@@ -46,16 +46,13 @@ struct TcParams {
     // tail split: the tiles of the last, partial wave [tail_first, ntotal) are cut into tail_z K ranges each so that they
     // spread over all SMs (448 tiles on 132 SMs: 3 + 52/132 rounds instead of 4); their partials are summed by a fix-up kernel
     int tail_first, tail_z, ntotal;
-    int tail_fix;                                 // 1: the K range that finishes LAST sums the tail_z partial tiles itself (no fix-up launch)
-    int* tail_cnt;                                // arrival counters of the tail tiles (zeroed before the launch)
-    FastDiv d_ntiles_p, d_cotiles, d_tiles_x, d_tiles_y, d_splits, d_tail_z;
+    FastDiv d_ntiles, d_cotiles, d_tiles_x, d_tiles_y, d_splits, d_tail_z;
     // Correlation on the same pipeline (corr_tc_forward): a unit = (sample, parity plane, 128-pixel tile of map 0, block of
     // cbw x cbh halo pixels of map 1); D[pixel][halo pixel] = <a, b> over C channels; the epilogue keeps the band that
     // lies inside the (2R+1)^2 displacement window.  W tiles are halo-pixel tiles of the pre-split map 1.
-    int corr, cR, cS, cD, cbw, cbh, cnx, cnt;
+    int cR, cS, cD, cbw, cbh, cnt;
     float cscale;
-    int cl, ntiles, ntiles_p, cotiles, total;     // cluster size (W multicast); pixel tiles (real / padded to cl), Co tiles, all tiles
-    float comp_a, comp_b;                         // RZ bias model: shrink(n MMAs) = comp_a + comp_b * n
+    int ntiles, cotiles, total;                   // pixel tiles, Co tiles, all tiles
     int gcs;                                      // tap-group packing for Ci <= 16: padded channels per tap (4/8/12/16), 0 = off
     // kernel-row packing for Ci <= 16 on a dense input (pixel stride == rcs floats, guard band around the blob): the kw taps
     // of one kernel row are CONTIGUOUS in memory for every output pixel, so one K block = 32 consecutive floats of that run.
@@ -64,7 +61,6 @@ struct TcParams {
     // the unshifted map, range of 32-pixel K segments); D[big channel][small channel] = sum over the segments' pixels.
     // Maps with few channels (wg_G = 8 .. 64 rows per tap) put 128 / wg_G taps side by side in one 128-row tile (wg_TPT).
     int wg_S, wg_ST, wg_BT, wg_segs, wg_segs_x, wg_sx, wg_G, wg_TPT, wg_taps;
-    int dbg;                                      // FN2_TC_DBG bits: 16 per-role wait-time profile
     short dy[49], dx[49], widx[49];
 };
 
@@ -89,7 +85,6 @@ struct TcTile {
     int n, u0, v0, co0, cls, tap0, ntaps, steps;
     int k0, split;                                // first K step of this unit, split index
     int slot;                                     // >= 0: raw partial sums go to workspace slot `slot` (tail split)
-    int tq;                                       // tail split: index of the tile among the tail tiles (slot / tail_z)
     bool valid;
 };
 // MODE (compile time, so that each instantiation's role loops stay small -- the all-in-one kernel had ~1900 SASS instructions in
@@ -138,23 +133,20 @@ __device__ __forceinline__ TcTile tc_decode_tile(const TcParams& p, int tile) {
         t.slot = tile - p.tail_first;
         int q;
         p.d_tail_z.divmod(t.slot, q, tseg);
-        t.tq = q;
         tile = p.tail_first + q;
     }
     if (p.splits > 1) { int q; p.d_splits.divmod(tile, q, t.split); tile = q; }   // splits of a tile run side by side (shared A tiles in L2)
     int pix, r, cot = 0;
-    p.d_ntiles_p.divmod(tile, r, pix);
+    p.d_ntiles.divmod(tile, r, pix);
     t.cls = 0;
     if (r) p.d_cotiles.divmod(r, t.cls, cot);
-    t.valid = pix < p.ntiles;
-    if (!t.valid) pix = 0;
     int tx, ty, q2;
     p.d_tiles_x.divmod(pix, q2, tx);
     p.d_tiles_y.divmod(q2, t.n, ty);
     t.u0 = ty * p.th; t.v0 = tx * p.tw;
     t.co0 = cot * NT;
     t.tap0 = p.cls_tap0[t.cls]; t.ntaps = p.cls_ntaps[t.cls];
-    if (t.u0 >= p.cls_Hu[t.cls] || t.v0 >= p.cls_Wu[t.cls]) t.valid = false;      // tile outside this (smaller) parity class
+    t.valid = t.u0 < p.cls_Hu[t.cls] && t.v0 < p.cls_Wu[t.cls];                   // false: tile outside this (smaller) parity class
     const int gsz = MODE == TC_GROUP ? 32 / p.gcs : 1;
     t.steps = MODE == TC_ROW ? p.rsteps : (MODE == TC_GROUP ? (t.ntaps + gsz - 1) / gsz : t.ntaps * p.cblocks);
     t.k0 = 0;
@@ -190,7 +182,7 @@ __device__ __forceinline__ void gather_taps(const unsigned char* base, int r0, i
 template <int NT, int MODE>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapW, const float* __restrict__ bias,
-               float* __restrict__ out, float* __restrict__ ws, const TcParams p, long long* __restrict__ prof) {
+               float* __restrict__ out, float* __restrict__ ws, const TcParams p) {
     using G = TcGeo<NT>;
     // MMA N: the correlation's halo block has cbw * cbh = 112 pixels (corr_tc_forward)
     constexpr int NM = MODE == TC_CORR ? 112 : NT;
@@ -199,34 +191,21 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + G::R * G::STAGE_BYTES + G::STG_BYTES);
     uint64_t* full = bars;                         // [R]  TMA bytes of the stage have landed
     uint64_t* done = bars + G::R;                  // [R]  MMAs of the step have retired: the stage is free
-    uint32_t* flag = reinterpret_cast<uint32_t*>(done + G::R);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     // Programmatic dependent launch: let the next kernel of the stream be scheduled as soon as every CTA of this one is
     // running, so that its CTAs take over SMs the moment ours exit and run their prologue (barrier init) there; it blocks
     // in griddepcontrol.wait (below, before its first global access) until this grid has completed.
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-    // CTAs of one cluster (p.cl consecutive blockIdx.x) always work on tiles with the same co0 and parity class, so they
-    // read the same W tiles: with p.cl > 1 each loads 1/cl of the rows and multicasts it to the whole cluster.  In that
-    // mode every CTA runs the full pipeline even for a tile outside the image/class (loads are zero-filled, nothing is
-    // stored); with p.cl == 1 such tiles are skipped.
-    const uint32_t crank = p.cl > 1 ? cluster_ctarank() : 0u;
-    const uint16_t cmask = (uint16_t)((1u << p.cl) - 1u);
-    const int wrows = NT / p.cl;                   // W rows this CTA loads per tile
     const int gsz = MODE == TC_GROUP ? 32 / p.gcs : 1;   // taps per K block when packing
-    const bool skip_invalid = p.cl == 1;
 
     if (tid == 0) {
-        // done[s]: one arrival per MMA warp (8) of every CTA that multicasts into this stage
-        for (int s = 0; s < G::R; s++) { mbar_init(&full[s], 1); mbar_init(&done[s], 8 * p.cl); }
+        // done[s]: one arrival per MMA warp (8)
+        for (int s = 0; s < G::R; s++) { mbar_init(&full[s], 1); mbar_init(&done[s], 8); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
-    if (p.cl > 1) cluster_sync_all();             // peers' barriers are initialised before any multicast can signal them
     asm volatile("griddepcontrol.wait;" ::: "memory");      // no-op unless launched with programmatic stream serialization
-    long long w0 = 0, w1 = 0;
-    const bool timed = prof != nullptr;
-    const long long t_start = clock64();
 
     if (warp < 4) {
         asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
@@ -237,17 +216,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
             int s = 0; uint32_t ph = 1u;                // ph: parity to wait on done[s]
             for (int tile = blockIdx.x; tile < p.total; tile += gridDim.x) {
                 const TcTile T = tc_decode_tile<NT, MODE>(p, tile);
-                if (!T.valid && skip_invalid) continue;
+                if (!T.valid) continue;
                 const int cx0 = T.v0 * p.su, cy0 = T.u0 * p.sv;
                 auto load_w = [&](unsigned char* st, uint64_t* bar, int c0, int blk) {
-                    unsigned char* wh = st + A_TILE_BYTES + crank * wrows * 128;
-                    if (p.cl > 1) {
-                        tma_load_4d_mc(wh, &mapW, bar, c0, T.co0 + crank * wrows, blk, 0, cmask);
-                        tma_load_4d_mc(wh + G::B_TILE_BYTES, &mapW, bar, c0, T.co0 + crank * wrows, blk, 1, cmask);
-                    } else {
-                        tma_load_4d(wh, &mapW, bar, c0, T.co0, blk, 0);
-                        tma_load_4d(wh + G::B_TILE_BYTES, &mapW, bar, c0, T.co0, blk, 1);
-                    }
+                    tma_load_4d(st + A_TILE_BYTES, &mapW, bar, c0, T.co0, blk, 0);
+                    tma_load_4d(st + A_TILE_BYTES + G::B_TILE_BYTES, &mapW, bar, c0, T.co0, blk, 1);
                 };
                 if constexpr (MODE == TC_CORR) {
                     const int py = T.cls / p.cS, px = T.cls % p.cS;
@@ -256,7 +229,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                     const uint32_t bbytes = (uint32_t)(p.cbw * p.cbh * 128);
 #pragma unroll 1
                     for (int i = 0; i < T.steps; i++) {
-                        mbar_wait_t(&done[s], ph, &w0, timed);
+                        mbar_wait(&done[s], ph);
                         unsigned char* st = smem + (size_t)s * G::STAGE_BYTES;
                         mbar_expect_tx(&full[s], (uint32_t)A_TILE_BYTES + 2u * bbytes);
                         tma_load_4d(st, &mapA, &full[s], i * 32, ax, ay, T.n);
@@ -275,7 +248,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                     const int tpt = p.wg_TPT, gbytes = p.wg_G * 128;
 #pragma unroll 1
                     for (int i = 0; i < T.steps; i++) {
-                        mbar_wait_t(&done[s], ph, &w0, timed);
+                        mbar_wait(&done[s], ph);
                         unsigned char* st = smem + (size_t)s * G::STAGE_BYTES;
                         mbar_expect_tx(&full[s], (uint32_t)G::STAGE_BYTES);
                         for (int j = 0; j < tpt; j++) {
@@ -294,7 +267,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                     int r = 0, kb = 0;
 #pragma unroll 1
                     for (int i = 0; i < T.steps; i++) {
-                        mbar_wait_t(&done[s], ph, &w0, timed);
+                        mbar_wait(&done[s], ph);
                         unsigned char* st = smem + (size_t)s * G::STAGE_BYTES;
                         mbar_expect_tx(&full[s], (uint32_t)G::STAGE_BYTES);
                         tma_load_4d(st, &mapA, &full[s], kb * 32, T.v0, cy0 + p.dy[r * p.rkw], T.n);
@@ -306,7 +279,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                     // several taps share one 32-wide K block: one small box {gcs channels, tw, th} per tap
                     const int box_bytes = 128 * gcs * 4;
                     for (int i = 0, t0 = 0; i < T.steps; i++, t0 += gsz) {
-                        mbar_wait_t(&done[s], ph, &w0, timed);
+                        mbar_wait(&done[s], ph);
                         unsigned char* st = smem + (size_t)s * G::STAGE_BYTES;
                         const int nt = min(gsz, T.ntaps - t0);
                         mbar_expect_tx(&full[s], (uint32_t)(nt * box_bytes + 2 * G::B_TILE_BYTES));
@@ -322,7 +295,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                     int cx = cx0 + p.dx[t], cy = cy0 + p.dy[t], wi = p.widx[t];
 #pragma unroll 1
                     for (int i = 0; i < T.steps; i++) {
-                        mbar_wait_t(&done[s], ph, &w0, timed);
+                        mbar_wait(&done[s], ph);
                         unsigned char* st = smem + (size_t)s * G::STAGE_BYTES;
                         mbar_expect_tx(&full[s], (uint32_t)G::STAGE_BYTES);
                         tma_load_4d(st, &mapA, &full[s], cb * 32, cx, cy, T.n);
@@ -347,7 +320,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
         uint32_t ph = 0;
         for (int tile = blockIdx.x; tile < p.total; tile += gridDim.x) {
             const TcTile T = tc_decode_tile<NT, MODE>(p, tile);
-            if (!T.valid && skip_invalid) continue;
+            if (!T.valid) continue;
             float acc[NH];
 #pragma unroll
             for (int j = 0; j < NH; j++) acc[j] = 0.f;
@@ -356,7 +329,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
             int in_chunk = 0;
 #pragma unroll 1
             for (int i = 0; i < T.steps; i++) {
-                mbar_wait_t(&full[s], ph, &w0, timed);
+                mbar_wait(&full[s], ph);
                 const unsigned char* st = smem + (size_t)s * G::STAGE_BYTES;
                 uint32_t ah[16], al[16];
                 if constexpr (MODE == TC_GROUP) {
@@ -419,15 +392,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                 for (int j = 0; j < (int)(sizeof(c) / sizeof(float)); j++) reg_fence(c[j]);
 #pragma unroll
                 for (int j = 0; j < (int)(sizeof(cx) / sizeof(float)); j++) reg_fence(cx[j]);
-                // this warp's MMAs of the step have retired: release the stage (to every CTA that multicasts into it)
+                // this warp's MMAs of the step have retired: release the stage
                 __syncwarp();
-                if (lane == 0) {
-                    if (p.cl > 1) { for (int r = 0; r < p.cl; r++) mbar_arrive_cluster(&done[s], (uint32_t)r); }
-                    else mbar_arrive(&done[s]);
-                }
+                if (lane == 0) mbar_arrive(&done[s]);
                 if (chunk_end) {
                     // mean truncation loss of the a_hi*w_hi chain of this chunk
-                    const float comp = p.comp_a + p.comp_b * (float)(G::MMAS_PER_STEP * (in_chunk + 1));
+                    const float comp = TRUNC_LOSS_PER_MMA * (float)(G::MMAS_PER_STEP * (in_chunk + 1));
                     if constexpr (G::WIDE) {
 #pragma unroll
                         for (int j = 0; j < NH; j++) acc[j] += fmaf(c[j], comp, c[j]) + (c[NH + j] + cx[j]);
@@ -492,49 +462,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                 continue;
             }
             const int u = T.u0 + yy, v = T.v0 + xx;
-            if (MODE == TC_PLAIN && T.slot >= 0 && p.tail_fix) {
-                // tail split, fixed up in the kernel: every K range stores its raw partial tile; the range that arrives LAST (an
-                // atomic counter per tile) sums the tail_z partials in slot order -- the order does not depend on who is last -- and
-                // writes the finished tile.
-                const bool live = T.valid && u < p.cls_Hu[T.cls] && v < p.cls_Wu[T.cls];
-                float* o = ws + ((long long)T.slot * 128 + m) * NT + hf * NH;
-#pragma unroll
-                for (int j = 0; j < NH; j += 4) *reinterpret_cast<float4*>(o + j) = *reinterpret_cast<const float4*>(srow + j);
-                __threadfence();
-                asm volatile("bar.sync 1, 256;" ::: "memory");
-                if (ct == 0) {
-                    const int prev = atomicAdd(p.tail_cnt + T.tq, 1);
-                    const bool l = prev == p.tail_z - 1;
-                    if (l) p.tail_cnt[T.tq] = 0;                         // everybody has arrived: leave the counter ready for the next launch
-                    *flag = l ? 1u : 0u;
-                }
-                asm volatile("bar.sync 1, 256;" ::: "memory");
-                const bool last = *flag != 0;
-                asm volatile("bar.sync 1, 256;" ::: "memory");            // flag is rewritten by the next tail unit
-                if (last && live) {
-                    __threadfence();
-                    const int oy = u * p.ou + p.cls_oy0[T.cls], ox = v * p.ov + p.cls_ox0[T.cls];
-                    float* dst = out + T.n * p.out_sn + (long long)oy * p.out_sh + (long long)ox * p.out_sw + T.co0 + hf * NH;
-                    const float* src = ws + ((long long)T.tq * p.tail_z * 128 + m) * NT + hf * NH;
-#pragma unroll 4
-                    for (int j = 0; j < NH; j += 4) {
-                        float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
-                        for (int z = 0; z < p.tail_z; z++) {
-                            const float4 x = __ldcg(reinterpret_cast<const float4*>(src + (long long)z * 128 * NT + j));
-                            a.x += x.x; a.y += x.y; a.z += x.z; a.w += x.w;
-                        }
-                        float r[4] = {a.x, a.y, a.z, a.w};
-#pragma unroll
-                        for (int e = 0; e < 4; e++) {
-                            if (p.has_bias) r[e] += __ldg(bias + T.co0 + hf * NH + j + e);
-                            if (p.relu) r[e] = r[e] > 0 ? r[e] : r[e] * p.slope;
-                        }
-                        *reinterpret_cast<float4*>(dst + j) = make_float4(r[0], r[1], r[2], r[3]);
-                    }
-                }
-                continue;
-            }
-            if (T.valid && u < p.cls_Hu[T.cls] && v < p.cls_Wu[T.cls]) {
+            if (u < p.cls_Hu[T.cls] && v < p.cls_Wu[T.cls]) {
                 const int oy = u * p.ou + p.cls_oy0[T.cls], ox = v * p.ov + p.cls_ox0[T.cls];
                 if (T.slot >= 0) {
                     // tail split: raw partial sums of this K range, [slot][128 pixels][NT]
@@ -563,12 +491,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
             }
         }
     }
-    if (prof && blockIdx.x == gridDim.x / 2 && lane == 0 && (warp == 0 || warp == 4)) {
-        long long* o = prof + (warp == 0 ? 0 : 4);
-        o[0] = clock64() - t_start; o[1] = w0; o[2] = w1; o[3] = 0;
-    }
     __syncthreads();
-    if (p.cl > 1) cluster_sync_all();             // no CTA leaves while a peer may still multicast into it / signal its barriers
 }
 
 __global__ void tc_pack_kernel(const float* __restrict__ w, float* __restrict__ wp, int Ci, int Co, int kh, int kw, int cip, int deconv) {
@@ -581,13 +504,7 @@ __global__ void tc_pack_kernel(const float* __restrict__ w, float* __restrict__ 
         const int r = t / kw, s = t % kw;
         float v = 0.f;
         if (ci < Ci) v = deconv ? w[(((long long)ci * Co + co) * kh + r) * kw + s] : w[(((long long)co * Ci + ci) * kh + r) * kw + s];
-        uint32_t h;
-        asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(h) : "f"(v));
-        const float hi = __uint_as_float(h);
-        uint32_t l;
-        asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(l) : "f"(v - hi));
-        wp[idx] = hi;
-        wp[per + idx] = __uint_as_float(l);
+        store_tf32_split(wp, per, idx, v);
     }
 }
 
@@ -604,13 +521,7 @@ __global__ void tc_pack_group_kernel(const float* __restrict__ w, float* __restr
         const int t = g * gs + j;
         float v = 0.f;
         if (j < gs && t < kh * kw && ci < Ci) v = w[(((long long)co * Ci + ci) * kh + t / kw) * kw + t % kw];
-        uint32_t h;
-        asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(h) : "f"(v));
-        const float hi = __uint_as_float(h);
-        uint32_t l;
-        asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(l) : "f"(v - hi));
-        wp[idx] = hi;
-        wp[per + idx] = __uint_as_float(l);
+        store_tf32_split(wp, per, idx, v);
     }
 }
 
@@ -626,13 +537,7 @@ __global__ void tc_pack_row_kernel(const float* __restrict__ w, float* __restric
         const int sx = kk / cs, ci = kk % cs;
         float v = 0.f;
         if (sx < kw && ci < Ci) v = w[(((long long)co * Ci + ci) * kh + r) * kw + sx];
-        uint32_t h;
-        asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(h) : "f"(v));
-        const float hi = __uint_as_float(h);
-        uint32_t l;
-        asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(l) : "f"(v - hi));
-        wp[idx] = hi;
-        wp[per + idx] = __uint_as_float(l);
+        store_tf32_split(wp, per, idx, v);
     }
 }
 
@@ -690,25 +595,17 @@ __global__ void tc_tail_reduce_kernel(const float* __restrict__ ws, const float*
     }
 }
 
-// Arrival counters of the in-kernel tail fix-up: a pool of zeroed regions handed out round-robin per launch (captured launches keep
-// theirs).  Every launch leaves its counters at zero again (the last arriver resets them), so a region may be reused as soon as the
-// launch that had it has finished; with 256 regions that is 256 tail-split launches later.
-constexpr int TAIL_CNT_REGION = 1024, TAIL_CNT_REGIONS = 256;
-static int* tc_tail_counters() {
-    static int* pool = nullptr;
-    static std::mutex mu;
-    static unsigned next = 0;
-    std::lock_guard<std::mutex> lk(mu);
-    if (!pool) {
-        if (cudaMalloc(&pool, (size_t)TAIL_CNT_REGION * TAIL_CNT_REGIONS * sizeof(int)) != cudaSuccess) { pool = nullptr; return nullptr; }
-        cudaMemset(pool, 0, (size_t)TAIL_CNT_REGION * TAIL_CNT_REGIONS * sizeof(int));
+int tc_enabled() {
+    static int v = -1;
+    if (v < 0) {
+        const char* e = getenv("FN2_TC");
+        v = (e && e[0] == '0') ? 0 : 1;
     }
-    return pool + (size_t)(next++ % TAIL_CNT_REGIONS) * TAIL_CNT_REGION;
+    return v;
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+}  // namespace
+
 EncodeTiledFn tc_encode_fn() {
     static EncodeTiledFn fn = nullptr;
     static std::once_flag once;
@@ -721,35 +618,10 @@ EncodeTiledFn tc_encode_fn() {
     return fn;
 }
 
-// FN2_TC_DBG & 16: per-role wait-time profile of CTA (0,0,0), printed by fn2_tc_prof_dump()
-int tc_pdl_enabled() {
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("FN2_TC_PDL"); v = (e && e[0] == '0') ? 0 : 1; }
-    return v;
-}
-int tc_num_sms() {
-    static int n = 0;
-    if (!n) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); if (n <= 0) n = 132; }
-    return n;
-}
-
-long long* tc_prof_buffer() {
-    static long long* buf = nullptr;
-    static int on = -1;
-    if (on < 0) { const char* e = getenv("FN2_TC_DBG"); on = (e && (atoi(e) & 16)) ? 1 : 0; if (on) { cudaMalloc(&buf, 16 * sizeof(long long)); cudaMemset(buf, 0, 16 * sizeof(long long)); } }
-    return buf;
-}
-
-int tc_enabled() {
-    static int v = -1;
-    if (v < 0) {
-        const char* e = getenv("FN2_TC");
-        v = (e && e[0] == '0') ? 0 : 1;
-    }
-    return v;
-}
-
-}  // namespace
+// output channels per tile (MMA N) of a layer with `co` output channels
+static int tc_nt(int co) { return (co % 128 == 0) ? 128 : (co % 64 == 0 ? 64 : (co % 32 == 0 ? 32 : 16)); }
+// K steps per accumulation chunk: NT == 128 chains the cross terms into the chunk accumulator too, so its chunks are one step
+static int tc_chunk_steps(int NT) { return NT == 128 ? 1 : 4; }
 
 // Small-Ci packing (plain convolutions with at most 16 input channels): mode 1 = tap groups (several taps share a 32-wide
 // K block, one small TMA box per tap), mode 2 = kernel rows (needs a dense input whose pixel stride equals the padded
@@ -758,13 +630,12 @@ struct TcSmallCi { int mode, cs, gs, ngroups, rblocks; };
 static TcSmallCi tc_small_ci(const fn2_conv_desc* d, int ci_stride) {
     TcSmallCi m = {0, 0, 0, 0, 0};
     if (d->deconv || d->ci > 16 || d->kh * d->kw < 2) return m;
-    if (getenv("FN2_TC_NOPACK")) return m;
     m.cs = (d->ci + 3) / 4 * 4;
     m.gs = 32 / m.cs;
     m.ngroups = (d->kh * d->kw + m.gs - 1) / m.gs;
     m.rblocks = (d->kw * m.cs + 31) / 32;
     m.mode = 1;
-    if (d->input_guard_bytes >= 512 && ci_stride == m.cs && d->kh * m.rblocks <= m.ngroups && !getenv("FN2_TC_NOROW")) m.mode = 2;
+    if (d->input_guard_bytes >= 512 && ci_stride == m.cs && d->kh * m.rblocks <= m.ngroups) m.mode = 2;
     return m;
 }
 
@@ -773,8 +644,7 @@ static TcSmallCi tc_small_ci(const fn2_conv_desc* d, int ci_stride) {
 // tail split plan for a layer with `tiles` tile units of `steps` K steps each: returns z (1 = off) and the first tail tile
 static int tc_tail_plan(long long tiles, int steps, int* first, int NT = 128) {
     *first = (int)tiles;
-    if (getenv("FN2_TC_NOTAIL")) return 1;
-    const int nsm = tc_num_sms();
+    const int nsm = num_sms();
     if (steps < 16) return 1;                       // (tiles <= nsm: everything is "tail" -- 112 tiles become 560 fifths on 132 SMs)
     const long long full = tiles / nsm * nsm, r = tiles - full;
     if (r == 0) return 1;
@@ -794,7 +664,7 @@ static int tc_tail_plan(long long tiles, int steps, int* first, int NT = 128) {
 }
 // tile count / K steps of a layer (same tiling rules as conv_tc_forward)
 static void tc_layer_geometry(const fn2_conv_desc* d, int N, int Ho, int Wo, int* NTo, long long* tiles, int* steps) {
-    const int NT = (d->co % 128 == 0) ? 128 : (d->co % 64 == 0 ? 64 : (d->co % 32 == 0 ? 32 : 16));
+    const int NT = tc_nt(d->co);
     const int sh = d->deconv ? d->stride_h : 1, sw = d->deconv ? d->stride_w : 1;
     const int Hu = (Ho + sh - 1) / sh, Wu = (Wo + sw - 1) / sw, ncls = min(sh, Ho) * min(sw, Wo);
     int tw = 8;
@@ -807,19 +677,11 @@ static void tc_layer_geometry(const fn2_conv_desc* d, int N, int Ho, int Wo, int
 }
 
 static int tc_split_plan(const fn2_conv_desc* d, int N, int Ho, int Wo) {
-    if (getenv("FN2_TC_NOSPLIT")) return 1;
     if (!d->deconv && d->ci <= 16) return 1;                       // small-Ci packing modes do not split
     if (d->co % 16) return 1;
-    const int NT = (d->co % 128 == 0) ? 128 : (d->co % 64 == 0 ? 64 : (d->co % 32 == 0 ? 32 : 16));
-    const int sh = d->deconv ? d->stride_h : 1, sw = d->deconv ? d->stride_w : 1;
-    const int Hu = (Ho + sh - 1) / sh, Wu = (Wo + sw - 1) / sw, ncls = min(sh, Ho) * min(sw, Wo);
-    int tw = 8;
-    while (tw < Wu && tw < 128) tw *= 2;
-    const int th = 128 / tw;
-    const long long tiles = (long long)N * ((Wu + tw - 1) / tw) * ((Hu + th - 1) / th) * (d->co / NT) * ncls;
-    const int ntaps = d->deconv ? max(1, d->kh / sh) * max(1, d->kw / sw) : d->kh * d->kw;
-    const int steps = ntaps * ((d->ci + 31) / 32);
-    const int nsm = tc_num_sms();
+    int NT, steps; long long tiles;
+    tc_layer_geometry(d, N, Ho, Wo, &NT, &tiles, &steps);
+    const int nsm = num_sms();
     if (tiles * 2 > nsm || steps < 32) return 1;
     int z = (int)(nsm / tiles);
     z = min(z, steps / 16);
@@ -915,35 +777,22 @@ int conv_tc_forward(const fn2_conv_desc* d, const T4& in, const float* wp, const
     if (conv_tn_applicable(d)) return conv_tn_forward(d, in, wp, bias, out, st);
     EncodeTiledFn enc = tc_encode_fn();
     if (!enc) { set_error("conv_tc: cuTensorMapEncodeTiled unavailable"); return FN2_ERR_CUDA; }
-    const int NT = (d->co % 128 == 0) ? 128 : (d->co % 64 == 0 ? 64 : (d->co % 32 == 0 ? 32 : 16));
+    const int NT = tc_nt(d->co);
     const int cip = (d->ci + 31) / 32 * 32;
     TcParams p;
-    p.corr = 0;
     p.N = in.n; p.Co = d->co; p.cblocks = cip / 32;
     p.Ho = out.h; p.Wo = out.w;
     p.splits = tc_split_plan(d, in.n, out.h, out.w);
     if (p.splits > 1 && (!ws || ws_floats < (size_t)p.splits * in.n * out.h * out.w * d->co)) p.splits = 1;
     p.out_sn = out.sn; p.out_sh = out.sh; p.out_sw = out.sw;
     p.relu = d->relu; p.has_bias = d->has_bias; p.slope = d->negative_slope;
-    // chunk length in K steps: NT == 128 chains the cross terms into the chunk accumulator too, so its chunks are one step
-    p.kd = NT == 128 ? 1 : 4;
-    if (const char* e = getenv(NT == 128 ? "FN2_TC_KD" : "FN2_TC_KDW")) { const int v = atoi(e); if (v >= 1 && v <= 1024) p.kd = v; }
-    const char* nocomp = getenv("FN2_TC_COMP");
-    // mean relative truncation loss of one chunk = comp_a + comp_b * n, n = a_hi*w_hi MMAs chained into the chunk accumulator
-    // (4 per step; with NT == 128 the 8 cross-term MMAs of a step precede them while the accumulator is still small).
-    // H100: ~1.1e-8 .. 1.3e-8 per truncating MMA and no constant term, from the mean signed errors of the tensor-core parity
-    // cases of tests/test_ops_gpu.py run with the earlier tensor core's constants (2.0e-8 + 1.67e-8 n overcorrected by 1e-7).
-    p.comp_a = 0.f;
-    p.comp_b = (nocomp && nocomp[0] == '0') ? 0.f : 1.3e-8f;
-    if (const char* e = getenv("FN2_TC_COMP_A")) p.comp_a = (float)atof(e);
-    if (const char* e = getenv("FN2_TC_COMP_B")) p.comp_b = (float)atof(e);
-    { const char* e = getenv("FN2_TC_DBG"); p.dbg = e ? atoi(e) : 0; }
+    // the kernel adds back the mean truncation loss of each chunk: TRUNC_LOSS_PER_MMA per a_hi*w_hi MMA chained into the
+    // chunk accumulator (4 per step; with NT == 128 the 8 cross-term MMAs of a step precede them while it is still small)
+    p.kd = tc_chunk_steps(NT);
 
     const TcSmallCi sm = tc_small_ci(d, (int)in.sw);
     p.gcs = sm.mode == 1 ? sm.cs : 0;
     p.rowmode = sm.mode == 2; p.rcs = sm.cs; p.rblocks = sm.rblocks; p.rsteps = d->kh * sm.rblocks; p.rkw = d->kw; p.rpad = d->pad_w; p.rW = in.w;
-    { const char* e = getenv("FN2_TC_CL"); p.cl = e ? atoi(e) : 1; if (p.cl != 1 && p.cl != 2 && p.cl != 4) p.cl = 1; if (NT / p.cl < 8) p.cl = NT / 8; }
-    if (p.cl > 1) p.splits = 1;                   // cluster mates must walk the same K steps to share W tiles
     // weights: [2][taps][Co][cip]   (group mode: [2][groups][Co][32])
     CUtensorMap mapW;
     {
@@ -951,7 +800,7 @@ int conv_tc_forward(const fn2_conv_desc* d, const T4& in, const float* wp, const
         const int nblk = sm.mode == 2 ? p.rsteps : (sm.mode == 1 ? sm.ngroups : d->kh * d->kw);
         cuuint64_t dims[4] = {(cuuint64_t)kin, (cuuint64_t)d->co, (cuuint64_t)nblk, 2};
         cuuint64_t strides[3] = {(cuuint64_t)kin * 4, (cuuint64_t)kin * d->co * 4, (cuuint64_t)kin * d->co * nblk * 4};
-        cuuint32_t box[4] = {32, (cuuint32_t)(NT / p.cl), 1, 1};
+        cuuint32_t box[4] = {32, (cuuint32_t)NT, 1, 1};
         cuuint32_t es[4] = {1, 1, 1, 1};
         CUresult r = enc(&mapW, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void*)wp, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
                          CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -985,37 +834,28 @@ int conv_tc_forward(const fn2_conv_desc* d, const T4& in, const float* wp, const
                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) { set_error("conv_tc: activation tensor map failed (%d)", (int)r); return FN2_ERR_CUDA; }
         p.ntiles = p.N * p.tiles_x * p.tiles_y;
-        p.ntiles_p = (p.ntiles + p.cl - 1) / p.cl * p.cl;
         p.cotiles = d->co / NT;
-        p.total = p.ntiles_p * p.cotiles * p.ncls * p.splits;
-        p.ntotal = p.total; p.tail_first = p.total; p.tail_z = 1; p.tail_fix = 0; p.tail_cnt = nullptr;
-        p.d_ntiles_p.init(p.ntiles_p); p.d_cotiles.init(p.cotiles); p.d_tiles_x.init(p.tiles_x); p.d_tiles_y.init(p.tiles_y);
+        p.total = p.ntiles * p.cotiles * p.ncls * p.splits;
+        p.ntotal = p.total; p.tail_first = p.total; p.tail_z = 1;
+        p.d_ntiles.init(p.ntiles); p.d_cotiles.init(p.cotiles); p.d_tiles_x.init(p.tiles_x); p.d_tiles_y.init(p.tiles_y);
         p.d_splits.init(max(1, p.splits)); p.d_tail_z.init(1);
-        if (p.splits == 1 && p.cl == 1 && !sm.mode && ws) {
+        if (p.splits == 1 && !sm.mode && ws) {
             int first = 0, steps_min = 1 << 30;
             for (int c = 0; c < p.ncls; c++) steps_min = min(steps_min, p.cls_ntaps[c] * p.cblocks);
             const int tz = tc_tail_plan(p.total, steps_min, &first, NT);
             if (tz > 1 && ws_floats >= (size_t)(p.total - first) * tz * 128 * NT) {
                 p.tail_first = first; p.tail_z = tz; p.d_tail_z.init(tz);
                 p.total = first + (p.ntotal - first) * tz;
-                // FN2_TC_TAILFIX=1: the last K range to arrive sums the partial tiles inside the kernel instead of a fix-up launch.
-                // Off by default: the last arriver's MMA warpgroups hold their SM while they re-read tail_z tiles, whereas the separate
-                // kernel spreads that over all SMs and overlaps the next layer's prologue (PDL).
-                static const bool fix = getenv("FN2_TC_TAILFIX") != nullptr;
-                p.tail_cnt = (fix && p.ntotal - first <= TAIL_CNT_REGION) ? tc_tail_counters() : nullptr;
-                p.tail_fix = p.tail_cnt ? 1 : 0;
             }
         }
         cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3((unsigned)min(p.total, tc_num_sms() / p.cl * p.cl), 1, 1);
+        cfg.gridDim = dim3((unsigned)min(p.total, num_sms()), 1, 1);
         cfg.blockDim = dim3(TC_THREADS);
         cfg.stream = st;
-        cudaLaunchAttribute attr[2];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = (unsigned)p.cl; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-        attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[1].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = attr; cfg.numAttrs = tc_pdl_enabled() ? 2 : 1;
+        cudaLaunchAttribute attr[1];
+        attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+        attr[0].val.programmaticStreamSerializationAllowed = 1;
+        cfg.attrs = attr; cfg.numAttrs = 1;
 #define FN2_TC_LAUNCH(NTV, MODEV)                                                                                       \
         {                                                                                                               \
             static bool attr_set = false;                                                                               \
@@ -1024,7 +864,7 @@ int conv_tc_forward(const fn2_conv_desc* d, const T4& in, const float* wp, const
                 attr_set = true;                                                                                        \
             }                                                                                                           \
             cfg.dynamicSmemBytes = TcGeo<NTV>::SMEM;                                                                    \
-            FN2_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<NTV, MODEV>, mapA, mapW, bias, out.p, ws, p, tc_prof_buffer())); \
+            FN2_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<NTV, MODEV>, mapA, mapW, bias, out.p, ws, p));                  \
         }
 #define FN2_TC_LAUNCH_NT(MODEV)                                                                                         \
         if (NT == 128) FN2_TC_LAUNCH(128, MODEV)                                                                        \
@@ -1037,7 +877,7 @@ int conv_tc_forward(const fn2_conv_desc* d, const T4& in, const float* wp, const
 #undef FN2_TC_LAUNCH_NT
 #undef FN2_TC_LAUNCH
         FN2_LAUNCH_CHECK();
-        if (p.tail_z > 1 && !p.tail_fix) {
+        if (p.tail_z > 1) {
             const long long work = (long long)(p.ntotal - p.tail_first) * 128 * (NT / 4);
             if (NT == 128) tc_tail_reduce_kernel<128><<<ew_grid(work, 256), 256, 0, st>>>(ws, bias, out.p, p);
             else if (NT == 64) tc_tail_reduce_kernel<64><<<ew_grid(work, 256), 256, 0, st>>>(ws, bias, out.p, p);
@@ -1153,19 +993,16 @@ static WgPlan wg_plan(const fn2_conv_desc* d, int N, int H, int W) {
     g.NT = g.Cs >= 128 ? 128 : (g.Cs >= 64 ? 64 : (g.Cs >= 32 ? 32 : 16));
     g.BT = (g.Cb + 127) / 128; g.ST = (g.Cs + g.NT - 1) / g.NT;
     g.G = 128;
-    if (g.Cb <= 64 && !getenv("FN2_WG_NOGROUP")) { g.G = 8; while (g.G < g.Cb) g.G *= 2; }
+    if (g.Cb <= 64) { g.G = 8; while (g.G < g.Cb) g.G *= 2; }
     g.TPT = 128 / g.G; g.TG = (g.taps + g.TPT - 1) / g.TPT;
     g.segs_x = (g.Ws + 31) / 32; g.segs = N * g.Hs * g.segs_x;
     const int base = g.TG * g.BT * g.ST;
-    int S = (3 * tc_num_sms() + base - 1) / base;
-    S = max(1, min(S, g.segs / 8));
-    if (const char* e = getenv("FN2_WG_SPLITS")) { const int v = atoi(e); if (v >= 1) S = min(v, max(1, g.segs)); }
-    g.S = S;
+    g.S = max(1, min((3 * num_sms() + base - 1) / base, g.segs / 8));
     g.Wq = (g.Wb + g.sx - 1) / g.sx + 3;          // + 3: room for the column delay of the 4 copies
     g.Wq_p = (g.Wq + 3) / 4 * 4; g.Ws_p = (g.Ws + 3) / 4 * 4;
     g.big_floats = up64((size_t)4 * N * g.Cb * g.Hb * g.sx * g.Wq_p);          // 4 copies, delayed by 0..3 columns
     g.small_floats = up64((size_t)2 * N * g.Cs * g.Hs * g.Ws_p);
-    g.part_floats = up64((size_t)base * S * 128 * g.NT);
+    g.part_floats = up64((size_t)base * g.S * 128 * g.NT);
     // the top diff is the small map of a convolution and the big map of a deconvolution
     g.bias_blocks = d->deconv ? ((g.Wq_p + 127) / 128) * (N * g.Hb * g.sx) : ((g.Ws_p + 127) / 128) * (N * g.Hs);
     g.bias_floats = d->has_bias ? up64((size_t)g.bias_blocks * d->co) : 0;
@@ -1260,7 +1097,7 @@ __global__ void wg_reduce_kernel(const float* __restrict__ part, float* __restri
 }
 
 int conv_tc_wgrad_eligible(const fn2_conv_desc* d) {
-    if (!tc_enabled() || getenv("FN2_WGRAD_SIMT") || d->engine == 1) return 0;      // engine 1 = `engine: CAFFE`: exact-FP32 SIMT everywhere
+    if (!tc_enabled() || d->engine == 1) return 0;      // engine 1 = `engine: CAFFE`: exact-FP32 SIMT everywhere
     if (d->kh * d->kw > 49 || d->stride_w > 8 || d->stride_h > 8) return 0;
     if (!tc_encode_fn()) return 0;
     return 1;
@@ -1307,15 +1144,11 @@ int conv_tc_wgrad(const fn2_conv_desc* d, const T4& bottom, const T4& top_diff, 
     memset(&p, 0, sizeof(p));
     p.N = g.N; p.Co = g.Cs; p.cblocks = 1;
     p.Ho = g.Hs; p.Wo = g.Ws;
-    p.splits = 1; p.cl = 1; p.tail_z = 1; p.su = g.sx; p.sv = g.sy; p.ou = p.ov = 1; p.ncls = 1;
+    p.splits = 1; p.tail_z = 1; p.su = g.sx; p.sv = g.sy; p.ou = p.ov = 1; p.ncls = 1;
     p.tw = 128; p.th = 1; p.tiles_x = p.tiles_y = 1;
     p.wg_S = g.S; p.wg_ST = g.ST; p.wg_BT = g.BT; p.wg_segs = g.segs; p.wg_segs_x = g.segs_x; p.wg_sx = g.sx;
     p.wg_G = g.G; p.wg_TPT = g.TPT; p.wg_taps = g.taps;
-    p.kd = g.NT == 128 ? 1 : 4;
-    if (const char* e = getenv(g.NT == 128 ? "FN2_TC_KD" : "FN2_TC_KDW")) { const int v = atoi(e); if (v >= 1 && v <= 1024) p.kd = v; }
-    const char* nocomp = getenv("FN2_TC_COMP");
-    p.comp_a = 0.f;
-    p.comp_b = (nocomp && nocomp[0] == '0') ? 0.f : 1.3e-8f;
+    p.kd = tc_chunk_steps(g.NT);
     for (int ky = 0; ky < d->kh; ky++)
         for (int kx = 0; kx < d->kw; kx++) {
             const int t = ky * d->kw + kx, q = kx - d->pad_w;
@@ -1345,13 +1178,9 @@ int conv_tc_wgrad(const fn2_conv_desc* d, const T4& bottom, const T4& top_diff, 
         if (r != CUDA_SUCCESS) { set_error("conv_tc_wgrad: small-map tensor map failed (%d)", (int)r); return FN2_ERR_CUDA; }
     }
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)min(p.total, tc_num_sms()), 1, 1);
+    cfg.gridDim = dim3((unsigned)min(p.total, num_sms()), 1, 1);
     cfg.blockDim = dim3(TC_THREADS);
     cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 1; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
 #define FN2_WG_LAUNCH(NTV)                                                                                              \
     {                                                                                                                   \
         static bool attr_set = false;                                                                                   \
@@ -1360,7 +1189,7 @@ int conv_tc_wgrad(const fn2_conv_desc* d, const T4& bottom, const T4& top_diff, 
             attr_set = true;                                                                                            \
         }                                                                                                               \
         cfg.dynamicSmemBytes = TcGeo<NTV>::SMEM;                                                                        \
-        FN2_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<NTV, TC_WGRAD>, mapA, mapB, (const float*)nullptr, (float*)nullptr, part, p, tc_prof_buffer())); \
+        FN2_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<NTV, TC_WGRAD>, mapA, mapB, (const float*)nullptr, (float*)nullptr, part, p)); \
     }
     if (g.NT == 128) FN2_WG_LAUNCH(128)
     else if (g.NT == 64) FN2_WG_LAUNCH(64)
@@ -1395,20 +1224,16 @@ int corr_tc_forward(const T4& b0, const T4& b1, const T4& top, int md, int s2, f
     constexpr int NT = 128;
     TcParams p;
     memset(&p, 0, sizeof(p));
-    p.corr = 1; p.cR = R; p.cS = S; p.cD = 2 * R + 1;
+    p.cR = R; p.cS = S; p.cD = 2 * R + 1;
     p.tw = 8; p.th = 16;                                                   // halo 28 x 36
     p.cbw = p.tw + 2 * R; p.cbh = 4;                                       // block = 4 full halo rows = 112 pixels (MMA N = 112)
-    p.cnx = 1; p.cnt = (p.th + 2 * R) / p.cbh;                             // 9 blocks
+    p.cnt = (p.th + 2 * R) / p.cbh;                             // 9 blocks
     p.cscale = 1.0f / (float)C;                                           // sumelems = k*k*C (correlation_layer.cu:108)
     p.N = N; p.Co = NT; p.cblocks = C / 32;
     p.Ho = H; p.Wo = W;
     p.out_sn = top.sn; p.out_sh = top.sh; p.out_sw = top.sw;
-    p.splits = 1; p.cl = 1; p.tail_z = 1; p.su = S; p.sv = S; p.ou = p.ov = 1; p.ncls = 1;
-    p.kd = 1;                                                             // NT == 128: one K step per chunk (see conv_tc_forward)
-    if (const char* e = getenv("FN2_TC_KD")) { const int v = atoi(e); if (v >= 1 && v <= 1024) p.kd = v; }
-    const char* nocomp = getenv("FN2_TC_COMP");
-    p.comp_a = 0.f;
-    p.comp_b = (nocomp && nocomp[0] == '0') ? 0.f : 1.3e-8f;
+    p.splits = 1; p.tail_z = 1; p.su = S; p.sv = S; p.ou = p.ov = 1; p.ncls = 1;
+    p.kd = tc_chunk_steps(NT);
     const int Ws = (W + S - 1) / S, Hs = (H + S - 1) / S;
     p.tiles_x = (Ws + p.tw - 1) / p.tw; p.tiles_y = (Hs + p.th - 1) / p.th;
     p.total = N * S * S * p.tiles_x * p.tiles_y * p.cnt;
@@ -1433,13 +1258,9 @@ int corr_tc_forward(const T4& b0, const T4& b1, const T4& top, int md, int s2, f
         if (r != CUDA_SUCCESS) { set_error("corr_tc: map-1 tensor map failed (%d)", (int)r); return FN2_ERR_CUDA; }
     }
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)min(p.total, tc_num_sms()), 1, 1);
+    cfg.gridDim = dim3((unsigned)min(p.total, num_sms()), 1, 1);
     cfg.blockDim = dim3(TC_THREADS);
     cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 1; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
     const int smem_bytes = TcGeo<NT>::SMEM;
     static bool attr_set = false;
     if (!attr_set) {
@@ -1447,18 +1268,9 @@ int corr_tc_forward(const T4& b0, const T4& b1, const T4& top, int md, int s2, f
         attr_set = true;
     }
     cfg.dynamicSmemBytes = smem_bytes;
-    FN2_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<NT, TC_CORR>, mapA, mapB, (const float*)nullptr, top.p, (float*)nullptr, p, tc_prof_buffer()));
+    FN2_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<NT, TC_CORR>, mapA, mapB, (const float*)nullptr, top.p, (float*)nullptr, p));
     FN2_LAUNCH_CHECK();
     return FN2_OK;
 }
 
 }  // namespace fn2
-
-extern "C" __attribute__((visibility("default"))) void fn2_tc_prof_dump(void) {
-    long long h[16];
-    long long* b = fn2::tc_prof_buffer();
-    if (!b) return;
-    cudaDeviceSynchronize();
-    cudaMemcpy(h, b, sizeof(h), cudaMemcpyDeviceToHost);
-    printf("tc prof (cycles) producer: total %lld wait_empty %lld | mma warp: total %lld wait_full %lld\n", h[0], h[1], h[4], h[5]);
-}

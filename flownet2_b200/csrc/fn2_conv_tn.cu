@@ -26,7 +26,6 @@
 // Warp roles: warp 0 TMA producer, warpgroups 1-2 the MMAs of pixels 0-63 / 64-127 and then, all 256 threads, the scatter
 // and write-out of the pass.  PDL as in fn2_conv_tc.cu.  Reference ops replaced: conv_layer.cu:8-23, deconv_layer.cu:8-23.
 #include <cuda.h>
-#include <mutex>
 
 #include "fn2_common.cuh"
 #include "fn2_tc_ptx.cuh"
@@ -57,7 +56,6 @@ struct TnParams {
     int ngmax;                                   // W tile rows in shared memory (max taps per pass * Co)
     int RA, RW, wres;                            // raw-A ring depth, W ring depth, 1 = all W stages resident in shared memory
     int total;                                   // units = N * nstrips * nseg
-    int dbg;                                     // FN2_TN_DBG bits (ablations, wrong results): 1 skip scatter, 2 skip write-out/zero, 4 skip MMAs, 128 skip group barriers
     float comp;                                  // mean RZ shrink of the 12*cblocks-MMA chain
     int relu, has_bias;
     float slope;
@@ -234,11 +232,9 @@ conv_tn_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
 #pragma unroll
                         for (int j = 0; j < TN_ACC_COLS / 2; j++) reg_fence(c[j]);
                         wgmma_fence();
-                        if (!(p.dbg & 4)) {
-                            if (p.ngmax == 96) tn_mma_step<96>(c, ah, al, dh, dl, cb != 0);
-                            else if (p.ngmax == 80) tn_mma_step<80>(c, ah, al, dh, dl, cb != 0);
-                            else tn_mma_step<64>(c, ah, al, dh, dl, cb != 0);
-                        }
+                        if (p.ngmax == 96) tn_mma_step<96>(c, ah, al, dh, dl, cb != 0);
+                        else if (p.ngmax == 80) tn_mma_step<80>(c, ah, al, dh, dl, cb != 0);
+                        else tn_mma_step<64>(c, ah, al, dh, dl, cb != 0);
                         wgmma_commit();
                         wgmma_wait_all();
 #pragma unroll
@@ -258,11 +254,11 @@ conv_tn_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                     }
                     asm volatile("bar.sync 3, 256;" ::: "memory");
                     const float* src = stg + m * STG + h * CH;
-                    const int ng = (p.dbg & 1) ? 0 : p.ngrp[ps];
+                    const int ng = p.ngrp[ps];
 #pragma unroll 1
                     for (int gi = 0; gi < ng; gi++) {
                         const int tl0 = p.grp[ps][gi].tl0, nrow = p.grp[ps][gi].nrow, oyr = p.grp[ps][gi].oyr;
-                        if (gi && !(p.dbg & 128)) tn_group_sync(h);   // the other 3 warps of this channel half may still add into the rows we now target
+                        if (gi) tn_group_sync(h);   // the other 3 warps of this channel half may still add into the rows we now target
                         int ring = rb + yrel0 + oyr;
                         if (ring >= p.RR) ring -= p.RR;
                         float* rowp = obuf + ring * rowstride + col0;
@@ -331,7 +327,7 @@ conv_tn_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                         }
                     }
 
-                    if (!(p.dbg & 128)) tn_group_sync(h);
+                    tn_group_sync(h);
                 }
                 // rows no later tile of this unit can touch: write them out (inside the segment / image) and clear them.  The two
                 // channel halves never meet in the ring, so each group of 4 warps flushes its own half on its own barrier.
@@ -340,7 +336,7 @@ conv_tn_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                 const bool do_flush = (k == U.ntiles - 1) || (++since_flush == p.F);
                 const int lo_row = flush_lo;
                 if (do_flush) { since_flush = 0; flush_lo = hi_row; }
-                if (do_flush && !(p.dbg & 2)) {
+                if (do_flush) {
                     constexpr int CG = CH / 4;                 // float4 groups per pixel in this half
                     constexpr int XPI = 128 / CG;              // columns per iteration
                     const int d128 = dt & 127;
@@ -363,11 +359,8 @@ conv_tn_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                             *reinterpret_cast<float4*>(dst + (long long)xi * p.out_sw) = make_float4(rv[0], rv[1], rv[2], rv[3]);
                         }
                     }
-                }
-                if (do_flush && !(p.dbg & 128)) tn_group_sync(h);
-                if (do_flush && !(p.dbg & 2)) {
+                    tn_group_sync(h);
                     const int n4 = (CH * p.CW) >> 2;           // this half of a ring row, a multiple of 4 floats (CW even)
-                    const int d128 = dt & 127;
                     for (int y = lo_row; y < hi_row; y++) {
                         int ring = rb + (y - touched_lo);
                         if (ring >= p.RR) ring -= p.RR;
@@ -375,8 +368,8 @@ conv_tn_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                         float4* z = reinterpret_cast<float4*>(obuf + ring * rowstride + h * CH * p.CW);
                         for (int e = d128; e < n4; e += 128) z[e] = make_float4(0.f, 0.f, 0.f, 0.f);
                     }
+                    tn_group_sync(h);
                 }
-                if (do_flush && !(p.dbg & 128)) tn_group_sync(h);
                 rb += advance;
                 while (rb >= p.RR) rb -= p.RR;
             }
@@ -389,21 +382,6 @@ conv_tn_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
 
 
 // ---- host ---------------------------------------------------------------------------------------------------------------
-typedef CUresult (*TnEncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                               const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                               CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-TnEncodeFn tn_encode_fn() {
-    static TnEncodeFn fn = nullptr;
-    static std::once_flag once;
-    std::call_once(once, [] {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-            fn = (TnEncodeFn)p;
-    });
-    return fn;
-}
-
 // packed weights: [hi|lo][pass * cblocks + cb][ngmax rows = (tap in pass, co)][32 channels of K block cb]
 __global__ void tn_pack_kernel(const float* __restrict__ w, float* __restrict__ wp, int Ci, int Co, int kh, int kw, int deconv,
                                int cblocks, int ngmax, TnParams p) {
@@ -422,13 +400,7 @@ __global__ void tn_pack_kernel(const float* __restrict__ w, float* __restrict__ 
             const int r = t / kw, s = t - r * kw;
             v = deconv ? w[(((long long)ci * Co + co) * kh + r) * kw + s] : w[(((long long)co * Ci + ci) * kh + r) * kw + s];
         }
-        uint32_t h;
-        asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(h) : "f"(v));
-        const float hi = __uint_as_float(h);
-        uint32_t l;
-        asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(l) : "f"(v - hi));
-        wp[idx] = hi;
-        wp[per + idx] = __uint_as_float(l);
+        store_tf32_split(wp, per, idx, v);
     }
 }
 
@@ -509,25 +481,19 @@ static bool tn_layer_plan(const fn2_conv_desc* d, TnParams* p) {
     // shift the strips so that strip 0's complete range starts at or just before output column 0
     p->cshift = -((xa + p->S - 1) / p->S);
     if (p->S * p->cshift + xa > 0) p->cshift -= 1;
-    // mean truncation loss of the accumulation chain: every MMA that adds a non-zero product truncates the accumulator, while
-    // slices beyond the last real channel add exact zeros and lose nothing.  H100: ~1.3e-8 of the accumulator per MMA (mean
-    // signed errors of tests/test_ops_gpu.py::test_conv_taps_on_n_engine at Ci = 40 / 64 / 96 imply 1.1e-8 / 1.33e-8 / 1.3e-8).
-    const char* nocomp = getenv("FN2_TC_COMP");
-    float bm = 1.3e-8f;
-    if (const char* e = getenv("FN2_TN_COMP_B")) bm = (float)atof(e);
-    p->comp = (nocomp && nocomp[0] == '0') ? 0.f : 3.f * bm * (float)((d->ci + 7) / 8);
+    // mean truncation loss of the accumulation chain: every MMA that adds a non-zero product truncates the accumulator (3 per
+    // 8-channel slice), while slices beyond the last real channel add exact zeros and lose nothing
+    p->comp = 3.f * TRUNC_LOSS_PER_MMA * (float)((d->ci + 7) / 8);
     // shared memory: raw-A ring + W (resident if it all fits, else a ring of 2..3 stages) + barriers + output ring.  The ring is
     // flushed (written out + cleared, two barriers) every F tiles; a larger F needs (F-1) * th * S more ring rows.
     const int wstage = 2 * p->ngmax * 128;
     const int nwall = p->npass * p->cblocks;
-    int fmax = 4;
-    if (const char* e = getenv("FN2_TN_F")) fmax = max(1, min(8, atoi(e)));
-    for (int F = fmax; F >= 1; F--) {
+    for (int F = 4; F >= 1; F--) {
         p->F = F; p->RR = span + (F - 1) * p->th * p->S;
         const int ring = p->RR * d->co * p->CW * 4;
         const int budget = 227 * 1024 - ring - 1024 - 256 - 128 * (p->ngmax + 4) * 4;      // ... - staging buffer
         p->RA = 4;
-        if (!getenv("FN2_TN_NORES") && p->RA * TN_A_BYTES + nwall * wstage <= budget) { p->wres = 1; p->RW = 0; return true; }
+        if (p->RA * TN_A_BYTES + nwall * wstage <= budget) { p->wres = 1; p->RW = 0; return true; }
         p->wres = 0;
         p->RW = min(3, (budget - p->RA * TN_A_BYTES) / wstage);
         if (p->RW >= 3) return true;                 // a 2-deep W ring costs more than the rarer flush saves (measured)
@@ -573,12 +539,11 @@ int conv_tn_plan(const fn2_conv_desc* d, int N, int Ho, int Wo, int* out8) {
 }
 
 int conv_tn_forward(const fn2_conv_desc* d, const T4& in, const float* wp, const float* bias, const T4& out, cudaStream_t st) {
-    TnEncodeFn enc = tn_encode_fn();
+    EncodeTiledFn enc = tc_encode_fn();
     if (!enc) { set_error("conv_tn: cuTensorMapEncodeTiled unavailable"); return FN2_ERR_CUDA; }
     TnParams p;
     if (!tn_layer_plan(d, &p)) { set_error("conv_tn: layer not eligible"); return FN2_ERR_INVALID; }
     p.N = in.n; p.Hin = in.h; p.Win = in.w; p.Ho = out.h; p.Wo = out.w;
-    { const char* e = getenv("FN2_TN_DBG"); p.dbg = e ? atoi(e) : 0; }
     p.relu = d->relu; p.has_bias = d->has_bias; p.slope = d->negative_slope;
     p.out_sn = out.sn; p.out_sh = out.sh; p.out_sw = out.sw;
     p.nstrips = (p.Wo - (p.S * p.cshift + p.xa) + p.S * p.stepx - 1) / (p.S * p.stepx);

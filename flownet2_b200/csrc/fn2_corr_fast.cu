@@ -200,7 +200,7 @@ corr_fast_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant
 
 // ---- rearrange: strided (n,c,h,w) view -> parity-planar ws[n][plane][c][Hs][Ws] ------------------------
 // `shift` empty columns precede every row of the map-1 planes: TMA needs the innermost start coordinate
-// of a box to be 16-byte aligned (measured: tools/tma_probe.cu), and the halo starts at xs0 - R, so the
+// of a box to be 16-byte aligned (measured), and the halo starts at xs0 - R, so the
 // planes are stored shifted by R mod 4 columns and the halo box starts at xs0 - R + shift = 0 (mod 4).
 // channel-fast (NHWC) source: 32 channels x 32 pixels tiles through shared memory (writes real pixels
 // only; corr_zero_pads_kernel clears the pad columns/rows).

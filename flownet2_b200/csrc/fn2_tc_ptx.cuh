@@ -1,9 +1,24 @@
-// wgmma / TMA / mbarrier PTX wrappers used by the tensor-core engine (fn2_conv_tc.cu); sm_90a.
+// wgmma / TMA / mbarrier PTX wrappers and constants shared by the tensor-core engines (fn2_conv_tc.cu, fn2_conv_tn.cu); sm_90a.
 #pragma once
 #include <cuda.h>
 #include "fn2_common.cuh"
 
 namespace fn2 {
+
+// The driver's cuTensorMapEncodeTiled, looked up once (fn2_conv_tc.cu); nullptr if the driver does not provide it.
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+EncodeTiledFn tc_encode_fn();
+
+// Mean relative loss of an FP32 accumulator per MMA that adds a non-zero product to it: the tensor core truncates (rounds
+// toward zero) its accumulator, so a chain of n MMAs shrinks the result by about n times this, and both engines add that
+// back.  H100: ~1.1e-8 .. 1.3e-8, from the mean signed errors of the tensor-core parity cases of tests/test_ops_gpu.py
+// (per-tap engine, and the taps-on-N engine at Ci = 40 / 64 / 96: 1.1e-8 / 1.33e-8 / 1.3e-8), with no constant term.
+// Recalibrating: build a side library with this set to 0, load it through FN2_LIB and run those tests; the mean signed error
+// ("shrink") they compute, divided by the number of MMAs the engine's compensation counts per chain, is the new value.
+constexpr float TRUNC_LOSS_PER_MMA = 1.3e-8f;
+
 namespace {
 
 // division by a launch constant without the ~40-instruction integer divide (the tile decode is on the critical path of the
@@ -39,36 +54,9 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
         if (++spins > (1u << 24)) __trap();       // a lost arrival becomes a launch error, never a hang
     }
 }
-// instrumented wait: accumulates the cycles spent waiting into *acc (debug profiling, FN2_TC_DBG & 16)
-__device__ __forceinline__ void mbar_wait_t(uint64_t* bar, uint32_t parity, long long* acc, bool timed) {
-    if (!timed) { mbar_wait(bar, parity); return; }
-    const long long t0 = clock64();
-    mbar_wait(bar, parity);
-    *acc += clock64() - t0;
-}
 __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3) {
     asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
                  ::"r"(su32(dst)), "l"(map), "r"(su32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-// the same box, delivered to the same shared-memory offset (and signalling the same barrier offset) of every CTA in cta_mask
-__device__ __forceinline__ void tma_load_4d_mc(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3, uint16_t cta_mask) {
-    asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4, %5, %6}], [%2], %7;"
-                 ::"r"(su32(dst)), "l"(map), "r"(su32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "h"(cta_mask) : "memory");
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .b32 rx;\n\t.reg .pred px;\n\telect.sync rx|px, 0xffffffff;\n\tselp.b32 %0, 1, 0, px;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
-// the same barrier in CTA `rank` of the cluster (release at cluster scope: our reads of the stage happen before the peer's
-// producer may overwrite it)
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
-    asm volatile("{\n\t.reg .b32 ra;\n\tmapa.shared::cluster.u32 ra, %0, %1;\n\tmbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}"
-                 ::"r"(su32(bar)), "r"(rank) : "memory");
 }
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
@@ -76,6 +64,16 @@ __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_grou
 // keeps the compiler from moving accesses of the accumulator registers across the asynchronous MMAs
 __device__ __forceinline__ void reg_fence(float& r) { asm volatile("" : "+f"(r)::"memory"); }
 __device__ __forceinline__ uint32_t to_tf32(float x) { return (__float_as_uint(x) + 0x1000u) & 0xffffe000u; }
+// weight packing: wp[idx] = v rounded to TF32, wp[per + idx] = the remainder rounded to TF32 (cvt.rna, which unlike
+// to_tf32 keeps a NaN a NaN)
+__device__ __forceinline__ void store_tf32_split(float* wp, long long per, long long idx, float v) {
+    uint32_t h, l;
+    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(h) : "f"(v));
+    const float hi = __uint_as_float(h);
+    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(l) : "f"(v - hi));
+    wp[idx] = hi;
+    wp[per + idx] = __uint_as_float(l);
+}
 // shared-memory matrix descriptor (sm_90 wgmma): K-major, SWIZZLE_128B, 8-row atoms of 1024 B, tile base 1024-byte aligned.
 // Adding 2 to the start-address field (+32 bytes) selects the next 8 TF32 columns of the swizzled tile.
 __device__ __forceinline__ uint64_t make_desc_sw128(uint32_t smem_addr) {

@@ -170,7 +170,7 @@ def test_no_compute_without_gpu_is_loud(fn2):
         fn2.Net(fn2.fill_template(fn2.model_template("FlowNet2-S"), 64, 64))
 
 
-def test_tcgen05_engine_plan_for_flownet2_shapes(fn2):
+def test_tensor_core_engine_plan_for_flownet2_shapes(fn2):
     """Host-side planning of the tensor-core convolution engine (no GPU needed): tile width, small-Ci packing mode, split-K for
     the small-spatial layers and the tail split of the last partial wave, at the BASELINE shapes (4 pairs, 1024x448)."""
     from flownet2_b200 import fn2_conv_desc

@@ -254,7 +254,7 @@ def test_full_size_properties(fn2, monkeypatch):
     """BASELINE.json's configuration (FlowNet2, 1024x436, 4 pairs) is too large for the CPU oracle; checked through
     size-independent properties instead: (1) replay determinism (eager pass == CUDA-graph replays, bit for bit),
     (2) batch independence: sample k of a batch-4 forward equals a batch-1 forward of that pair (different tile schedules and
-    K splits, so within the flow tolerance, not bitwise), (3) the two convolution engines agree: tcgen05 3xTF32 vs exact-FP32
+    K splits, so within the flow tolerance, not bitwise), (3) the two convolution engines agree: wgmma 3xTF32 vs exact-FP32
     SIMT within 1e-4 of the flow scale, (4) correlation layer: tensor-core path vs FP32 path on the real conv3 features."""
     W, H, B = 1024, 436, 4
     proto = fn2.fill_template(fn2.model_template("FlowNet2"), W, H)

@@ -5,8 +5,6 @@ mean) are compared BIT-EXACT (same expression order, no FMA contraction on eithe
 Correlation and conv/deconv reduce in a different order than the oracle -> 1e-5 relative to the
 magnitude of the result (the reference's own conv tests use 1e-4, test_convolution_layer.cpp:256).
 """
-import os
-
 import numpy as np
 import pytest
 
@@ -251,7 +249,7 @@ TC_CASES = [
 
 
 @pytest.mark.parametrize("case", TC_CASES)
-def test_conv_tcgen05_engine(ops, case):
+def test_conv_tensor_core_engine(ops, case):
     """3xTF32 tensor-core engine (engine=2 fails loudly if the shape is not eligible): same tolerance as the FP32
     SIMT engine, and no systematic shrink (the tensor core's round-toward-zero accumulation is drained/compensated)."""
     N, Ci, H, W, Co, k, s, p, deconv = case
@@ -329,7 +327,7 @@ ROW_CASES = [
 
 
 @pytest.mark.parametrize("case", ROW_CASES)
-def test_conv_tcgen05_row_mode(ops, case):
+def test_conv_tensor_core_row_mode(ops, case):
     """The guard band is filled with NaN: the row runs of edge pixels reach into it (and into the neighbouring image
     rows), and none of that may leak into the result."""
     N, Ci, H, W, Co, k, s, p = case
@@ -456,37 +454,3 @@ def test_error_paths(fn2, ops):
     with pytest.raises(fn2.Fn2Error, match="2 channels"):
         ops.flow_warp(a, a)
 
-
-_SWITCH_CODE = r"""
-import numpy as np, torch
-from flownet2_b200 import ops
-from oracle import oracle as O
-r = np.random.default_rng(29)
-N, Ci, H, W, Co = 1, 64, 16, 64, 128
-x = r.standard_normal((N, Ci, H, W)).astype(np.float32)
-w = (r.standard_normal((Co, Ci, 3, 3)) * np.sqrt(2.0 / (Ci * 9))).astype(np.float32)
-b = r.standard_normal(Co).astype(np.float32)
-want = O.relu(O.conv_fwd(x, w, b, 1, 1, f64acc=True), 0.1)
-xt = torch.from_numpy(x).cuda().contiguous(memory_format=torch.channels_last)
-got = ops.conv2d(xt, torch.from_numpy(w).cuda(), torch.from_numpy(b).cuda(), 1, 1, False, 0.1, 2)
-got = got.contiguous().cpu().numpy()
-print(float(np.abs(got - want).max() / max(1.0, np.abs(want).max())))
-"""
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("switch", [{"FN2_TC_TAILFIX": "1"}, {"FN2_TC_CL": "2"}, {"FN2_TC_CL": "4"}])
-def test_conv_tensor_core_optional_paths(switch):
-    """The tensor-core engine's opt-in paths (read once per process, hence a subprocess): the in-kernel fix-up of the tail split
-    (8 tiles of 128 pixels, fewer than the SMs: every tile's K loop is split) and cluster launches with multicast weight tiles.
-    Same tolerance as the default path."""
-    import subprocess
-    import sys
-    from flownet2_b200 import ops
-    plan = ops.conv_plan(64, 128, 3, 1, 1, False, 1, 16, 64, 64)
-    assert plan[0] == 128 and plan[3] == 0 and plan[6] > 1, plan          # tail split planned (tail K ranges > 1)
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    out = subprocess.run([sys.executable, "-c", _SWITCH_CODE], capture_output=True, text=True, cwd=root, env=dict(os.environ, **switch))
-    assert out.returncode == 0, out.stderr[-2000:]
-    err = float(out.stdout.strip().splitlines()[-1])
-    assert err <= 1e-6, err

@@ -11,8 +11,8 @@ run() {  # name tool args...
     grep -E "ERROR SUMMARY|RACECHECK SUMMARY|passed|failed" gpurun_out/san_${name}_${tool}.log | tail -4 >> gpurun_out/r02_sanitizer_summary.txt
 }
 : > gpurun_out/r02_sanitizer_summary.txt
-run tc_ops memcheck python -m pytest tests/test_ops_gpu.py -q -x -k "tcgen05 or taps_on_n"
-run tc_ops racecheck python -m pytest tests/test_ops_gpu.py -q -x -k "tcgen05 or taps_on_n"
+run tc_ops memcheck python -m pytest tests/test_ops_gpu.py -q -x -k "tensor_core or taps_on_n"
+run tc_ops racecheck python -m pytest tests/test_ops_gpu.py -q -x -k "tensor_core or taps_on_n"
 run wgrad memcheck python -m pytest tests/test_train_gpu.py -q -x -k "conv_backward"
 run wgrad racecheck python -m pytest tests/test_train_gpu.py -q -x -k "c3x3_s1_wide or c5x5_s2_w57 or d4x4_s2_wide"
 run net_c memcheck python -m pytest tests/test_train_gpu.py -q -x -k "without_fusion"

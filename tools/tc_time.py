@@ -36,5 +36,4 @@ for (N, Ci, H, W, Co, k, s, p) in [(4, 473, 56, 128, 256, 3, 1, 1), (4, 12, 448,
     except Exception:
         clk = 1.98e9                                 # H100 SXM maximum SM clock
     rounds = (tiles + sms - 1) // sms
-    if hasattr(l, "fn2_tc_prof_dump"): l.fn2_tc_prof_dump()
-    print("DBG=%s %s: %.3f ms, %d tiles (%d rounds) x %d steps -> %.0f cycles/step @%.2fGHz" % (os.environ.get("FN2_TC_DBG", "0"), (N, Ci, H, W, Co, k, s), ms, tiles, rounds, steps, ms * 1e-3 * clk / rounds / steps, clk / 1e9), flush=True)
+    print("%s: %.3f ms, %d tiles (%d rounds) x %d steps -> %.0f cycles/step @%.2fGHz" % ((N, Ci, H, W, Co, k, s), ms, tiles, rounds, steps, ms * 1e-3 * clk / rounds / steps, clk / 1e9), flush=True)
