@@ -72,6 +72,20 @@ inline bool valid(const fn2_tensor* t) {
     return t && t->data && t->n > 0 && t->c > 0 && t->h > 0 && t->w > 0;
 }
 
+// Output parity classes and kernel-tap table of a convolution or deconvolution (fn2_conv.cu), shared by the per-tap engines.
+// Class c covers the output pixels (u*ou + oy0[c], v*ov + ox0[c]), u < Hu[c], v < Wu[c]; its taps t = tap0[c] ..
+// tap0[c] + ntaps[c] - 1 read the input at (u*stride_h + dy[t], v*stride_w + dx[t]) (stride 1 for a deconvolution) with the
+// weights of kernel position widx[t].  A convolution is one class with all taps.  A deconvolution (gather form of col2im,
+// util/im2col.cpp:158-190) has one class per output parity (oy mod stride_h, ox mod stride_w) present in the output, holding
+// the taps that reach it: every tap belongs to exactly one class, and a class may have none.
+// Needs kh*kw <= 49 and, for a deconvolution, stride_h*stride_w <= 16.
+struct ConvTaps {
+    int ncls, ou, ov;
+    int Hu[16], Wu[16], oy0[16], ox0[16], tap0[16], ntaps[16];
+    short dy[49], dx[49], widx[49];
+};
+void conv_taps(const fn2_conv_desc* d, int Ho, int Wo, ConvTaps* c);
+
 inline int num_sms() {
     static int sms = 0;
     if (!sms) {

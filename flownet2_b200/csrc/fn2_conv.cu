@@ -15,13 +15,22 @@
 
 namespace fn2 {
 
+// per-tap tensor-core engine (fn2_conv_tc.cu)
 int conv_tc_eligible(const fn2_conv_desc* d, const T4& in, const T4& out);
 int conv_tc_forward(const fn2_conv_desc* d, const T4& in, const float* wp, const float* bias,
                     const T4& out, float* ws, size_t ws_floats, cudaStream_t st);
-size_t conv_tc_workspace_floats(const fn2_conv_desc* d, int N, int Ho, int Wo);
-int conv_tc_plan(const fn2_conv_desc* d, int N, int Ho, int Wo, int ci_stride, int* out8);
-int conv_tc_packed_floats(const fn2_conv_desc* d, int ci_stride, size_t* floats);
+size_t conv_tc_workspace_floats(const fn2_conv_desc* d, int N, int W, int Ho, int Wo);
+void conv_tc_plan(const fn2_conv_desc* d, int N, int W, int Ho, int Wo, int ci_stride, int* out8);
+size_t conv_tc_packed_floats(const fn2_conv_desc* d, int ci_stride);
 int conv_tc_pack(const fn2_conv_desc* d, int ci_stride, const float* w, float* wp, cudaStream_t st);
+// taps-on-N tensor-core engine for few output channels at high resolution (fn2_conv_tn.cu); it takes precedence over the
+// per-tap engine for the layers it applies to
+int conv_tn_applicable(const fn2_conv_desc* d);
+size_t conv_tn_packed_floats(const fn2_conv_desc* d);
+int conv_tn_pack(const fn2_conv_desc* d, const float* w, float* wp, cudaStream_t st);
+int conv_tn_plan(const fn2_conv_desc* d, int N, int Ho, int Wo, int* out8);
+int conv_tn_forward(const fn2_conv_desc* d, const T4& in, const float* wp, const float* bias, const T4& out, cudaStream_t st);
+// FP32 SIMT engine for NHWC tensors (fn2_conv_nhwc.cu)
 int conv_nhwc_eligible(const fn2_conv_desc* d, const T4& in, const T4& out);
 size_t conv_nhwc_workspace_floats(const fn2_conv_desc* d, int N, int Ho, int Wo);
 int conv_nhwc_forward(const fn2_conv_desc* d, const T4& in, const float* wp, const float* bias, const T4& out,
@@ -638,6 +647,31 @@ static int make_params(const fn2_conv_desc* d, const T4& in, const T4& out, Conv
     return FN2_OK;
 }
 
+static inline int floordiv(int a, int b) { return (a >= 0) ? a / b : -((-a + b - 1) / b); }
+
+void conv_taps(const fn2_conv_desc* d, int Ho, int Wo, ConvTaps* c) {
+    const int sh = d->deconv ? d->stride_h : 1, sw = d->deconv ? d->stride_w : 1;
+    c->ncls = 0; c->ou = sh; c->ov = sw;
+    int nt = 0;
+    for (int py = 0; py < min(sh, Ho); py++)
+        for (int px = 0; px < min(sw, Wo); px++) {
+            const int k = c->ncls++;
+            c->Hu[k] = (Ho - py + sh - 1) / sh; c->Wu[k] = (Wo - px + sw - 1) / sw;
+            c->oy0[k] = py; c->ox0[k] = px; c->tap0[k] = nt;
+            for (int r = 0; r < d->kh; r++) {
+                if (((py + d->pad_h - r) % sh + sh) % sh) continue;        // deconvolution: oy = iy*sh - pad + r
+                for (int s = 0; s < d->kw; s++) {
+                    if (((px + d->pad_w - s) % sw + sw) % sw) continue;
+                    c->dy[nt] = (short)(d->deconv ? floordiv(py + d->pad_h - r, sh) : r - d->pad_h);
+                    c->dx[nt] = (short)(d->deconv ? floordiv(px + d->pad_w - s, sw) : s - d->pad_w);
+                    c->widx[nt] = (short)(r * d->kw + s);
+                    nt++;
+                }
+            }
+            c->ntaps[k] = nt - c->tap0[k];
+        }
+}
+
 }  // namespace fn2
 
 using namespace fn2;
@@ -661,11 +695,8 @@ int fn2_conv_out_shape(const fn2_conv_desc* d, int H, int W, int* Ho, int* Wo) {
 // what the tensor-core engine needs (padded channel count of the bottom tensor).
 int fn2_conv_packed_floats(const fn2_conv_desc* d, int ci_stride, size_t* floats) {
     FN2_CHECK_ARG(d && floats, "conv_packed_floats: null argument");
-    size_t simt = (size_t)d->kh * d->kw * d->ci * d->co;
-    size_t tc = 0;
-    int rc = conv_tc_packed_floats(d, ci_stride, &tc);
-    if (rc) return rc;
-    *floats = simt + tc;
+    const size_t simt = (size_t)d->kh * d->kw * d->ci * d->co;
+    *floats = simt + (conv_tn_applicable(d) ? conv_tn_packed_floats(d) : conv_tc_packed_floats(d, ci_stride));
     return FN2_OK;
 }
 
@@ -676,6 +707,7 @@ int fn2_conv_pack_weights(const fn2_conv_desc* d, int ci_stride, const float* ca
     pack_weights_kernel<<<ew_grid(total, 256), 256, 0, (cudaStream_t)stream>>>(
         caffe_weights_dev, packed_dev, d->ci, d->co, d->kh, d->kw, d->ci, d->deconv);
     FN2_LAUNCH_CHECK();
+    if (conv_tn_applicable(d)) return conv_tn_pack(d, caffe_weights_dev, packed_dev + total, (cudaStream_t)stream);
     return conv_tc_pack(d, ci_stride, caffe_weights_dev, packed_dev + total, (cudaStream_t)stream);
 }
 
@@ -684,7 +716,9 @@ int fn2_conv_plan(const fn2_conv_desc* d, int N, int H, int W, int ci_stride, in
     int Ho, Wo;
     int rc = fn2_conv_out_shape(d, H, W, &Ho, &Wo);
     if (rc) return rc;
-    conv_tc_plan(d, N, Ho, Wo, ci_stride, plan8);
+    for (int i = 0; i < 8; i++) plan8[i] = 0;
+    if (conv_tn_applicable(d)) conv_tn_plan(d, N, Ho, Wo, plan8);
+    else conv_tc_plan(d, N, W, Ho, Wo, ci_stride, plan8);
     return FN2_OK;
 }
 
@@ -693,7 +727,8 @@ int fn2_conv_workspace_bytes(const fn2_conv_desc* d, int N, int H, int W, size_t
     int Ho, Wo;
     int rc = fn2_conv_out_shape(d, H, W, &Ho, &Wo);
     if (rc) return rc;
-    *bytes = max(conv_nhwc_workspace_floats(d, N, Ho, Wo), conv_tc_workspace_floats(d, N, Ho, Wo)) * sizeof(float);
+    const size_t tc = conv_tn_applicable(d) ? 0 : conv_tc_workspace_floats(d, N, W, Ho, Wo);
+    *bytes = max(conv_nhwc_workspace_floats(d, N, Ho, Wo), tc) * sizeof(float);
     return FN2_OK;
 }
 
@@ -708,8 +743,11 @@ int fn2_conv_forward(const fn2_conv_desc* d, const fn2_tensor* bottom, const flo
     if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     const long long simt_floats = (long long)d->kh * d->kw * d->ci * d->co;
-    if (d->engine != 1 && conv_tc_eligible(d, in, out))
-        return conv_tc_forward(d, in, packed_weights_dev + simt_floats, bias_dev, out, (float*)workspace, workspace_bytes / sizeof(float), st);
+    if (d->engine != 1 && conv_tc_eligible(d, in, out)) {
+        const float* tcw = packed_weights_dev + simt_floats;
+        if (conv_tn_applicable(d)) return conv_tn_forward(d, in, tcw, bias_dev, out, st);
+        return conv_tc_forward(d, in, tcw, bias_dev, out, (float*)workspace, workspace_bytes / sizeof(float), st);
+    }
     FN2_CHECK_ARG(d->engine != 2, "conv: tensor-core engine requested but the shape/layout is not eligible");
     if (!d->deconv && d->ci <= 4 && d->co >= 32 && out.sc == 1 && d->kh * d->kw * d->ci <= 200) {
         p.cis = d->ci;
@@ -733,7 +771,7 @@ int fn2_conv_forward(const fn2_conv_desc* d, const fn2_tensor* bottom, const flo
         if (C4 <= 8) {
             const int grid = (int)min((long long)num_sms() * 8, (M + 255) / 256);
 #define FN2_PF_THREAD(C)                                                                                                   \
-            case C: if (k3 && d->pad_h == 1 && d->pad_w == 1 && !getenv("FN2_PF_NOTILE")) {                                \
+            case C: if (k3 && d->pad_h == 1 && d->pad_w == 1) {                                                            \
                         const size_t tsm = smem + (size_t)10 * 34 * (C + 1) * sizeof(float4);                               \
                         const int tgrid = (int)min((long long)num_sms() * 4, (long long)p.N * ((p.Wo + 31) / 32) * ((p.Ho + 7) / 8)); \
                         if (tsm > 48 * 1024) FN2_CUDA(cudaFuncSetAttribute(conv_pf3_tile_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tsm)); \

@@ -243,8 +243,6 @@ __global__ void conv_nhwc_reduce_kernel(const float* __restrict__ partial, const
     }
 }
 
-static inline int floordiv(int a, int b) { return (a >= 0) ? a / b : -((-a + b - 1) / b); }
-
 int conv_nhwc_eligible(const fn2_conv_desc* d, const T4& in, const T4& out) {
     if (in.sc != 1 || out.sc != 1) return 0;
     if (d->co % 4 || d->co < 8) return 0;
@@ -299,63 +297,30 @@ int conv_nhwc_forward(const fn2_conv_desc* d, const T4& in, const float* wp, con
         else if (bn == 64) conv_nhwc_kernel<64><<<grid, 256, 0, st>>>(in.p, wp, bias, out.p, partial, p);
         else conv_nhwc_kernel<32><<<grid, 256, 0, st>>>(in.p, wp, bias, out.p, partial, p);
     };
-    if (!d->deconv) {
-        p.Hu = out.h; p.Wu = out.w; p.su = d->stride_h; p.sv = d->stride_w; p.ou = p.ov = 1; p.oy0 = p.ox0 = 0;
-        p.ntaps = d->kh * d->kw;
-        for (int r = 0; r < d->kh; r++)
-            for (int s = 0; s < d->kw; s++) {
-                const int t = r * d->kw + s;
-                p.dy[t] = (short)(r - d->pad_h); p.dx[t] = (short)(s - d->pad_w); p.widx[t] = (short)t;
-            }
+    ConvTaps tp;
+    conv_taps(d, out.h, out.w, &tp);
+    p.su = d->deconv ? 1 : d->stride_h; p.sv = d->deconv ? 1 : d->stride_w; p.ou = tp.ou; p.ov = tp.ov;
+    // one launch per output parity class (a convolution has one)
+    for (int c = 0; c < tp.ncls; c++) {
+        p.Hu = tp.Hu[c]; p.Wu = tp.Wu[c]; p.oy0 = tp.oy0[c]; p.ox0 = tp.ox0[c];
+        p.ntaps = tp.ntaps[c];
+        for (int t = 0; t < p.ntaps; t++) {
+            p.dy[t] = tp.dy[tp.tap0[c] + t]; p.dx[t] = tp.dx[tp.tap0[c] + t]; p.widx[t] = tp.widx[tp.tap0[c] + t];
+        }
         const long long M = (long long)p.N * p.Hu * p.Wu;
         dim3 grid((unsigned)((M + NB_M - 1) / NB_M), (unsigned)((d->co + bn - 1) / bn), 1);
-        p.splits = plan_splits(M, d->co, d->ci, p.ntaps);
+        p.splits = p.ntaps > 0 ? plan_splits(M, d->co, d->ci, p.ntaps) : 1;
         if (p.splits > 1 && ws && ws_floats >= (size_t)p.splits * M * d->co) {
             grid.z = p.splits;
             launch(grid, ws);
             FN2_LAUNCH_CHECK();
             conv_nhwc_reduce_kernel<<<ew_grid(M * p.Co, 256), 256, 0, st>>>(ws, bias, out.p, p.splits, p);
-            FN2_LAUNCH_CHECK();
-            return FN2_OK;
+        } else {
+            p.splits = 1;
+            launch(grid, nullptr);     // a class without taps still gets bias (+ReLU)
         }
-        p.splits = 1;
-        launch(grid, nullptr);
         FN2_LAUNCH_CHECK();
-        return FN2_OK;
     }
-    // deconvolution: one launch per output parity class
-    const int sh = d->stride_h, sw = d->stride_w;
-    for (int py = 0; py < sh; py++)
-        for (int px = 0; px < sw; px++) {
-            if (py >= out.h || px >= out.w) continue;
-            p.Hu = (out.h - py + sh - 1) / sh; p.Wu = (out.w - px + sw - 1) / sw;
-            p.su = p.sv = 1; p.ou = sh; p.ov = sw; p.oy0 = py; p.ox0 = px;
-            int nt = 0;
-            for (int r = 0; r < d->kh; r++) {
-                if (((py + d->pad_h - r) % sh + sh) % sh) continue;        // oy = iy*sh - pad + r
-                for (int s = 0; s < d->kw; s++) {
-                    if (((px + d->pad_w - s) % sw + sw) % sw) continue;
-                    p.dy[nt] = (short)floordiv(py + d->pad_h - r, sh);
-                    p.dx[nt] = (short)floordiv(px + d->pad_w - s, sw);
-                    p.widx[nt] = (short)(r * d->kw + s);
-                    nt++;
-                }
-            }
-            p.ntaps = nt;
-            const long long M = (long long)p.N * p.Hu * p.Wu;
-            dim3 grid((unsigned)((M + NB_M - 1) / NB_M), (unsigned)((d->co + bn - 1) / bn), 1);
-            p.splits = nt > 0 ? plan_splits(M, d->co, d->ci, nt) : 1;
-            if (p.splits > 1 && ws && ws_floats >= (size_t)p.splits * M * d->co) {
-                grid.z = p.splits;
-                launch(grid, ws);
-                FN2_LAUNCH_CHECK();
-                conv_nhwc_reduce_kernel<<<ew_grid(M * p.Co, 256), 256, 0, st>>>(ws, bias, out.p, p.splits, p);
-            } else {
-                p.splits = 1;
-                launch(grid, nullptr);     // nt == 0 still writes bias (+ReLU) to this class
-            }
-            FN2_LAUNCH_CHECK();
-        }
     return FN2_OK;
 }
 

@@ -36,17 +36,18 @@ struct TcParams {
     int N, su, sv, ou, ov;                        // sub-grid / mapping (see fn2_conv_nhwc.cu)
     int ncls;                                     // output parity classes handled by this launch (grid.z)
     int cls_Hu[4], cls_Wu[4], cls_oy0[4], cls_ox0[4], cls_tap0[4], cls_ntaps[4];
-    int Co, cblocks;                              // cblocks = ceil(Ci / 32)
+    int cblocks;                                  // ceil(Ci / 32)
     long long out_sn, out_sh, out_sw;
     int relu, has_bias;
     float slope;
     int tw, th, tiles_x, tiles_y;
     int kd;                                       // channel blocks per tensor-core accumulation chain
-    int splits, Ho, Wo;                           // split-K: K ranges per tile (partials go to the workspace), output size
-    // tail split: the tiles of the last, partial wave [tail_first, ntotal) are cut into tail_z K ranges each so that they
-    // spread over all SMs (448 tiles on 132 SMs: 3 + 52/132 rounds instead of 4); their partials are summed by a fix-up kernel
-    int tail_first, tail_z, ntotal;
-    FastDiv d_ntiles, d_cotiles, d_tiles_x, d_tiles_y, d_splits, d_tail_z;
+    int Ho, Wo;                                   // output size
+    // K split (tc_split_plan): the tiles [split_first, ntotal) are cut into split_z K ranges each, which run on different SMs
+    // as consecutive tile units; their raw partial tiles go to the workspace and tc_split_reduce_kernel sums them.
+    // split_z = 1: unsplit (split_first = ntotal).
+    int split_first, split_z, ntotal;
+    FastDiv d_ntiles, d_cotiles, d_tiles_x, d_tiles_y, d_split_z;
     // Correlation on the same pipeline (corr_tc_forward): a unit = (sample, parity plane, 128-pixel tile of map 0, block of
     // cbw x cbh halo pixels of map 1); D[pixel][halo pixel] = <a, b> over C channels; the epilogue keeps the band that
     // lies inside the (2R+1)^2 displacement window.  W tiles are halo-pixel tiles of the pre-split map 1.
@@ -83,18 +84,34 @@ template <int NT> struct TcGeo {
 // one output tile: 128 pixels (th x tw) of one sample and parity class, NT output channels
 struct TcTile {
     int n, u0, v0, co0, cls, tap0, ntaps, steps;
-    int k0, split;                                // first K step of this unit, split index
-    int slot;                                     // >= 0: raw partial sums go to workspace slot `slot` (tail split)
+    int k0;                                       // first K step of this unit
+    int slot;                                     // >= 0: raw partial sums go to workspace slot `slot` (K split)
     bool valid;
 };
 // MODE (compile time, so that each instantiation's role loops stay small -- the all-in-one kernel had ~1900 SASS instructions in
 // the converter loop and stalled on instruction fetch): 0 plain K blocks, 1 tap groups, 2 kernel rows, 3 correlation
 enum { TC_PLAIN = 0, TC_GROUP = 1, TC_ROW = 2, TC_CORR = 3, TC_WGRAD = 4 };
 
+// whole tile `tile` of the plain, tap-group and kernel-row modes: sample, pixel origin, Co tile, parity class and its taps
+template <int NT>
+__device__ __forceinline__ void tc_whole_tile(const TcParams& p, int tile, TcTile& t) {
+    int pix, r, cot = 0;
+    p.d_ntiles.divmod(tile, r, pix);
+    t.cls = 0;
+    if (r) p.d_cotiles.divmod(r, t.cls, cot);
+    int tx, ty, q2;
+    p.d_tiles_x.divmod(pix, q2, tx);
+    p.d_tiles_y.divmod(q2, t.n, ty);
+    t.u0 = ty * p.th; t.v0 = tx * p.tw;
+    t.co0 = cot * NT;
+    t.tap0 = p.cls_tap0[t.cls]; t.ntaps = p.cls_ntaps[t.cls];
+    t.valid = t.u0 < p.cls_Hu[t.cls] && t.v0 < p.cls_Wu[t.cls];                   // false: tile outside this (smaller) parity class
+}
+
 template <int NT, int MODE>
 __device__ __forceinline__ TcTile tc_decode_tile(const TcParams& p, int tile) {
     TcTile t;
-    t.split = 0; t.slot = -1;
+    t.slot = -1;
     if constexpr (MODE == TC_CORR) {
         // unit -> (halo block, tile x, tile y, plane, sample); co0 carries the halo block, cls the parity plane
         int r = tile / p.cnt;
@@ -116,7 +133,7 @@ __device__ __forceinline__ TcTile tc_decode_tile(const TcParams& p, int tile) {
     if constexpr (MODE == TC_WGRAD) {
         // unit -> (K range, small-channel tile, big-channel tile, tap); u0 carries the first big channel, slot the unit itself
         int q = tile / p.wg_S;
-        t.split = tile - q * p.wg_S;
+        const int split = tile - q * p.wg_S;
         const int q2 = q / p.wg_ST;
         t.co0 = (q - q2 * p.wg_ST) * NT;
         t.tap0 = q2 / p.wg_BT;
@@ -124,40 +141,24 @@ __device__ __forceinline__ TcTile tc_decode_tile(const TcParams& p, int tile) {
         t.tap0 *= p.wg_TPT;                                        // first tap of the group
         t.n = 0; t.v0 = 0; t.cls = 0; t.ntaps = 1; t.slot = tile; t.valid = true;
         const int per = (p.wg_segs + p.wg_S - 1) / p.wg_S;
-        t.k0 = min(p.wg_segs, t.split * per);
+        t.k0 = min(p.wg_segs, split * per);
         t.steps = min(p.wg_segs, t.k0 + per) - t.k0;
         return t;
     }
-    int tseg = 0;
-    if (p.tail_z > 1 && tile >= p.tail_first) {
-        t.slot = tile - p.tail_first;
+    int seg = 0;
+    if (p.split_z > 1 && tile >= p.split_first) {              // the K ranges of a split tile run side by side (shared A tiles in L2)
+        t.slot = tile - p.split_first;
         int q;
-        p.d_tail_z.divmod(t.slot, q, tseg);
-        tile = p.tail_first + q;
+        p.d_split_z.divmod(t.slot, q, seg);
+        tile = p.split_first + q;
     }
-    if (p.splits > 1) { int q; p.d_splits.divmod(tile, q, t.split); tile = q; }   // splits of a tile run side by side (shared A tiles in L2)
-    int pix, r, cot = 0;
-    p.d_ntiles.divmod(tile, r, pix);
-    t.cls = 0;
-    if (r) p.d_cotiles.divmod(r, t.cls, cot);
-    int tx, ty, q2;
-    p.d_tiles_x.divmod(pix, q2, tx);
-    p.d_tiles_y.divmod(q2, t.n, ty);
-    t.u0 = ty * p.th; t.v0 = tx * p.tw;
-    t.co0 = cot * NT;
-    t.tap0 = p.cls_tap0[t.cls]; t.ntaps = p.cls_ntaps[t.cls];
-    t.valid = t.u0 < p.cls_Hu[t.cls] && t.v0 < p.cls_Wu[t.cls];                   // false: tile outside this (smaller) parity class
+    tc_whole_tile<NT>(p, tile, t);
     const int gsz = MODE == TC_GROUP ? 32 / p.gcs : 1;
     t.steps = MODE == TC_ROW ? p.rsteps : (MODE == TC_GROUP ? (t.ntaps + gsz - 1) / gsz : t.ntaps * p.cblocks);
     t.k0 = 0;
-    if (p.splits > 1) {
-        const int per = (t.steps + p.splits - 1) / p.splits;
-        t.k0 = min(t.steps, t.split * per);
-        t.steps = min(t.steps, t.k0 + per) - t.k0;
-    }
     if (t.slot >= 0) {
-        const int per = (t.steps + p.tail_z - 1) / p.tail_z;
-        t.k0 = min(t.steps, tseg * per);
+        const int per = (t.steps + p.split_z - 1) / p.split_z;
+        t.k0 = min(t.steps, seg * per);
         t.steps = min(t.steps, t.k0 + per) - t.k0;
     }
     return t;
@@ -465,13 +466,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
             if (u < p.cls_Hu[T.cls] && v < p.cls_Wu[T.cls]) {
                 const int oy = u * p.ou + p.cls_oy0[T.cls], ox = v * p.ov + p.cls_ox0[T.cls];
                 if (T.slot >= 0) {
-                    // tail split: raw partial sums of this K range, [slot][128 pixels][NT]
+                    // K split: raw partial sums of this K range, [slot][128 pixels][NT]
                     float* o = ws + ((long long)T.slot * 128 + m) * NT + hf * NH;
-#pragma unroll
-                    for (int j = 0; j < NH; j += 4) *reinterpret_cast<float4*>(o + j) = *reinterpret_cast<const float4*>(srow + j);
-                } else if (p.splits > 1) {
-                    // raw partial sums, dense [split][n][oy][ox][Co]; bias / ReLU are applied by the fixed-order reduction
-                    float* o = ws + ((((long long)T.split * p.N + T.n) * p.Ho + oy) * p.Wo + ox) * p.Co + T.co0 + hf * NH;
 #pragma unroll
                     for (int j = 0; j < NH; j += 4) *reinterpret_cast<float4*>(o + j) = *reinterpret_cast<const float4*>(srow + j);
                 } else {
@@ -541,47 +537,23 @@ __global__ void tc_pack_row_kernel(const float* __restrict__ w, float* __restric
     }
 }
 
-// fixed-order sum of the split-K partials + bias + ReLU (4 channels per thread)
-__global__ void tc_splitk_reduce_kernel(const float* __restrict__ ws, const float* __restrict__ bias, float* __restrict__ out, TcParams p) {
-    const int c4 = p.Co / 4;
-    const long long per = (long long)p.N * p.Ho * p.Wo * c4;
-    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < per; idx += (long long)gridDim.x * blockDim.x) {
-        const int c = (int)(idx % c4) * 4;
-        long long m = idx / c4;
-        float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
-        for (int z = 0; z < p.splits; z++) {
-            const float4 v = *reinterpret_cast<const float4*>(ws + ((long long)z * p.N * p.Ho * p.Wo + m) * p.Co + c);
-            a.x += v.x; a.y += v.y; a.z += v.z; a.w += v.w;
-        }
-        if (p.has_bias) { a.x += __ldg(bias + c); a.y += __ldg(bias + c + 1); a.z += __ldg(bias + c + 2); a.w += __ldg(bias + c + 3); }
-        if (p.relu) {
-            a.x = a.x > 0 ? a.x : a.x * p.slope; a.y = a.y > 0 ? a.y : a.y * p.slope;
-            a.z = a.z > 0 ? a.z : a.z * p.slope; a.w = a.w > 0 ? a.w : a.w * p.slope;
-        }
-        const int ox = (int)(m % p.Wo); m /= p.Wo;
-        const int oy = (int)(m % p.Ho);
-        const int n = (int)(m / p.Ho);
-        *reinterpret_cast<float4*>(out + n * p.out_sn + (long long)oy * p.out_sh + (long long)ox * p.out_sw + c) = a;
-    }
-}
-
-// fix-up of the tail split: fixed-order sum of the tail_z partial tiles + bias + ReLU, one thread per (tile row, 4 channels)
+// fix-up of a K-split layer: fixed-order sum of the split_z partial tiles of every split tile + bias + ReLU, one thread per
+// (tile row, 4 channels)
 template <int NT>
-__global__ void tc_tail_reduce_kernel(const float* __restrict__ ws, const float* __restrict__ bias, float* __restrict__ out, TcParams p) {
-    const int ntail = p.ntotal - p.tail_first;
-    const long long per = (long long)ntail * 128 * (NT / 4);
-    TcParams q = p;
-    q.tail_z = 1;                                  // decode whole tiles
+__global__ void tc_split_reduce_kernel(const float* __restrict__ ws, const float* __restrict__ bias, float* __restrict__ out, const TcParams p) {
+    const int nsplit = p.ntotal - p.split_first;
+    const long long per = (long long)nsplit * 128 * (NT / 4);
     for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < per; idx += (long long)gridDim.x * blockDim.x) {
         const int c = (int)(idx % (NT / 4)) * 4;
         const int m = (int)((idx / (NT / 4)) % 128);
         const int t = (int)(idx / ((NT / 4) * 128));
-        const TcTile T = tc_decode_tile<NT, TC_PLAIN>(q, p.tail_first + t);     // the tail split only exists in plain mode
+        TcTile T;
+        tc_whole_tile<NT>(p, p.split_first + t, T);
         const int u = T.u0 + m / p.tw, v = T.v0 + m % p.tw;
         if (!T.valid || u >= p.cls_Hu[T.cls] || v >= p.cls_Wu[T.cls]) continue;
         float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
-        for (int z = 0; z < p.tail_z; z++) {
-            const float4 x = *reinterpret_cast<const float4*>(ws + (((long long)t * p.tail_z + z) * 128 + m) * NT + c);
+        for (int z = 0; z < p.split_z; z++) {
+            const float4 x = *reinterpret_cast<const float4*>(ws + (((long long)t * p.split_z + z) * 128 + m) * NT + c);
             a.x += x.x; a.y += x.y; a.z += x.z; a.w += x.w;
         }
         const int co = T.co0 + c;
@@ -639,12 +611,19 @@ static TcSmallCi tc_small_ci(const fn2_conv_desc* d, int ci_stride) {
     return m;
 }
 
-// Split-K plan: layers whose tile list cannot fill the GPU (the 7x16 .. 14x32 maps of conv5/conv6/deconv5 with
-// K = 9 * 1024) cut every tile's K loop into `z` ranges that run on different SMs.
-// tail split plan for a layer with `tiles` tile units of `steps` K steps each: returns z (1 = off) and the first tail tile
-static int tc_tail_plan(long long tiles, int steps, int* first, int NT = 128) {
-    *first = (int)tiles;
+// K split of a layer with `tiles` tile units of `steps` K steps each (the fewest of any parity class): returns z (1 = unsplit)
+// and the first split tile.
+//  * Tile lists that cannot fill the GPU (the 7x16 .. 14x32 maps of conv5/conv6/deconv5 with K = 9 * 1024) split every tile.
+//  * Otherwise the tiles of the last, partial wave are split so that they spread over all SMs (448 tiles on 132 SMs:
+//    3 + 52/132 rounds instead of 4).
+static int tc_split_plan(long long tiles, int steps, int NT, int* first) {
     const int nsm = num_sms();
+    *first = 0;
+    if (tiles * 2 <= nsm && steps >= 32) {
+        const int z = min(min((int)(nsm / tiles), steps / 16), 8);
+        if (z >= 2) return z;
+    }
+    *first = (int)tiles;
     if (steps < 16) return 1;                       // (tiles <= nsm: everything is "tail" -- 112 tiles become 560 fifths on 132 SMs)
     const long long full = tiles / nsm * nsm, r = tiles - full;
     if (r == 0) return 1;
@@ -662,100 +641,109 @@ static int tc_tail_plan(long long tiles, int steps, int* first, int NT = 128) {
     *first = (int)full;
     return bz;
 }
-// tile count / K steps of a layer (same tiling rules as conv_tc_forward)
-static void tc_layer_geometry(const fn2_conv_desc* d, int N, int Ho, int Wo, int* NTo, long long* tiles, int* steps) {
-    const int NT = tc_nt(d->co);
-    const int sh = d->deconv ? d->stride_h : 1, sw = d->deconv ? d->stride_w : 1;
-    const int Hu = (Ho + sh - 1) / sh, Wu = (Wo + sw - 1) / sw, ncls = min(sh, Ho) * min(sw, Wo);
+
+// layer shapes the engine takes: whole 16-channel output tiles, at most 49 taps, convolution stride <= 2, deconvolution
+// stride 1 or 2 (at most 4 parity classes)
+static bool tc_takes(const fn2_conv_desc* d) {
+    if (d->co % 16 || d->kh * d->kw > 49 || d->stride_h > 2 || d->stride_w > 2) return false;
+    return !d->deconv || d->stride_h == d->stride_w;
+}
+
+// The engine's plan of one layer: every TcParams field of a forward launch except the output view, and the small-Ci packing.
+struct TcPlan {
+    TcParams p;
+    TcSmallCi sm;
+    int NT, steps;                                // output channels per tile, K steps per tile (the fewest of any parity class)
+};
+// W: input width (kernel-row packing), ci_stride: input pixel stride, ws_floats: workspace available for a K split (a K split
+// that does not fit runs unsplit).  Returns false for a layer the engine does not take, including a deconvolution with a
+// parity class that no tap reaches.
+static bool tc_plan(const fn2_conv_desc* d, int N, int W, int Ho, int Wo, int ci_stride, size_t ws_floats, TcPlan* pl) {
+    if (!tc_takes(d)) return false;
+    ConvTaps tp;
+    conv_taps(d, Ho, Wo, &tp);
+    TcParams* p = &pl->p;
+    TcSmallCi* sm = &pl->sm;
+    memset(p, 0, sizeof(*p));
+    const int NT = pl->NT = tc_nt(d->co);
+    p->N = N; p->cblocks = (d->ci + 31) / 32;
+    p->Ho = Ho; p->Wo = Wo;
+    p->relu = d->relu; p->has_bias = d->has_bias; p->slope = d->negative_slope;
+    // the kernel adds back the mean truncation loss of each chunk: TRUNC_LOSS_PER_MMA per a_hi*w_hi MMA chained into the
+    // chunk accumulator (4 per step; with NT == 128 the 8 cross-term MMAs of a step precede them while it is still small)
+    p->kd = tc_chunk_steps(NT);
+    *sm = tc_small_ci(d, ci_stride);
+    p->gcs = sm->mode == 1 ? sm->cs : 0;
+    p->rowmode = sm->mode == 2; p->rcs = sm->cs; p->rblocks = sm->rblocks; p->rsteps = d->kh * sm->rblocks;
+    p->rkw = d->kw; p->rpad = d->pad_w; p->rW = W;
+    // A box element strides: the convolution stride (x, y); a deconvolution's classes are stride-1 convolutions
+    p->su = d->deconv ? 1 : d->stride_w; p->sv = d->deconv ? 1 : d->stride_h;
+    p->ou = tp.ou; p->ov = tp.ov; p->ncls = tp.ncls;
+    int steps = 1 << 30, Wmax = 0, Hmax = 0;
+    for (int c = 0; c < tp.ncls; c++) {
+        if (!tp.ntaps[c]) return false;
+        p->cls_Hu[c] = tp.Hu[c]; p->cls_Wu[c] = tp.Wu[c]; p->cls_oy0[c] = tp.oy0[c]; p->cls_ox0[c] = tp.ox0[c];
+        p->cls_tap0[c] = tp.tap0[c]; p->cls_ntaps[c] = tp.ntaps[c];
+        steps = min(steps, tp.ntaps[c] * p->cblocks);
+        Wmax = max(Wmax, tp.Wu[c]); Hmax = max(Hmax, tp.Hu[c]);
+    }
+    memcpy(p->dy, tp.dy, sizeof(p->dy)); memcpy(p->dx, tp.dx, sizeof(p->dx)); memcpy(p->widx, tp.widx, sizeof(p->widx));
+    if (sm->mode == 1) steps = sm->ngroups;
+    if (sm->mode == 2) steps = p->rsteps;
+    pl->steps = steps;
+    // tile shape: widest power of two covering the (largest) row, 128 pixels per tile
     int tw = 8;
-    while (tw < Wu && tw < 128) tw *= 2;
-    const int th = 128 / tw;
-    *tiles = (long long)N * ((Wu + tw - 1) / tw) * ((Hu + th - 1) / th) * (d->co / NT) * ncls;
-    const int ntaps = d->deconv ? max(1, d->kh / sh) * max(1, d->kw / sw) : d->kh * d->kw;
-    *steps = ntaps * ((d->ci + 31) / 32);
-    *NTo = NT;
+    while (tw < Wmax && tw < 128) tw *= 2;
+    p->tw = tw; p->th = 128 / tw;
+    p->tiles_x = (Wmax + p->tw - 1) / p->tw; p->tiles_y = (Hmax + p->th - 1) / p->th;
+    p->ntiles = N * p->tiles_x * p->tiles_y;
+    p->cotiles = d->co / NT;
+    p->ntotal = p->ntiles * p->cotiles * p->ncls;
+    int first = p->ntotal, z = 1;
+    if (!sm->mode) z = tc_split_plan(p->ntotal, steps, NT, &first);           // small-Ci packing modes do not split
+    if (z > 1 && ws_floats < (size_t)(p->ntotal - first) * z * 128 * NT) { z = 1; first = p->ntotal; }
+    p->split_first = first; p->split_z = z;
+    p->total = first + (p->ntotal - first) * z;
+    p->d_ntiles.init(p->ntiles); p->d_cotiles.init(p->cotiles); p->d_tiles_x.init(p->tiles_x); p->d_tiles_y.init(p->tiles_y);
+    p->d_split_z.init(z);
+    return true;
 }
 
-static int tc_split_plan(const fn2_conv_desc* d, int N, int Ho, int Wo) {
-    if (!d->deconv && d->ci <= 16) return 1;                       // small-Ci packing modes do not split
-    if (d->co % 16) return 1;
-    int NT, steps; long long tiles;
-    tc_layer_geometry(d, N, Ho, Wo, &NT, &tiles, &steps);
-    const int nsm = num_sms();
-    if (tiles * 2 > nsm || steps < 32) return 1;
-    int z = (int)(nsm / tiles);
-    z = min(z, steps / 16);
-    z = min(z, 8);
-    return z < 2 ? 1 : z;
+// workspace of the layer's K split; the pixel stride does not matter: only the small-Ci modes depend on it, and they never split
+size_t conv_tc_workspace_floats(const fn2_conv_desc* d, int N, int W, int Ho, int Wo) {
+    TcPlan pl;
+    if (!tc_plan(d, N, W, Ho, Wo, d->ci, SIZE_MAX, &pl) || pl.p.split_z == 1) return 0;
+    return (size_t)(pl.p.ntotal - pl.p.split_first) * pl.p.split_z * 128 * pl.NT;
 }
 
-// taps-on-N engine for few output channels at high resolution (fn2_conv_tn.cu)
-int conv_tn_applicable(const fn2_conv_desc* d);
-size_t conv_tn_packed_floats(const fn2_conv_desc* d);
-int conv_tn_pack(const fn2_conv_desc* d, const float* w, float* wp, cudaStream_t st);
-int conv_tn_plan(const fn2_conv_desc* d, int N, int Ho, int Wo, int* out8);
-int conv_tn_forward(const fn2_conv_desc* d, const T4& in, const float* wp, const float* bias, const T4& out, cudaStream_t st);
-
-size_t conv_tc_workspace_floats(const fn2_conv_desc* d, int N, int Ho, int Wo) {
-    if (conv_tn_applicable(d)) return 0;
-    const int z = tc_split_plan(d, N, Ho, Wo);
-    if (z > 1) return (size_t)z * N * Ho * Wo * d->co;
-    if (d->co % 16 || (!d->deconv && d->ci <= 16)) return 0;
-    int NT, steps, first; long long tiles;
-    tc_layer_geometry(d, N, Ho, Wo, &NT, &tiles, &steps);
-    const int tz = tc_tail_plan(tiles, steps, &first, NT);
-    return tz > 1 ? (size_t)(tiles - first) * tz * 128 * NT : 0;
-}
-
-// Host-side plan of the tensor-core engine for one layer shape (introspection for tests and tools; needs no GPU):
-// out = {NT, tile units, K steps per tile, small-Ci mode (0 plain, 1 tap groups, 2 kernel rows), uniform K splits,
-//        first tail tile, tail K ranges, 0}
-int conv_tc_plan(const fn2_conv_desc* d, int N, int Ho, int Wo, int ci_stride, int* out8) {
-    for (int i = 0; i < 8; i++) out8[i] = 0;
-    if (d->co % 16) return 0;
-    if (conv_tn_applicable(d)) return conv_tn_plan(d, N, Ho, Wo, out8);
-    int NT, steps; long long tiles;
-    tc_layer_geometry(d, N, Ho, Wo, &NT, &tiles, &steps);
-    const TcSmallCi sm = tc_small_ci(d, ci_stride);
-    if (sm.mode == 1) steps = sm.ngroups;
-    if (sm.mode == 2) steps = d->kh * sm.rblocks;
-    out8[0] = NT; out8[1] = (int)tiles; out8[2] = steps; out8[3] = sm.mode;
-    out8[4] = tc_split_plan(d, N, Ho, Wo);
-    out8[5] = (int)tiles; out8[6] = 1;
-    if (out8[4] == 1 && !sm.mode) { int first = 0; out8[6] = tc_tail_plan(tiles, steps, &first, NT); out8[5] = first; }
-    return 1;
+// plan8 (fn2_conv_plan): {NT, tile units, K steps per tile, small-Ci mode (0 plain, 1 tap groups, 2 kernel rows), first split
+// tile, K ranges per split tile, 0, 0}; left 0 for a layer the engine does not take
+void conv_tc_plan(const fn2_conv_desc* d, int N, int W, int Ho, int Wo, int ci_stride, int* out8) {
+    TcPlan pl;
+    if (!tc_plan(d, N, W, Ho, Wo, ci_stride, SIZE_MAX, &pl)) return;
+    out8[0] = pl.NT; out8[1] = pl.p.ntotal; out8[2] = pl.steps; out8[3] = pl.sm.mode;
+    out8[4] = pl.p.split_first; out8[5] = pl.p.split_z;
 }
 
 int conv_tc_eligible(const fn2_conv_desc* d, const T4& in, const T4& out) {
     if (!tc_enabled()) return 0;
     if (in.sc != 1 || out.sc != 1) return 0;
-    if (d->co % 16) return 0;
-    if (d->deconv && (d->stride_h != 2 || d->stride_w != 2) && (d->stride_h != 1 || d->stride_w != 1)) return 0;
-    if (d->kh * d->kw > 49) return 0;
-    if (d->stride_h > 2 || d->stride_w > 2) return 0;
+    if (!tc_takes(d)) return 0;
     if (((uintptr_t)in.p & 15) || (in.sw & 3) || (in.sh & 3) || (in.sn & 3)) return 0;
     if (((uintptr_t)out.p & 15) || (out.sw & 3) || (out.sh & 3) || (out.sn & 3)) return 0;
     if (!tc_encode_fn()) return 0;
     return 1;
 }
 
-int conv_tc_packed_floats(const fn2_conv_desc* d, int ci_stride, size_t* floats) {
-    if (conv_tn_applicable(d)) { *floats = conv_tn_packed_floats(d); return FN2_OK; }
-    const int cip = (d->ci + 31) / 32 * 32;
+size_t conv_tc_packed_floats(const fn2_conv_desc* d, int ci_stride) {
+    if (d->co % 16) return 0;
     const TcSmallCi sm = tc_small_ci(d, ci_stride);
-    if (sm.mode) {
-        const int nblk = sm.mode == 2 ? d->kh * sm.rblocks : sm.ngroups;
-        *floats = (d->co % 16 == 0) ? (size_t)2 * nblk * d->co * 32 : 0;
-        return FN2_OK;
-    }
-    *floats = (d->co % 16 == 0) ? (size_t)2 * d->kh * d->kw * d->co * cip : 0;
-    return FN2_OK;
+    if (sm.mode) return (size_t)2 * (sm.mode == 2 ? d->kh * sm.rblocks : sm.ngroups) * d->co * 32;
+    return (size_t)2 * d->kh * d->kw * d->co * ((d->ci + 31) / 32 * 32);
 }
 
 int conv_tc_pack(const fn2_conv_desc* d, int ci_stride, const float* w, float* wp, cudaStream_t st) {
-    if (conv_tn_applicable(d)) return conv_tn_pack(d, w, wp, st);
-    size_t floats = 0;
-    conv_tc_packed_floats(d, ci_stride, &floats);
+    const size_t floats = conv_tc_packed_floats(d, ci_stride);
     if (!floats) return FN2_OK;
     const int cip = (d->ci + 31) / 32 * 32;
     const TcSmallCi sm = tc_small_ci(d, ci_stride);
@@ -770,32 +758,22 @@ int conv_tc_pack(const fn2_conv_desc* d, int ci_stride, const float* w, float* w
     return FN2_OK;
 }
 
-static inline int floordiv_i(int a, int b) { return (a >= 0) ? a / b : -((-a + b - 1) / b); }
-
 int conv_tc_forward(const fn2_conv_desc* d, const T4& in, const float* wp, const float* bias, const T4& out, float* ws, size_t ws_floats,
                     cudaStream_t st) {
-    if (conv_tn_applicable(d)) return conv_tn_forward(d, in, wp, bias, out, st);
     EncodeTiledFn enc = tc_encode_fn();
     if (!enc) { set_error("conv_tc: cuTensorMapEncodeTiled unavailable"); return FN2_ERR_CUDA; }
-    const int NT = tc_nt(d->co);
-    const int cip = (d->ci + 31) / 32 * 32;
-    TcParams p;
-    p.N = in.n; p.Co = d->co; p.cblocks = cip / 32;
-    p.Ho = out.h; p.Wo = out.w;
-    p.splits = tc_split_plan(d, in.n, out.h, out.w);
-    if (p.splits > 1 && (!ws || ws_floats < (size_t)p.splits * in.n * out.h * out.w * d->co)) p.splits = 1;
+    TcPlan pl;
+    if (!tc_plan(d, in.n, in.w, out.h, out.w, (int)in.sw, ws ? ws_floats : 0, &pl)) {
+        set_error("conv_tc: layer not supported (deconvolution parity class without taps)"); return FN2_ERR_INVALID;
+    }
+    TcParams& p = pl.p;
+    const TcSmallCi& sm = pl.sm;
+    const int NT = pl.NT, su = p.su, sv = p.sv;
     p.out_sn = out.sn; p.out_sh = out.sh; p.out_sw = out.sw;
-    p.relu = d->relu; p.has_bias = d->has_bias; p.slope = d->negative_slope;
-    // the kernel adds back the mean truncation loss of each chunk: TRUNC_LOSS_PER_MMA per a_hi*w_hi MMA chained into the
-    // chunk accumulator (4 per step; with NT == 128 the 8 cross-term MMAs of a step precede them while it is still small)
-    p.kd = tc_chunk_steps(NT);
-
-    const TcSmallCi sm = tc_small_ci(d, (int)in.sw);
-    p.gcs = sm.mode == 1 ? sm.cs : 0;
-    p.rowmode = sm.mode == 2; p.rcs = sm.cs; p.rblocks = sm.rblocks; p.rsteps = d->kh * sm.rblocks; p.rkw = d->kw; p.rpad = d->pad_w; p.rW = in.w;
     // weights: [2][taps][Co][cip]   (group mode: [2][groups][Co][32])
     CUtensorMap mapW;
     {
+        const int cip = p.cblocks * 32;
         const int kin = sm.mode ? 32 : cip;
         const int nblk = sm.mode == 2 ? p.rsteps : (sm.mode == 1 ? sm.ngroups : d->kh * d->kw);
         cuuint64_t dims[4] = {(cuuint64_t)kin, (cuuint64_t)d->co, (cuuint64_t)nblk, 2};
@@ -806,16 +784,8 @@ int conv_tc_forward(const fn2_conv_desc* d, const T4& in, const float* wp, const
                          CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) { set_error("conv_tc: weight tensor map failed (%d)", (int)r); return FN2_ERR_CUDA; }
     }
-    auto run = [&](int su, int sv) -> int {
-        // tile shape: widest power of two covering the (largest) row, 128 pixels per tile
-        int Wmax = 0, Hmax = 0;
-        for (int c = 0; c < p.ncls; c++) { Wmax = max(Wmax, p.cls_Wu[c]); Hmax = max(Hmax, p.cls_Hu[c]); }
-        int tw = 8;
-        while (tw < Wmax && tw < 128) tw *= 2;
-        p.tw = tw; p.th = 128 / tw;
-        p.tiles_x = (Wmax + p.tw - 1) / p.tw; p.tiles_y = (Hmax + p.th - 1) / p.th;
-        p.su = su; p.sv = sv;
-        CUtensorMap mapA;
+    CUtensorMap mapA;
+    {
         cuuint64_t dims[4] = {(cuuint64_t)in.c, (cuuint64_t)in.w, (cuuint64_t)in.h, (cuuint64_t)in.n};
         cuuint64_t strides[3] = {(cuuint64_t)in.sw * 4, (cuuint64_t)in.sh * 4, (cuuint64_t)in.sn * 4};
         cuuint32_t box[4] = {(cuuint32_t)(p.gcs ? p.gcs : 32), (cuuint32_t)(p.tw * su), (cuuint32_t)(p.th * sv), 1};
@@ -833,99 +803,45 @@ int conv_tc_forward(const fn2_conv_desc* d, const T4& in, const float* wp, const
                          p.gcs ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) { set_error("conv_tc: activation tensor map failed (%d)", (int)r); return FN2_ERR_CUDA; }
-        p.ntiles = p.N * p.tiles_x * p.tiles_y;
-        p.cotiles = d->co / NT;
-        p.total = p.ntiles * p.cotiles * p.ncls * p.splits;
-        p.ntotal = p.total; p.tail_first = p.total; p.tail_z = 1;
-        p.d_ntiles.init(p.ntiles); p.d_cotiles.init(p.cotiles); p.d_tiles_x.init(p.tiles_x); p.d_tiles_y.init(p.tiles_y);
-        p.d_splits.init(max(1, p.splits)); p.d_tail_z.init(1);
-        if (p.splits == 1 && !sm.mode && ws) {
-            int first = 0, steps_min = 1 << 30;
-            for (int c = 0; c < p.ncls; c++) steps_min = min(steps_min, p.cls_ntaps[c] * p.cblocks);
-            const int tz = tc_tail_plan(p.total, steps_min, &first, NT);
-            if (tz > 1 && ws_floats >= (size_t)(p.total - first) * tz * 128 * NT) {
-                p.tail_first = first; p.tail_z = tz; p.d_tail_z.init(tz);
-                p.total = first + (p.ntotal - first) * tz;
-            }
-        }
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3((unsigned)min(p.total, num_sms()), 1, 1);
-        cfg.blockDim = dim3(TC_THREADS);
-        cfg.stream = st;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[0].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = attr; cfg.numAttrs = 1;
+    }
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3((unsigned)min(p.total, num_sms()), 1, 1);
+    cfg.blockDim = dim3(TC_THREADS);
+    cfg.stream = st;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr; cfg.numAttrs = 1;
 #define FN2_TC_LAUNCH(NTV, MODEV)                                                                                       \
-        {                                                                                                               \
-            static bool attr_set = false;                                                                               \
-            if (!attr_set) {                                                                                            \
-                FN2_CUDA(cudaFuncSetAttribute(conv_tc_kernel<NTV, MODEV>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcGeo<NTV>::SMEM)); \
-                attr_set = true;                                                                                        \
-            }                                                                                                           \
-            cfg.dynamicSmemBytes = TcGeo<NTV>::SMEM;                                                                    \
-            FN2_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<NTV, MODEV>, mapA, mapW, bias, out.p, ws, p));                  \
-        }
+    {                                                                                                                   \
+        static bool attr_set = false;                                                                                   \
+        if (!attr_set) {                                                                                                \
+            FN2_CUDA(cudaFuncSetAttribute(conv_tc_kernel<NTV, MODEV>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcGeo<NTV>::SMEM)); \
+            attr_set = true;                                                                                            \
+        }                                                                                                               \
+        cfg.dynamicSmemBytes = TcGeo<NTV>::SMEM;                                                                        \
+        FN2_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<NTV, MODEV>, mapA, mapW, bias, out.p, ws, p));                      \
+    }
 #define FN2_TC_LAUNCH_NT(MODEV)                                                                                         \
-        if (NT == 128) FN2_TC_LAUNCH(128, MODEV)                                                                        \
-        else if (NT == 64) FN2_TC_LAUNCH(64, MODEV)                                                                     \
-        else if (NT == 32) FN2_TC_LAUNCH(32, MODEV)                                                                     \
-        else FN2_TC_LAUNCH(16, MODEV)
-        if (sm.mode == 2) { FN2_TC_LAUNCH_NT(TC_ROW) }
-        else if (sm.mode == 1) { FN2_TC_LAUNCH_NT(TC_GROUP) }
-        else { FN2_TC_LAUNCH_NT(TC_PLAIN) }
+    if (NT == 128) FN2_TC_LAUNCH(128, MODEV)                                                                            \
+    else if (NT == 64) FN2_TC_LAUNCH(64, MODEV)                                                                         \
+    else if (NT == 32) FN2_TC_LAUNCH(32, MODEV)                                                                         \
+    else FN2_TC_LAUNCH(16, MODEV)
+    if (sm.mode == 2) { FN2_TC_LAUNCH_NT(TC_ROW) }
+    else if (sm.mode == 1) { FN2_TC_LAUNCH_NT(TC_GROUP) }
+    else { FN2_TC_LAUNCH_NT(TC_PLAIN) }
 #undef FN2_TC_LAUNCH_NT
 #undef FN2_TC_LAUNCH
+    FN2_LAUNCH_CHECK();
+    if (p.split_z > 1) {
+        const long long work = (long long)(p.ntotal - p.split_first) * 128 * (NT / 4);
+        if (NT == 128) tc_split_reduce_kernel<128><<<ew_grid(work, 256), 256, 0, st>>>(ws, bias, out.p, p);
+        else if (NT == 64) tc_split_reduce_kernel<64><<<ew_grid(work, 256), 256, 0, st>>>(ws, bias, out.p, p);
+        else if (NT == 32) tc_split_reduce_kernel<32><<<ew_grid(work, 256), 256, 0, st>>>(ws, bias, out.p, p);
+        else tc_split_reduce_kernel<16><<<ew_grid(work, 256), 256, 0, st>>>(ws, bias, out.p, p);
         FN2_LAUNCH_CHECK();
-        if (p.tail_z > 1) {
-            const long long work = (long long)(p.ntotal - p.tail_first) * 128 * (NT / 4);
-            if (NT == 128) tc_tail_reduce_kernel<128><<<ew_grid(work, 256), 256, 0, st>>>(ws, bias, out.p, p);
-            else if (NT == 64) tc_tail_reduce_kernel<64><<<ew_grid(work, 256), 256, 0, st>>>(ws, bias, out.p, p);
-            else if (NT == 32) tc_tail_reduce_kernel<32><<<ew_grid(work, 256), 256, 0, st>>>(ws, bias, out.p, p);
-            else tc_tail_reduce_kernel<16><<<ew_grid(work, 256), 256, 0, st>>>(ws, bias, out.p, p);
-            FN2_LAUNCH_CHECK();
-        }
-        if (p.splits > 1) {
-            tc_splitk_reduce_kernel<<<ew_grid((long long)p.N * p.Ho * p.Wo * (p.Co / 4), 256), 256, 0, st>>>(ws, bias, out.p, p);
-            FN2_LAUNCH_CHECK();
-        }
-        return FN2_OK;
-    };
-    if (!d->deconv) {
-        p.ncls = 1;
-        p.cls_Hu[0] = out.h; p.cls_Wu[0] = out.w; p.ou = p.ov = 1; p.cls_oy0[0] = p.cls_ox0[0] = 0;
-        p.cls_tap0[0] = 0; p.cls_ntaps[0] = d->kh * d->kw;
-        for (int r = 0; r < d->kh; r++)
-            for (int s = 0; s < d->kw; s++) {
-                const int t = r * d->kw + s;
-                p.dy[t] = (short)(r - d->pad_h); p.dx[t] = (short)(s - d->pad_w); p.widx[t] = (short)t;
-            }
-        return run(d->stride_w, d->stride_h);
     }
-    // deconvolution: all output parity classes in one launch (grid.z); every kernel tap belongs to exactly one class
-    const int sh = d->stride_h, sw = d->stride_w;
-    p.ou = sh; p.ov = sw; p.ncls = 0;
-    int nt = 0;
-    for (int py = 0; py < sh; py++)
-        for (int px = 0; px < sw; px++) {
-            if (py >= out.h || px >= out.w) continue;
-            const int c = p.ncls++;
-            p.cls_Hu[c] = (out.h - py + sh - 1) / sh; p.cls_Wu[c] = (out.w - px + sw - 1) / sw;
-            p.cls_oy0[c] = py; p.cls_ox0[c] = px; p.cls_tap0[c] = nt;
-            for (int r = 0; r < d->kh; r++) {
-                if (((py + d->pad_h - r) % sh + sh) % sh) continue;
-                for (int s = 0; s < d->kw; s++) {
-                    if (((px + d->pad_w - s) % sw + sw) % sw) continue;
-                    p.dy[nt] = (short)floordiv_i(py + d->pad_h - r, sh);
-                    p.dx[nt] = (short)floordiv_i(px + d->pad_w - s, sw);
-                    p.widx[nt] = (short)(r * d->kw + s);
-                    nt++;
-                }
-            }
-            p.cls_ntaps[c] = nt - p.cls_tap0[c];
-            if (p.cls_ntaps[c] == 0) { set_error("conv_tc: deconvolution parity class without taps"); return FN2_ERR_INVALID; }
-        }
-    return run(1, 1);
+    return FN2_OK;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -1142,9 +1058,9 @@ int conv_tc_wgrad(const fn2_conv_desc* d, const T4& bottom, const T4& top_diff, 
     }
     TcParams p;
     memset(&p, 0, sizeof(p));
-    p.N = g.N; p.Co = g.Cs; p.cblocks = 1;
+    p.N = g.N; p.cblocks = 1;
     p.Ho = g.Hs; p.Wo = g.Ws;
-    p.splits = 1; p.tail_z = 1; p.su = g.sx; p.sv = g.sy; p.ou = p.ov = 1; p.ncls = 1;
+    p.split_z = 1; p.su = g.sx; p.sv = g.sy; p.ou = p.ov = 1; p.ncls = 1;
     p.tw = 128; p.th = 1; p.tiles_x = p.tiles_y = 1;
     p.wg_S = g.S; p.wg_ST = g.ST; p.wg_BT = g.BT; p.wg_segs = g.segs; p.wg_segs_x = g.segs_x; p.wg_sx = g.sx;
     p.wg_G = g.G; p.wg_TPT = g.TPT; p.wg_taps = g.taps;
@@ -1157,7 +1073,7 @@ int conv_tc_wgrad(const fn2_conv_desc* d, const T4& bottom, const T4& top_diff, 
             p.dy[t] = (short)(ky - d->pad_h); p.dx[t] = (short)(shift + dl); p.widx[t] = (short)(par | (dl << 4));
         }
     p.total = g.TG * g.BT * g.ST * g.S;
-    p.ntotal = p.total; p.tail_first = p.total;
+    p.ntotal = p.total; p.split_first = p.total;
     CUtensorMap mapA, mapB;
     {
         cuuint64_t dims[4] = {(cuuint64_t)g.Wq, (cuuint64_t)g.Hb * g.sx, (cuuint64_t)g.Cb, (cuuint64_t)4 * g.N};
@@ -1229,15 +1145,15 @@ int corr_tc_forward(const T4& b0, const T4& b1, const T4& top, int md, int s2, f
     p.cbw = p.tw + 2 * R; p.cbh = 4;                                       // block = 4 full halo rows = 112 pixels (MMA N = 112)
     p.cnt = (p.th + 2 * R) / p.cbh;                             // 9 blocks
     p.cscale = 1.0f / (float)C;                                           // sumelems = k*k*C (correlation_layer.cu:108)
-    p.N = N; p.Co = NT; p.cblocks = C / 32;
+    p.N = N; p.cblocks = C / 32;
     p.Ho = H; p.Wo = W;
     p.out_sn = top.sn; p.out_sh = top.sh; p.out_sw = top.sw;
-    p.splits = 1; p.tail_z = 1; p.su = S; p.sv = S; p.ou = p.ov = 1; p.ncls = 1;
+    p.split_z = 1; p.su = S; p.sv = S; p.ou = p.ov = 1; p.ncls = 1;
     p.kd = tc_chunk_steps(NT);
     const int Ws = (W + S - 1) / S, Hs = (H + S - 1) / S;
     p.tiles_x = (Ws + p.tw - 1) / p.tw; p.tiles_y = (Hs + p.th - 1) / p.th;
     p.total = N * S * S * p.tiles_x * p.tiles_y * p.cnt;
-    p.ntotal = p.total; p.tail_first = p.total;
+    p.ntotal = p.total; p.split_first = p.total;
     CUtensorMap mapA, mapB;
     {
         cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};

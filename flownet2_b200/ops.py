@@ -185,7 +185,8 @@ def mean_subtract(top, mean_pp=None, mean_pc=None, per_pixel=False):
 
 
 def conv_plan(ci, co, k, stride, pad, deconv, n, h, w, ci_stride):
-    """fn2_conv_plan: the tensor-core engines' host-side plan for a layer shape (8 ints, see include/fn2.h)."""
+    """fn2_conv_plan: the tensor-core engines' host-side plan for a layer shape (8 ints, see include/fn2.h): NT, tile units,
+    K steps per tile, mode, first split tile, K ranges per split tile."""
     d = fn2_conv_desc(ci, co, k, k, stride, stride, pad, pad, 1 if deconv else 0, 1, 0, 0.0, 0, 0)
     plan = (C.c_int32 * 8)()
     check(lib().fn2_conv_plan(C.byref(d), n, h, w, ci_stride, plan))

@@ -184,8 +184,11 @@ FN2_API int fn2_conv_out_shape(const fn2_conv_desc* d, int H, int W, int* Ho, in
  * Passing a NULL / too small workspace is allowed: the kernel then runs unsplit. */
 FN2_API int fn2_conv_workspace_bytes(const fn2_conv_desc* d, int N, int H, int W, size_t* bytes);
 /* Host-side plan of the tensor-core engine for a layer shape (introspection; needs no GPU): plan8 = {NT (output channels per
- * tile; 0 = not eligible by channel count), tile units, K steps per tile, small-Ci mode (0 plain K blocks, 1 tap groups,
- * 2 kernel rows), uniform K splits, first tail tile, K ranges per tail tile, 0}. */
+ * tile; 0 = a shape the engine does not take), tile units, K steps per tile, small-Ci mode (0 plain K blocks, 1 tap groups,
+ * 2 kernel rows), first split tile, K ranges per split tile (1 = unsplit), 0, 0}.  The tiles from the first split tile on
+ * have their K loops cut into that many ranges, which run on different SMs: all tiles of a layer whose tile list cannot fill
+ * the GPU, else the tiles of the last, partial wave.  The taps-on-N engine (mode 3) reports {-accumulator columns of the
+ * widest pass, 0, K blocks, 3, passes, strips, 0, 0}. */
 FN2_API int fn2_conv_plan(const fn2_conv_desc* d, int N, int H, int W, int ci_stride, int32_t* plan8);
 FN2_API int fn2_conv_forward(const fn2_conv_desc* d, const fn2_tensor* bottom,
                              const float* packed_weights_dev, const float* bias_dev,

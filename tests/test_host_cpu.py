@@ -170,9 +170,10 @@ def test_no_compute_without_gpu_is_loud(fn2):
         fn2.Net(fn2.fill_template(fn2.model_template("FlowNet2-S"), 64, 64))
 
 
-def test_tensor_core_engine_plan_for_flownet2_shapes(fn2):
-    """Host-side planning of the tensor-core convolution engine (no GPU needed): tile width, small-Ci packing mode, split-K for
-    the small-spatial layers and the tail split of the last partial wave, at the BASELINE shapes (4 pairs, 1024x448)."""
+def test_tensor_core_engine_split_plan_for_flownet2_shapes(fn2):
+    """Host-side planning of the tensor-core convolution engine (no GPU needed): tile width, small-Ci packing mode and the K
+    split, read from plan8 slots 4-5 (first split tile, K ranges per split tile): every tile of the small-spatial layers, the
+    tiles of the last partial wave elsewhere, at the BASELINE shapes (4 pairs, 1024x448)."""
     from flownet2_b200 import fn2_conv_desc
     lib = fn2.lib()
 
@@ -195,12 +196,12 @@ def test_tensor_core_engine_plan_for_flownet2_shapes(fn2):
     assert pl[3] == 1
     # conv3_1: 448 tiles -> the tiles of the last, partial wave (448 mod the SM count) are K-split, partials fit the workspace
     pl, ws = plan(473, 256, 3, 1, 1, 56, 128)
-    assert pl[0] == 128 and pl[1] == 448 and pl[2] == 9 * 15 and pl[4] == 1
-    tail = 448 - pl[5]
-    assert 0 < tail < 448 // 3 and 2 <= pl[6] <= 8 and ws >= tail * pl[6] * 128 * 128 * 4
-    # conv6_1: 28 tiles with K = 9*1024 -> uniform split-K over the SMs
+    assert pl[0] == 128 and pl[1] == 448 and pl[2] == 9 * 15
+    tail = 448 - pl[4]
+    assert 0 < tail < 448 // 3 and 2 <= pl[5] <= 8 and ws >= tail * pl[5] * 128 * 128 * 4
+    # conv6_1: 32 tiles with K = 9*1024 -> every tile is K-split over the SMs
     pl, ws = plan(1024, 1024, 3, 1, 1, 7, 16)
-    assert pl[1] == 32 and 2 <= pl[4] <= 8 and ws >= pl[4] * 4 * 7 * 16 * 1024 * 4
+    assert pl[1] == 32 and pl[4] == 0 and 2 <= pl[5] <= 8 and ws >= pl[1] * pl[5] * 128 * 128 * 4
     # fusion interconv0: 16 output channels at full resolution -> taps-on-N engine (mode 3): two passes of 5 + 4 taps x 16 = 80
     # accumulator columns, K = 3 blocks of 32 channels, 35 strips of 30 complete columns
     pl, ws = plan(82, 16, 3, 1, 1, 448, 1024, cis=96)
@@ -216,13 +217,41 @@ def test_tensor_core_engine_plan_for_flownet2_shapes(fn2):
             "F.lib().fn2_conv_plan(C.byref(d), 4, 448, 1024, 96, o); print(list(o))")
     out = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, env=dict(os.environ, FN2_TN="0"), cwd=ROOT)
     pl = eval(out.stdout.strip().splitlines()[-1])
-    assert pl[0] == 16 and pl[3] == 0 and pl[4] == 1 and pl[2] == 27
+    assert pl[0] == 16 and pl[3] == 0 and pl[4] > 0 and pl[2] == 27
     # flow predictor (2 output channels) is not a tensor-core layer
     pl, _ = plan(194, 2, 3, 1, 1, 112, 256)
     assert pl[0] == 0
     # deconv5: 4 parity classes of 2x2 taps
     pl, _ = plan(1024, 512, 4, 2, 1, 7, 16, deconv=1)
     assert pl[0] == 128 and pl[2] == 4 * 32
+    # a 1x1 stride-2 deconvolution leaves three parity classes without taps: not a tensor-core layer
+    pl, ws = plan(256, 128, 1, 2, 0, 14, 32, deconv=1)
+    assert pl == [0] * 8
+
+
+def test_tensor_core_engine_plan_golden(fn2):
+    """fn2_conv_plan over a sweep of conv / deconv descriptors (tests/golden/make_conv_plan_golden.py): engine, NT, tiles, K
+    steps, small-Ci mode and K split unchanged.  The workspace is unchanged too, except for layers that split every tile: their
+    partial tiles take tiles * z * 128 * NT floats (at least the dense N * Ho * Wo * Co of the output they cover)."""
+    from flownet2_b200 import fn2_conv_desc
+    from tests.golden.make_conv_plan_golden import INT_FIELDS
+    lib = fn2.lib()
+    g = np.load(os.path.join(GOLD, "conv_plan_golden.npz"))
+    assert len(g["plan"]) > 7000 and g["uniform"].sum() > 500 and (g["plan"][:, 3] == 3).sum() > 100
+    bad = []
+    for row, (N, H, W, cis), want, ws_want, uniform in zip(g["desc"], g["shape"], g["plan"], g["ws"], g["uniform"]):
+        d = fn2_conv_desc(**dict(zip(INT_FIELDS, (int(v) for v in row))), negative_slope=0.1)
+        out = (C.c_int32 * 8)()
+        assert lib.fn2_conv_plan(C.byref(d), int(N), int(H), int(W), int(cis), out) == 0
+        ws = C.c_size_t()
+        assert lib.fn2_conv_workspace_bytes(C.byref(d), int(N), int(H), int(W), C.byref(ws)) == 0
+        got = list(out)
+        if uniform:
+            assert got[4] == 0
+            ws_want = max(int(ws_want), got[1] * got[5] * 128 * got[0] * 4)
+        if got != want.tolist() or ws.value != ws_want:
+            bad.append((row.tolist(), (N, H, W, cis), want.tolist(), got, int(ws_want), ws.value))
+    assert not bad, (len(bad), bad[:5])
 
 
 AUG_LAYER = """
