@@ -57,6 +57,11 @@ struct T4 {
     __host__ __device__ bool is_nhwc() const {
         return sc == 1 && sh == (long long)w * sw && sn == (long long)h * w * sw;
     }
+    // every pixel starts on a 16-byte boundary with its channels contiguous, so it can be read as float4 groups; how many
+    // groups a pixel may be read as (its extent) is for the caller to check
+    bool px_float4() const {
+        return sc == 1 && !((uintptr_t)p & 15) && !(sn & 3) && !(sh & 3) && !(sw & 3);
+    }
 };
 
 inline T4 view(const fn2_tensor* t) {

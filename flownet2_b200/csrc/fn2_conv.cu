@@ -244,7 +244,9 @@ __global__ void __launch_bounds__(256) conv_smallco_kernel(T4 in, const float* _
 }
 
 // Tiny path (Co <= 4 and Ci <= 32: flow upsamplers 2->2, full-resolution flow predictors): one thread per
-// output pixel, all weights staged in shared memory.
+// output pixel, all weights staged in shared memory.  A deconvolution output (oy, ox) is reached only by the kernel rows
+// r = (oy + ph) mod sh, + sh, ..., reading input rows (oy + ph) / sh, - 1, ... (columns alike): those taps are visited in
+// ascending order, and skipped only when they fall outside the input, exactly as in_coord() decides.
 template <bool DECONV>
 __global__ void __launch_bounds__(256) conv_tiny_kernel(T4 in, const float* __restrict__ wp,
                                                         const float* __restrict__ bias, T4 out, ConvP p) {
@@ -253,15 +255,19 @@ __global__ void __launch_bounds__(256) conv_tiny_kernel(T4 in, const float* __re
     for (int i = threadIdx.x; i < nw; i += blockDim.x) wsm[i] = wp[i];
     __syncthreads();
     const long long M = (long long)p.N * p.Ho * p.Wo;
+    const int rstep = DECONV ? p.sh : 1, sstep = DECONV ? p.sw : 1, istep = DECONV ? -1 : 1;
     for (long long m = blockIdx.x * (long long)blockDim.x + threadIdx.x; m < M; m += (long long)gridDim.x * blockDim.x) {
         const int ox = (int)(m % p.Wo);
         const int oy = (int)((m / p.Wo) % p.Ho);
         const int n = (int)(m / ((long long)p.Wo * p.Ho));
         float acc[4] = {0.f, 0.f, 0.f, 0.f};
-        for (int r = 0; r < p.kh; r++)
-            for (int s = 0; s < p.kw; s++) {
-                int iy, ix;
-                if (!in_coord<DECONV>(p, oy, ox, r, s, iy, ix)) continue;
+        const int ty = oy + p.ph, tx = ox + p.pw;
+        const int r0 = DECONV ? ty % p.sh : 0, iy0 = DECONV ? ty / p.sh : oy * p.sh - p.ph;
+        const int s0 = DECONV ? tx % p.sw : 0, ix0 = DECONV ? tx / p.sw : ox * p.sw - p.pw;
+        for (int r = r0, iy = iy0; r < p.kh; r += rstep, iy += istep) {
+            if (iy < 0 || iy >= p.H) continue;
+            for (int s = s0, ix = ix0; s < p.kw; s += sstep, ix += istep) {
+                if (ix < 0 || ix >= p.W) continue;
                 const float* ip = in.p + in.off(n, 0, iy, ix);
                 const float* w = wsm + (r * p.kw + s) * p.Ci * p.Co;
                 for (int ci = 0; ci < p.Ci; ci++) {
@@ -271,6 +277,7 @@ __global__ void __launch_bounds__(256) conv_tiny_kernel(T4 in, const float* __re
                         if (j < p.Co) acc[j] = fmaf(a, w[ci * p.Co + j], acc[j]);
                 }
             }
+        }
 #pragma unroll
         for (int j = 0; j < 4; j++) {
             if (j >= p.Co) break;
@@ -284,8 +291,12 @@ __global__ void __launch_bounds__(256) conv_tiny_kernel(T4 in, const float* __re
 
 // Flow predictors (Co == 2, NHWC input): the layers are memory bound (a few MFLOP per MB), so the kernels below read
 // every input pixel as float4 vectors and keep the [tap][ci] weight pairs in shared memory.
-//   conv_pf_thread_kernel: Ci <= 32 (full-resolution fusion predictors) -- one thread per output pixel
-//   conv_pf_warp_kernel:   larger Ci -- one warp per output pixel, lanes stride the channel vectors, shuffle reduce
+//   conv_pf3_tile_kernel:  3x3 / stride 1, Ci <= 32 (the full-resolution fusion predictors) -- one block per 32 x 8 outputs
+//   conv_pf_thread_kernel: other shapes with Ci <= 32 (the backward-data operator of the 4x4 / stride-2 flow upsamplers)
+//                          -- one thread per output pixel
+//   conv_pf3_warp_kernel:  3x3 / stride 1, larger Ci (the other predict_flow layers) -- one warp per 4 outputs of a row
+//   conv_pf_warp_kernel:   other shapes with larger Ci -- one warp per output pixel, lanes stride the channel vectors,
+//                          shuffle reduce
 // Channels [Ci, 4*C4) are blob padding: their weights are zero (the padding itself is finite, the arena is zero-filled).
 __device__ __forceinline__ void pf_stage_weights(float2* wsm, const float* __restrict__ wp, int taps, int Ci, int C4) {
     const int cp = C4 * 4;
@@ -373,50 +384,10 @@ __global__ void __launch_bounds__(256) conv_pf_warp_kernel(T4 in, const float* _
     }
 }
 
-// 3x3 / stride 1 specialisations of the two flow-predictor kernels (every predict_flow layer of FlowNet2): compile-time tap
-// loops so that the loads of a kernel row are in flight together.
-template <int C4>
-__global__ void __launch_bounds__(256) conv_pf3_thread_kernel(T4 in, const float* __restrict__ wp, const float* __restrict__ bias, T4 out, ConvP p) {
-    extern __shared__ float2 pf_wsm[];
-    pf_stage_weights(pf_wsm, wp, 9, p.Ci, C4);
-    const long long M = (long long)p.N * p.Ho * p.Wo;
-    for (long long m = blockIdx.x * (long long)blockDim.x + threadIdx.x; m < M; m += (long long)gridDim.x * blockDim.x) {
-        const int ox = (int)(m % p.Wo);
-        const int oy = (int)((m / p.Wo) % p.Ho);
-        const int n = (int)(m / ((long long)p.Wo * p.Ho));
-        float a0 = 0.f, a1 = 0.f;
-#pragma unroll
-        for (int r = 0; r < 3; r++) {
-            const int iy = oy - p.ph + r;
-            if (iy < 0 || iy >= p.H) continue;
-            float4 a[3][C4];
-#pragma unroll
-            for (int s = 0; s < 3; s++) {
-                const int ix = ox - p.pw + s;
-                const bool ok = ix >= 0 && ix < p.W;
-                const float4* ip = reinterpret_cast<const float4*>(in.p + in.off(n, 0, iy, ok ? ix : ox));
-#pragma unroll
-                for (int q = 0; q < C4; q++) a[s][q] = ok ? __ldg(ip + q) : make_float4(0.f, 0.f, 0.f, 0.f);
-            }
-#pragma unroll
-            for (int s = 0; s < 3; s++) {
-                const float4* w = reinterpret_cast<const float4*>(pf_wsm + (r * 3 + s) * C4 * 4);
-#pragma unroll
-                for (int q = 0; q < C4; q++) {
-                    const float4 w01 = w[2 * q], w23 = w[2 * q + 1];
-                    a0 = fmaf(a[s][q].x, w01.x, a0); a1 = fmaf(a[s][q].x, w01.y, a1);
-                    a0 = fmaf(a[s][q].y, w01.z, a0); a1 = fmaf(a[s][q].y, w01.w, a1);
-                    a0 = fmaf(a[s][q].z, w23.x, a0); a1 = fmaf(a[s][q].z, w23.y, a1);
-                    a0 = fmaf(a[s][q].w, w23.z, a0); a1 = fmaf(a[s][q].w, w23.w, a1);
-                }
-            }
-        }
-        pf_store(out, p, bias, n, oy, ox, a0, a1);
-    }
-}
-// Shared-memory tiled variant of the thread-per-pixel predictor for Ci <= 32: a block of 256 threads produces a 32 x 8 output
-// tile from a 34 x 10 input halo that is fetched with fully coalesced 128-bit loads (the direct version reads 64..128-byte
-// pixels at a 64..128-byte lane stride: 16 L1 wavefronts per load instruction).  Same accumulation order, bit-identical.
+// 3x3 / stride 1 predictor for Ci <= 32, any padding: a block of 256 threads produces a 32 x 8 output tile from the 34 x 10
+// input halo at (bx*32 - pw, by*8 - ph), fetched with fully coalesced 128-bit loads (a thread per output pixel would read
+// 64..128-byte pixels at a 64..128-byte lane stride: 16 L1 wavefronts per load instruction).  Halo pixels outside the input
+// are zero.
 template <int C4>
 __global__ void __launch_bounds__(256) conv_pf3_tile_kernel(T4 in, const float* __restrict__ wp, const float* __restrict__ bias, T4 out, ConvP p) {
     extern __shared__ float2 pf_wsm[];
@@ -443,7 +414,7 @@ __global__ void __launch_bounds__(256) conv_pf3_tile_kernel(T4 in, const float* 
         float a0 = 0.f, a1 = 0.f;
 #pragma unroll
         for (int r = 0; r < 3; r++) {
-            if (oy - p.ph + r < 0 || oy - p.ph + r >= p.H) continue;                 // same skipping as the direct kernel
+            if (oy - p.ph + r < 0 || oy - p.ph + r >= p.H) continue;                 // columns outside add the halo's zeros
 #pragma unroll
             for (int s_ = 0; s_ < 3; s_++) {
                 const float4* a = tile + ((ty + r) * HW + tx + s_) * PS;
@@ -533,48 +504,6 @@ __global__ void __launch_bounds__(256) conv_pf3_warp_kernel(T4 in, const float* 
     }
 }
 
-// Flow upsamplers (Deconvolution 4x4, stride 2, Ci, Co <= 4): an output pixel is reached by exactly the 2x2 taps whose parity
-// matches, so only those are visited (conv_tiny_kernel<true> tests all 16).  Same tap and channel order as the generic kernel,
-// hence bit-identical results.
-__global__ void __launch_bounds__(256) deconv_s2_tiny_kernel(T4 in, const float* __restrict__ wp, const float* __restrict__ bias, T4 out, ConvP p) {
-    extern __shared__ float wsm[];                    // [kh*kw][Ci][Co]
-    const int nw = p.kh * p.kw * p.Ci * p.Co;
-    for (int i = threadIdx.x; i < nw; i += blockDim.x) wsm[i] = wp[i];
-    __syncthreads();
-    const long long M = (long long)p.N * p.Ho * p.Wo;
-    for (long long m = blockIdx.x * (long long)blockDim.x + threadIdx.x; m < M; m += (long long)gridDim.x * blockDim.x) {
-        const int ox = (int)(m % p.Wo);
-        const int oy = (int)((m / p.Wo) % p.Ho);
-        const int n = (int)(m / ((long long)p.Wo * p.Ho));
-        float acc[4] = {0.f, 0.f, 0.f, 0.f};
-        const int ty = oy + p.ph, tx = ox + p.pw;
-        for (int r = ty & 1; r < p.kh; r += 2) {
-            const int iy = (ty - r) >> 1;
-            if (ty - r < 0 || iy >= p.H) continue;
-            for (int s_ = tx & 1; s_ < p.kw; s_ += 2) {
-                const int ix = (tx - s_) >> 1;
-                if (tx - s_ < 0 || ix >= p.W) continue;
-                const float* ip = in.p + in.off(n, 0, iy, ix);
-                const float* w = wsm + (r * p.kw + s_) * p.Ci * p.Co;
-                for (int ci = 0; ci < p.Ci; ci++) {
-                    const float a = __ldg(ip + ci * in.sc);
-#pragma unroll
-                    for (int j = 0; j < 4; j++)
-                        if (j < p.Co) acc[j] = fmaf(a, w[ci * p.Co + j], acc[j]);
-                }
-            }
-        }
-#pragma unroll
-        for (int j = 0; j < 4; j++) {
-            if (j >= p.Co) break;
-            float v = acc[j];
-            if (p.has_bias) v += __ldg(bias + j);
-            if (p.relu) v = v > 0 ? v : v * p.slope;
-            out.p[out.off(n, j, oy, ox)] = v;
-        }
-    }
-}
-
 // Caffe weights -> packed [k][co].  conv: w[co][ci][r][s]; deconv: w[ci][co][r][s].
 __global__ void pack_weights_kernel(const float* __restrict__ w, float* __restrict__ wp, int Ci, int Co,
                                     int kh, int kw, int cis, int deconv) {
@@ -643,8 +572,48 @@ static int make_params(const fn2_conv_desc* d, const T4& in, const T4& out, Conv
                   "conv: top must be (%d,%d,%d,%d), got (%d,%d,%d,%d)", in.n, d->co, Ho, Wo, out.n, out.c, out.h, out.w);
     p->Ci = d->ci; p->Co = d->co; p->kh = d->kh; p->kw = d->kw; p->sh = d->stride_h; p->sw = d->stride_w;
     p->ph = d->pad_h; p->pw = d->pad_w; p->H = in.h; p->W = in.w; p->Ho = Ho; p->Wo = Wo; p->N = in.n;
+    p->cis = d->ci; p->K = d->kh * d->kw * d->ci;
     p->relu = d->relu; p->has_bias = d->has_bias; p->slope = d->negative_slope;
     return FN2_OK;
+}
+
+// The SIMT kernels, in the order simt_route tries them.
+enum class SimtRoute { fewci, nhwc, pf3_tile, pf_thread, pf3_warp, pf_warp, tiny, smallco, igemm };
+
+// smem: dynamic shared memory bytes; C4: float4 groups per input pixel of the flow predictors; nhwc plans its own launches
+struct SimtLaunch { SimtRoute route; dim3 grid; size_t smem; int C4; };
+
+// Which SIMT kernel runs a layer the tensor-core engines do not take, and its launch geometry.
+static SimtLaunch simt_route(const fn2_conv_desc* d, const T4& in, const T4& out) {
+    const long long M = (long long)out.n * out.h * out.w;
+    const int taps = d->kh * d->kw, C4 = (d->ci + 3) / 4;
+    if (!d->deconv && d->ci <= 4 && d->co >= 32 && out.sc == 1 && taps * d->ci <= 200)
+        return {SimtRoute::fewci, dim3((unsigned)(M / out.w * ((out.w + FEW_PX - 1) / FEW_PX))), (size_t)FEW_PX * taps * d->ci * sizeof(float), 0};
+    if (conv_nhwc_eligible(d, in, out)) return {SimtRoute::nhwc, dim3(), 0, 0};
+    const size_t pf_smem = (size_t)taps * C4 * 4 * sizeof(float2);
+    if (!d->deconv && d->co == 2 && in.px_float4() && in.sw >= 4 * C4 && pf_smem <= 200 * 1024) {
+        const bool k3 = d->kh == 3 && d->kw == 3 && d->stride_h == 1 && d->stride_w == 1;
+        if (C4 <= 8 && k3) {
+            const long long tiles = (long long)out.n * ((out.w + 31) / 32) * ((out.h + 7) / 8);
+            return {SimtRoute::pf3_tile, dim3((unsigned)min((long long)num_sms() * 4, tiles)),
+                    pf_smem + (size_t)10 * 34 * (C4 + 1) * sizeof(float4), C4};
+        }
+        if (C4 <= 8) return {SimtRoute::pf_thread, dim3((unsigned)min((long long)num_sms() * 8, (M + 255) / 256)), pf_smem, C4};
+        const long long per_sm = max((size_t)1, min((size_t)8, (size_t)(220 * 1024) / (pf_smem + 1024)));
+        const long long warps = k3 ? (long long)out.n * out.h * ((out.w + 3) / 4) : M;       // pf3_warp: 4 outputs of a row
+        return {k3 ? SimtRoute::pf3_warp : SimtRoute::pf_warp, dim3((unsigned)min(num_sms() * per_sm, (warps + 7) / 8)), pf_smem, C4};
+    }
+    if (d->co <= 4 && d->ci <= 32) return {SimtRoute::tiny, dim3(ew_grid(M, 256)), (size_t)taps * d->ci * d->co * sizeof(float), 0};
+    if (d->co <= 4) return {SimtRoute::smallco, dim3(ew_grid(M * 32, 256)), 0, 0};
+    return {SimtRoute::igemm, dim3((unsigned)((M + BM - 1) / BM), (unsigned)((d->co + BN - 1) / BN)), 0, 0};
+}
+
+// conv_pf3_tile_kernel<C4> or conv_pf_thread_kernel<C4>, for C4 in 1..8
+template <int C = 1>
+static auto pf_thread_kernel(bool tile, int C4) -> decltype(&conv_pf_thread_kernel<1>) {
+    if constexpr (C < 8)
+        if (C4 > C) return pf_thread_kernel<C + 1>(tile, C4);
+    return tile ? conv_pf3_tile_kernel<C> : conv_pf_thread_kernel<C>;
 }
 
 static inline int floordiv(int a, int b) { return (a >= 0) ? a / b : -((-a + b - 1) / b); }
@@ -749,73 +718,27 @@ int fn2_conv_forward(const fn2_conv_desc* d, const fn2_tensor* bottom, const flo
         return conv_tc_forward(d, in, tcw, bias_dev, out, (float*)workspace, workspace_bytes / sizeof(float), st);
     }
     FN2_CHECK_ARG(d->engine != 2, "conv: tensor-core engine requested but the shape/layout is not eligible");
-    if (!d->deconv && d->ci <= 4 && d->co >= 32 && out.sc == 1 && d->kh * d->kw * d->ci <= 200) {
-        p.cis = d->ci;
-        const int xt = (p.Wo + FEW_PX - 1) / FEW_PX;
-        const size_t smem = (size_t)FEW_PX * d->kh * d->kw * d->ci * sizeof(float);
-        conv_fewci_kernel<<<(unsigned)(p.N * p.Ho * xt), 256, smem, st>>>(in, packed_weights_dev, bias_dev, out, p);
+    const SimtLaunch L = simt_route(d, in, out);
+    // Dynamic shared memory above the default 48 KB needs the kernel's limit raised (per device) to what the launch uses.
+    auto launch = [&](auto kernel, auto... c4) -> int {
+        if (L.smem > 48 * 1024) FN2_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.smem));
+        kernel<<<L.grid, 256, L.smem, st>>>(in, packed_weights_dev, bias_dev, out, p, c4...);
         FN2_LAUNCH_CHECK();
         return FN2_OK;
-    }
-    if (conv_nhwc_eligible(d, in, out))
+    };
+    switch (L.route) {
+    case SimtRoute::fewci: return launch(conv_fewci_kernel);
+    case SimtRoute::nhwc:
         return conv_nhwc_forward(d, in, packed_weights_dev, bias_dev, out, (float*)workspace, workspace_bytes / sizeof(float), st);
-    p.cis = d->ci;
-    p.K = d->kh * d->kw * p.cis;
-    const long long M = (long long)p.N * p.Ho * p.Wo;
-    const int C4 = (d->ci + 3) / 4;
-    const bool pf_ok = !d->deconv && d->co == 2 && in.sc == 1 && in.sw >= 4 * C4 && !((uintptr_t)in.p & 15) && !(in.sw & 3) &&
-                       !(in.sh & 3) && !(in.sn & 3) && (size_t)d->kh * d->kw * C4 * 4 * sizeof(float2) <= 200 * 1024;
-    if (pf_ok) {
-        const size_t smem = (size_t)d->kh * d->kw * C4 * 4 * sizeof(float2);
-        const bool k3 = d->kh == 3 && d->kw == 3 && d->stride_h == 1 && d->stride_w == 1;
-        if (C4 <= 8) {
-            const int grid = (int)min((long long)num_sms() * 8, (M + 255) / 256);
-#define FN2_PF_THREAD(C)                                                                                                   \
-            case C: if (k3 && d->pad_h == 1 && d->pad_w == 1) {                                                            \
-                        const size_t tsm = smem + (size_t)10 * 34 * (C + 1) * sizeof(float4);                               \
-                        const int tgrid = (int)min((long long)num_sms() * 4, (long long)p.N * ((p.Wo + 31) / 32) * ((p.Ho + 7) / 8)); \
-                        if (tsm > 48 * 1024) FN2_CUDA(cudaFuncSetAttribute(conv_pf3_tile_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tsm)); \
-                        conv_pf3_tile_kernel<C><<<tgrid, 256, tsm, st>>>(in, packed_weights_dev, bias_dev, out, p);            \
-                    } else if (k3) conv_pf3_thread_kernel<C><<<grid, 256, smem, st>>>(in, packed_weights_dev, bias_dev, out, p);  \
-                    else conv_pf_thread_kernel<C><<<grid, 256, smem, st>>>(in, packed_weights_dev, bias_dev, out, p);      \
-                    break;
-            switch (C4) { FN2_PF_THREAD(1) FN2_PF_THREAD(2) FN2_PF_THREAD(3) FN2_PF_THREAD(4) FN2_PF_THREAD(5) FN2_PF_THREAD(6)
-                          FN2_PF_THREAD(7) FN2_PF_THREAD(8) }
-#undef FN2_PF_THREAD
-        } else {
-            static size_t smem_set = 0;
-            if (smem > 48 * 1024 && smem > smem_set) {
-                FN2_CUDA(cudaFuncSetAttribute(conv_pf_warp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(200 * 1024)));
-                FN2_CUDA(cudaFuncSetAttribute(conv_pf3_warp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(200 * 1024)));
-                smem_set = 200 * 1024;
-            }
-            const int per_sm = (int)max((size_t)1, min((size_t)8, (size_t)(220 * 1024) / (smem + 1024)));
-            if (k3) {
-                const long long groups = (long long)p.N * p.Ho * ((p.Wo + 3) / 4);
-                const int grid = (int)min((long long)num_sms() * per_sm, (groups + 7) / 8);
-                conv_pf3_warp_kernel<<<grid, 256, smem, st>>>(in, packed_weights_dev, bias_dev, out, p, C4);
-            } else {
-                const int grid = (int)min((long long)num_sms() * per_sm, (M + 7) / 8);
-                conv_pf_warp_kernel<<<grid, 256, smem, st>>>(in, packed_weights_dev, bias_dev, out, p, C4);
-            }
-        }
-    } else if (d->co <= 4 && d->ci <= 32) {
-        const size_t smem = (size_t)p.K * p.Co * sizeof(float);
-        const int grid = ew_grid(M, 256);
-        if (d->deconv && d->stride_h == 2 && d->stride_w == 2) deconv_s2_tiny_kernel<<<grid, 256, smem, st>>>(in, packed_weights_dev, bias_dev, out, p);
-        else if (d->deconv) conv_tiny_kernel<true><<<grid, 256, smem, st>>>(in, packed_weights_dev, bias_dev, out, p);
-        else           conv_tiny_kernel<false><<<grid, 256, smem, st>>>(in, packed_weights_dev, bias_dev, out, p);
-    } else if (d->co <= 4) {
-        const int grid = ew_grid(M * 32, 256);
-        if (d->deconv) conv_smallco_kernel<true, 4><<<grid, 256, 0, st>>>(in, packed_weights_dev, bias_dev, out, p);
-        else           conv_smallco_kernel<false, 4><<<grid, 256, 0, st>>>(in, packed_weights_dev, bias_dev, out, p);
-    } else {
-        dim3 grid((unsigned)((M + BM - 1) / BM), (unsigned)((d->co + BN - 1) / BN));
-        if (d->deconv) conv_igemm_kernel<true><<<grid, 256, 0, st>>>(in, packed_weights_dev, bias_dev, out, p);
-        else           conv_igemm_kernel<false><<<grid, 256, 0, st>>>(in, packed_weights_dev, bias_dev, out, p);
+    case SimtRoute::pf3_tile: return launch(pf_thread_kernel(true, L.C4));
+    case SimtRoute::pf_thread: return launch(pf_thread_kernel(false, L.C4));
+    case SimtRoute::pf3_warp: return launch(conv_pf3_warp_kernel, L.C4);
+    case SimtRoute::pf_warp: return launch(conv_pf_warp_kernel, L.C4);
+    case SimtRoute::tiny: return launch(d->deconv ? conv_tiny_kernel<true> : conv_tiny_kernel<false>);
+    case SimtRoute::smallco: return launch(d->deconv ? conv_smallco_kernel<true, 4> : conv_smallco_kernel<false, 4>);
+    case SimtRoute::igemm: return launch(d->deconv ? conv_igemm_kernel<true> : conv_igemm_kernel<false>);
     }
-    FN2_LAUNCH_CHECK();
-    return FN2_OK;
+    return FN2_ERR_INVALID;                 // not reached: every route returns above
 }
 
 }  // extern "C"

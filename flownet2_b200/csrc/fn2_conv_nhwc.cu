@@ -289,8 +289,8 @@ int conv_nhwc_forward(const fn2_conv_desc* d, const T4& in, const float* wp, con
     p.in_sn = in.sn; p.in_sh = in.sh; p.in_sw = in.sw;
     p.out_sn = out.sn; p.out_sh = out.sh; p.out_sw = out.sw;
     p.relu = d->relu; p.has_bias = d->has_bias; p.slope = d->negative_slope;
-    p.vec_in = ((uintptr_t)in.p % 16 == 0) && in.sn % 4 == 0 && in.sh % 4 == 0 && in.sw % 4 == 0;
-    p.vec_out = ((uintptr_t)out.p % 16 == 0) && out.sn % 4 == 0 && out.sh % 4 == 0 && out.sw % 4 == 0;
+    p.vec_in = in.px_float4();          // both views are channel-fast (conv_nhwc_eligible)
+    p.vec_out = out.px_float4();
     const int bn = pick_bn(d->co);
     auto launch = [&](dim3 grid, float* partial) {
         if (bn == 128) conv_nhwc_kernel<128><<<grid, 256, 0, st>>>(in.p, wp, bias, out.p, partial, p);

@@ -571,7 +571,7 @@ __global__ void fill_kernel(T4 dst, float v) {
 struct PxView { T4 t; int vr; };
 static PxView px_view(const T4& t) {
     PxView v; v.t = t;
-    v.vr = t.sc == 1 && !((uintptr_t)t.p & 15) && !(t.sw & 3) && !(t.sh & 3) && !(t.sn & 3) && t.sw >= (t.c + 3) / 4 * 4;
+    v.vr = t.px_float4() && t.sw >= (t.c + 3) / 4 * 4;
     return v;
 }
 __device__ __forceinline__ float4 px_load(const PxView& v, long long o, int c0) {
@@ -838,7 +838,7 @@ int fn2_flow_warp_forward(const fn2_tensor* image, const fn2_tensor* flow, const
     float fill = 0.f;
     if (fill_nan) { unsigned u = 0xFFE00000u; memcpy(&fill, &u, 4); }
     const long long total = (long long)out.n * out.h * out.w;
-    const int vec4 = img.sc == 1 && img.c <= 4 && img.sw >= 4 && !((uintptr_t)img.p & 15) && !(img.sw & 3) && !(img.sh & 3) && !(img.sn & 3);
+    const int vec4 = img.px_float4() && img.c <= 4 && img.sw >= 4;
     flow_warp_fwd_kernel<<<ew_grid(total, 256), 256, 0, (cudaStream_t)stream>>>(img, fl, out, fill, vec4);
     FN2_LAUNCH_CHECK();
     return FN2_OK;
@@ -894,7 +894,7 @@ int fn2_warp_block_forward(const fn2_tensor* flow_in, const fn2_tensor* image0, 
     FN2_CHECK_ARG(fx <= 1.f && fy <= 1.f, "warp_block: the flow must be up-sampled (use the layer chain otherwise)");
     float fill = 0.f;
     if (fill_nan) { unsigned u = 0xFFE00000u; memcpy(&fill, &u, 4); }
-    const int vec4 = i1.sc == 1 && i1.c <= 4 && i1.sw >= 4 && !((uintptr_t)i1.p & 15) && !(i1.sw & 3) && !(i1.sh & 3) && !(i1.sn & 3);
+    const int vec4 = i1.px_float4() && i1.c <= 4 && i1.sw >= 4;
     const long long total = (long long)ff.n * ff.h * ff.w;
     warp_block_kernel<<<ew_grid(total, 256), 256, 0, (cudaStream_t)stream>>>(fin, i0, i1, ff, wp, er, en, fs, fx, fy, scale_coeff, fill, vec4);
     FN2_LAUNCH_CHECK();
@@ -1000,7 +1000,7 @@ int fn2_channel_norm_forward(const fn2_tensor* bottom, const fn2_tensor* top, vo
     FN2_CHECK_ARG(out.c == 1 && out.n == in.n && out.h == in.h && out.w == in.w,
                   "channel_norm: top must be (N,1,H,W) (channel_norm_layer.cpp:29)");
     const long long total = (long long)in.n * in.h * in.w;
-    const int vec4 = in.sc == 1 && in.c <= 4 && in.sw >= 4 && !((uintptr_t)in.p & 15) && !(in.sw & 3) && !(in.sh & 3) && !(in.sn & 3);
+    const int vec4 = in.px_float4() && in.c <= 4 && in.sw >= 4;
     channel_norm_kernel<<<ew_grid(total, 256), 256, 0, (cudaStream_t)stream>>>(in, out, vec4);
     FN2_LAUNCH_CHECK();
     return FN2_OK;
