@@ -91,6 +91,16 @@ struct ConvTaps {
 };
 void conv_taps(const fn2_conv_desc* d, int Ho, int Wo, ConvTaps* c);
 
+// Geometry of a Correlation (dims 2) or Correlation1D (dims 1) layer (fn2_corr.cu, corr_geometry): top pixel (x, y) compares
+// the k x k patch of bottom0 at (x*s1 + md - pad, y*s1 + y0) with the bottom1 patch displaced by
+// ((tc % Dx + xs) * s2, (tc / Dx + ys) * s2) for top channel tc; R = md / s2.
+struct CorrGeo {
+    int dims;
+    int topC, topH, topW;
+    int k, s1, md, pad, y0;
+    int Dx, xs, ys, s2, R;
+};
+
 inline int num_sms() {
     static int sms = 0;
     if (!sms) {

@@ -1118,22 +1118,14 @@ int conv_tc_wgrad(const fn2_conv_desc* d, const T4& bottom, const T4& top_diff, 
     return FN2_OK;
 }
 
-int corr_tc_eligible(const T4& b0, const T4& b1, const T4& top, int md, int s2) {
-    if (!tc_enabled() || getenv("FN2_CORR_NOTC")) return 0;
-    if (s2 < 1 || s2 > 2 || md % s2 || md / s2 != 10) return 0;            // halo blocks are laid out for R = 10
-    if (b0.c % 32 || b0.sc != 1 || b1.sc != 1 || top.sc != 1) return 0;
-    if (((uintptr_t)b0.p & 15) || (b0.sw & 3) || (b0.sh & 3) || (b0.sn & 3)) return 0;
-    if (((uintptr_t)b1.p & 15) || (b1.sw & 3) || (b1.sh & 3) || (b1.sn & 3)) return 0;
-    if (!tc_encode_fn()) return 0;
-    return 1;
-}
+// The correlation route itself is chosen in fn2_corr.cu (corr_fwd_route); this says whether the tensor cores may take it.
+bool corr_tc_available() { return tc_enabled() && tc_encode_fn(); }
 size_t corr_tc_workspace_floats(int N, int C, int H, int W) { return (size_t)2 * N * H * W * C; }
 
-int corr_tc_forward(const T4& b0, const T4& b1, const T4& top, int md, int s2, float* ws, size_t ws_floats, cudaStream_t st) {
+// R = 10, s2 <= 2, C % 32 == 0, channel-fast maps with 16-byte aligned pixels; ws holds corr_tc_workspace_floats
+int corr_tc_forward(const T4& b0, const T4& b1, const T4& top, int R, int s2, float* ws, cudaStream_t st) {
     EncodeTiledFn enc = tc_encode_fn();
-    if (!enc) { set_error("corr_tc: cuTensorMapEncodeTiled unavailable"); return FN2_ERR_CUDA; }
-    const int N = b0.n, C = b0.c, H = b0.h, W = b0.w, S = s2, R = md / s2;
-    if (!ws || ws_floats < corr_tc_workspace_floats(N, C, H, W)) { set_error("corr_tc: workspace too small"); return FN2_ERR_WORKSPACE; }
+    const int N = b0.n, C = b0.c, H = b0.h, W = b0.w, S = s2;
     float* hi = ws; float* lo = ws + (size_t)N * H * W * C;
     corr_split_kernel<<<ew_grid((long long)N * H * W * (C / 4), 256), 256, 0, st>>>(b1.p, b1.sn, b1.sh, b1.sw, N, H, W, C, hi, lo);
     FN2_LAUNCH_CHECK();
@@ -1178,11 +1170,7 @@ int corr_tc_forward(const T4& b0, const T4& b1, const T4& top, int md, int s2, f
     cfg.blockDim = dim3(TC_THREADS);
     cfg.stream = st;
     const int smem_bytes = TcGeo<NT>::SMEM;
-    static bool attr_set = false;
-    if (!attr_set) {
-        FN2_CUDA(cudaFuncSetAttribute(conv_tc_kernel<NT, TC_CORR>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
-        attr_set = true;
-    }
+    FN2_CUDA(cudaFuncSetAttribute(conv_tc_kernel<NT, TC_CORR>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
     cfg.dynamicSmemBytes = smem_bytes;
     FN2_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<NT, TC_CORR>, mapA, mapB, (const float*)nullptr, top.p, (float*)nullptr, p));
     FN2_LAUNCH_CHECK();

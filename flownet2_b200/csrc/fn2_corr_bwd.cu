@@ -1,4 +1,4 @@
-// Correlation backward (2-D and 1-D, MULTIPLY and SUBTRACT) and the Correlation1D forward.
+// Correlation backward (2-D and 1-D, MULTIPLY and SUBTRACT), on the geometry of fn2_corr.cu (CorrGeo).
 //
 // Reference: CorrelateDataBackward0/1 (correlation_layer.cu:118-249), ...Subtract (:298-427), correlation_layer1d.cu:48-420.
 // The reference launches one thread per bottom element that walks all displacements and, inside, the range of top positions
@@ -11,9 +11,14 @@
 //   SUBTRACT uses the reference's sign map in place of M / M': s(q) = (bottom0[q] >= bottom1[q]) ? +1 : -1 evaluated AT THE
 //   DISPLACED position for both gradients (:327-329, :397-399), +s for bottom0 and -s for bottom1, and +-1 (not 0) outside
 //   the image, because the reference compares its two zero-padded copies there.
-// For FlowNet2-C's layer (k = 1, stride_1 = 1, pad = md) G is topdiff itself.  The apply step is one shared-memory tiled kernel:
-// an 8 x 8 pixel tile keeps its G rows (64 x D floats) resident and streams the (8 + 2*reach)^2 halo of M in 8-channel chunks;
-// thread = (pixel, 2 channels), D fused multiply-adds per chunk and channel, fixed summation order (no atomics).
+// When k = 1, stride_1 = 1 and pad = md, G is topdiff itself (identity G); otherwise corr_patchsum_kernel forms it first.
+// Routes (corr_bwd_plan, corr_backward):
+//   * fast  -- FlowNet2-C's layer (MULTIPLY, identity G, 21 x 21 displacements, stride_2 <= 2, C % 32 == 0) on channel-fast
+//              maps with 16-byte aligned pixels: corr_bwd_fast_kernel on the stride_2 parity planes.  Workspace N*H*W*D.
+//   * tiled -- everything else: one shared-memory tiled apply kernel.  An 8 x 8 pixel tile keeps its G rows (64 x D floats)
+//              resident and streams the (8 + 2*reach)^2 halo of M in 8-channel chunks; thread = (pixel, 2 channels), D fused
+//              multiply-adds per chunk and channel, fixed summation order (no atomics).  Workspace: N*H*W*D for the patch sum
+//              unless G is the identity, plus N*H*W*C for the SUBTRACT sign map.
 #include "fn2_common.cuh"
 
 namespace fn2 {
@@ -134,42 +139,6 @@ __global__ void __launch_bounds__(256) corr_apply_kernel(const float* __restrict
                 if (c + 1 < p.C) out.p[out.off(n, c + 1, y, x)] = a1 * p.scale;
             }
         }
-    }
-}
-
-// Correlation1D forward (correlation_layer1d.cu:48-112): displacement in x only, rows are not padded; one warp per output
-// pixel and displacement group, lanes over channels, shuffle reduction (fixed order).
-__global__ void __launch_bounds__(128) corr1d_fwd_kernel(T4 b0, T4 b1, T4 top, int pad, int k, int md, int s1, int s2, int x_shift, int type) {
-    extern __shared__ float patch[];                  // [k*k][C]
-    const int x = blockIdx.x, y = blockIdx.y, n = blockIdx.z;
-    const int C = b0.c, H = b0.h, W = b0.w;
-    const int x1 = x * s1 + md - pad, y1 = y * s1;     // upper-left of the patch, unpadded coordinates (:56-57)
-    for (int idx = threadIdx.x; idx < k * k * C; idx += blockDim.x) {
-        const int ch = idx % C, ji = idx / C;
-        const int yy = y1 + ji / k, xx = x1 + ji % k;
-        patch[idx] = (yy >= 0 && yy < H && xx >= 0 && xx < W) ? b0.p[b0.off(n, ch, yy, xx)] : 0.f;
-    }
-    __syncthreads();
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int sumelems = k * k * C;
-    for (int tc = warp; tc < top.c; tc += 4) {
-        const int s2o = (tc + x_shift) * s2;             // :83
-        float acc = 0.f;
-        for (int j = 0; j < k; j++) {
-            const int yy = y1 + j;
-            for (int i = 0; i < k; i++) {
-                const int xx = x1 + s2o + i;
-                const bool inb = yy >= 0 && yy < H && xx >= 0 && xx < W;
-                const float* ap = patch + (j * k + i) * C;
-                for (int ch = lane; ch < C; ch += 32) {
-                    const float b = inb ? b1.p[b1.off(n, ch, yy, xx)] : 0.f;
-                    acc += type == 0 ? ap[ch] * b : fabsf(ap[ch] - b);
-                }
-            }
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-        if (lane == 0) top.p[top.off(n, tc, y, x)] = acc / (float)sumelems;
     }
 }
 
@@ -294,28 +263,37 @@ __global__ void corr_shift_kernel(T4 td, float* __restrict__ gx, int R, int S) {
     }
 }
 
-static bool corr_fast_ok(const T4& b0, const T4& b1, const T4& td, const T4& d0, const T4& d1, const CbP& p, int corr_type, int s2) {
-    if (getenv("FN2_CORR_BWD_SLOW")) return false;
-    if (corr_type != 0 || !p.identity_g || p.D != CF_DW * CF_DW || s2 < 1 || s2 > 2 || p.reach_x != CF_R * s2 || p.C % 32) return false;
-    const T4* ts[4] = {&b0, &b1, &d0, &d1};
-    for (const T4* t : ts)
-        if (t->sc != 1 || ((uintptr_t)t->p & 15) || (t->sw & 3) || (t->sh & 3) || (t->sn & 3)) return false;
-    return true;
+
+// Backward route of a layer, from its shape.  G is the top diff itself when the patch walk is the identity (k 1, stride_1 1,
+// pad = md); otherwise the tiled route first forms the patch sum.  FlowNet2-C's class -- MULTIPLY, G = top diff, the 21 x 21
+// displacement grid, stride_2 <= 2, C % 32 == 0 -- takes the fast kernel when the four bottom maps are channel-fast with
+// 16-byte aligned pixels too (corr_backward); it stages the shifted top diff in the workspace.
+struct CorrBwdPlan {
+    bool fast;              // shape of the fast route
+    bool patch_sum;         // the tiled route needs the patch sum
+    size_t g_floats;        // N*H*W*D: the fast route's shifted top diff, or the patch sum
+    size_t s_floats;        // SUBTRACT: the sign map, N*H*W*C
+    size_t tiled_floats() const { return (patch_sum ? g_floats : 0) + s_floats; }
+};
+
+CorrBwdPlan corr_bwd_plan(const CorrGeo& g, int N, int C, int H, int W, int corr_type) {
+    CorrBwdPlan pl;
+    pl.patch_sum = !(g.k == 1 && g.s1 == 1 && g.pad == g.md && g.topH == H && g.topW == W);
+    pl.fast = corr_type == 0 && !pl.patch_sum && g.topC == CF_DW * CF_DW && g.Dx == CF_DW && g.xs == -CF_R && g.ys == -CF_R &&
+              g.s2 <= 2 && C % 32 == 0;
+    pl.g_floats = (size_t)N * H * W * g.topC;
+    pl.s_floats = corr_type == 1 ? (size_t)N * H * W * C : 0;
+    return pl;
 }
 
-static int corr_fast_run(const T4& b0, const T4& b1, const T4& td, const T4& d0, const T4& d1, const CbP& p, int s2, float* ws, cudaStream_t st) {
+int corr_fast_run(const T4& b0, const T4& b1, const T4& td, const T4& d0, const T4& d1, const CbP& p, int s2, float* ws, cudaStream_t st) {
     CfP f;
     f.N = p.N; f.C = p.C; f.H = p.H; f.W = p.W; f.S = s2; f.scale = p.scale; f.cchunks = p.C / 32;
     const int Hp = (p.H + s2 - 1) / s2, Wp = (p.W + s2 - 1) / s2;
     f.tiles_y = (Hp + CF_TH - 1) / CF_TH; f.tiles_x = (Wp + CF_TW - 1) / CF_TW;
     const int units = f.N * s2 * s2 * f.tiles_y * f.tiles_x * f.cchunks;
-    static bool attr = false;
-    if (!attr) {
-        FN2_CUDA(cudaFuncSetAttribute(corr_bwd_fast_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, CF_SMEM));
-        FN2_CUDA(cudaFuncSetAttribute(corr_bwd_fast_kernel<-1>, cudaFuncAttributeMaxDynamicSharedMemorySize, CF_SMEM));
-        attr = true;
-    }
     const int grid = min(units, num_sms());
+    FN2_CUDA(cudaFuncSetAttribute(corr_bwd_fast_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, CF_SMEM));
     corr_bwd_fast_kernel<1><<<grid, 256, CF_SMEM, st>>>(td, b1, d0, f);
     FN2_LAUNCH_CHECK();
     corr_shift_kernel<<<ew_grid((long long)p.N * p.H * p.W * p.D, 256), 256, 0, st>>>(td, ws, CF_R, s2);
@@ -323,24 +301,16 @@ static int corr_fast_run(const T4& b0, const T4& b1, const T4& td, const T4& d0,
     T4 gx;
     gx.p = ws; gx.n = p.N; gx.c = p.D; gx.h = p.H; gx.w = p.W;
     gx.sc = 1; gx.sw = p.D; gx.sh = (long long)p.W * p.D; gx.sn = (long long)p.H * p.W * p.D;
+    FN2_CUDA(cudaFuncSetAttribute(corr_bwd_fast_kernel<-1>, cudaFuncAttributeMaxDynamicSharedMemorySize, CF_SMEM));
     corr_bwd_fast_kernel<-1><<<grid, 256, CF_SMEM, st>>>(gx, b0, d1, f);
     FN2_LAUNCH_CHECK();
     return FN2_OK;
 }
 
-int corr_bwd_run(const T4& b0, const T4& b1, const T4& td, const T4& d0, const T4& d1, CbP& p, int corr_type, float* ws, size_t ws_floats,
-                 cudaStream_t st, int s2_2d = 0) {
-    if (s2_2d > 0 && corr_fast_ok(b0, b1, td, d0, d1, p, corr_type, s2_2d)) {
-        if (!ws || ws_floats < (size_t)p.N * p.H * p.W * p.D) { set_error("correlation_backward: workspace too small"); return FN2_ERR_WORKSPACE; }
-        return corr_fast_run(b0, b1, td, d0, d1, p, s2_2d, ws, st);
-    }
-    const size_t gfloats = p.identity_g ? 0 : (size_t)p.N * p.H * p.W * p.D;
-    const size_t sfloats = corr_type == 1 ? (size_t)p.N * p.H * p.W * p.C : 0;
-    if (gfloats + sfloats > ws_floats || (!ws && gfloats + sfloats)) { set_error("correlation_backward: workspace too small (%zu floats needed)", gfloats + sfloats); return FN2_ERR_WORKSPACE; }
-    float* g = ws;
-    float* sgn = ws + gfloats;
+int corr_tiled_run(const T4& b0, const T4& b1, const T4& td, const T4& d0, const T4& d1, CbP& p, int corr_type, float* g,
+                   float* sgn, cudaStream_t st) {
     if (!p.identity_g) {
-        corr_patchsum_kernel<<<ew_grid((long long)gfloats, 256), 256, 0, st>>>(td, g, p);
+        corr_patchsum_kernel<<<ew_grid((long long)p.N * p.H * p.W * p.D, 256), 256, 0, st>>>(td, g, p);
         FN2_LAUNCH_CHECK();
     }
     T4 m0 = b1, m1 = b0;
@@ -356,13 +326,12 @@ int corr_bwd_run(const T4& b0, const T4& b1, const T4& td, const T4& d0, const T
     const int hw = CB_TILE + 2 * p.reach_x, hh = CB_TILE + 2 * p.reach_y;
     const size_t smem = ((size_t)64 * p.D + (size_t)hh * hw * CB_CH) * sizeof(float);
     if (smem > 220 * 1024) { set_error("correlation_backward: displacement window too large for the tiled kernel (%zu B)", smem); return FN2_ERR_INVALID; }
-    static size_t set0 = 0, set1 = 0;
-    if (smem > set0) { FN2_CUDA(cudaFuncSetAttribute(corr_apply_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); set0 = smem; }
-    if (smem > set1) { FN2_CUDA(cudaFuncSetAttribute(corr_apply_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); set1 = smem; }
     const int tiles = p.N * ((p.H + CB_TILE - 1) / CB_TILE) * ((p.W + CB_TILE - 1) / CB_TILE);
     const int grid = min(tiles, num_sms());
+    if (smem > 48 * 1024) FN2_CUDA(cudaFuncSetAttribute(corr_apply_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     corr_apply_kernel<0><<<grid, 256, smem, st>>>(g, td, m0, d0, p, s0);
     FN2_LAUNCH_CHECK();
+    if (smem > 48 * 1024) FN2_CUDA(cudaFuncSetAttribute(corr_apply_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     corr_apply_kernel<1><<<grid, 256, smem, st>>>(g, td, m1, d1, p, s1);
     FN2_LAUNCH_CHECK();
     return FN2_OK;
@@ -370,78 +339,35 @@ int corr_bwd_run(const T4& b0, const T4& b1, const T4& td, const T4& d0, const T
 
 }  // namespace
 
-size_t corr_bwd_workspace_floats(int N, int C, int H, int W, int D, int k, int s1, int pad, int md, int topH, int topW, int corr_type, int one_d) {
-    const bool ident = k == 1 && s1 == 1 && pad == md && topH == H && topW == W;
-    // (the identity case of the 2-D MULTIPLY layer may take the fast path, which stages the shifted top diff there)
-    return ((ident && (one_d || corr_type == 1)) ? 0 : (size_t)N * H * W * D) + (corr_type == 1 ? (size_t)N * H * W * C : 0);
+size_t corr_bwd_workspace_floats(const CorrGeo& g, int N, int C, int H, int W, int corr_type) {
+    const CorrBwdPlan pl = corr_bwd_plan(g, N, C, H, W, corr_type);
+    return pl.fast ? pl.g_floats : pl.tiled_floats();
 }
 
-// 2-D layer: top channel tc <-> displacement ((tc / Dw - R) * s2, (tc % Dw - R) * s2)   (correlation_layer.cu:81-82)
-int corr_bwd_2d(const T4& b0, const T4& b1, const T4& td, const T4& d0, const T4& d1, int pad, int k, int md, int s1, int s2, int corr_type,
-                float* ws, size_t ws_floats, cudaStream_t st) {
+int corr_backward(const CorrGeo& g, const T4& b0, const T4& b1, const T4& td, const T4& d0, const T4& d1, int corr_type,
+                  float* ws, size_t ws_floats, cudaStream_t st) {
+    const CorrBwdPlan pl = corr_bwd_plan(g, b0.n, b0.c, b0.h, b0.w, corr_type);
+    if (g.topC > 441) { set_error("correlation_backward: more than 441 displacements"); return FN2_ERR_INVALID; }
     CbP p;
     memset(&p, 0, sizeof(p));
     p.N = b0.n; p.C = b0.c; p.H = b0.h; p.W = b0.w;
-    const int R = md / s2, Dw = 2 * R + 1;
-    p.D = Dw * Dw;
-    if (p.D > 441) { set_error("correlation_backward: more than 441 displacements"); return FN2_ERR_INVALID; }
-    p.topH = td.h; p.topW = td.w; p.k = k; p.s1 = s1; p.md = md; p.pad = pad; p.ypatch_off = md - pad;
-    for (int tc = 0; tc < p.D; tc++) { p.dy[tc] = (short)((tc / Dw - R) * s2); p.dx[tc] = (short)((tc % Dw - R) * s2); }
-    p.reach_y = p.reach_x = R * s2;
-    p.identity_g = (k == 1 && s1 == 1 && pad == md && td.h == b0.h && td.w == b0.w) ? 1 : 0;
-    p.scale = 1.f / (float)(k * k * p.C);
-    return corr_bwd_run(b0, b1, td, d0, d1, p, corr_type, ws, ws_floats, st, s2);
-}
-
-// 1-D layer: tc <-> (0, (tc + x_shift) * s2), x_shift = -R (both directions or left only) or 0 (right only)
-static int corr1d_geometry(int md, int s2, int single_direction, int* D, int* x_shift) {
-    const int R = md / s2;
-    *D = single_direction != 0 ? R + 1 : 2 * R + 1;          // correlation_layer1d.cpp:64-68
-    // correlation_layer1d.cu Forward_gpu: -R, "to the left" -grid_width (sic: one stride_2 step beyond -max_displacement), "to the right" 0
-    *x_shift = single_direction == 1 ? 0 : (single_direction == -1 ? -(R + 1) : -R);
-    return R;
-}
-
-int corr1d_shape(int H, int W, int pad, int k, int md, int s1, int s2, int single_direction, int* tc, int* th, int* tw) {
-    if (k < 1 || k % 2 == 0) { set_error("Odd kernel size required (correlation_layer1d.cpp:22)"); return FN2_ERR_INVALID; }
-    if (s1 < 1 || s2 < 1 || md < 0 || pad < 0) { set_error("correlation1d: bad stride/displacement/pad"); return FN2_ERR_INVALID; }
-    if (single_direction < -1 || single_direction > 1) { set_error("single_direction must be -1 (left), 0 (off), or 1 (right)"); return FN2_ERR_INVALID; }
-    const int kr = (k - 1) / 2, border = md + kr;
-    const int w = (int)ceilf((float)(W + 2 * pad - border * 2) / (float)s1);     // :55
-    const int h = (int)ceilf((float)(H - kr * 2) / (float)s1);                   // :56 (rows are not padded)
-    if (w < 1 || h < 1) { set_error("Correlation cannot be done with current settings. Neighborhood and kernel don't fit in blob"); return FN2_ERR_INVALID; }
-    int D, xs;
-    corr1d_geometry(md, s2, single_direction, &D, &xs);
-    *tc = D; *th = h; *tw = w;
-    return FN2_OK;
-}
-
-int corr1d_forward(const T4& b0, const T4& b1, const T4& top, int pad, int k, int md, int s1, int s2, int single_direction, int corr_type,
-                   cudaStream_t st) {
-    int D, xs;
-    corr1d_geometry(md, s2, single_direction, &D, &xs);
-    const size_t smem = (size_t)k * k * b0.c * sizeof(float);
-    if (smem > 200 * 1024) { set_error("correlation1d: k*k*C patch does not fit in shared memory"); return FN2_ERR_INVALID; }
-    if (smem > 48 * 1024) FN2_CUDA(cudaFuncSetAttribute(corr1d_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    dim3 grid(top.w, top.h, b0.n);
-    corr1d_fwd_kernel<<<grid, 128, smem, st>>>(b0, b1, top, pad, k, md, s1, s2, xs, corr_type);
-    FN2_LAUNCH_CHECK();
-    return FN2_OK;
-}
-
-int corr_bwd_1d(const T4& b0, const T4& b1, const T4& td, const T4& d0, const T4& d1, int pad, int k, int md, int s1, int s2,
-                int single_direction, int corr_type, float* ws, size_t ws_floats, cudaStream_t st) {
-    CbP p;
-    memset(&p, 0, sizeof(p));
-    p.N = b0.n; p.C = b0.c; p.H = b0.h; p.W = b0.w;
-    int xs;
-    const int R = corr1d_geometry(md, s2, single_direction, &p.D, &xs);
-    p.topH = td.h; p.topW = td.w; p.k = k; p.s1 = s1; p.md = md; p.pad = pad; p.ypatch_off = 0;
-    for (int tc = 0; tc < p.D; tc++) { p.dy[tc] = 0; p.dx[tc] = (short)((tc + xs) * s2); }
-    p.reach_y = 0; p.reach_x = (single_direction == -1 ? R + 1 : R) * s2;
-    p.identity_g = (k == 1 && s1 == 1 && pad == md && td.h == b0.h && td.w == b0.w) ? 1 : 0;
-    p.scale = 1.f / (float)(k * k * p.C);
-    return corr_bwd_run(b0, b1, td, d0, d1, p, corr_type, ws, ws_floats, st);
+    p.D = g.topC;
+    p.topH = g.topH; p.topW = g.topW; p.k = g.k; p.s1 = g.s1; p.md = g.md; p.pad = g.pad; p.ypatch_off = g.y0;
+    for (int tc = 0; tc < p.D; tc++) {
+        p.dy[tc] = (short)((tc / g.Dx + g.ys) * g.s2);
+        p.dx[tc] = (short)((tc % g.Dx + g.xs) * g.s2);
+    }
+    p.reach_x = max(-g.xs, g.Dx - 1 + g.xs) * g.s2;
+    p.reach_y = max(-g.ys, g.topC / g.Dx - 1 + g.ys) * g.s2;
+    p.identity_g = pl.patch_sum ? 0 : 1;
+    p.scale = 1.f / (float)(g.k * g.k * p.C);
+    if (pl.fast && b0.px_float4() && b1.px_float4() && d0.px_float4() && d1.px_float4()) {
+        if (!ws || ws_floats < pl.g_floats) { set_error("correlation_backward: workspace too small"); return FN2_ERR_WORKSPACE; }
+        return corr_fast_run(b0, b1, td, d0, d1, p, g.s2, ws, st);
+    }
+    const size_t need = pl.tiled_floats();
+    if (need > ws_floats || (!ws && need)) { set_error("correlation_backward: workspace too small (%zu floats needed)", need); return FN2_ERR_WORKSPACE; }
+    return corr_tiled_run(b0, b1, td, d0, d1, p, corr_type, ws, ws + (pl.patch_sum ? pl.g_floats : 0), st);
 }
 
 }  // namespace fn2

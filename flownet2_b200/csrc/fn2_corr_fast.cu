@@ -1,6 +1,7 @@
-// Fast Correlation path for the FlowNet2 parameter class: MULTIPLY, kernel_size 1, stride_1 1,
-// pad == max_displacement, stride_2 | max_displacement  (FlowNet2-C: pad 20, md 20, s2 2 -> 21x21 = 441
-// displacements).  Reference: CorrelateData, correlation_layer.cu:46-114 (+ rearrange :24-42).
+// FP32 fast Correlation route for the FlowNet2 parameter class: MULTIPLY, kernel_size 1, stride_1 1,
+// pad == max_displacement, stride_2 | max_displacement, radius R = md / stride_2 of 10 or 4 (the instantiated ones), C % 8 == 0
+// (FlowNet2-C: pad 20, md 20, s2 2 -> 21x21 = 441 displacements).  fn2_corr.cu chooses the route (corr_fwd_plan,
+// corr_fwd_route).  Reference: CorrelateData, correlation_layer.cu:46-114 (+ rearrange :24-42).
 //
 // Design (FP32 SIMT -- the north_star forbids tensor cores for this gather-reduce):
 //   * stride_2 = S samples only displacements that are multiples of S, so an output pixel only ever
@@ -18,11 +19,7 @@
 //     needed at all: every (pixel, displacement) sum lives in exactly one thread.
 //   * epilogue: divide by C (sumelems, :106-108) and store straight into the strided top view (NCHW for
 //     drop-in use, NHWC/concat view inside the engine).
-#include <cuda.h>
-#include <mutex>
-#include <unordered_map>
-
-#include "fn2_common.cuh"
+#include "fn2_tc_ptx.cuh"
 
 namespace fn2 {
 
@@ -46,31 +43,6 @@ template <int R> struct Geo {
     static constexpr int STAGE_BYTES = (A_STAGE + B_STAGE) * 4;
     static constexpr int SMEM = NST * STAGE_BYTES + 1024;
 };
-
-// ---- PTX helpers (mbarrier + TMA), see blackwell_cuda_programming.md Guideline 15 ----------------------
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    uint32_t done = 0, spins = 0;
-    while (true) {
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.b32 %0, 1, 0, p;\n\t}"
-                     : "=r"(done) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-        if (done) break;
-        if (++spins > (1u << 24)) __trap();       // never hang the GPU: a lost arrival becomes a launch error
-    }
-}
-__device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3) {
-    asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-                 ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
 
 struct FastP {
     int N, C, H, W;          // bottoms
@@ -249,25 +221,8 @@ __global__ void corr_rearrange_generic_kernel(T4 in, float* __restrict__ ws, int
     }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn encode_fn() {
-    static EncodeTiledFn fn = nullptr;
-    static std::once_flag once;
-    std::call_once(once, [] {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-            q == cudaDriverEntryPointSuccess)
-            fn = (EncodeTiledFn)p;
-    });
-    return fn;
-}
-
 int make_map(CUtensorMap* m, float* base, int Ws, int Hs, int C, int NP, int bw, int bh) {
-    EncodeTiledFn fn = encode_fn();
+    EncodeTiledFn fn = tc_encode_fn();
     if (!fn) { set_error("cuTensorMapEncodeTiled is not available from the driver"); return FN2_ERR_CUDA; }
     cuuint64_t dims[4] = {(cuuint64_t)Ws, (cuuint64_t)Hs, (cuuint64_t)C, (cuuint64_t)NP};
     cuuint64_t strides[3] = {(cuuint64_t)Ws * 4, (cuuint64_t)Ws * Hs * 4, (cuuint64_t)Ws * Hs * C * 4};
@@ -317,11 +272,7 @@ int launch(const T4& b0, const T4& b1, const T4& top, int S, float* ws, cudaStre
     if (rc) return rc;
     rc = make_map(&mapB, dst[1], pitch[1], p.Hs, p.C, p.N * S * S, G::BW, G::BH);
     if (rc) return rc;
-    static bool attr_set = false;
-    if (!attr_set) {
-        FN2_CUDA(cudaFuncSetAttribute(corr_fast_kernel<R>, cudaFuncAttributeMaxDynamicSharedMemorySize, G::SMEM));
-        attr_set = true;
-    }
+    FN2_CUDA(cudaFuncSetAttribute(corr_fast_kernel<R>, cudaFuncAttributeMaxDynamicSharedMemorySize, G::SMEM));
     const int grid = p.N * S * S * p.tiles_x * p.tiles_y;
     corr_fast_kernel<R><<<grid, G::THREADS, G::SMEM, st>>>(mapA, mapB, top, p);
     FN2_LAUNCH_CHECK();
@@ -330,32 +281,14 @@ int launch(const T4& b0, const T4& b1, const T4& top, int S, float* ws, cudaStre
 
 }  // namespace
 
-int corr_fast_eligible(const T4& b0, const T4& b1, const T4& top, int pad, int k, int md, int s1, int s2, int type) {
-    if (type != 0 || k != 1 || s1 != 1 || pad != md || s2 < 1 || md % s2) return 0;
-    const int R = md / s2;
-    if (R != 10 && R != 4) return 0;                   // instantiated radii
-    if (b0.c % CC) return 0;
-    if ((long long)b0.n * s2 * s2 > 65535LL * 1024) return 0;
-    (void)b1; (void)top;
-    return 1;
+size_t corr_fast_workspace_bytes(int N, int C, int H, int W, int R, int s2) {
+    return (size_t)N * s2 * s2 * C * sub_extent(H, s2) * (ws_width(W, s2, 0) + ws_width(W, s2, R % 4)) * sizeof(float);
 }
 
-int corr_fast_workspace(int N, int C, int H, int W, int md, int s2, size_t* bytes) {
-    const int R = md / s2;
-    *bytes = (size_t)N * s2 * s2 * C * sub_extent(H, s2) * (ws_width(W, s2, 0) + ws_width(W, s2, R % 4)) * sizeof(float);
-    return FN2_OK;
-}
-
-int corr_fast_forward(const T4& b0, const T4& b1, const T4& top, int md, int s2, void* ws, size_t ws_bytes, cudaStream_t st) {
-    size_t need = 0;
-    corr_fast_workspace(b0.n, b0.c, b0.h, b0.w, md, s2, &need);
-    if (ws_bytes < need) { set_error("correlation: workspace too small"); return FN2_ERR_WORKSPACE; }
+// R = 10 or 4; ws holds corr_fast_workspace_bytes
+int corr_fast_forward(const T4& b0, const T4& b1, const T4& top, int R, int s2, void* ws, cudaStream_t st) {
     if (((uintptr_t)ws & 127) != 0) { set_error("correlation: workspace must be 128-byte aligned"); return FN2_ERR_INVALID; }
-    const int R = md / s2;
-    if (R == 10) return launch<10>(b0, b1, top, s2, (float*)ws, st);
-    if (R == 4) return launch<4>(b0, b1, top, s2, (float*)ws, st);
-    set_error("corr_fast: radius %d not instantiated", R);
-    return FN2_ERR_INVALID;
+    return R == 10 ? launch<10>(b0, b1, top, s2, (float*)ws, st) : launch<4>(b0, b1, top, s2, (float*)ws, st);
 }
 
 }  // namespace fn2

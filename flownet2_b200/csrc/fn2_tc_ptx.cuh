@@ -1,4 +1,5 @@
-// wgmma / TMA / mbarrier PTX wrappers and constants shared by the tensor-core engines (fn2_conv_tc.cu, fn2_conv_tn.cu); sm_90a.
+// wgmma / TMA / mbarrier PTX wrappers and constants shared by the tensor-core engines (fn2_conv_tc.cu, fn2_conv_tn.cu) and the
+// FP32 fast correlation (fn2_corr_fast.cu: mbarrier, TMA and the tensor-map encoder); sm_90a.
 #pragma once
 #include <cuda.h>
 #include "fn2_common.cuh"

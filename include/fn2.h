@@ -68,7 +68,9 @@ FN2_API int fn2_correlation_forward(const fn2_tensor* bottom0, const fn2_tensor*
                                     void* workspace, size_t workspace_bytes, void* stream);
 /* Gradients w.r.t. both bottoms: CorrelateDataBackward0/1 (:118-249), ...Subtract (:298-427), driver :508-600.  Computed through
  * the factorisation described in flownet2_b200/csrc/fn2_corr_bwd.cu (channel-free patch sum of top_diff, then a tiled
- * displacement-sum against the other map); needs workspace unless kernel_size 1, stride_1 1, pad == max_displacement, MULTIPLY. */
+ * displacement-sum against the other map).  Workspace: N*H*W*D floats for the patch sum unless kernel_size 1, stride_1 1,
+ * pad == max_displacement, and for FlowNet2-C's fast route (MULTIPLY, that identity patch walk, 21 x 21 displacements,
+ * stride_2 <= 2, C % 32 == 0); plus N*H*W*C floats for the SUBTRACT sign map. */
 FN2_API int fn2_correlation_backward_workspace_bytes(int N, int C, int H, int W, int pad, int kernel_size, int max_displacement,
                                                      int stride1, int stride2, int corr_type, size_t* bytes);
 FN2_API int fn2_correlation_backward(const fn2_tensor* bottom0, const fn2_tensor* bottom1,

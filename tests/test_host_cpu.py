@@ -254,6 +254,40 @@ def test_tensor_core_engine_plan_golden(fn2):
     assert not bad, (len(bad), bad[:5])
 
 
+def test_correlation_workspace_golden(fn2):
+    """Workspace queries of Correlation and Correlation1D over a sweep of layer shapes (tests/golden/make_corr_ws_golden.py).
+    Where a route uses workspace the size is the recorded one: the FP32 fast forward (MULTIPLY, k 1, stride_1 1, pad = md,
+    md % stride_2 == 0, R = 4 or 10, C % 8 == 0), the fast backward (the same with R = 10, stride_2 <= 2, C % 32 == 0), the
+    backward's patch sum (unless k 1, stride_1 1, pad = md) and its SUBTRACT sign map.  Every other shape needs none."""
+    lib = fn2.lib()
+    g = np.load(os.path.join(GOLD, "corr_ws_golden.npz"))
+    assert len(g["params"]) > 6000
+    bad, dropped = [], 0
+    for p, fwd_want, bwd_want in zip(g["params"], g["fwd"], g["bwd"]):
+        dims, N, Cc, H, W, pad, k, md, s1, s2, sd, typ = (int(v) for v in p)
+        R = md // s2
+        ident = k == 1 and s1 == 1 and pad == md
+        b = C.c_size_t()
+        if dims == 2:
+            assert lib.fn2_correlation_workspace_bytes(N, Cc, H, W, pad, k, md, s1, s2, typ, C.byref(b)) == 0
+            fast = typ == 0 and ident and md % s2 == 0 and R in (4, 10) and Cc % 8 == 0
+            want = int(fwd_want) if fast else 0
+            dropped += want != fwd_want
+            if b.value != want:
+                bad.append(("fwd", p.tolist(), int(fwd_want), b.value))
+            assert lib.fn2_correlation_backward_workspace_bytes(N, Cc, H, W, pad, k, md, s1, s2, typ, C.byref(b)) == 0
+            uses = not ident or typ == 1 or (R == 10 and s2 <= 2 and Cc % 32 == 0)
+        else:
+            assert lib.fn2_correlation1d_backward_workspace_bytes(N, Cc, H, W, pad, k, md, s1, s2, sd, typ, C.byref(b)) == 0
+            uses = not ident or typ == 1
+        want = int(bwd_want) if uses else 0
+        dropped += want != bwd_want
+        if b.value != want:
+            bad.append(("bwd", p.tolist(), int(bwd_want), b.value))
+    assert not bad, (len(bad), bad[:5])
+    assert dropped > 0 and (g["fwd"] > 0).sum() > 50
+
+
 AUG_LAYER = """
 layer {
   name: "aug" type: "DataAugmentation" bottom: "img" top: "aug"

@@ -255,7 +255,8 @@ def test_full_size_properties(fn2, monkeypatch):
     size-independent properties instead: (1) replay determinism (eager pass == CUDA-graph replays, bit for bit),
     (2) batch independence: sample k of a batch-4 forward equals a batch-1 forward of that pair (different tile schedules and
     K splits, so within the flow tolerance, not bitwise), (3) the two convolution engines agree: wgmma 3xTF32 vs exact-FP32
-    SIMT within 1e-4 of the flow scale, (4) correlation layer: tensor-core path vs FP32 path on the real conv3 features."""
+    SIMT within 1e-4 of the flow scale, (4) correlation layer: tensor-core route vs the FP32 fast route on the net's own conv3
+    features (NCHW copies, which the tensor-core route does not take)."""
     W, H, B = 1024, 436, 4
     proto = fn2.fill_template(fn2.model_template("FlowNet2"), W, H)
     img0, img1 = smooth_images(rng(99), B, H, W)
@@ -268,20 +269,22 @@ def test_full_size_properties(fn2, monkeypatch):
     assert np.isfinite(f1).all() and f1.shape == (B, 2, H, W)
     assert maxabs(f1, f2) == 0.0 and maxabs(f1, f3) == 0.0
     scale = max(1.0, float(np.abs(f1).max()))
-    corr_tc = net.blobs["net1_corr"].data.copy() if "net1_corr" in net.blobs else None
+    if "net1_corr" in net.blobs:
+        from flownet2_b200 import ops
+        corr_tc = net.blobs["net1_corr"].data
+        a, b = (torch.from_numpy(net.blobs[n].data).cuda() for n in ("net1_conv3a", "net1_conv3b"))
+        corr_fp32 = ops.correlation(a, b, 20, 1, 20, 1, 2).cpu().numpy()
+        corr_fp32 = np.where(corr_fp32 > 0, corr_fp32, corr_fp32 * np.float32(0.1))     # net1_ReLU_corr runs in place
+        assert maxabs(corr_fp32, corr_tc) <= 1e-5 * max(1.0, float(np.abs(corr_fp32).max()))
     del net
     one = fn2.Net(proto, weights, fn2.TEST, batch=1)
     g = one.forward(img0=img0[2:3], img1=img1[2:3])["predict_flow_final"]
     assert maxabs(g, f1[2:3]) <= 1e-4 * scale, (maxabs(g, f1[2:3]), scale)
     del one
     monkeypatch.setenv("FN2_CONV_ENGINE", "simt")
-    monkeypatch.setenv("FN2_CORR_NOTC", "1")
     simt = fn2.Net(proto, weights, fn2.TEST, batch=B)
     h = simt.forward(img0=img0, img1=img1)["predict_flow_final"]
     assert maxabs(h, f1) <= 1e-4 * scale, (maxabs(h, f1), scale)
-    if corr_tc is not None:
-        corr_fp32 = simt.blobs["net1_corr"].data
-        assert maxabs(corr_fp32, corr_tc) <= 1e-5 * max(1.0, float(np.abs(corr_fp32).max()))
 
 
 def test_fused_warp_block_is_bit_identical_to_the_layer_chain(fn2, monkeypatch):
