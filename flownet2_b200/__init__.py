@@ -66,12 +66,14 @@ def lib():
                      "fn2_net_graph_active", "fn2_net_backward", "fn2_net_clear_param_diffs", "fn2_net_launches_per_backward"):
             getattr(l, name).argtypes = [C.c_void_p]
         l.fn2_net_param_diff_arena.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t)]
+        l.fn2_net_trainable_diff_span.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t)]
         l.fn2_net_set_diff.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p]
         l.fn2_net_get_diff.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p]
         l.fn2_net_param_shape.argtypes = [C.c_void_p, C.c_char_p, C.c_int, C.POINTER(C.c_int)]
         l.fn2_net_get_param.argtypes = [C.c_void_p, C.c_char_p, C.c_int, C.c_int, C.c_void_p]
         l.fn2_net_layer_need_backward.argtypes = [C.c_void_p, C.c_int]
         l.fn2_net_copy_trained_layers.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
+        l.fn2_net_copy_trained_layers_prefixed.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_char_p]
         l.fn2_net_to_caffemodel.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_size_t)]
         l.fn2_net_to_hdf5.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_size_t)]
         l.fn2_caffemodel_to_hdf5.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_size_t)]
@@ -147,7 +149,8 @@ def fill_template(text, width, height):
 
 
 def train_template(name="FlowNet2-C"):
-    """Text of models/<name>_train.prototxt.template (the authored FlowNet2-C training graph of BASELINE config 5)."""
+    """Text of models/<name>_train.prototxt.template: the authored training graphs of the FlowNet2 schedule, FlowNet2-C
+    (BASELINE config 5), FlowNet2-CS, FlowNet2-CSS, FlowNet2-SD and FlowNet2 (the fusion stage)."""
     p = os.path.join(os.path.dirname(_HERE), "models", "%s_train.prototxt.template" % name)
     with open(p) as f:
         return f.read()
@@ -237,12 +240,14 @@ class Net(object):
         except Exception:
             pass
 
-    def copy_from(self, weights):
+    def copy_from(self, weights, prefix=""):
+        """Load a .caffemodel (path or bytes).  Source layer X fills layer prefix + X; source layers with no target are ignored
+        (the FlowNet2 stage hand-over: FlowNet2-C_train into FlowNet2-CS_train with prefix="net1_")."""
         if isinstance(weights, str):
             with open(weights, "rb") as f:
                 weights = f.read()
         buf = (C.c_char * len(weights)).from_buffer_copy(weights)
-        check(lib().fn2_net_copy_trained_layers(self._h, buf, len(weights)))
+        check(lib().fn2_net_copy_trained_layers_prefixed(self._h, buf, len(weights), prefix.encode()))
 
     def fill_params(self, seed=1701):
         check(lib().fn2_net_fill_params(self._h, int(seed)))
@@ -331,6 +336,12 @@ class Net(object):
     def param_diff_arena(self):
         p, n = C.c_void_p(), C.c_size_t()
         check(lib().fn2_net_param_diff_arena(self._h, C.byref(p), C.byref(n)))
+        return p.value, n.value
+
+    def trainable_diff_span(self):
+        """(device pointer, bytes): the range of param_diff_arena() that holds every gradient the backward pass writes."""
+        p, n = C.c_void_p(), C.c_size_t()
+        check(lib().fn2_net_trainable_diff_span(self._h, C.byref(p), C.byref(n)))
         return p.value, n.value
 
     def layer_need_backward(self):

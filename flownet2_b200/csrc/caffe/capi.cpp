@@ -64,6 +64,14 @@ int fn2_net_copy_trained_layers(fn2_net* net, const void* caffemodel, size_t byt
     FN2_CATCH
 }
 
+int fn2_net_copy_trained_layers_prefixed(fn2_net* net, const void* caffemodel, size_t bytes, const char* prefix) {
+    if (!net || !caffemodel || !prefix) { fn2::set_error("copy_trained_layers_prefixed: null argument"); return FN2_ERR_INVALID; }
+    FN2_TRY
+        net->net->CopyTrainedLayersFrom(caffemodel, bytes, prefix);
+        return FN2_OK;
+    FN2_CATCH
+}
+
 int fn2_net_to_caffemodel(fn2_net* net, void* buf, size_t* bytes) {
     if (!net || !bytes) { fn2::set_error("to_caffemodel: null argument"); return FN2_ERR_INVALID; }
     FN2_TRY
@@ -197,6 +205,13 @@ int fn2_net_param_diff_arena(fn2_net* net, void** dev_ptr, size_t* bytes) {
     if (!net || !dev_ptr || !bytes) { fn2::set_error("param_diff_arena: null argument"); return FN2_ERR_INVALID; }
     FN2_TRY
         net->net->ParamDiffArena(dev_ptr, bytes);
+        return FN2_OK;
+    FN2_CATCH
+}
+int fn2_net_trainable_diff_span(fn2_net* net, void** dev_ptr, size_t* bytes) {
+    if (!net || !dev_ptr || !bytes) { fn2::set_error("trainable_diff_span: null argument"); return FN2_ERR_INVALID; }
+    FN2_TRY
+        net->net->TrainableDiffSpan(dev_ptr, bytes);
         return FN2_OK;
     FN2_CATCH
 }

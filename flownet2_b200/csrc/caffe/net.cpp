@@ -106,12 +106,16 @@ void Net<Dtype>::Init(const NetParameter& param) {
 }
 
 // Resample(LINEAR, 2 bottoms, up-sampling a 2-channel flow) -> FlowWarp(img1, flow) -> Eltwise(img0, warped; 1, -1) -> ChannelNorm,
-// and Eltwise(flow; coeff): FlowNet2's hand-over between stacked networks.  Deploy nets only (no backward through the fused pass).
+// and Eltwise(flow; coeff): FlowNet2's hand-over between stacked networks.  The fused pass has no backward, so a block fuses only
+// when none of its five layers needs backward -- always in FlowNet2's graphs, deploy or training, because the Resample layer
+// stops the gradient.
 template <typename Dtype>
 void Net<Dtype>::FuseWarpBlocks() {
     absorbed_.assign(layers_.size(), 0);
-    if (phase_ != TEST || getenv("FN2_NO_WARPFUSE")) return;
+    if (getenv("FN2_NO_WARPFUSE")) return;
     const int L = (int)layers_.size();
+    vector<char> layer_need, blob_need;
+    NeedBackward(&layer_need, &blob_need);
     auto consumers = [&](int blob, int after) {
         vector<int> c;
         for (int j = after + 1; j < L; j++) for (int b : bottom_id_vecs_[j]) if (b == blob) { c.push_back(j); break; }
@@ -151,8 +155,8 @@ void Net<Dtype>::FuseWarpBlocks() {
         if (wb.norm < 0) continue;
         // the second image must exist before the Resample layer runs, and everything has to sit on one stream
         const int members[4] = {wb.warp, wb.sub, wb.norm, wb.scale};
-        bool ok = true;
-        for (int m : members) if (!layer_stream_.empty() && layer_stream_[m] != layer_stream_[r]) ok = false;
+        bool ok = !layer_need[r];
+        for (int m : members) if (layer_need[m] || (!layer_stream_.empty() && layer_stream_[m] != layer_stream_[r])) ok = false;
         auto produced_before = [&](int blob) {
             for (int j = r; j < L; j++) for (int t : top_id_vecs_[j]) if (t == blob) return false;
             return true;
@@ -309,14 +313,14 @@ static vector<int> strip_leading_ones(const vector<int>& s) {
 // layer may not have more blobs than the target, every target blob must be present; the blob takes the dataset's shape
 // (hdf5_load_nd_dataset, util/hdf5.cpp:20-76).  Parsed by the minimal reader of hdf5_min.cpp (no HDF5 library in this image).
 template <typename Dtype>
-void Net<Dtype>::CopyTrainedLayersFromHDF5(const void* h5, size_t bytes) {
+void Net<Dtype>::CopyTrainedLayersFromHDF5(const void* h5, size_t bytes, const string& prefix) {
     Caffe::stream() = stream_;
     H5File f(h5, bytes);
     CHECK(f.has("/data")) << "Error reading weights: the file has no /data group";
     std::map<string, int> index;
     for (size_t i = 0; i < layer_names_.size(); i++) index[layer_names_[i]] = (int)i;
     for (const string& src : f.links("/data")) {
-        auto it = index.find(src);
+        auto it = index.find(prefix + src);
         if (it == index.end()) continue;                               // "Ignoring source layer"
         auto& target = layers_[it->second]->blobs();
         const string base = "/data/" + src;
@@ -348,14 +352,14 @@ void Net<Dtype>::CopyTrainedLayersFromHDF5(const void* h5, size_t bytes) {
 }
 
 template <typename Dtype>
-void Net<Dtype>::CopyTrainedLayersFrom(const void* caffemodel, size_t bytes) {
+void Net<Dtype>::CopyTrainedLayersFrom(const void* caffemodel, size_t bytes, const string& prefix) {
     static const unsigned char h5sig[8] = {0x89, 'H', 'D', 'F', '\r', '\n', 0x1a, '\n'};
-    if (bytes >= 8 && !memcmp(caffemodel, h5sig, 8)) { CopyTrainedLayersFromHDF5(caffemodel, bytes); return; }   // .caffemodel.h5
+    if (bytes >= 8 && !memcmp(caffemodel, h5sig, 8)) { CopyTrainedLayersFromHDF5(caffemodel, bytes, prefix); return; }   // .caffemodel.h5
     Caffe::stream() = stream_;
     vector<LayerBlobs> src = ParseCaffemodel(caffemodel, bytes);
     for (const LayerBlobs& sl : src) {
         size_t ti = 0;
-        while (ti != layer_names_.size() && layer_names_[ti] != sl.name) ++ti;
+        while (ti != layer_names_.size() && layer_names_[ti] != prefix + sl.name) ++ti;
         if (ti == layer_names_.size()) continue;                               // "Ignoring source layer"
         auto& target = layers_[ti]->blobs();
         if (layers_[ti]->DoesUseCustomCopyBlobs()) {                            // net.cpp:769-780 (fork)
@@ -547,6 +551,32 @@ void Net<Dtype>::MarkActivationsOnDevice() {
 }
 
 // ---- backward -----------------------------------------------------------------------------------------------------------
+template <typename Dtype>
+float Net<Dtype>::lr_mult(int layer, int param) const {
+    const LayerParameter& lp = layers_[layer]->layer_param();
+    return param < lp.m->count("param") ? lp.m->msg("param", param).f("lr_mult", 1.f) : 1.f;      // ParamSpec default 1
+}
+
+// Which layers need backward and which blobs carry a gradient, from the graph alone (net.cpp:120-170, :223-262): a layer needs
+// backward if it has a parameter with lr_mult != 0 or a bottom that needs it (every input blob with force_backward), and it
+// allows backward.  propagate_down: false then cuts single bottoms in PlanBackward.  The warp-block fusion and the trainable
+// span of the gradient arena follow the same rule.
+template <typename Dtype>
+void Net<Dtype>::NeedBackward(vector<char>* layer_need, vector<char>* blob_need) const {
+    const int L = (int)layers_.size();
+    layer_need->assign(L, 0);
+    blob_need->assign(blobs_.size(), 0);
+    if (force_backward_) for (int b : net_input_blob_indices_) (*blob_need)[b] = 1;       // net.cpp:96-100, :262-267
+    for (int i = 0; i < L; i++) {
+        bool need = false;
+        for (size_t pi = 0; pi < layers_[i]->blobs().size(); pi++) if (lr_mult(i, (int)pi) != 0.f) need = true;
+        for (int b : bottom_id_vecs_[i]) if ((*blob_need)[b]) need = true;
+        if (!layers_[i]->AllowBackward()) need = false;
+        (*layer_need)[i] = need;
+        for (int t : top_id_vecs_[i]) if (need) (*blob_need)[t] = 1;
+    }
+}
+
 // Same decisions as Net::Init's backward bookkeeping (net.cpp:120-170 need_backward / blobs_under_loss, :210-262), made once:
 //  * a layer needs backward if it has parameters or a bottom that needs it, and AllowBackward();
 //  * it runs only if one of its tops lies under a loss (or under a SetDiff seed);
@@ -557,21 +587,8 @@ template <typename Dtype>
 void Net<Dtype>::PlanBackward() {
     if (bw_planned_) return;
     const int L = (int)layers_.size(), B = (int)blobs_.size();
-    vector<char> blob_need(B, 0), under_loss(B, 0);
-    vector<char> layer_need(L, 0);
-    if (force_backward_) for (int b : net_input_blob_indices_) blob_need[b] = 1;       // net.cpp:96-100, :262-267
-    for (int i = 0; i < L; i++) {
-        bool need = false;                                           // a parameter with lr_mult != 0 (net.cpp:223-262; default 1)
-        for (size_t pi = 0; pi < layers_[i]->blobs().size(); pi++) {
-            const LayerParameter& lpp = layers_[i]->layer_param();
-            const float lr = (int)pi < lpp.m->count("param") ? lpp.m->msg("param", (int)pi).f("lr_mult", 1.f) : 1.f;
-            if (lr != 0.f) need = true;
-        }
-        for (int b : bottom_id_vecs_[i]) if (blob_need[b]) need = true;
-        if (!layers_[i]->AllowBackward()) need = false;
-        layer_need[i] = need;
-        for (int t : top_id_vecs_[i]) blob_need[t] = need ? 1 : blob_need[t];
-    }
+    vector<char> layer_need, blob_need, under_loss(B, 0);
+    NeedBackward(&layer_need, &blob_need);
     for (int s : bw_seeds_) under_loss[s] = 1;
     vector<std::pair<int, Dtype> > loss_tops;
     for (int i = 0; i < L; i++)
@@ -661,6 +678,24 @@ template <typename Dtype>
 void Net<Dtype>::ParamDiffArena(void** dev, size_t* bytes) {
     BuildDiffArena();
     *dev = diff_arena_; *bytes = arena_floats_ * sizeof(Dtype);
+}
+
+// Parameters the backward pass writes (lr_mult != 0 in a layer that needs backward) as one range of the gradient arena: a
+// stage trained on top of frozen predecessors all-reduces this range only, not the predecessors' gradients, which stay zero.
+template <typename Dtype>
+void Net<Dtype>::TrainableDiffSpan(void** dev, size_t* bytes) {
+    BuildDiffArena();
+    vector<char> layer_need, blob_need;
+    NeedBackward(&layer_need, &blob_need);
+    size_t off = 0, lo = arena_floats_, hi = 0;
+    for (size_t i = 0; i < layers_.size(); i++)
+        for (size_t pi = 0; pi < layers_[i]->blobs().size(); pi++) {
+            const size_t padded = ((size_t)layers_[i]->blobs()[pi]->count() + 63) / 64 * 64;
+            if (layer_need[i] && lr_mult((int)i, (int)pi) != 0.f) { lo = std::min(lo, off); hi = off + padded; }
+            off += padded;
+        }
+    if (hi == 0) lo = 0;
+    *dev = diff_arena_ + lo; *bytes = (hi - lo) * sizeof(Dtype);
 }
 
 template <typename Dtype>

@@ -25,13 +25,16 @@ class Net {
     void SetDiff(const string& blob, const Dtype* host_nchw);
     void GetDiff(const string& blob, Dtype* host_nchw);
     void ParamDiffArena(void** dev, size_t* bytes);
+    void TrainableDiffSpan(void** dev, size_t* bytes);
     int launches_per_backward() const { return launches_per_backward_; }
     const vector<char>& layer_need_backward() { PlanBackward(); return bw_run_; }
     void Sync();
     cudaStream_t stream() const { return stream_; }
 
-    void CopyTrainedLayersFrom(const void* caffemodel, size_t bytes);     // net.cpp:752-802 (binary proto) / :823-870 (HDF5, by signature)
-    void CopyTrainedLayersFromHDF5(const void* h5, size_t bytes);
+    // net.cpp:752-802 (binary proto) / :823-870 (HDF5, by signature).  Source layer X fills target layer prefix + X (a stage's
+    // trained sub-network inside the next stage's graph: conv1 -> net1_conv1); source layers with no target are ignored.
+    void CopyTrainedLayersFrom(const void* caffemodel, size_t bytes, const string& prefix = "");
+    void CopyTrainedLayersFromHDF5(const void* h5, size_t bytes, const string& prefix = "");
     std::string ToCaffemodel();
     void FillParams(uint64_t seed);
     void ParamsChanged();
@@ -74,6 +77,8 @@ class Net {
     struct WarpBlock { int resample, warp, sub, norm, scale; float coeff; int fill_nan; };
     std::map<int, WarpBlock> warp_head_;        // by the Resample layer's index
     vector<char> absorbed_;
+    float lr_mult(int layer, int param) const;
+    void NeedBackward(vector<char>* layer_need, vector<char>* blob_need) const;
     void PlanBackward();
     void BuildDiffArena();
     // backward plan (static per graph + seed set): which layers run, per bottom whether the gradient is wanted and whether it is

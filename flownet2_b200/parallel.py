@@ -79,8 +79,10 @@ def gather_flows_to_root(local, out=None, dst=0):
     return None
 
 
-def grad_arena_tensor(net):
-    ptr, nbytes = net.param_diff_arena()
+def grad_arena_tensor(net, trainable_only=False):
+    """The gradient arena as a torch view; trainable_only: just the part the backward pass writes (net.trainable_diff_span()),
+    which is what a stage trained on frozen predecessors has to all-reduce."""
+    ptr, nbytes = net.trainable_diff_span() if trainable_only else net.param_diff_arena()
     return torch.as_tensor(DevicePtr(ptr, nbytes // 4), device="cuda")
 
 

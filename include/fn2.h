@@ -273,6 +273,9 @@ FN2_API int fn2_net_create_batch(const char* prototxt_text, int phase, int batch
 FN2_API void fn2_net_destroy(fn2_net* net);
 /* Load weights from the bytes of a .caffemodel (binary NetParameter). */
 FN2_API int fn2_net_copy_trained_layers(fn2_net* net, const void* caffemodel, size_t bytes);
+/* Same, with source layer X filling target layer prefix + X (FlowNet2's stage hand-over: a FlowNet2-C caffemodel into the
+ * net1_ layers of FlowNet2-CS, FlowNet2-SD into the netsd_ layers of FlowNet2).  Source layers with no target are ignored. */
+FN2_API int fn2_net_copy_trained_layers_prefixed(fn2_net* net, const void* caffemodel, size_t bytes, const char* prefix);
 /* Serialise current parameters as a .caffemodel.  Call with buf==NULL to query the size. */
 FN2_API int fn2_net_to_caffemodel(fn2_net* net, void* buf, size_t* bytes);
 /* Fill parameters from the prototxt's fillers (deterministic given seed); used for synthetic
@@ -317,6 +320,9 @@ FN2_API int fn2_net_clear_param_diffs(fn2_net* net);
 FN2_API int fn2_net_set_diff(fn2_net* net, const char* blob, const float* host_nchw);
 FN2_API int fn2_net_get_diff(fn2_net* net, const char* blob, float* host_nchw);
 FN2_API int fn2_net_param_diff_arena(fn2_net* net, void** dev_ptr, size_t* bytes);
+/* The smallest range of that arena covering every parameter the backward pass writes (lr_mult != 0 in a layer that needs
+ * backward).  A stage trained on top of frozen predecessors all-reduces only this range; the rest of the arena stays zero. */
+FN2_API int fn2_net_trainable_diff_span(fn2_net* net, void** dev_ptr, size_t* bytes);
 FN2_API int fn2_net_param_shape(fn2_net* net, const char* layer, int index, int shape[4]);
 FN2_API int fn2_net_get_param(fn2_net* net, const char* layer, int index, int diff, float* host);
 FN2_API int fn2_net_launches_per_backward(fn2_net* net);

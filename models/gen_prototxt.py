@@ -8,7 +8,7 @@ caffe.proto and the template variables of scripts/run-flownet.py:39-48
 ($TARGET_WIDTH$, $TARGET_HEIGHT$, $ADAPTED_WIDTH$, $ADAPTED_HEIGHT$, $SCALE_WIDTH$, $SCALE_HEIGHT$),
 input blobs img0/img1 and output blob predict_flow_final (run-flownet.py:66-70,98).
 
-    python models/gen_prototxt.py        # rewrites models/*_deploy.prototxt.template
+    python models/gen_prototxt.py        # rewrites models/*_deploy.prototxt.template and models/*_train.prototxt.template
 """
 import os
 
@@ -18,6 +18,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 class P:
     def __init__(self):
         self.s = []
+        self.frozen = False          # conv() then gives every parameter blob lr_mult 0 / decay_mult 0 (a frozen predecessor)
 
     def add(self, text):
         self.s.append(text)
@@ -53,9 +54,13 @@ def preprocess(p):
     return "img0_nomean_resize", "img1_nomean_resize"
 
 
-def conv_body(num_output, k, stride, pad, bias_value=0.0):
-    return ("  param {\n    lr_mult: 1\n    decay_mult: 1\n  }\n  param {\n    lr_mult: 1\n    decay_mult: 0\n  }\n"
-            "  convolution_param {\n    num_output: %d\n    pad: %d\n    kernel_size: %d\n    stride: %d\n"
+FROZEN = "  param {\n    lr_mult: 0\n    decay_mult: 0\n  }\n"
+
+
+def conv_body(num_output, k, stride, pad, bias_value=0.0, frozen=False):
+    params = FROZEN * 2 if frozen else ("  param {\n    lr_mult: 1\n    decay_mult: 1\n  }\n"
+                                        "  param {\n    lr_mult: 1\n    decay_mult: 0\n  }\n")
+    return (params + "  convolution_param {\n    num_output: %d\n    pad: %d\n    kernel_size: %d\n    stride: %d\n"
             "    weight_filler {\n      type: \"msra\"\n    }\n    bias_filler {\n      type: \"constant\"\n"
             "      value: %g\n    }\n    engine: CUDNN\n  }\n" % (num_output, pad, k, stride, bias_value))
 
@@ -67,7 +72,7 @@ def conv(p, pre, name, bottoms, tops, num_output, k, stride, relu=True, deconv=F
     if pad is None:
         pad = (k - 1) // 2 if not deconv else 1
     p.layer(pre + name, "Deconvolution" if deconv else "Convolution", bottoms, tops,
-            conv_body(num_output, k, stride, pad))
+            conv_body(num_output, k, stride, pad, frozen=p.frozen))
     if relu:
         for i, t in enumerate(tops):
             p.layer("%sReLU_%s%s" % (pre, name, "" if len(tops) == 1 else "_%d" % i), "ReLU", [t], [t], RELU)
@@ -205,12 +210,17 @@ def build_c():
     return p.text()
 
 
-def css_body(p, a, b):
+def css_body(p, a, b, stages=(2, 3), frozen=()):
+    """FlowNet-C (net1_) and one FlowNet-S per entry of `stages`, each fed through a warp block; prefixes in `frozen` get
+    lr_mult 0."""
+    p.frozen = "net1_" in frozen
     flow = flownet_c(p, "net1_", a, b)
-    for k in (2, 3):
+    for k in stages:
         full, scaled, warped, err = warp_block(p, "net%d_in_" % k, flow, a, b)
         concat(p, "net%d_Concat_input" % k, [a, b, warped, scaled, err], "net%d_input" % k)
+        p.frozen = "net%d_" % k in frozen
         flow = flownet_s(p, "net%d_" % k, "net%d_input" % k)
+    p.frozen = False
     return flow
 
 
@@ -234,6 +244,20 @@ def build_full():
     flow_css = css_body(p, a, b)
     concat(p, "netsd_Concat_input", [a, b], "netsd_input")
     flow_sd = flownet_sd(p, "netsd_", "netsd_input")
+    flow = fusion(p, a, b, flow_css, flow_sd)
+    # fusion output is already in pixels at ADAPTED size
+    p.layer("Resample_final", "Resample", [flow], ["predict_flow_resize"],
+            "  resample_param {\n    width: $TARGET_WIDTH$\n    height: $TARGET_HEIGHT$\n    type: LINEAR\n"
+            "    antialias: true\n  }\n")
+    p.layer("scale_conv1", "Convolution", ["predict_flow_resize"], ["predict_flow_final"],
+            "  param {\n    lr_mult: 0\n    decay_mult: 0\n  }\n  convolution_param {\n    num_output: 2\n    pad: 0\n"
+            "    kernel_size: 1\n    stride: 1\n    bias_term: false\n    weight_filler {\n      type: \"diagonal\"\n"
+            "      diag_val: $SCALE_WIDTH$\n      diag_val: $SCALE_HEIGHT$\n    }\n  }\n")
+    return p.text()
+
+
+def fusion(p, a, b, flow_css, flow_sd):
+    """The fusion network on the CSS and SD flows: -> fuse_predict_flow0, flow in pixels at the input's resolution."""
     # fusion inputs at full (adapted) resolution
     full1, _, _, err1 = warp_block(p, "fuse_css_", flow_css, a, b)
     full2, _, _, err2 = warp_block(p, "fuse_sd_", flow_sd, a, b)
@@ -257,15 +281,7 @@ def build_full():
     concat(p, pre + "Concat0", [pre + "conv0", pre + "deconv0", pre + "upsampled_flow1_to_0"], pre + "concat0")
     conv(p, pre, "interconv0", [pre + "concat0"], [pre + "interconv0"], 16, 3, 1, relu=False)
     conv(p, pre, "predict_flow0", [pre + "interconv0"], [pre + "predict_flow0"], 2, 3, 1, relu=False)
-    # fusion output is already in pixels at ADAPTED size
-    p.layer("Resample_final", "Resample", [pre + "predict_flow0"], ["predict_flow_resize"],
-            "  resample_param {\n    width: $TARGET_WIDTH$\n    height: $TARGET_HEIGHT$\n    type: LINEAR\n"
-            "    antialias: true\n  }\n")
-    p.layer("scale_conv1", "Convolution", ["predict_flow_resize"], ["predict_flow_final"],
-            "  param {\n    lr_mult: 0\n    decay_mult: 0\n  }\n  convolution_param {\n    num_output: 2\n    pad: 0\n"
-            "    kernel_size: 1\n    stride: 1\n    bias_term: false\n    weight_filler {\n      type: \"diagonal\"\n"
-            "      diag_val: $SCALE_WIDTH$\n      diag_val: $SCALE_HEIGHT$\n    }\n  }\n")
-    return p.text()
+    return pre + "predict_flow0"
 
 
 # ---- FlowNet2-C training net (BASELINE.json config 5) ------------------------------------------------------------------------
@@ -280,9 +296,10 @@ def _gen(kind, exp, mean, spread):
 EIGVEC = [0.51, 0.56, 0.65, 0.79, 0.01, -0.62, 0.35, -0.83, 0.44]
 
 
-def build_c_train():
-    p = P()
-    p.add('name: "FlowNet2-C-train"\n')
+def train_head(p, name, scale_gt=True):
+    """Input frames and ground truth, augmentation of both frames and of the flow -> img0_aug, img1_aug, and the ground truth
+    flow_gt_aug (pixels) or, with scale_gt, scaled_flow_gt_aug (network scale, x 0.05)."""
+    p.add('name: "%s"\n' % name)
     p.layer("data", "Input", [], ["img0", "img1", "flow_gt"],
             "  input_param {\n" + "".join("    shape { dim: $BATCH$ dim: %d dim: $DATA_HEIGHT$ dim: $DATA_WIDTH$ }\n" % c for c in (3, 3, 2)) + "  }\n")
     for i in (0, 1):
@@ -312,18 +329,82 @@ def build_c_train():
             "  propagate_down: false\n  propagate_down: false\n  augmentation_param {\n" + common + eig + "  }\n")
     p.layer("flow_aug", "FlowAugmentation", ["flow_gt", "img0_aug_params", "img1_aug_params"], ["flow_gt_aug"],
             "  augmentation_param {\n    crop_width: $TARGET_WIDTH$\n    crop_height: $TARGET_HEIGHT$\n  }\n")
-    scale(p, "scale_gt", "flow_gt_aug", "scaled_flow_gt_aug", "0.05")
-    flownet_c(p, "", "img0_aug", "img1_aug")
-    for lvl, wgt in ((6, 0.32), (5, 0.08), (4, 0.02), (3, 0.01), (2, 0.005)):
-        p.layer("Downsample%d" % lvl, "Downsample", ["scaled_flow_gt_aug", "predict_flow%d" % lvl], ["blob_gt%d" % lvl],
+    if scale_gt:
+        scale(p, "scale_gt", "flow_gt_aug", "scaled_flow_gt_aug", "0.05")
+    return "img0_aug", "img1_aug"
+
+
+LOSS_WEIGHTS = ((6, 0.32), (5, 0.08), (4, 0.02), (3, 0.01), (2, 0.005))
+# NOT-IN-REF and without a public source: the fusion network's loss weights (flow in pixels at 1/4, 1/2 and full resolution)
+FUSION_LOSS_WEIGHTS = ((2, 0.005), (1, 0.01), (0, 0.02))
+
+
+def losses(p, gt, pre, weights=LOSS_WEIGHTS):
+    """End-point-error loss of <pre>predict_flow<level> against the ground truth `gt` downsampled to its size, per level."""
+    for lvl, wgt in weights:
+        pred = "%spredict_flow%d" % (pre, lvl)
+        p.layer("Downsample%d" % lvl, "Downsample", [gt, pred], ["blob_gt%d" % lvl],
                 "  propagate_down: false\n  propagate_down: false\n")
-        p.layer("flow_loss%d" % lvl, "L1Loss", ["predict_flow%d" % lvl, "blob_gt%d" % lvl], ["flow_loss%d" % lvl],
+        p.layer("flow_loss%d" % lvl, "L1Loss", [pred, "blob_gt%d" % lvl], ["flow_loss%d" % lvl],
                 "  loss_weight: %g\n  l1_loss_param {\n    l2_per_location: true\n  }\n" % wgt)
+
+
+def build_c_train():
+    p = P()
+    a, b = train_head(p, "FlowNet2-C-train")
+    flownet_c(p, "", a, b)
+    losses(p, "scaled_flow_gt_aug", "")
+    return p.text()
+
+
+# ---- the stacked FlowNet2 training schedule: each stage trains its newest sub-network on top of frozen predecessors -----------
+# NOT-IN-REF like the C template (the reference ships no training prototxts): the stages of Ilg et al. (CVPR'17) -- CS on a
+# frozen C, CSS on a frozen CS, SD on its own, the fusion network on a frozen CSS and a frozen SD.  Layer names are those of
+# the deploy templates, so a trained caffemodel loads into the matching deploy net by name.  The warp blocks read the
+# augmented frames; Resample allows no backward, so no gradient ever reaches a warp block or a frozen predecessor.
+def build_cs_train():
+    p = P()
+    a, b = train_head(p, "FlowNet2-CS-train")
+    css_body(p, a, b, stages=(2,), frozen=("net1_",))
+    losses(p, "scaled_flow_gt_aug", "net2_")
+    return p.text()
+
+
+def build_css_train():
+    p = P()
+    a, b = train_head(p, "FlowNet2-CSS-train")
+    css_body(p, a, b, frozen=("net1_", "net2_"))
+    losses(p, "scaled_flow_gt_aug", "net3_")
+    return p.text()
+
+
+def build_sd_train():
+    p = P()
+    a, b = train_head(p, "FlowNet2-SD-train")
+    concat(p, "Concat_input", [a, b], "input")
+    flownet_sd(p, "", "input")
+    losses(p, "scaled_flow_gt_aug", "")
+    return p.text()
+
+
+def build_full_train():
+    """The fusion stage.  The fusion network predicts flow in pixels, so its ground truth is not scaled."""
+    p = P()
+    a, b = train_head(p, "FlowNet2-train", scale_gt=False)
+    flow_css = css_body(p, a, b, frozen=("net1_", "net2_", "net3_"))
+    concat(p, "netsd_Concat_input", [a, b], "netsd_input")
+    p.frozen = True
+    flow_sd = flownet_sd(p, "netsd_", "netsd_input")
+    p.frozen = False
+    fusion(p, a, b, flow_css, flow_sd)
+    losses(p, "flow_gt_aug", "fuse_", FUSION_LOSS_WEIGHTS)
     return p.text()
 
 
 MODELS = {"FlowNet2-S": build_s, "FlowNet2-C": build_c, "FlowNet2-CSS": build_css, "FlowNet2-SD": build_sd,
           "FlowNet2": build_full}
+TRAIN_MODELS = {"FlowNet2-C": build_c_train, "FlowNet2-CS": build_cs_train, "FlowNet2-CSS": build_css_train,
+                "FlowNet2-SD": build_sd_train, "FlowNet2": build_full_train}
 
 if __name__ == "__main__":
     for name, fn in MODELS.items():
@@ -331,7 +412,8 @@ if __name__ == "__main__":
         with open(path, "w") as f:
             f.write(fn())
         print("wrote", path)
-    path = os.path.join(HERE, "FlowNet2-C_train.prototxt.template")
-    with open(path, "w") as f:
-        f.write(build_c_train())
-    print("wrote", path)
+    for name, fn in TRAIN_MODELS.items():
+        path = os.path.join(HERE, "%s_train.prototxt.template" % name)
+        with open(path, "w") as f:
+            f.write(fn())
+        print("wrote", path)
