@@ -62,6 +62,8 @@ struct T4 {
     bool px_float4() const {
         return sc == 1 && !((uintptr_t)p & 15) && !(sn & 3) && !(sh & 3) && !(sw & 3);
     }
+    // every pixel can be read as ceil(c/4) float4 groups (lanes beyond c are padding or a neighbour's channels)
+    bool px_float4_groups() const { return px_float4() && sw >= 4 * ((c + 3) / 4); }
 };
 
 inline T4 view(const fn2_tensor* t) {

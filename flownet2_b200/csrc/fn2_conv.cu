@@ -591,7 +591,7 @@ static SimtLaunch simt_route(const fn2_conv_desc* d, const T4& in, const T4& out
         return {SimtRoute::fewci, dim3((unsigned)(M / out.w * ((out.w + FEW_PX - 1) / FEW_PX))), (size_t)FEW_PX * taps * d->ci * sizeof(float), 0};
     if (conv_nhwc_eligible(d, in, out)) return {SimtRoute::nhwc, dim3(), 0, 0};
     const size_t pf_smem = (size_t)taps * C4 * 4 * sizeof(float2);
-    if (!d->deconv && d->co == 2 && in.px_float4() && in.sw >= 4 * C4 && pf_smem <= 200 * 1024) {
+    if (!d->deconv && d->co == 2 && in.px_float4_groups() && pf_smem <= 200 * 1024) {
         const bool k3 = d->kh == 3 && d->kw == 3 && d->stride_h == 1 && d->stride_w == 1;
         if (C4 <= 8 && k3) {
             const long long tiles = (long long)out.n * ((out.w + 31) / 32) * ((out.h + 7) / 8);

@@ -1,5 +1,6 @@
-// Streaming (HBM-bound) layers of the FlowNet2 forward path: FlowWarp, Resample,
-// DataAugmentation kernels, ReLU, Eltwise, ChannelNorm, strided copy/fill.
+// Streaming (HBM-bound) layers: FlowWarp, Resample, DataAugmentation kernels, ChannelNorm, the warp block, and the
+// element-wise ops of the forward and backward passes (ReLU and its backward, Eltwise SUM, y = alpha*x + beta*y, strided
+// copy and fill).
 //
 // This translation unit is compiled with -fmad=false: every expression below is evaluated
 // with separately rounded multiplies and adds in the order written, which is also how the CPU
@@ -10,6 +11,7 @@
 // blobs (drop-in use) and the engine's NHWC activations / concat views.
 #include <math.h>
 #include <cfloat>
+#include <initializer_list>
 
 #include "fn2_common.cuh"
 
@@ -439,38 +441,6 @@ __global__ void mean_subtract_kernel(T4 top, T4 mean, const float* __restrict__ 
 // ---------------------------------------------------------------------------------------------
 // Glue.
 // ---------------------------------------------------------------------------------------------
-// ReLU: relu_layer.cu:9-14  x > 0 ? x : x*slope
-__global__ void relu_kernel(T4 in, T4 out, float slope) {
-    const long long total = out.count();
-    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
-         idx += (long long)gridDim.x * blockDim.x) {
-        const int c = (int)(idx % out.c);
-        long long r = idx / out.c;
-        const int x = (int)(r % out.w); r /= out.w;
-        const int y = (int)(r % out.h);
-        const int n = (int)(r / out.h);
-        const float v = in.p[in.off(n, c, y, x)];
-        out.p[out.off(n, c, y, x)] = v > 0 ? v : v * slope;
-    }
-}
-
-struct EltArgs { T4 b[4]; float coeff[4]; int nb; };
-// Eltwise SUM: eltwise_layer.cpp:59-65 (zero, then axpy in bottom order).
-__global__ void eltwise_sum_kernel(EltArgs a, T4 out) {
-    const long long total = out.count();
-    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
-         idx += (long long)gridDim.x * blockDim.x) {
-        const int x = (int)(idx % out.w);
-        long long r = idx / out.w;
-        const int c = (int)(r % out.c); r /= out.c;
-        const int y = (int)(r % out.h);
-        const int n = (int)(r / out.h);
-        float acc = 0.f;
-        for (int b = 0; b < a.nb; b++) acc = acc + a.coeff[b] * a.b[b].p[a.b[b].off(n, c, y, x)];
-        out.p[out.off(n, c, y, x)] = acc;
-    }
-}
-
 // ChannelNorm: channel_norm_layer.cu:17-30.
 __global__ void channel_norm_kernel(T4 in, T4 out, int vec4) {
     const long long total = (long long)in.n * in.h * in.w;
@@ -495,30 +465,6 @@ __global__ void channel_norm_kernel(T4 in, T4 out, int vec4) {
     }
 }
 
-// Strided copy (Concat, layout conversion).  Two index decodings so that either side can be
-// the coalesced one: SRC_CFAST decodes channel-fastest (good when src or dst is NHWC).
-template <bool CFAST>
-__global__ void copy_kernel(T4 src, T4 dst) {
-    const long long total = dst.count();
-    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
-         idx += (long long)gridDim.x * blockDim.x) {
-        int n, c, y, x;
-        if (CFAST) {
-            c = (int)(idx % dst.c);
-            long long r = idx / dst.c;
-            x = (int)(r % dst.w); r /= dst.w;
-            y = (int)(r % dst.h);
-            n = (int)(r / dst.h);
-        } else {
-            x = (int)(idx % dst.w);
-            long long r = idx / dst.w;
-            y = (int)(r % dst.h); r /= dst.h;
-            c = (int)(r % dst.c);
-            n = (int)(r / dst.c);
-        }
-        dst.p[dst.off(n, c, y, x)] = src.p[src.off(n, c, y, x)];
-    }
-}
 // Tiled transpose copy between a channel-planar side and a channel-fast side: 32 pixels x 32
 // channels per tile through shared memory so that both global sides are coalesced.
 __global__ void copy_transpose_kernel(T4 src, T4 dst, int src_cfast) {
@@ -547,33 +493,24 @@ __global__ void copy_transpose_kernel(T4 src, T4 dst, int src_cfast) {
     }
 }
 
-__global__ void fill_kernel(T4 dst, float v) {
-    const long long total = dst.count();
-    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
-         idx += (long long)gridDim.x * blockDim.x) {
-        const int c = (int)(idx % dst.c);
-        long long r = idx / dst.c;
-        const int x = (int)(r % dst.w); r /= dst.w;
-        const int y = (int)(r % dst.h);
-        const int n = (int)(r / dst.h);
-        dst.p[dst.off(n, c, y, x)] = v;
-    }
-}
-
 // ---------------------------------------------------------------------------------------------
-// Channel-fast ("NHWC") variants of the element-wise kernels: one thread per (pixel, group of 4 channels), 128-bit
-// accesses where the view allows them.  Same per-element arithmetic as the generic kernels above (bit-identical).
-// vr: the view may be READ as float4 groups (16-byte aligned pixels; lanes beyond C are padding or a neighbour's
-// channels -- read, never used).  WRITES never touch a lane beyond C: a view cannot tell whether those lanes are its own
-// padding or a sibling's channels inside a zero-copy Concat parent (a 2-channel child of a 2+2 parent has the same strides as
-// a dense 2-channel blob), so the tail group is stored lane by lane; padding stays zero from the allocation.
+// Element-wise ops: ReLU (relu_layer.cu:9-14) and its backward (relu_layer.cu:29-38), Eltwise SUM (eltwise_layer.cpp:59-65),
+// y = alpha*x + beta*y, copy and fill.  Each op is a functor over its views that computes one float4 of lanes at a place
+// `at` and stores them; ew_run picks one of two routes for it:
+//   * channel groups, when every view the op touches is channel-fast and pixel-linear (T4::is_nhwc: every NHWC blob and
+//     every concat child): thread = (pixel p, channels c0..c0+3), each view's lanes at p * sw + c0, float4 where the view
+//     allows (vr below);
+//   * strided, otherwise: thread = one element, in lane x; channel-fastest when the destination is channel-fast, else
+//     width-fastest.
+// Both routes evaluate the same expression per element, so they agree bit for bit.
+//
+// vr: the view may be READ as float4 groups (lanes beyond C are padding or a neighbour's channels -- read, never used).
+// WRITES never touch a lane beyond C: a view cannot tell whether those lanes are its own padding or a sibling's channels
+// inside a zero-copy Concat parent (a 2-channel child of a 2+2 parent has the same strides as a dense 2-channel blob), so the
+// tail group is stored lane by lane; padding stays zero from the allocation.
 // ---------------------------------------------------------------------------------------------
 struct PxView { T4 t; int vr; };
-static PxView px_view(const T4& t) {
-    PxView v; v.t = t;
-    v.vr = t.px_float4() && t.sw >= (t.c + 3) / 4 * 4;
-    return v;
-}
+static PxView px_view(const T4& t) { return {t, t.px_float4_groups()}; }
 __device__ __forceinline__ float4 px_load(const PxView& v, long long o, int c0) {
     if (v.vr) return *reinterpret_cast<const float4*>(v.t.p + o + c0);
     float4 r = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -591,49 +528,114 @@ __device__ __forceinline__ void px_store(const PxView& v, long long o, int c0, f
     if (c0 + 2 < v.t.c) v.t.p[o + c0 + 2] = r.z;
     if (c0 + 3 < v.t.c) v.t.p[o + c0 + 3] = r.w;
 }
-#define FN2_PX_DECODE(T)                                                                       \
-        const int g = (int)(idx % G);                                                          \
-        long long r_ = idx / G;                                                                \
-        const int x = (int)(r_ % (T).w); r_ /= (T).w;                                          \
-        const int y = (int)(r_ % (T).h);                                                       \
-        const int n = (int)(r_ / (T).h);                                                       \
-        const int c0 = 4 * g;
+// Channel-group route: lanes c0..c0+3 of pixel p.  F4: every view the op touches is read and written as whole float4 groups
+// (C a multiple of 4, every blob of a conv stack): straight-line 128-bit accesses.  Its loads may take the read-only path
+// even where the op writes a view it reads (axpby, an in-place ReLU backward): every element is read only by the thread
+// that writes it, and before it does.
+template <bool F4> struct GroupAt {
+    long long p; int c0;
+    __device__ float4 load(const PxView& v) const {
+        return F4 ? __ldg(reinterpret_cast<const float4*>(v.t.p + p * v.t.sw + c0)) : px_load(v, p * v.t.sw, c0);
+    }
+    __device__ void store(const PxView& v, float4 r) const {
+        if (F4) *reinterpret_cast<float4*>(v.t.p + p * v.t.sw + c0) = r;
+        else px_store(v, p * v.t.sw, c0, r);
+    }
+};
+// Strided route: element (n, c, y, x) in lane x; the other lanes are never stored.
+struct ElemAt {
+    int n, c, y, x;
+    __device__ float4 load(const PxView& v) const { return make_float4(v.t.p[v.t.off(n, c, y, x)], 0.f, 0.f, 0.f); }
+    __device__ void store(const PxView& v, float4 r) const { v.t.p[v.t.off(n, c, y, x)] = r.x; }
+};
+template <class F> __device__ __forceinline__ float4 lanes(F f, float4 a) { return make_float4(f(a.x), f(a.y), f(a.z), f(a.w)); }
+template <class F> __device__ __forceinline__ float4 lanes(F f, float4 a, float4 b) {
+    return make_float4(f(a.x, b.x), f(a.y, b.y), f(a.z, b.z), f(a.w, b.w));
+}
 
-struct EltPx { PxView b[4]; float coeff[4]; int nb; };
-__global__ void eltwise_sum_px_kernel(EltPx a, PxView out) {
-    const int G = (out.t.c + 3) / 4;
-    const long long total = (long long)out.t.n * out.t.h * out.t.w * G;
-    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
-        FN2_PX_DECODE(out.t)
+struct ReluOp {                                   // x > 0 ? x : x * slope
+    PxView in, out; float slope;
+    template <class At> __device__ void operator()(const At& at) const {
+        const float s = slope;
+        at.store(out, lanes([s](float v) { return v > 0 ? v : v * s; }, at.load(in)));
+    }
+};
+// dx (+)= dy * (y > 0 ? 1 : slope) from the layer's TOP data (in-place ReLU keeps no bottom data; for slope > 0 the sign is the
+// same).  The product is rounded before it is added, as in the reference, where ReLU writes it and a Split layer adds it in.
+struct ReluBwdOp {
+    PxView data, dy, dx; float slope; int accumulate;
+    template <class At> __device__ void operator()(const At& at) const {
+        const float s = slope;
+        float4 g = lanes([s](float t, float d) { return d * (t > 0.f ? 1.f : s); }, at.load(data), at.load(dy));
+        if (accumulate) g = lanes([](float o, float v) { return o + v; }, at.load(dx), g);
+        at.store(dx, g);
+    }
+};
+struct EltwiseSumOp {                             // zero, then acc + coeff * b in bottom order
+    PxView b[4]; float coeff[4]; int nb; PxView out;
+    template <class At> __device__ void operator()(const At& at) const {
         float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-        for (int b = 0; b < a.nb; b++) {
-            const float4 v = px_load(a.b[b], a.b[b].t.off(n, 0, y, x), c0);
-            acc.x = acc.x + a.coeff[b] * v.x; acc.y = acc.y + a.coeff[b] * v.y;
-            acc.z = acc.z + a.coeff[b] * v.z; acc.w = acc.w + a.coeff[b] * v.w;
+        for (int i = 0; i < nb; i++) {
+            const float k = coeff[i];
+            acc = lanes([k](float a, float v) { return a + k * v; }, acc, at.load(b[i]));
         }
-        px_store(out, out.t.off(n, 0, y, x), c0, acc);
+        at.store(out, acc);
     }
-}
-__global__ void relu_px_kernel(PxView in, PxView out, float slope) {
-    const int G = (out.t.c + 3) / 4;
-    const long long total = (long long)out.t.n * out.t.h * out.t.w * G;
+};
+struct AxpbyOp {                                  // y = alpha * x + beta * y; beta == 0 does not read y
+    PxView x, y; float alpha, beta;
+    template <class At> __device__ void operator()(const At& at) const {
+        const float a = alpha, b = beta;
+        const float4 xv = at.load(x);
+        if (b == 0.f) at.store(y, lanes([a](float v) { return a * v; }, xv));
+        else at.store(y, lanes([a, b](float v, float w) { return fmaf(a, v, b * w); }, xv, at.load(y)));
+    }
+};
+struct CopyOp {
+    PxView src, dst;
+    template <class At> __device__ void operator()(const At& at) const { at.store(dst, at.load(src)); }
+};
+struct FillOp {
+    PxView dst; float v;
+    template <class At> __device__ void operator()(const At& at) const { at.store(dst, make_float4(v, v, v, v)); }
+};
+
+template <bool F4, class Op>
+__global__ void ew_group_kernel(Op op, long long pixels, int G) {
+    const long long total = pixels * G;
     for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
-        FN2_PX_DECODE(out.t)
-        float4 v = px_load(in, in.t.off(n, 0, y, x), c0);
-        v.x = v.x > 0 ? v.x : v.x * slope; v.y = v.y > 0 ? v.y : v.y * slope;
-        v.z = v.z > 0 ? v.z : v.z * slope; v.w = v.w > 0 ? v.w : v.w * slope;
-        px_store(out, out.t.off(n, 0, y, x), c0, v);
+        const long long p = idx / G;
+        op(GroupAt<F4>{p, 4 * (int)(idx - p * G)});
     }
 }
-__global__ void copy_px_kernel(PxView src, PxView dst) {
-    const int G = (dst.t.c + 3) / 4;
-    const long long total = (long long)dst.t.n * dst.t.h * dst.t.w * G;
+template <class Op>
+__global__ void ew_strided_kernel(Op op, T4 dst) {
+    const long long total = dst.count();
     for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
-        FN2_PX_DECODE(dst.t)
-        px_store(dst, dst.t.off(n, 0, y, x), c0, px_load(src, src.t.off(n, 0, y, x), c0));
+        int n, c, y, x;
+        long long r = idx;
+        if (dst.sc == 1) { c = (int)(r % dst.c); r /= dst.c; x = (int)(r % dst.w); r /= dst.w; y = (int)(r % dst.h); n = (int)(r / dst.h); }
+        else { x = (int)(r % dst.w); r /= dst.w; y = (int)(r % dst.h); r /= dst.h; c = (int)(r % dst.c); n = (int)(r / dst.c); }
+        op(ElemAt{n, c, y, x});
     }
 }
-#undef FN2_PX_DECODE
+// Runs op over dst's elements; srcs: the other views op touches.
+template <class Op>
+static int ew_run(const Op& op, const T4& dst, std::initializer_list<T4> srcs, void* stream) {
+    bool group = dst.is_nhwc(), f4 = dst.c % 4 == 0 && dst.px_float4_groups();
+    for (const T4& s : srcs) { group = group && s.is_nhwc(); f4 = f4 && s.px_float4_groups(); }
+    cudaStream_t st = (cudaStream_t)stream;
+    if (group) {
+        const long long pixels = (long long)dst.n * dst.h * dst.w;
+        const int G = (dst.c + 3) / 4;
+        if (f4) ew_group_kernel<true><<<ew_grid(pixels * G, 256), 256, 0, st>>>(op, pixels, G);
+        else ew_group_kernel<false><<<ew_grid(pixels * G, 256), 256, 0, st>>>(op, pixels, G);
+    } else {
+        ew_strided_kernel<<<ew_grid(dst.count(), 256), 256, 0, st>>>(op, dst);
+    }
+    FN2_LAUNCH_CHECK();
+    return FN2_OK;
+}
 
 // ---------------------------------------------------------------------------------------------
 // Training-time augmentations of DataAugmentation (3-channel data).  Chromatic-eigen: ComputeChromaticEigenspace
@@ -838,7 +840,7 @@ int fn2_flow_warp_forward(const fn2_tensor* image, const fn2_tensor* flow, const
     float fill = 0.f;
     if (fill_nan) { unsigned u = 0xFFE00000u; memcpy(&fill, &u, 4); }
     const long long total = (long long)out.n * out.h * out.w;
-    const int vec4 = img.px_float4() && img.c <= 4 && img.sw >= 4;
+    const int vec4 = img.c <= 4 && img.px_float4_groups();
     flow_warp_fwd_kernel<<<ew_grid(total, 256), 256, 0, (cudaStream_t)stream>>>(img, fl, out, fill, vec4);
     FN2_LAUNCH_CHECK();
     return FN2_OK;
@@ -852,8 +854,8 @@ int fn2_flow_warp_backward(const fn2_tensor* image, const fn2_tensor* flow,
     T4 img = view(image), fl = view(flow), wd = view(warped_diff), id = view(image_diff), fd = view(flow_diff);
     FN2_CHECK_ARG(fl.c == 2 && fd.c == 2 && same_dims(img, wd) && same_dims(img, id) && same_dims(fl, fd),
                   "flow_warp_backward: shape mismatch");
-    fill_kernel<<<ew_grid(id.count(), 256), 256, 0, (cudaStream_t)stream>>>(id, 0.f);
-    FN2_LAUNCH_CHECK();
+    const int rc = fn2_fill(image_diff, 0.f, stream);
+    if (rc) return rc;
     const long long total = (long long)img.n * img.h * img.w;
     flow_warp_bwd_kernel<<<ew_grid(total, 256), 256, 0, (cudaStream_t)stream>>>(img, fl, wd, id, fd);
     FN2_LAUNCH_CHECK();
@@ -894,7 +896,7 @@ int fn2_warp_block_forward(const fn2_tensor* flow_in, const fn2_tensor* image0, 
     FN2_CHECK_ARG(fx <= 1.f && fy <= 1.f, "warp_block: the flow must be up-sampled (use the layer chain otherwise)");
     float fill = 0.f;
     if (fill_nan) { unsigned u = 0xFFE00000u; memcpy(&fill, &u, 4); }
-    const int vec4 = i1.px_float4() && i1.c <= 4 && i1.sw >= 4;
+    const int vec4 = i1.px_float4_groups();           // i1.c <= 4, checked above
     const long long total = (long long)ff.n * ff.h * ff.w;
     warp_block_kernel<<<ew_grid(total, 256), 256, 0, (cudaStream_t)stream>>>(fin, i0, i1, ff, wp, er, en, fs, fx, fy, scale_coeff, fill, vec4);
     FN2_LAUNCH_CHECK();
@@ -959,39 +961,40 @@ int fn2_relu_forward(const fn2_tensor* bottom, const fn2_tensor* top, float nega
     FN2_CHECK_ARG(valid(bottom) && valid(top), "relu: null/empty tensor");
     T4 in = view(bottom), out = view(top);
     FN2_CHECK_ARG(same_dims(in, out), "relu: shape mismatch");
-    if (in.sc == 1 && out.sc == 1) {
-        const long long groups = (long long)out.n * out.h * out.w * ((out.c + 3) / 4);
-        relu_px_kernel<<<ew_grid(groups, 256), 256, 0, (cudaStream_t)stream>>>(px_view(in), px_view(out), negative_slope);
-    } else
-    relu_kernel<<<ew_grid(out.count(), 256), 256, 0, (cudaStream_t)stream>>>(in, out, negative_slope);
-    FN2_LAUNCH_CHECK();
-    return FN2_OK;
+    return ew_run(ReluOp{px_view(in), px_view(out), negative_slope}, out, {in}, stream);
+}
+
+int fn2_relu_backward(const fn2_tensor* top_data, const fn2_tensor* top_diff, const fn2_tensor* bottom_diff, float negative_slope,
+                      int accumulate, void* stream) {
+    FN2_CHECK_ARG(valid(top_data) && valid(top_diff) && valid(bottom_diff), "relu_backward: null/empty tensor");
+    T4 d = view(top_data), dy = view(top_diff), dx = view(bottom_diff);
+    FN2_CHECK_ARG(same_dims(d, dy) && same_dims(d, dx), "relu_backward: shape mismatch");
+    return ew_run(ReluBwdOp{px_view(d), px_view(dy), px_view(dx), negative_slope, accumulate}, dx, {d, dy}, stream);
 }
 
 int fn2_eltwise_sum(const fn2_tensor* const* bottoms, const float* coeffs, int num_bottoms,
                     const fn2_tensor* top, void* stream) {
     FN2_CHECK_ARG(bottoms && valid(top) && num_bottoms >= 1 && num_bottoms <= 4,
                   "eltwise_sum: need 1..4 bottoms");
-    EltArgs a;
-    a.nb = num_bottoms;
-    T4 out = view(top);
+    T4 out = view(top), b[4] = {out, out, out, out};
+    EltwiseSumOp op{};
+    op.nb = num_bottoms;
+    op.out = px_view(out);
     for (int i = 0; i < num_bottoms; i++) {
         FN2_CHECK_ARG(valid(bottoms[i]), "eltwise_sum: null bottom");
-        a.b[i] = view(bottoms[i]);
-        FN2_CHECK_ARG(same_dims(a.b[i], out), "eltwise_sum: shape mismatch (eltwise_layer.cpp:33)");
-        a.coeff[i] = coeffs ? coeffs[i] : 1.0f;
+        b[i] = view(bottoms[i]);
+        FN2_CHECK_ARG(same_dims(b[i], out), "eltwise_sum: shape mismatch (eltwise_layer.cpp:33)");
+        op.b[i] = px_view(b[i]);
+        op.coeff[i] = coeffs ? coeffs[i] : 1.0f;
     }
-    bool cfast = out.sc == 1;
-    for (int i = 0; i < num_bottoms; i++) cfast = cfast && a.b[i].sc == 1;
-    if (cfast) {
-        EltPx e; e.nb = a.nb;
-        for (int i = 0; i < a.nb; i++) { e.b[i] = px_view(a.b[i]); e.coeff[i] = a.coeff[i]; }
-        const long long groups = (long long)out.n * out.h * out.w * ((out.c + 3) / 4);
-        eltwise_sum_px_kernel<<<ew_grid(groups, 256), 256, 0, (cudaStream_t)stream>>>(e, px_view(out));
-    } else
-    eltwise_sum_kernel<<<ew_grid(out.count(), 256), 256, 0, (cudaStream_t)stream>>>(a, out);
-    FN2_LAUNCH_CHECK();
-    return FN2_OK;
+    return ew_run(op, out, {b[0], b[1], b[2], b[3]}, stream);
+}
+
+int fn2_axpby(const fn2_tensor* x, float alpha, const fn2_tensor* y, float beta, void* stream) {
+    FN2_CHECK_ARG(valid(x) && valid(y), "axpby: null/empty tensor");
+    T4 xv = view(x), yv = view(y);
+    FN2_CHECK_ARG(same_dims(xv, yv), "axpby: shape mismatch");
+    return ew_run(AxpbyOp{px_view(xv), px_view(yv), alpha, beta}, yv, {xv}, stream);
 }
 
 int fn2_channel_norm_forward(const fn2_tensor* bottom, const fn2_tensor* top, void* stream) {
@@ -1000,7 +1003,7 @@ int fn2_channel_norm_forward(const fn2_tensor* bottom, const fn2_tensor* top, vo
     FN2_CHECK_ARG(out.c == 1 && out.n == in.n && out.h == in.h && out.w == in.w,
                   "channel_norm: top must be (N,1,H,W) (channel_norm_layer.cpp:29)");
     const long long total = (long long)in.n * in.h * in.w;
-    const int vec4 = in.px_float4() && in.c <= 4 && in.sw >= 4;
+    const int vec4 = in.c <= 4 && in.px_float4_groups();
     channel_norm_kernel<<<ew_grid(total, 256), 256, 0, (cudaStream_t)stream>>>(in, out, vec4);
     FN2_LAUNCH_CHECK();
     return FN2_OK;
@@ -1017,16 +1020,10 @@ int fn2_copy(const fn2_tensor* src, const fn2_tensor* dst, void* stream) {
         const long long hw = (long long)d.h * d.w;
         dim3 grid((unsigned)((hw + 31) / 32), (unsigned)((d.c + 31) / 32), (unsigned)d.n);
         copy_transpose_kernel<<<grid, dim3(32, 8), 0, st>>>(s, d, s_cf ? 1 : 0);
-    } else if (s_cf && d_cf) {
-        const long long groups = (long long)d.n * d.h * d.w * ((d.c + 3) / 4);
-        copy_px_kernel<<<ew_grid(groups, 256), 256, 0, st>>>(px_view(s), px_view(d));
-    } else if (d_cf || (s_cf && !d_pl)) {
-        copy_kernel<true><<<ew_grid(d.count(), 256), 256, 0, st>>>(s, d);
-    } else {
-        copy_kernel<false><<<ew_grid(d.count(), 256), 256, 0, st>>>(s, d);
+        FN2_LAUNCH_CHECK();
+        return FN2_OK;
     }
-    FN2_LAUNCH_CHECK();
-    return FN2_OK;
+    return ew_run(CopyOp{px_view(s), px_view(d)}, d, {s}, stream);
 }
 
 int fn2_chromatic_eigenspace(const fn2_tensor* data, const float* eigvec9_dev, float* space_dev, void* stream) {
@@ -1074,9 +1071,7 @@ int fn2_apply_effects(const fn2_tensor* data, const float* effects_dev, float ma
 int fn2_fill(const fn2_tensor* dst, float value, void* stream) {
     FN2_CHECK_ARG(valid(dst), "fill: null/empty tensor");
     T4 d = view(dst);
-    fill_kernel<<<ew_grid(d.count(), 256), 256, 0, (cudaStream_t)stream>>>(d, value);
-    FN2_LAUNCH_CHECK();
-    return FN2_OK;
+    return ew_run(FillOp{px_view(d), value}, d, {}, stream);
 }
 
 }  // extern "C"

@@ -1,13 +1,10 @@
-// Training-side kernels of the FlowNet2-C training step (BASELINE.json config 5) behind the C-ABI:
-//   * gradient plumbing: y = alpha*x + beta*y over strided views (Eltwise / Concat / Split-less fan-out accumulation), leaky
-//     ReLU backward (relu_layer.cu:29-38)
-//   * convolution / deconvolution gradients w.r.t. weights and bias (base_conv_layer.cpp:352-395 weight_gpu_gemm /
-//     backward_gpu_bias): FP32 SIMT outer-product GEMM over the pixels, split over pixel ranges with a fixed-order reduction
-//     (deterministic; the reference's cuBLAS order is unpinned).  The gradients w.r.t. the DATA reuse the forward engines with
-//     derived weights (fn2_conv_backward_data: a stride-1 convolution's adjoint is a convolution with flipped, transposed
-//     weights; a stride-2 convolution's adjoint is the deconvolution with the same weights and vice versa).
-//   * L1Loss (l1loss_layer.cu:67-195), Downsample (downsample_layer.cu:15-80), FlowAugmentation
-//     (flow_augmentation_layer.cu:24-166), GenerateAugmentationParameters (generate_augmentation_parameters_layer.cu) kernels.
+// Convolution and deconvolution gradients behind the C-ABI:
+//   * gradients w.r.t. weights and bias (base_conv_layer.cpp:352-395 weight_gpu_gemm / backward_gpu_bias): on the tensor-core
+//     engine where it takes the layer (fn2_conv_tc.cu), else an FP32 SIMT outer-product GEMM over the pixels, split over
+//     pixel ranges with a fixed-order reduction (deterministic; the reference's cuBLAS order is unpinned);
+//   * the descriptor and derived weights of the gradient w.r.t. the DATA, which reuses the forward engines
+//     (fn2_conv_backward_data_desc: a stride-1 convolution's adjoint is a convolution with flipped, transposed weights; a
+//     stride-2 convolution's adjoint is the deconvolution with the same weights and vice versa).
 #include "fn2_common.cuh"
 
 namespace fn2 {
@@ -19,71 +16,6 @@ int conv_tc_wgrad(const fn2_conv_desc* d, const T4& bottom, const T4& top_diff, 
                   size_t ws_floats, cudaStream_t st);
 
 namespace {
-
-// ---- y = alpha * x + beta * y ----------------------------------------------------------------------------------------
-__global__ void axpby_kernel(T4 x, float alpha, T4 y, float beta) {
-    const long long total = y.count();
-    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
-        // channel fastest when the destination is channel-fast, else width fastest
-        int n, c, h, w;
-        long long r = idx;
-        if (y.sc == 1) { c = (int)(r % y.c); r /= y.c; w = (int)(r % y.w); r /= y.w; h = (int)(r % y.h); n = (int)(r / y.h); }
-        else { w = (int)(r % y.w); r /= y.w; h = (int)(r % y.h); r /= y.h; c = (int)(r % y.c); n = (int)(r / y.c); }
-        const float xv = x.p[x.off(n, c, h, w)];
-        float* yp = y.p + y.off(n, c, h, w);
-        *yp = beta == 0.f ? alpha * xv : fmaf(alpha, xv, beta * *yp);
-    }
-}
-
-// both views channel-fast and pixel-linear (pixel p at p * sw), channels a multiple of 4: 128-bit accesses
-__global__ void axpby_vec_kernel(const float* __restrict__ x, long long xs, float alpha, float* __restrict__ y, long long ys, float beta,
-                                 long long pixels, int c4) {
-    const long long total = pixels * c4;
-    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
-        const long long p = idx / c4;
-        const int c = (int)(idx - p * c4) * 4;
-        const float4 xv = *reinterpret_cast<const float4*>(x + p * xs + c);
-        float4* yp = reinterpret_cast<float4*>(y + p * ys + c);
-        float4 o;
-        if (beta == 0.f) { o.x = alpha * xv.x; o.y = alpha * xv.y; o.z = alpha * xv.z; o.w = alpha * xv.w; }
-        else {
-            const float4 yv = *yp;
-            o.x = fmaf(alpha, xv.x, beta * yv.x); o.y = fmaf(alpha, xv.y, beta * yv.y);
-            o.z = fmaf(alpha, xv.z, beta * yv.z); o.w = fmaf(alpha, xv.w, beta * yv.w);
-        }
-        *yp = o;
-    }
-}
-
-// dx (+)= dy * (y > 0 ? 1 : slope); `data` is the layer's TOP data (in-place ReLU keeps no bottom data; for slope > 0 the
-// sign is the same, which is what the reference's in-place ReLU relies on, relu_layer.cu:29-38)
-__global__ void relu_bwd_kernel(T4 data, T4 dy, T4 dx, float slope, int accumulate) {
-    const long long total = dx.count();
-    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
-        int n, c, h, w;
-        long long r = idx;
-        if (dx.sc == 1) { c = (int)(r % dx.c); r /= dx.c; w = (int)(r % dx.w); r /= dx.w; h = (int)(r % dx.h); n = (int)(r / dx.h); }
-        else { w = (int)(r % dx.w); r /= dx.w; h = (int)(r % dx.h); r /= dx.h; c = (int)(r % dx.c); n = (int)(r / dx.c); }
-        const float g = dy.p[dy.off(n, c, h, w)] * (data.p[data.off(n, c, h, w)] > 0.f ? 1.f : slope);
-        float* o = dx.p + dx.off(n, c, h, w);
-        *o = accumulate ? *o + g : g;
-    }
-}
-
-// dense channel-fast maps with identical strides (every blob pair Net::Backward passes): 128-bit accesses
-__global__ void relu_bwd_vec_kernel(const float* __restrict__ data, const float* __restrict__ dy, float* __restrict__ dx, long long pixels,
-                                    int c4, long long pstride, float slope, int accumulate) {
-    const long long total = pixels * c4;
-    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
-        const long long off = (idx / c4) * pstride + (idx % c4) * 4;
-        const float4 d = *reinterpret_cast<const float4*>(data + off), g = *reinterpret_cast<const float4*>(dy + off);
-        float4 o = make_float4(g.x * (d.x > 0.f ? 1.f : slope), g.y * (d.y > 0.f ? 1.f : slope), g.z * (d.z > 0.f ? 1.f : slope),
-                               g.w * (d.w > 0.f ? 1.f : slope));
-        float4* out = reinterpret_cast<float4*>(dx + off);
-        if (accumulate) { const float4 p = *out; o.x += p.x; o.y += p.y; o.z += p.z; o.w += p.w; }
-        *out = o;
-    }
-}
 
 // ---- bias gradient: db[c] = sum over (n, y, x) of dy, two stages, fixed order ---------------------------------------------
 __global__ void bias_grad_partial_kernel(T4 dy, float* __restrict__ part, int chunks) {
@@ -221,44 +153,6 @@ __global__ void flip_transpose_kernel(const float* __restrict__ w, float* __rest
 using namespace fn2;
 
 extern "C" {
-
-int fn2_axpby(const fn2_tensor* x, float alpha, const fn2_tensor* y, float beta, void* stream) {
-    FN2_CHECK_ARG(valid(x) && valid(y), "axpby: null/empty tensor");
-    T4 xv = view(x), yv = view(y);
-    FN2_CHECK_ARG(same_dims(xv, yv), "axpby: shape mismatch");
-    auto linear = [](const T4& t) { return t.sc == 1 && t.c >= 4 && !(t.sw & 3) && t.sh == (long long)t.w * t.sw && t.sn == (long long)t.h * t.sh &&
-                                           !((uintptr_t)t.p & 15); };
-    if (linear(xv) && linear(yv)) {
-        // whole float4 groups through the vector kernel, the (c mod 4) tail channels (concat-sized blobs: 1026, 770, ...) through the scalar one
-        const long long pixels = (long long)yv.n * yv.h * yv.w;
-        const int cv = yv.c & ~3;
-        axpby_vec_kernel<<<ew_grid(pixels * (cv / 4), 256), 256, 0, (cudaStream_t)stream>>>(xv.p, xv.sw, alpha, yv.p, yv.sw, beta, pixels, cv / 4);
-        FN2_LAUNCH_CHECK();
-        if (cv == yv.c) return FN2_OK;
-        xv.p += cv; yv.p += cv; xv.c -= cv; yv.c -= cv;
-    }
-    axpby_kernel<<<ew_grid(yv.count(), 256), 256, 0, (cudaStream_t)stream>>>(xv, alpha, yv, beta);
-    FN2_LAUNCH_CHECK();
-    return FN2_OK;
-}
-
-int fn2_relu_backward(const fn2_tensor* top_data, const fn2_tensor* top_diff, const fn2_tensor* bottom_diff, float negative_slope,
-                      int accumulate, void* stream) {
-    FN2_CHECK_ARG(valid(top_data) && valid(top_diff) && valid(bottom_diff), "relu_backward: null/empty tensor");
-    T4 d = view(top_data), dy = view(top_diff), dx = view(bottom_diff);
-    FN2_CHECK_ARG(same_dims(d, dy) && same_dims(d, dx), "relu_backward: shape mismatch");
-    auto dense = [](const T4& t) { return t.sc == 1 && !(t.c & 3) && !(t.sw & 3) && t.sh == (long long)t.w * t.sw && t.sn == (long long)t.h * t.sh &&
-                                          !((uintptr_t)t.p & 15); };
-    if (dense(d) && dense(dy) && dense(dx) && d.sw == dy.sw && d.sw == dx.sw) {
-        const long long pixels = (long long)d.n * d.h * d.w;
-        relu_bwd_vec_kernel<<<ew_grid(pixels * (d.c / 4), 256), 256, 0, (cudaStream_t)stream>>>(d.p, dy.p, dx.p, pixels, d.c / 4, d.sw, negative_slope, accumulate);
-        FN2_LAUNCH_CHECK();
-        return FN2_OK;
-    }
-    relu_bwd_kernel<<<ew_grid(dx.count(), 256), 256, 0, (cudaStream_t)stream>>>(d, dy, dx, negative_slope, accumulate);
-    FN2_LAUNCH_CHECK();
-    return FN2_OK;
-}
 
 int fn2_conv_backward_params_workspace_bytes(const fn2_conv_desc* d, int N, int H, int W, size_t* bytes) {
     FN2_CHECK_ARG(d && bytes, "conv_backward_params_workspace_bytes: null argument");

@@ -275,10 +275,12 @@ def conv2d_backward(x, weight, top_diff, stride=1, pad=0, deconv=False, bias=Tru
     return dx, wd, bd
 
 
-def relu_backward(top_data, top_diff, negative_slope=0.0):
-    out = torch.empty_like(top_diff)
+def relu_backward(top_data, top_diff, negative_slope=0.0, out=None, accumulate=False):
+    """-> out (a new tensor if None) = top_diff * (top_data > 0 ? 1 : negative_slope), added to out's values if accumulate."""
+    if out is None:
+        out = torch.empty_like(top_diff)
     a, b, c = desc(top_data), desc(top_diff), desc(out)
-    check(lib().fn2_relu_backward(C.byref(a), C.byref(b), C.byref(c), negative_slope, 0, _stream()))
+    check(lib().fn2_relu_backward(C.byref(a), C.byref(b), C.byref(c), negative_slope, 1 if accumulate else 0, _stream()))
     return out
 
 
@@ -288,15 +290,17 @@ def axpby(x, alpha, y, beta):
     return y
 
 
-def relu(x, negative_slope=0.0):
-    out = torch.empty_like(x)
+def relu(x, negative_slope=0.0, out=None):
+    if out is None:
+        out = torch.empty_like(x)
     dx, do = desc(x), desc(out)
     check(lib().fn2_relu_forward(C.byref(dx), C.byref(do), negative_slope, _stream()))
     return out
 
 
-def eltwise_sum(bottoms, coeffs=None):
-    out = torch.empty_like(bottoms[0])
+def eltwise_sum(bottoms, coeffs=None, out=None):
+    if out is None:
+        out = torch.empty_like(bottoms[0])
     ds = [desc(b) for b in bottoms]
     arr = (C.POINTER(fn2_tensor) * len(ds))(*[C.pointer(d) for d in ds])
     cf = (C.c_float * len(ds))(*(coeffs if coeffs else [1.0] * len(ds)))
@@ -315,4 +319,10 @@ def channel_norm(x):
 def copy(src, dst):
     ds, dd = desc(src), desc(dst)
     check(lib().fn2_copy(C.byref(ds), C.byref(dd), _stream()))
+    return dst
+
+
+def fill(dst, value):
+    dd = desc(dst)
+    check(lib().fn2_fill(C.byref(dd), value, _stream()))
     return dst

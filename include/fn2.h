@@ -242,7 +242,7 @@ FN2_API int fn2_flow_augmentation(const fn2_tensor* flow, const fn2_tensor* top,
 /* ------------------------------------------------------------------------------------ */
 /* Glue: ReLU (relu_layer.cu:9-14), Eltwise SUM with coeffs (eltwise_layer.cu),           */
 /* ChannelNorm (channel_norm_layer.cu:17-30), strided copy (Concat concat_layer.cu,        */
-/* layout conversion).                                                                    */
+/* layout conversion), axpby, ReLU backward, fill.  Bit-exact on every layout.            */
 /* ------------------------------------------------------------------------------------ */
 FN2_API int fn2_relu_forward(const fn2_tensor* bottom, const fn2_tensor* top, float negative_slope,
                              void* stream);
@@ -253,7 +253,8 @@ FN2_API int fn2_copy(const fn2_tensor* src, const fn2_tensor* dst, void* stream)
 /* y = alpha * x + beta * y over strided views (gradient accumulation for blobs with several consumers; Eltwise / Concat /
  * Split backward: eltwise_layer.cu, concat_layer.cu, split_layer.cu).  beta == 0 overwrites without reading y. */
 FN2_API int fn2_axpby(const fn2_tensor* x, float alpha, const fn2_tensor* y, float beta, void* stream);
-/* ReLULayer::Backward_gpu (relu_layer.cu:29-38) from the TOP data (valid for in-place use with negative_slope >= 0). */
+/* ReLULayer::Backward_gpu (relu_layer.cu:29-38) from the TOP data (valid for in-place use with negative_slope >= 0):
+ * g = top_diff * (top_data > 0 ? 1 : negative_slope), rounded; bottom_diff = accumulate ? bottom_diff + g : g. */
 FN2_API int fn2_relu_backward(const fn2_tensor* top_data, const fn2_tensor* top_diff, const fn2_tensor* bottom_diff,
                               float negative_slope, int accumulate, void* stream);
 FN2_API int fn2_fill(const fn2_tensor* dst, float value, void* stream);
