@@ -113,6 +113,8 @@ def lib():
         l.fn2_conv_flip_transpose_weights.argtypes = [D, C.c_void_p, C.c_void_p, C.c_void_p]
         l.fn2_eltwise_sum.argtypes = [C.POINTER(T), C.POINTER(C.c_float), C.c_int, T, C.c_void_p]
         l.fn2_channel_norm_forward.argtypes = [T, T, C.c_void_p]
+        l.fn2_warp_block_forward.argtypes = [T] * 8 + [C.c_float, C.c_int, C.c_void_p]
+        l.fn2_downsample_forward.argtypes = [T, T, C.c_void_p]
         l.fn2_copy.argtypes = [T, T, C.c_void_p]
         l.fn2_fill.argtypes = [T, C.c_float, C.c_void_p]
         l.fn2_write_flo.argtypes = [C.c_char_p, C.c_void_p, C.c_int, C.c_int]

@@ -120,5 +120,38 @@ inline int ew_grid(long long total, int block) {
     long long cap = (long long)num_sms() * 8;
     return (int)(need < cap ? (need > 0 ? need : 1) : cap);
 }
+// Launches kernel over total work items (ew_grid(total, 256) CTAs of 256 threads) on stream: FN2_OK or the launch error.
+template <class... P, class... A>
+inline int ew_launch(void (*kernel)(P...), long long total, void* stream, const A&... args) {
+    kernel<<<ew_grid(total, 256), 256, 0, (cudaStream_t)stream>>>(args...);
+    FN2_LAUNCH_CHECK();
+    return FN2_OK;
+}
+
+// Grid-stride loops of the per-pixel and per-element kernels.  Each thread visits the same indices in the same order whatever
+// the kernel does with them, so per-thread partial sums (L1Loss, the eigenspace statistics) and index-seeded noise stay fixed.
+// f(n, y, x) for every pixel of an n x h x w extent, x fastest.
+template <class F>
+__device__ __forceinline__ void for_each_pixel(int n, int h, int w, const F& f) {
+    const long long total = (long long)n * h * w;
+    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x)
+        f((int)(idx / ((long long)w * h)), (int)((idx / w) % h), (int)(idx % w));
+}
+// (n, c, y, x) of element i of t in NCHW-logical order (x fastest, then y, c, n)
+struct Idx4 { int n, c, y, x; };
+__device__ __forceinline__ Idx4 nchw_index(const T4& t, long long i) {
+    Idx4 r;
+    r.x = (int)(i % t.w); i /= t.w;
+    r.y = (int)(i % t.h); i /= t.h;
+    r.c = (int)(i % t.c); r.n = (int)(i / t.c);
+    return r;
+}
+// f(e, idx) for every element of t: e its (n, c, y, x), idx its NCHW-logical linear index
+template <class F>
+__device__ __forceinline__ void for_each_element(const T4& t, const F& f) {
+    const long long total = t.count();
+    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x)
+        f(nchw_index(t, idx), idx);
+}
 
 }  // namespace fn2

@@ -5,10 +5,14 @@
 // cuBLAS dot products through six intermediate blobs.  Here ONE pass over the two bottoms computes the masked loss sum and the
 // not-NaN count per block, a second tiny kernel reduces the block partials in a fixed order (deterministic; cublasSdot's order is
 // not) and writes loss and normaliser; the backward recomputes difference, masks and signs from the bottoms instead of reading
-// stored intermediates: 2 reads forward, 2 reads + 2 writes backward, nothing else touches HBM.
+// stored intermediates: 2 reads forward, 2 reads + 2 writes backward, nothing else touches HBM.  Both passes call the same
+// device functions for the difference and the per-location sum with its plateau mask (l1_diff, l1_keep, l2_location), so they
+// see the same masks.
 // state (device, 4 floats): [0] loss, [1] normalize_coeff, [2] masked sum, [3] not-NaN count.
 //
-// Downsample (downsample_layer.cu:15-80): weighted box average around the rounded source position, NaN aware.
+// Downsample (downsample_layer.cu:15-80): weighted box average around the rounded source position, NaN aware; the narrow and
+// the wide kernel share the centre, the tap and the final value (ds_centre, ds_tap, ds_value).
+// This file is compiled with FMA contraction (unlike fn2_ops.cu): moving code between the two changes its rounding.
 // FlowAugmentation (flow_augmentation_layer.cu:24-66): flow field of the augmented pair from the two spatial transforms.
 #include "fn2_common.cuh"
 
@@ -21,39 +25,45 @@ struct L1P {
     float wsum, eps, plateau;
 };
 
-// per-location value / counts; shared by forward and backward so that both see the same masks
-struct L1Loc {
-    float s;            // l2: sum_c w * d^2 after the plateau mask
-    bool plateau_kill;  // l2: location masked by the plateau
-};
+// The per-element difference of the Eltwise layer: bottom0 - bottom1, or bottom0 alone
+__device__ __forceinline__ float l1_diff(const T4& a, const T4& b, const L1P& p, int n, int c, int y, int x) {
+    float d = a.p[a.off(n, c, y, x)];
+    if (p.two) d -= b.p[b.off(n, c, y, x)];
+    return d;
+}
+// L1 route: d counts (FindNotNaNs, then MaskPlateauValues)
+__device__ __forceinline__ bool l1_keep(const L1P& p, float d) { return d == d && !(p.plateau_on && fabsf(d) < p.plateau); }
+// L2 route: the per-location sum s = sum_c wsum * d^2 over the not-NaN d (KillMasked, Power(2), then the 1x1 sum convolution),
+// zeroed by the plateau mask (MaskPlateauValuesInitial + KillMasked), which kill reports.  cnt counts the not-NaN d.
+__device__ __forceinline__ float l2_location(const T4& a, const T4& b, const L1P& p, int n, int y, int x, float& cnt, bool& kill) {
+    float s = 0.f;
+    for (int c = 0; c < a.c; c++) {
+        const float d = l1_diff(a, b, p, n, c, y, x);
+        const bool ok = d == d;
+        cnt += ok ? 1.f : 0.f;
+        const float dz = ok ? d : 0.f;
+        s += p.wsum * (dz * dz);
+    }
+    kill = p.plateau_on && fabsf(s) < p.plateau * p.plateau;
+    return kill ? 0.f : s;
+}
 
 template <bool L2>
 __global__ void l1loss_fwd_kernel(T4 a, T4 b, L1P p, float* __restrict__ part /* [grid][2] */) {
-    const long long P = (long long)a.n * a.h * a.w;
     float loss = 0.f, cnt = 0.f;
-    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < P; idx += (long long)gridDim.x * blockDim.x) {
-        const int x = (int)(idx % a.w);
-        const long long r = idx / a.w;
-        const int y = (int)(r % a.h), n = (int)(r / a.h);
-        float s = 0.f;
-        for (int c = 0; c < a.c; c++) {
-            float d = a.p[a.off(n, c, y, x)];
-            if (p.two) d -= b.p[b.off(n, c, y, x)];
-            const bool ok = d == d;                                     // FindNotNaNs
-            cnt += ok ? 1.f : 0.f;
-            if (L2) {
-                const float dz = ok ? d : 0.f;                          // KillMasked
-                s += p.wsum * (dz * dz);                                // Power(2) then the 1x1 sum convolution
-            } else {
-                const bool keep = ok && !(p.plateau_on && fabsf(d) < p.plateau);   // MaskPlateauValues
-                loss += keep ? fabsf(d) : 0.f;                          // d * sign(d)
+    for_each_pixel(a.n, a.h, a.w, [&](int n, int y, int x) {
+        if constexpr (L2) {
+            bool kill;
+            const float s = l2_location(a, b, p, n, y, x, cnt, kill);
+            loss += sqrtf(s + p.eps);                                   // Power(0.5, shift = epsilon)
+        } else {
+            for (int c = 0; c < a.c; c++) {
+                const float d = l1_diff(a, b, p, n, c, y, x);
+                cnt += d == d ? 1.f : 0.f;
+                loss += l1_keep(p, d) ? fabsf(d) : 0.f;                 // d * sign(d)
             }
         }
-        if (L2) {
-            if (p.plateau_on && fabsf(s) < p.plateau * p.plateau) s = 0.f;        // MaskPlateauValuesInitial + KillMasked
-            loss += sqrtf(s + p.eps);                                   // Power(0.5, shift = epsilon)
-        }
-    }
+    });
     __shared__ float sl[32], sc[32];
     for (int o = 16; o; o >>= 1) { loss += __shfl_xor_sync(0xffffffffu, loss, o); cnt += __shfl_xor_sync(0xffffffffu, cnt, o); }
     if ((threadIdx.x & 31) == 0) { sl[threadIdx.x >> 5] = loss; sc[threadIdx.x >> 5] = cnt; }
@@ -81,120 +91,104 @@ __global__ void l1loss_final_kernel(const float* __restrict__ part, int blocks, 
 template <bool L2>
 __global__ void l1loss_bwd_kernel(T4 a, T4 b, L1P p, const float* __restrict__ state, const float* __restrict__ top_diff,
                                   T4 da, T4 db, int prop_a, int prop_b, int acc_a, int acc_b) {
-    const long long P = (long long)a.n * a.h * a.w;
     const float alpha = top_diff[0] / state[1];                         // l1loss_layer.cu:152
-    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < P; idx += (long long)gridDim.x * blockDim.x) {
-        const int x = (int)(idx % a.w);
-        const long long r = idx / a.w;
-        const int y = (int)(r % a.h), n = (int)(r / a.h);
+    for_each_pixel(a.n, a.h, a.w, [&](int n, int y, int x) {
         float gs = 0.f;
         if (L2) {
-            float s = 0.f;
-            for (int c = 0; c < a.c; c++) {
-                float d = a.p[a.off(n, c, y, x)];
-                if (p.two) d -= b.p[b.off(n, c, y, x)];
-                const float dz = d == d ? d : 0.f;
-                s += p.wsum * (dz * dz);
-            }
-            const bool kill = p.plateau_on && fabsf(s) < p.plateau * p.plateau;
-            if (kill) s = 0.f;
+            float cnt = 0.f;
+            bool kill;
+            const float s = l2_location(a, b, p, n, y, x, cnt, kill);
             const float root = sqrtf(s + p.eps);
             // PowerLayer::Backward (power_layer.cu:49-84): shift != 0: top_data / (x + shift) * power; shift == 0: top_data / x * power
             gs = (root / (s + p.eps)) * 0.5f * alpha;
             if (kill) gs = 0.f;                                         // KillMasked(plateau_l2_) on the sum's diff
         }
         for (int c = 0; c < a.c; c++) {
-            float d = a.p[a.off(n, c, y, x)];
-            if (p.two) d -= b.p[b.off(n, c, y, x)];
-            const bool ok = d == d;
+            const float d = l1_diff(a, b, p, n, c, y, x);
             float g;
             if (L2) {
+                const bool ok = d == d;
                 const float dz = ok ? d : 0.f;
                 g = (2.f * dz) * (p.wsum * gs);                         // Power(2) backward of the sum convolution's backward
                 if (!ok) g = 0.f;                                       // KillMasked(mask_)
             } else {
-                const bool keep = ok && !(p.plateau_on && fabsf(d) < p.plateau);
+                const bool keep = l1_keep(p, d);
                 const float dz = keep ? d : 0.f;
                 g = keep ? alpha * (dz > 0.f ? 1.f : -1.f) : 0.f;       // ComputeSign: 0 -> -1
             }
             if (prop_a) { float* o = da.p + da.off(n, c, y, x); *o = acc_a ? *o + g : g; }
             if (prop_b && p.two) { float* o = db.p + db.off(n, c, y, x); *o = acc_b ? *o - g : -g; }
         }
-    }
+    });
 }
 
 // ---- Downsample ------------------------------------------------------------------------------------------------------------
+// Output (dx, dy) averages the source window around the rounded centre (bx, by) with tent weights of radius (wscale, hscale).
+// The narrow kernel takes one output per thread, the wide one a block per output (ds_wide).
+struct DsCentre { float bx, by; int ix, iy; };
+__device__ __forceinline__ DsCentre ds_centre(const T4& src, const T4& dst, int dx, int dy) {
+    DsCentre r;
+    r.bx = ((float)dx / (float)(dst.w - 1)) * (float)(src.w - 1);
+    r.by = ((float)dy / (float)(dst.h - 1)) * (float)(src.h - 1);
+    r.ix = (int)roundf(r.bx); r.iy = (int)roundf(r.by);
+    return r;
+}
+// Adds source pixel (sx, sy) of channel (n, c): a NaN sample adds its weight to wnan instead of val and wsum.
+__device__ __forceinline__ void ds_tap(const T4& src, int n, int c, int sx, int sy, const DsCentre& o, float wscale, float hscale,
+                                       float& val, float& wsum, float& wnan) {
+    if (sx < 0 || sy < 0 || sx >= src.w || sy >= src.h) return;
+    float sample = src.p[src.off(n, c, sy, sx)];
+    float wgt = fmaxf(0.f, 1.f - fabsf((float)sx - o.bx) / wscale) * fmaxf(0.f, 1.f - fabsf((float)sy - o.by) / hscale);
+    if (sample != sample) { wnan += wgt; sample = 0.f; wgt = 0.f; }
+    val += sample * wgt;
+    wsum += wgt;
+}
+// NaN when NaN samples carry more than half of the weight, else the weighted mean
+__device__ __forceinline__ float ds_value(float val, float wsum, float wnan) {
+    return (wnan / wsum > 0.5f) ? __int_as_float(0x7fffffff) : val / wsum;
+}
+
 __global__ void downsample_kernel(T4 src, T4 dst, float wscale, float hscale, int wrad, int hrad) {
-    const long long total = dst.count();
-    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
-        const int dx = (int)(idx % dst.w);
-        long long r = idx / dst.w;
-        const int dy = (int)(r % dst.h); r /= dst.h;
-        const int c = (int)(r % dst.c), n = (int)(r / dst.c);
-        const float bx = ((float)dx / (float)(dst.w - 1)) * (float)(src.w - 1);
-        const float by = ((float)dy / (float)(dst.h - 1)) * (float)(src.h - 1);
-        const int ix = (int)roundf(bx), iy = (int)roundf(by);
+    for_each_element(dst, [&](Idx4 e, long long) {
+        const DsCentre o = ds_centre(src, dst, e.x, e.y);
         float val = 0.f, wsum = 0.f, wnan = 0.f;
-        for (int yo = -hrad; yo <= hrad; yo++) {
-            const int sy = iy + yo;
-            for (int xo = -wrad; xo <= wrad; xo++) {
-                const int sx = ix + xo;
-                if (sx < 0 || sy < 0 || sx >= src.w || sy >= src.h) continue;
-                float sample = src.p[src.off(n, c, sy, sx)];
-                float wgt = fmaxf(0.f, 1.f - fabsf((float)sx - bx) / wscale) * fmaxf(0.f, 1.f - fabsf((float)sy - by) / hscale);
-                if (sample != sample) { wnan += wgt; sample = 0.f; wgt = 0.f; }
-                val += sample * wgt;
-                wsum += wgt;
-            }
-        }
-        dst.p[dst.off(n, c, dy, dx)] = (wnan / wsum > 0.5f) ? __int_as_float(0x7fffffff) : val / wsum;
-    }
+        for (int yo = -hrad; yo <= hrad; yo++)
+            for (int xo = -wrad; xo <= wrad; xo++) ds_tap(src, e.n, e.c, o.ix + xo, o.iy + yo, o, wscale, hscale, val, wsum, wnan);
+        dst.p[dst.off(e.n, e.c, e.y, e.x)] = ds_value(val, wsum, wnan);
+    });
 }
 
 // Wide windows (the 1/64 level averages 161 x 151 source pixels per output): one warp-group per output element, the window
 // spread over the threads, fixed-order tree reduction.
 __global__ void downsample_wide_kernel(T4 src, T4 dst, float wscale, float hscale, int wrad, int hrad) {
-    const long long idx = blockIdx.x;
-    const int dx = (int)(idx % dst.w);
-    long long r = idx / dst.w;
-    const int dy = (int)(r % dst.h); r /= dst.h;
-    const int c = (int)(r % dst.c), n = (int)(r / dst.c);
-    const float bx = ((float)dx / (float)(dst.w - 1)) * (float)(src.w - 1);
-    const float by = ((float)dy / (float)(dst.h - 1)) * (float)(src.h - 1);
-    const int ix = (int)roundf(bx), iy = (int)roundf(by);
+    const Idx4 e = nchw_index(dst, blockIdx.x);
+    const DsCentre o = ds_centre(src, dst, e.x, e.y);
     const int ww = 2 * wrad + 1, wh = 2 * hrad + 1;
     float val = 0.f, wsum = 0.f, wnan = 0.f;
-    for (int t = threadIdx.x; t < ww * wh; t += blockDim.x) {
-        const int sy = iy - hrad + t / ww, sx = ix - wrad + t % ww;
-        if (sx < 0 || sy < 0 || sx >= src.w || sy >= src.h) continue;
-        float sample = src.p[src.off(n, c, sy, sx)];
-        float wgt = fmaxf(0.f, 1.f - fabsf((float)sx - bx) / wscale) * fmaxf(0.f, 1.f - fabsf((float)sy - by) / hscale);
-        if (sample != sample) { wnan += wgt; sample = 0.f; wgt = 0.f; }
-        val += sample * wgt;
-        wsum += wgt;
-    }
+    for (int t = threadIdx.x; t < ww * wh; t += blockDim.x)
+        ds_tap(src, e.n, e.c, o.ix - wrad + t % ww, o.iy - hrad + t / ww, o, wscale, hscale, val, wsum, wnan);
     __shared__ float s[3][8];
-    for (int o = 16; o; o >>= 1) {
-        val += __shfl_xor_sync(0xffffffffu, val, o); wsum += __shfl_xor_sync(0xffffffffu, wsum, o); wnan += __shfl_xor_sync(0xffffffffu, wnan, o);
+    for (int k = 16; k; k >>= 1) {
+        val += __shfl_xor_sync(0xffffffffu, val, k); wsum += __shfl_xor_sync(0xffffffffu, wsum, k); wnan += __shfl_xor_sync(0xffffffffu, wnan, k);
     }
     if ((threadIdx.x & 31) == 0) { s[0][threadIdx.x >> 5] = val; s[1][threadIdx.x >> 5] = wsum; s[2][threadIdx.x >> 5] = wnan; }
     __syncthreads();
     if (threadIdx.x == 0) {
         val = wsum = wnan = 0.f;
         for (int i = 0; i < (int)(blockDim.x >> 5); i++) { val += s[0][i]; wsum += s[1][i]; wnan += s[2][i]; }
-        dst.p[dst.off(n, c, dy, dx)] = (wnan / wsum > 0.5f) ? __int_as_float(0x7fffffff) : val / wsum;
+        dst.p[dst.off(e.n, e.c, e.y, e.x)] = ds_value(val, wsum, wnan);
     }
 }
+
+// The wide kernel, a block of 256 threads per output, when the window has at least one tap per thread and the outputs fit
+// in one grid row (at most 2^20 blocks); one thread per output otherwise.
+static bool ds_wide(int wrad, int hrad, long long outputs) { return (2 * wrad + 1) * (2 * hrad + 1) >= 256 && outputs <= (1 << 20); }
 
 // ---- FlowAugmentation ------------------------------------------------------------------------------------------------------
 // m1 / m2: 6 floats per sample in NAME order t0..t5 (x' = x*t0 + y*t2 + t4, y' = x*t1 + y*t3 + t5); m2 is already inverted.
 __global__ void flow_aug_kernel(T4 src, T4 dst, const float* __restrict__ m1, const float* __restrict__ m2) {
-    const long long total = (long long)dst.n * dst.h * dst.w;
     const long long src_count = src.count();
-    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
-        const int xi = (int)(idx % dst.w);
-        const long long r = idx / dst.w;
-        const int yi = (int)(r % dst.h), n = (int)(r / dst.h);
+    for_each_pixel(dst.n, dst.h, dst.w, [&](int n, int yi, int xi) {
         const float x = (float)xi, y = (float)yi;
         const float* a = m1 + 6 * n;
         const float* b = m2 + 6 * n;
@@ -208,21 +202,23 @@ __global__ void flow_aug_kernel(T4 src, T4 dst, const float* __restrict__ m1, co
         long long ov = (long long)src.w * ((long long)src.h * (2 * n + 1) + sy) + sx;
         ou = max(0LL, min(ou, src_count - 1));
         ov = max(0LL, min(ov, src_count - 1));
-        auto at = [&](long long lin) {
-            const int w = (int)(lin % src.w); long long q = lin / src.w;
-            const int h = (int)(q % src.h); q /= src.h;
-            const int c = (int)(q % src.c), nn = (int)(q / src.c);
-            return src.p[src.off(nn, c, h, w)];
-        };
+        auto at = [&](long long lin) { const Idx4 e = nchw_index(src, lin); return src.p[src.off(e.n, e.c, e.y, e.x)]; };
         const float x2 = x1 + at(ou), y2 = y1 + at(ov);
         const float x3 = x2 * b[0] + y2 * b[2] + b[4];
         const float y3 = x2 * b[1] + y2 * b[3] + b[5];
         dst.p[dst.off(n, 0, yi, xi)] = x3 - x;
         dst.p[dst.off(n, 1, yi, xi)] = y3 - y;
-    }
+    });
 }
 
 int loss_grid(long long P) { return (int)max(1LL, min((long long)num_sms() * 4, (P + 255) / 256)); }
+
+L1P l1_params(const fn2_l1loss_desc* d, const T4& a, bool two) {
+    L1P p;
+    p.l2_per_location = d->l2_per_location; p.two = two ? 1 : 0; p.plateau_on = d->plateau > 0.f; p.plateau = d->plateau;
+    p.eps = d->epsilon; p.wsum = d->l2_prescale_by_channels ? 1.f / (float)a.c : 1.f;
+    return p;
+}
 
 }  // namespace
 }  // namespace fn2
@@ -245,9 +241,7 @@ int fn2_l1loss_forward(const fn2_tensor* bottom0, const fn2_tensor* bottom1, con
     const long long P = (long long)a.n * a.h * a.w;
     const int grid = loss_grid(P);
     FN2_CHECK_ARG(workspace_bytes >= (size_t)grid * 2 * sizeof(float), "l1loss_forward: workspace too small");
-    L1P p;
-    p.l2_per_location = d->l2_per_location; p.two = bottom1 ? 1 : 0; p.plateau_on = d->plateau > 0.f; p.plateau = d->plateau;
-    p.eps = d->epsilon; p.wsum = d->l2_prescale_by_channels ? 1.f / (float)a.c : 1.f;
+    const L1P p = l1_params(d, a, bottom1);
     cudaStream_t st = (cudaStream_t)stream;
     if (p.l2_per_location) l1loss_fwd_kernel<true><<<grid, 256, 0, st>>>(a, b, p, (float*)workspace);
     else l1loss_fwd_kernel<false><<<grid, 256, 0, st>>>(a, b, p, (float*)workspace);
@@ -266,9 +260,7 @@ int fn2_l1loss_backward(const fn2_tensor* bottom0, const fn2_tensor* bottom1, co
     if (bottom1) { b = view(bottom1); FN2_CHECK_ARG(same_dims(a, b), "l1loss_backward: bottoms differ in shape"); }
     if (bottom0_diff) { da = view(bottom0_diff); FN2_CHECK_ARG(same_dims(a, da), "l1loss_backward: bottom0 diff shape"); }
     if (bottom1_diff) { FN2_CHECK_ARG(bottom1, "l1loss_backward: diff for a missing bottom"); db = view(bottom1_diff); FN2_CHECK_ARG(same_dims(a, db), "l1loss_backward: bottom1 diff shape"); }
-    L1P p;
-    p.l2_per_location = d->l2_per_location; p.two = bottom1 ? 1 : 0; p.plateau_on = d->plateau > 0.f; p.plateau = d->plateau;
-    p.eps = d->epsilon; p.wsum = d->l2_prescale_by_channels ? 1.f / (float)a.c : 1.f;
+    const L1P p = l1_params(d, a, bottom1);
     const int grid = loss_grid((long long)a.n * a.h * a.w);
     cudaStream_t st = (cudaStream_t)stream;
     if (p.l2_per_location)
@@ -286,10 +278,8 @@ int fn2_downsample_forward(const fn2_tensor* bottom, const fn2_tensor* top, void
     if (s.h == t.h && s.w == t.w) return fn2_copy(bottom, top, stream);            // downsample_layer.cpp:55-58 (shared data)
     const float wscale = (float)(s.w - 1) / (float)(t.w - 1), hscale = (float)(s.h - 1) / (float)(t.h - 1);
     const int wrad = (int)ceilf(wscale), hrad = (int)ceilf(hscale);
-    if ((2 * wrad + 1) * (2 * hrad + 1) >= 256 && t.count() <= (1 << 20))
-        downsample_wide_kernel<<<(unsigned)t.count(), 256, 0, (cudaStream_t)stream>>>(s, t, wscale, hscale, wrad, hrad);
-    else
-        downsample_kernel<<<ew_grid(t.count(), 256), 256, 0, (cudaStream_t)stream>>>(s, t, wscale, hscale, wrad, hrad);
+    if (!ds_wide(wrad, hrad, t.count())) return ew_launch(downsample_kernel, t.count(), stream, s, t, wscale, hscale, wrad, hrad);
+    downsample_wide_kernel<<<(unsigned)t.count(), 256, 0, (cudaStream_t)stream>>>(s, t, wscale, hscale, wrad, hrad);
     FN2_LAUNCH_CHECK();
     return FN2_OK;
 }
@@ -298,9 +288,7 @@ int fn2_flow_augmentation(const fn2_tensor* flow, const fn2_tensor* top, const f
     FN2_CHECK_ARG(valid(flow) && valid(top) && mats1_dev && mats2_inverse_dev, "flow_augmentation: null argument");
     T4 s = view(flow), t = view(top);
     FN2_CHECK_ARG(s.c == 2 && t.c == 2 && s.n == t.n, "flow_augmentation: flow blobs need 2 channels and equal num");
-    flow_aug_kernel<<<ew_grid((long long)t.n * t.h * t.w, 256), 256, 0, (cudaStream_t)stream>>>(s, t, mats1_dev, mats2_inverse_dev);
-    FN2_LAUNCH_CHECK();
-    return FN2_OK;
+    return ew_launch(flow_aug_kernel, (long long)t.n * t.h * t.w, stream, s, t, mats1_dev, mats2_inverse_dev);
 }
 
 }  // extern "C"

@@ -8,7 +8,9 @@
 // layers are compared bit-for-bit.  They are bandwidth-bound; FMA contraction buys nothing.
 //
 // All kernels take strided tensor views (fn2::T4) so the same code serves the reference's NCHW
-// blobs (drop-in use) and the engine's NHWC activations / concat views.
+// blobs (drop-in use) and the engine's NHWC activations / concat views.  The per-pixel kernels run the grid-stride loops of
+// fn2_common.cuh.  The warp block is built from the device functions of the stand-alone FlowWarp, Resample, Eltwise and
+// ChannelNorm kernels: the compiler inlines the same functions in both places, so its tops are bit-identical to the layer chain's.
 #include <math.h>
 #include <cfloat>
 #include <initializer_list>
@@ -22,65 +24,74 @@ namespace fn2 {
 // One thread per output pixel; the reference's NCHW->NHWC transpose pass (.cu:24-52) is not
 // needed: taps are read straight from the strided view.
 // ---------------------------------------------------------------------------------------------
-__global__ void flow_warp_fwd_kernel(T4 img, T4 flow, T4 out, float fill, int vec4) {
-    const long long total = (long long)out.n * out.h * out.w;
-    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
-         idx += (long long)gridDim.x * blockDim.x) {
-        const int x = (int)(idx % out.w);
-        const int y = (int)((idx / out.w) % out.h);
-        const int n = (int)(idx / ((long long)out.w * out.h));
-        const float fx = flow.p[flow.off(n, 0, y, x)];
-        const float fy = flow.p[flow.off(n, 1, y, x)];
-        const float x2 = (float)x + fx;
-        const float y2 = (float)y + fy;
-        const int width = img.w, height = img.h;
-        if (x2 >= 0 && y2 >= 0 && x2 < width && y2 < height) {      // flow_warp_layer.cpp:86
-            const int ix2_L = (int)x2;
-            const int iy2_T = (int)y2;
-            const int ix2_R = min(ix2_L + 1, width - 1);
-            const int iy2_B = min(iy2_T + 1, height - 1);
-            const float alpha = x2 - ix2_L;
-            const float beta = y2 - iy2_T;
-            const float cTL = (1 - alpha) * (1 - beta);
-            const float cTR = alpha * (1 - beta);
-            const float cBL = (1 - alpha) * beta;
-            const float cBR = alpha * beta;
-            const long long oTL = img.off(n, 0, iy2_T, ix2_L), oTR = img.off(n, 0, iy2_T, ix2_R);
-            const long long oBL = img.off(n, 0, iy2_B, ix2_L), oBR = img.off(n, 0, iy2_B, ix2_R);
-            if (vec4) {
-                // channel-fast image with <= 4 channels in 16-byte pixels: one 128-bit load per tap (same arithmetic per channel)
-                const float4 TL = __ldg(reinterpret_cast<const float4*>(img.p + oTL)), TR = __ldg(reinterpret_cast<const float4*>(img.p + oTR));
-                const float4 BL = __ldg(reinterpret_cast<const float4*>(img.p + oBL)), BR = __ldg(reinterpret_cast<const float4*>(img.p + oBR));
-                const float tl[4] = {TL.x, TL.y, TL.z, TL.w}, tr[4] = {TR.x, TR.y, TR.z, TR.w};
-                const float bl[4] = {BL.x, BL.y, BL.z, BL.w}, br[4] = {BR.x, BR.y, BR.z, BR.w};
+// Bilinear taps of the image point (x + u, y + v): inside tells whether it lies in the image (else the output is the fill
+// value); then the four weights and the offsets of the four taps' channel 0.
+struct WarpTaps {
+    bool inside;
+    float cTL, cTR, cBL, cBR;
+    long long oTL, oTR, oBL, oBR;
+};
+__device__ __forceinline__ WarpTaps warp_taps(const T4& img, int n, int y, int x, float u, float v) {
+    WarpTaps t;
+    const float x2 = (float)x + u;
+    const float y2 = (float)y + v;
+    const int width = img.w, height = img.h;
+    t.inside = x2 >= 0 && y2 >= 0 && x2 < width && y2 < height;      // flow_warp_layer.cpp:86
+    if (!t.inside) return t;
+    const int ix2_L = (int)x2;
+    const int iy2_T = (int)y2;
+    const int ix2_R = min(ix2_L + 1, width - 1);
+    const int iy2_B = min(iy2_T + 1, height - 1);
+    const float alpha = x2 - ix2_L;
+    const float beta = y2 - iy2_T;
+    t.cTL = (1 - alpha) * (1 - beta);
+    t.cTR = alpha * (1 - beta);
+    t.cBL = (1 - alpha) * beta;
+    t.cBR = alpha * beta;
+    t.oTL = img.off(n, 0, iy2_T, ix2_L); t.oTR = img.off(n, 0, iy2_T, ix2_R);
+    t.oBL = img.off(n, 0, iy2_B, ix2_L); t.oBR = img.off(n, 0, iy2_B, ix2_R);
+    return t;
+}
+__device__ __forceinline__ float warp_mix(const WarpTaps& t, float TL, float TR, float BL, float BR) {
+    return ((t.cTL * TL + t.cTR * TR) + t.cBL * BL) + t.cBR * BR;
+}
+// Warped value of channel c (strided form)
+__device__ __forceinline__ float warp_channel(const WarpTaps& t, const T4& img, int c) {
+    const long long o = c * img.sc;
+    return warp_mix(t, __ldg(img.p + t.oTL + o), __ldg(img.p + t.oTR + o), __ldg(img.p + t.oBL + o), __ldg(img.p + t.oBR + o));
+}
+// Warped values of channels 0..3 (float4 form: every pixel is one 16-byte group, one 128-bit load per tap)
+__device__ __forceinline__ void warp_group(const WarpTaps& t, const T4& img, float v[4]) {
+    const float4 TL = __ldg(reinterpret_cast<const float4*>(img.p + t.oTL)), TR = __ldg(reinterpret_cast<const float4*>(img.p + t.oTR));
+    const float4 BL = __ldg(reinterpret_cast<const float4*>(img.p + t.oBL)), BR = __ldg(reinterpret_cast<const float4*>(img.p + t.oBR));
+    v[0] = warp_mix(t, TL.x, TR.x, BL.x, BR.x);
+    v[1] = warp_mix(t, TL.y, TR.y, BL.y, BR.y);
+    v[2] = warp_mix(t, TL.z, TR.z, BL.z, BR.z);
+    v[3] = warp_mix(t, TL.w, TR.w, BL.w, BR.w);
+}
+
+// F4: every image pixel is one float4 group (px_one_group).
+template <bool F4>
+__global__ void flow_warp_fwd_kernel(T4 img, T4 flow, T4 out, float fill) {
+    for_each_pixel(out.n, out.h, out.w, [&](int n, int y, int x) {
+        const WarpTaps t = warp_taps(img, n, y, x, flow.p[flow.off(n, 0, y, x)], flow.p[flow.off(n, 1, y, x)]);
+        if (F4 && t.inside) {
+            float v[4];
+            warp_group(t, img, v);
 #pragma unroll
-                for (int c = 0; c < 4; c++)
-                    if (c < img.c) out.p[out.off(n, c, y, x)] = ((cTL * tl[c] + cTR * tr[c]) + cBL * bl[c]) + cBR * br[c];
-                continue;
-            }
-            for (int c = 0; c < img.c; c++) {
-                const float TL = __ldg(img.p + oTL + c * img.sc);
-                const float TR = __ldg(img.p + oTR + c * img.sc);
-                const float BL = __ldg(img.p + oBL + c * img.sc);
-                const float BR = __ldg(img.p + oBR + c * img.sc);
-                out.p[out.off(n, c, y, x)] = ((cTL * TL + cTR * TR) + cBL * BL) + cBR * BR;
-            }
+            for (int c = 0; c < 4; c++)
+                if (c < img.c) out.p[out.off(n, c, y, x)] = v[c];
         } else {
-            for (int c = 0; c < img.c; c++) out.p[out.off(n, c, y, x)] = fill;
+            for (int c = 0; c < img.c; c++) out.p[out.off(n, c, y, x)] = t.inside ? warp_channel(t, img, c) : fill;
         }
-    }
+    });
 }
 
 // FlowWarp backward.  Reference: flow_warp_layer.cu:170-229 / flow_warp_layer.cpp:120-198.
 // image_diff must be zero-filled by the caller side (done in the entry point).  Scatter via
 // atomicAdd exactly like the reference (order-nondeterministic in the last ulp).
 __global__ void flow_warp_bwd_kernel(T4 img, T4 flow, T4 wdiff, T4 idiff, T4 fdiff) {
-    const long long total = (long long)img.n * img.h * img.w;
-    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
-         idx += (long long)gridDim.x * blockDim.x) {
-        const int x = (int)(idx % img.w);
-        const int y = (int)((idx / img.w) % img.h);
-        const int n = (int)(idx / ((long long)img.w * img.h));
+    for_each_pixel(img.n, img.h, img.w, [&](int n, int y, int x) {
         const float x2 = (float)x + flow.p[flow.off(n, 0, y, x)];
         const float y2 = (float)y + flow.p[flow.off(n, 1, y, x)];
         const int width = img.w, height = img.h;
@@ -106,116 +117,7 @@ __global__ void flow_warp_bwd_kernel(T4 img, T4 flow, T4 wdiff, T4 idiff, T4 fdi
         }
         fdiff.p[fdiff.off(n, 0, y, x)] = du;
         fdiff.p[fdiff.off(n, 1, y, x)] = dv;
-    }
-}
-
-// ---------------------------------------------------------------------------------------------
-// Warp block between two stacked networks (FlowNet2-CSS / FlowNet2): the chain
-//   Resample(LINEAR, up-sampling) -> FlowWarp -> Eltwise(img0 - warped) -> ChannelNorm, and Eltwise(coeff * flow)
-// as ONE pass: one thread per full-resolution pixel computes the interpolated flow, samples the second image, and writes all
-// five tops (most of them channel ranges of the next network's input concat).  Every value goes through exactly the
-// expressions of the stand-alone kernels below (resample_kernel<2>, flow_warp_fwd_kernel, eltwise_sum_kernel with coefficients
-// (1, -1) resp. (coeff), channel_norm_kernel; this file is compiled -fmad=false), so the tops are bit-identical to the layer
-// chain's.  References: resample_layer.cu:40-95, flow_warp_layer.cu:59-122, eltwise_layer.cu:36-60, channel_norm_layer.cu:17-30.
-// ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ float triangleCoeffW(float x) {
-    if (-1 <= x && x < 0) return x + 1;
-    if (0 <= x && x <= 1) return 1 - x;
-    return 0;
-}
-__global__ void warp_block_kernel(T4 fin, T4 img0, T4 img1, T4 ffull, T4 warped, T4 err, T4 errn, T4 fscaled, float fx, float fy,
-                                  float coeff, float fill, int vec4) {
-    const long long total = (long long)ffull.n * ffull.h * ffull.w;
-    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
-        const int x_out = (int)(idx % ffull.w);
-        const int y_out = (int)((idx / ffull.w) % ffull.h);
-        const int n = (int)(idx / ((long long)ffull.w * ffull.h));
-        // ---- Resample (LINEAR, no antialias: up-sampling), 2 channels: resample_kernel<2> with the window of <= 8 columns
-        const float x_in = (x_out * fx + fy / 2.0f) - 0.5f;
-        const float y_in = (y_out * fy + fx / 2.0f) - 0.5f;
-        const int x_in_round = (int)roundf(x_in);
-        const int y_in_round = (int)roundf(y_in);
-        const float ax = 1.0f / 1.0f, ay = 1.0f / 1.0f;
-        const int rx = (fx < 1.0f) ? 2 : (int)ceilf(2.0f / ax);
-        const int ry = (fy < 1.0f) ? 2 : (int)ceilf(2.0f / ay);
-        const int xl = max(x_in_round - rx, (int)floorf(x_in - 1.0f / ax)), xh = min(x_in_round + rx, (int)ceilf(x_in + 1.0f / ax));
-        const int yl = max(y_in_round - ry, (int)floorf(y_in - 1.0f / ay)), yh = min(y_in_round + ry, (int)ceilf(y_in + 1.0f / ay));
-        float tx_[8];
-#pragma unroll
-        for (int k = 0; k < 8; k++) {
-            const float dx = x_in - (xl + k);
-            tx_[k] = (ax * triangleCoeffW(ax * dx)) * ay;
-        }
-        float sum0 = 0.f, sum1 = 0.f, wsum = 0.f;
-        for (int y = yl; y <= yh; y++) {
-            if (y < 0 || y >= fin.h) continue;
-            const float dy = y_in - y;
-            const float cy = triangleCoeffW(ay * dy);
-#pragma unroll
-            for (int k = 0; k < 8; k++) {
-                const int x = xl + k;
-                if (x > xh) break;
-                if (x < 0 || x >= fin.w) continue;
-                const float w = tx_[k] * cy;
-                if (w == 0.f) continue;
-                const float* ip = fin.p + fin.off(n, 0, y, x);
-                sum0 = sum0 + w * __ldg(ip);
-                sum1 = sum1 + w * __ldg(ip + fin.sc);
-                wsum += w;
-            }
-        }
-        const float f0 = (!wsum) ? 0 : (sum0 / wsum), f1 = (!wsum) ? 0 : (sum1 / wsum);
-        ffull.p[ffull.off(n, 0, y_out, x_out)] = f0;
-        ffull.p[ffull.off(n, 1, y_out, x_out)] = f1;
-        // ---- Eltwise(coeff): acc = 0 + coeff * v
-        fscaled.p[fscaled.off(n, 0, y_out, x_out)] = 0.f + coeff * f0;
-        fscaled.p[fscaled.off(n, 1, y_out, x_out)] = 0.f + coeff * f1;
-        // ---- FlowWarp of img1 (flow_warp_fwd_kernel)
-        const float x2 = (float)x_out + f0;
-        const float y2 = (float)y_out + f1;
-        const int width = img1.w, height = img1.h;
-        float wv[4] = {fill, fill, fill, fill};
-        if (x2 >= 0 && y2 >= 0 && x2 < width && y2 < height) {
-            const int ix2_L = (int)x2;
-            const int iy2_T = (int)y2;
-            const int ix2_R = min(ix2_L + 1, width - 1);
-            const int iy2_B = min(iy2_T + 1, height - 1);
-            const float alpha = x2 - ix2_L;
-            const float beta = y2 - iy2_T;
-            const float cTL = (1 - alpha) * (1 - beta);
-            const float cTR = alpha * (1 - beta);
-            const float cBL = (1 - alpha) * beta;
-            const float cBR = alpha * beta;
-            const long long oTL = img1.off(n, 0, iy2_T, ix2_L), oTR = img1.off(n, 0, iy2_T, ix2_R);
-            const long long oBL = img1.off(n, 0, iy2_B, ix2_L), oBR = img1.off(n, 0, iy2_B, ix2_R);
-            if (vec4) {
-                const float4 TL = __ldg(reinterpret_cast<const float4*>(img1.p + oTL)), TR = __ldg(reinterpret_cast<const float4*>(img1.p + oTR));
-                const float4 BL = __ldg(reinterpret_cast<const float4*>(img1.p + oBL)), BR = __ldg(reinterpret_cast<const float4*>(img1.p + oBR));
-                const float tl[4] = {TL.x, TL.y, TL.z, TL.w}, tr[4] = {TR.x, TR.y, TR.z, TR.w};
-                const float bl[4] = {BL.x, BL.y, BL.z, BL.w}, br[4] = {BR.x, BR.y, BR.z, BR.w};
-#pragma unroll
-                for (int c = 0; c < 4; c++) wv[c] = ((cTL * tl[c] + cTR * tr[c]) + cBL * bl[c]) + cBR * br[c];
-            } else {
-                for (int c = 0; c < img1.c; c++) {
-                    const float TL = __ldg(img1.p + oTL + c * img1.sc);
-                    const float TR = __ldg(img1.p + oTR + c * img1.sc);
-                    const float BL = __ldg(img1.p + oBL + c * img1.sc);
-                    const float BR = __ldg(img1.p + oBR + c * img1.sc);
-                    wv[c] = ((cTL * TL + cTR * TR) + cBL * BL) + cBR * BR;
-                }
-            }
-        }
-        // ---- Eltwise(1, -1): acc = (0 + 1 * a) + (-1) * b, then ChannelNorm
-        float norm = 0;
-        for (int c = 0; c < img1.c; c++) {
-            warped.p[warped.off(n, c, y_out, x_out)] = wv[c];
-            float acc = 0.f + 1.0f * img0.p[img0.off(n, c, y_out, x_out)];
-            acc = acc + (-1.0f) * wv[c];
-            err.p[err.off(n, c, y_out, x_out)] = acc;
-            norm = norm + acc * acc;
-        }
-        errn.p[errn.off(n, 0, y_out, x_out)] = sqrtf(norm);
-    }
+    });
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -233,94 +135,157 @@ __device__ __forceinline__ float triangleCoeff(float x) {
     if (0 <= x && x <= 1) return 1 - x;
     return 0;
 }
+// Source coordinate of output coordinate o; f is this axis's in/out ratio, g the other axis's (the swapped offsets).
+__device__ __forceinline__ float resample_src(int o, float f, float g) { return (o * f + g / 2.0f) - 0.5f; }
 
-// One thread per output pixel, all channels: the filter weights depend on the pixel only, and every channel accumulates
-// its taps in the reference's order (y outer, x inner), so each channel's result is bit-identical to the per-element
-// formulation.  Taps whose weight is exactly zero are skipped: sum + 0*v == sum and wsum + 0 == wsum for finite v (the
-// triangle filter of an up-sampling has 21 zero taps out of 25).
-template <int TYPE>   // 1 nearest, 2 linear(triangle), 3 cubic
-__global__ void resample_kernel(T4 in, T4 out, float fx, float fy, int antialias) {
-    const long long total = (long long)out.n * out.h * out.w;
-    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
-         idx += (long long)gridDim.x * blockDim.x) {
-        const int x_out = (int)(idx % out.w);
-        const int y_out = (int)((idx / out.w) % out.h);
-        const int n = (int)(idx / ((long long)out.w * out.h));
-        const float x_in = (x_out * fx + fy / 2.0f) - 0.5f;
-        const float y_in = (y_out * fy + fx / 2.0f) - 0.5f;
+// Filter window of TYPE 2 (triangle) or 3 (cubic) around the source point (x_in, y_in).  One thread per output pixel, all
+// channels: the filter weights depend on the pixel only, and every channel accumulates its taps in the reference's order
+// (y outer, x inner), so each channel's result is bit-identical to the per-element formulation.  The filters vanish outside
+// |ax*dx| < support, so only the taps of the reference's window that can carry weight are visited, and taps whose weight is
+// exactly zero are skipped: sum + 0*v == sum and wsum + 0 == wsum for finite v (the triangle filter of an up-sampling has 21
+// zero taps out of 25).
+template <int TYPE> struct ResampleWindow {
+    static constexpr int MAXT = 8;
+    float x_in, y_in, ax, ay;
+    int xl, xh, yl, yh;
+    bool pre;                     // at most MAXT columns: tx holds the x factors
+    float tx[MAXT];
+    __device__ static float coeff(float d) { return (TYPE == 3) ? bicubicCoeff(d) : triangleCoeff(d); }
+    // (ax * cx) * ay of column x: the first two products of the reference's weight expression
+    __device__ float xfactor(int x) const { return (ax * coeff(ax * (x_in - x))) * ay; }
+    __device__ ResampleWindow(float x_in_, float y_in_, float fx, float fy, int antialias) : x_in(x_in_), y_in(y_in_) {
+        const int kernel_width = (TYPE == 3) ? 4 : 2;
+        ax = 1.0f / (antialias ? fx : 1.0f);
+        ay = 1.0f / (antialias ? fy : 1.0f);
         const int x_in_round = (int)roundf(x_in);
         const int y_in_round = (int)roundf(y_in);
-        if (TYPE == 1) {
-            // the reference does not clamp (resample_layer.cu:120-123) and can read out of
-            // bounds; clamp instead (documented deviation)
-            const int xr = min(max(x_in_round, 0), in.w - 1);
-            const int yr = min(max(y_in_round, 0), in.h - 1);
-            for (int c = 0; c < out.c; c++) out.p[out.off(n, c, y_out, x_out)] = in.p[in.off(n, c, yr, xr)];
-            continue;
-        }
-        const int kernel_width = (TYPE == 3) ? 4 : 2;
-        const float ax = 1.0f / (antialias ? fx : 1.0f);
-        const float ay = 1.0f / (antialias ? fy : 1.0f);
         const int rx = (fx < 1.0f) ? 2 : (int)ceilf((float)kernel_width / ax);
         const int ry = (fy < 1.0f) ? 2 : (int)ceilf((float)kernel_width / ay);
-        // the filters vanish outside |ax*dx| < support: only the taps of the reference's window that can carry weight are
-        // visited (every skipped tap has weight exactly 0, see above)
         const float sup = (TYPE == 3) ? 2.0f : 1.0f;
-        const int xl = max(x_in_round - rx, (int)floorf(x_in - sup / ax)), xh = min(x_in_round + rx, (int)ceilf(x_in + sup / ax));
-        const int yl = max(y_in_round - ry, (int)floorf(y_in - sup / ay)), yh = min(y_in_round + ry, (int)ceilf(y_in + sup / ay));
-        // x factors ((ax * cx) * ay, the first two products of the reference's weight expression) once per pixel when the
-        // window is narrow (always, except for strong down-sampling)
-        constexpr int MAXT = 8;
-        float tx_[MAXT];
-        const bool pre = xh - xl < MAXT;
+        xl = max(x_in_round - rx, (int)floorf(x_in - sup / ax)); xh = min(x_in_round + rx, (int)ceilf(x_in + sup / ax));
+        yl = max(y_in_round - ry, (int)floorf(y_in - sup / ay)); yh = min(y_in_round + ry, (int)ceilf(y_in + sup / ay));
+        pre = xh - xl < MAXT;
         if (pre) {
 #pragma unroll
-            for (int k = 0; k < MAXT; k++) {
-                const float dx = x_in - (xl + k);
-                const float cx = (TYPE == 3) ? bicubicCoeff(ax * dx) : triangleCoeff(ax * dx);
-                tx_[k] = (ax * cx) * ay;
-            }
-        }
-        for (int c0 = 0; c0 < out.c; c0 += 4) {
-            const int nc = min(4, out.c - c0);
-            float sum[4] = {0.f, 0.f, 0.f, 0.f};
-            float wsum = 0;
-            for (int y = yl; y <= yh; y++) {
-                if (y < 0 || y >= in.h) continue;
-                const float dy = y_in - y;
-                const float cy = (TYPE == 3) ? bicubicCoeff(ay * dy) : triangleCoeff(ay * dy);
-#pragma unroll
-                for (int k = 0; k < MAXT; k++) {
-                    const int x = xl + k;
-                    if (!pre || x > xh) break;
-                    if (x < 0 || x >= in.w) continue;
-                    const float w = tx_[k] * cy;
-                    if (w == 0.f) continue;
-                    const float* ip = in.p + in.off(n, c0, y, x);
-#pragma unroll
-                    for (int j = 0; j < 4; j++)
-                        if (j < nc) sum[j] = sum[j] + w * __ldg(ip + (long long)j * in.sc);
-                    wsum += w;
-                }
-                if (!pre)
-                for (int x = xl; x <= xh; x++) {
-                    if (x < 0 || x >= in.w) continue;
-                    const float dx = x_in - x;
-                    const float cx = (TYPE == 3) ? bicubicCoeff(ax * dx) : triangleCoeff(ax * dx);
-                    const float w = (ax * cx) * ay * cy;
-                    if (w == 0.f) continue;
-                    const float* ip = in.p + in.off(n, c0, y, x);
-#pragma unroll
-                    for (int j = 0; j < 4; j++)
-                        if (j < nc) sum[j] = sum[j] + w * __ldg(ip + (long long)j * in.sc);
-                    wsum += w;
-                }
-            }
-#pragma unroll
-            for (int j = 0; j < 4; j++)
-                if (j < nc) out.p[out.off(n, c0 + j, y_out, x_out)] = (!wsum) ? 0 : (sum[j] / wsum);
+            for (int k = 0; k < MAXT; k++) tx[k] = xfactor(xl + k);
         }
     }
+    // sum[j] += w * in(n, c0 + j, y, x) over the window's taps for j < nc; returns the sum of the weights
+    __device__ float accumulate(const T4& in, int n, int c0, int nc, float sum[4]) const {
+        float wsum = 0;
+        for (int y = yl; y <= yh; y++) {
+            if (y < 0 || y >= in.h) continue;
+            const float cy = coeff(ay * (y_in - y));
+            for (int x0 = xl; x0 <= xh; x0 += MAXT) {     // one pass when pre
+#pragma unroll
+                for (int k = 0; k < MAXT; k++) {
+                    const int x = x0 + k;
+                    if (x > xh) break;
+                    if (x < 0 || x >= in.w) continue;
+                    const float w = (pre ? tx[k] : xfactor(x)) * cy;
+                    if (w == 0.f) continue;
+                    const float* ip = in.p + in.off(n, c0, y, x);
+#pragma unroll
+                    for (int j = 0; j < 4; j++)
+                        if (j < nc) sum[j] = sum[j] + w * __ldg(ip + (long long)j * in.sc);
+                    wsum += w;
+                }
+            }
+        }
+        return wsum;
+    }
+    __device__ static float value(float sum, float wsum) { return (!wsum) ? 0 : (sum / wsum); }
+};
+
+template <int TYPE>   // 1 nearest, 2 linear(triangle), 3 cubic
+__global__ void resample_kernel(T4 in, T4 out, float fx, float fy, int antialias) {
+    for_each_pixel(out.n, out.h, out.w, [&](int n, int y_out, int x_out) {
+        const float x_in = resample_src(x_out, fx, fy), y_in = resample_src(y_out, fy, fx);
+        if constexpr (TYPE == 1) {
+            // the reference does not clamp (resample_layer.cu:120-123) and can read out of
+            // bounds; clamp instead (documented deviation)
+            const int xr = min(max((int)roundf(x_in), 0), in.w - 1);
+            const int yr = min(max((int)roundf(y_in), 0), in.h - 1);
+            for (int c = 0; c < out.c; c++) out.p[out.off(n, c, y_out, x_out)] = in.p[in.off(n, c, yr, xr)];
+        } else {
+            const ResampleWindow<TYPE> win(x_in, y_in, fx, fy, antialias);
+            for (int c0 = 0; c0 < out.c; c0 += 4) {
+                const int nc = min(4, out.c - c0);
+                float sum[4] = {0.f, 0.f, 0.f, 0.f};
+                const float wsum = win.accumulate(in, n, c0, nc, sum);
+#pragma unroll
+                for (int j = 0; j < 4; j++)
+                    if (j < nc) out.p[out.off(n, c0 + j, y_out, x_out)] = ResampleWindow<TYPE>::value(sum[j], wsum);
+            }
+        }
+    });
+}
+
+// ---------------------------------------------------------------------------------------------
+// ChannelNorm (channel_norm_layer.cu:17-30) and the Eltwise SUM term (eltwise_layer.cpp:59-65).
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ float eltwise_term(float acc, float k, float v) { return acc + k * v; }
+// ChannelNorm's running sum of squares; the output is its square root
+__device__ __forceinline__ float norm_term(float norm, float v) { return norm + v * v; }
+
+// F4: every input pixel is one float4 group (px_one_group).
+template <bool F4>
+__global__ void channel_norm_kernel(T4 in, T4 out) {
+    for_each_pixel(in.n, in.h, in.w, [&](int n, int y, int x) {
+        float norm = 0;
+        if (F4) {
+            const float4 q = *reinterpret_cast<const float4*>(in.p + in.off(n, 0, y, x));
+            const float v[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+            for (int c = 0; c < 4; c++) if (c < in.c) norm = norm_term(norm, v[c]);
+        } else {
+            for (int c = 0; c < in.c; c++) norm = norm_term(norm, in.p[in.off(n, c, y, x)]);
+        }
+        out.p[out.off(n, 0, y, x)] = sqrtf(norm);
+    });
+}
+
+// ---------------------------------------------------------------------------------------------
+// Warp block between two stacked networks (FlowNet2-CSS / FlowNet2): the chain
+//   Resample(LINEAR, up-sampling) -> FlowWarp -> Eltwise(img0 - warped) -> ChannelNorm, and Eltwise(coeff * flow)
+// as ONE pass: one thread per full-resolution pixel computes the interpolated flow, samples the second image, and writes all
+// five tops (most of them channel ranges of the next network's input concat).  Every value comes from the device functions
+// of the stand-alone kernels above (ResampleWindow<2> without antialias on channels 0-1, warp_taps / warp_group /
+// warp_channel, eltwise_term with coefficients (1, -1) resp. (coeff), norm_term), so the tops are bit-identical to the layer
+// chain's.  F4: every image1 pixel is one float4 group (px_one_group).
+// ---------------------------------------------------------------------------------------------
+template <bool F4>
+__global__ void warp_block_kernel(T4 fin, T4 img0, T4 img1, T4 ffull, T4 warped, T4 err, T4 errn, T4 fscaled, float fx, float fy,
+                                  float coeff, float fill) {
+    for_each_pixel(ffull.n, ffull.h, ffull.w, [&](int n, int y, int x) {
+        const ResampleWindow<2> win(resample_src(x, fx, fy), resample_src(y, fy, fx), fx, fy, 0);
+        float f[4] = {0.f, 0.f, 0.f, 0.f};
+        const float wsum = win.accumulate(fin, n, 0, 2, f);
+#pragma unroll
+        for (int c = 0; c < 2; c++) {
+            f[c] = ResampleWindow<2>::value(f[c], wsum);
+            ffull.p[ffull.off(n, c, y, x)] = f[c];
+            fscaled.p[fscaled.off(n, c, y, x)] = eltwise_term(0.f, coeff, f[c]);
+        }
+        const WarpTaps t = warp_taps(img1, n, y, x, f[0], f[1]);
+        float wv[4] = {fill, fill, fill, fill};
+        if (t.inside && F4) warp_group(t, img1, wv);
+        if (t.inside && !F4) {
+#pragma unroll
+            for (int c = 0; c < 4; c++)
+                if (c < img1.c) wv[c] = warp_channel(t, img1, c);
+        }
+        float norm = 0;
+#pragma unroll
+        for (int c = 0; c < 4; c++) {
+            if (c >= img1.c) break;
+            warped.p[warped.off(n, c, y, x)] = wv[c];
+            const float e = eltwise_term(eltwise_term(0.f, 1.0f, img0.p[img0.off(n, c, y, x)]), -1.0f, wv[c]);
+            err.p[err.off(n, c, y, x)] = e;
+            norm = norm_term(norm, e);
+        }
+        errn.p[errn.off(n, 0, y, x)] = sqrtf(norm);
+    });
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -333,12 +298,7 @@ __global__ void resample_kernel(T4 in, T4 out, float fx, float fy, int antialias
 __device__ __forceinline__ float clampf(float f, float a, float b) { return fmaxf(a, fminf(f, b)); }
 
 __global__ void spatial_aug_kernel(T4 src, T4 dst, const float* __restrict__ mats) {
-    const long long total = (long long)dst.n * dst.h * dst.w;
-    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
-         idx += (long long)gridDim.x * blockDim.x) {
-        const int x = (int)(idx % dst.w);
-        const int y = (int)((idx / dst.w) % dst.h);
-        const int n = (int)(idx / ((long long)dst.w * dst.h));
+    for_each_pixel(dst.n, dst.h, dst.w, [&](int n, int y, int x) {
         const float* m = mats + 6 * n;
         float xpos = (x * m[0] + y * m[2]) + m[4];
         float ypos = (x * m[1] + y * m[3]) + m[5];
@@ -359,17 +319,12 @@ __global__ void spatial_aug_kernel(T4 src, T4 dst, const float* __restrict__ mat
             // term order TL, BR, BL, TR (data_augmentation_layer.cu:62-65)
             dst.p[dst.off(n, c, y, x)] = ((cTL * TL + cBR * BR) + cBL * BL) + cTR * TR;
         }
-    }
+    });
 }
 
 // ColorContrastAugmentation: data_augmentation_layer.cu:73-117 (in place, 3 channels).
 __global__ void color_contrast_kernel(T4 d, const float* __restrict__ chroma, float max_multiplier) {
-    const long long total = (long long)d.n * d.h * d.w;
-    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
-         idx += (long long)gridDim.x * blockDim.x) {
-        const int x = (int)(idx % d.w);
-        const int y = (int)((idx / d.w) % d.h);
-        const int n = (int)(idx / ((long long)d.w * d.h));
+    for_each_pixel(d.n, d.h, d.w, [&](int n, int y, int x) {
         const float* ch = chroma + 6 * n;
         float rgb[3];
         float mean_in = 0, mean_out = 0;
@@ -387,23 +342,18 @@ __global__ void color_contrast_kernel(T4 d, const float* __restrict__ chroma, fl
             v = 0.5f + (v - 0.5f) * ch[2];
             d.p[d.off(n, c, y, x)] = clampf(v, 0.f, max_multiplier);
         }
-    }
+    });
 }
 
-// Running mean update: data_augmentation_layer.cu:600-607 (scal, axpy per sample, scal).
+// Running mean update: data_augmentation_layer.cu:600-607 (scal, axpy per sample, scal).  One thread per (c, y, x).
 __global__ void mean_update_kernel(T4 top, T4 mean, float num_iter) {
-    const long long total = (long long)top.c * top.h * top.w;
-    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
-         idx += (long long)gridDim.x * blockDim.x) {
-        const int x = (int)(idx % top.w);
-        const int y = (int)((idx / top.w) % top.h);
-        const int c = (int)(idx / ((long long)top.w * top.h));
+    for_each_pixel(top.c, top.h, top.w, [&](int c, int y, int x) {
         float* mp = mean.p + mean.off(0, c, y, x);
         float m = *mp * (num_iter - 1.0f);
         const float inv = 1.0f / (float)top.n;
         for (int n = 0; n < top.n; n++) m = m + inv * top.p[top.off(n, c, y, x)];
         *mp = m * (1.0f / num_iter);
-    }
+    });
 }
 // Per-channel average of the mean image (caffe_gpu_gemv with ones, :608); one CTA per channel,
 // double accumulation (the cuBLAS order is unpinned).
@@ -424,45 +374,11 @@ __global__ void mean_per_channel_kernel(T4 mean, float* __restrict__ mean_pc) {
 }
 // Mean subtraction :610-634.
 __global__ void mean_subtract_kernel(T4 top, T4 mean, const float* __restrict__ mean_pc, int per_pixel) {
-    const long long total = top.count();
-    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
-         idx += (long long)gridDim.x * blockDim.x) {
-        const int x = (int)(idx % top.w);
-        long long r = idx / top.w;
-        const int c = (int)(r % top.c); r /= top.c;
-        const int y = (int)(r % top.h);
-        const int n = (int)(r / top.h);
-        const float m = per_pixel ? mean.p[mean.off(0, c, y, x)] : mean_pc[c];
-        float* t = top.p + top.off(n, c, y, x);
+    for_each_element(top, [&](Idx4 e, long long) {
+        const float m = per_pixel ? mean.p[mean.off(0, e.c, e.y, e.x)] : mean_pc[e.c];
+        float* t = top.p + top.off(e.n, e.c, e.y, e.x);
         *t = *t - m;
-    }
-}
-
-// ---------------------------------------------------------------------------------------------
-// Glue.
-// ---------------------------------------------------------------------------------------------
-// ChannelNorm: channel_norm_layer.cu:17-30.
-__global__ void channel_norm_kernel(T4 in, T4 out, int vec4) {
-    const long long total = (long long)in.n * in.h * in.w;
-    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
-         idx += (long long)gridDim.x * blockDim.x) {
-        const int x = (int)(idx % in.w);
-        const int y = (int)((idx / in.w) % in.h);
-        const int n = (int)(idx / ((long long)in.w * in.h));
-        float norm = 0;
-        if (vec4) {
-            const float4 q = *reinterpret_cast<const float4*>(in.p + in.off(n, 0, y, x));
-            const float v[4] = {q.x, q.y, q.z, q.w};
-#pragma unroll
-            for (int c = 0; c < 4; c++) if (c < in.c) norm = norm + v[c] * v[c];
-        } else {
-            for (int c = 0; c < in.c; c++) {
-                const float v = in.p[in.off(n, c, y, x)];
-                norm = norm + v * v;
-            }
-        }
-        out.p[out.off(n, 0, y, x)] = sqrtf(norm);
-    }
+    });
 }
 
 // Tiled transpose copy between a channel-planar side and a channel-fast side: 32 pixels x 32
@@ -577,7 +493,7 @@ struct EltwiseSumOp {                             // zero, then acc + coeff * b 
         float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
         for (int i = 0; i < nb; i++) {
             const float k = coeff[i];
-            acc = lanes([k](float a, float v) { return a + k * v; }, acc, at.load(b[i]));
+            acc = lanes([k](float a, float v) { return eltwise_term(a, k, v); }, acc, at.load(b[i]));
         }
         at.store(out, acc);
     }
@@ -624,17 +540,11 @@ template <class Op>
 static int ew_run(const Op& op, const T4& dst, std::initializer_list<T4> srcs, void* stream) {
     bool group = dst.is_nhwc(), f4 = dst.c % 4 == 0 && dst.px_float4_groups();
     for (const T4& s : srcs) { group = group && s.is_nhwc(); f4 = f4 && s.px_float4_groups(); }
-    cudaStream_t st = (cudaStream_t)stream;
-    if (group) {
-        const long long pixels = (long long)dst.n * dst.h * dst.w;
-        const int G = (dst.c + 3) / 4;
-        if (f4) ew_group_kernel<true><<<ew_grid(pixels * G, 256), 256, 0, st>>>(op, pixels, G);
-        else ew_group_kernel<false><<<ew_grid(pixels * G, 256), 256, 0, st>>>(op, pixels, G);
-    } else {
-        ew_strided_kernel<<<ew_grid(dst.count(), 256), 256, 0, st>>>(op, dst);
-    }
-    FN2_LAUNCH_CHECK();
-    return FN2_OK;
+    if (!group) return ew_launch(ew_strided_kernel<Op>, dst.count(), stream, op, dst);
+    const long long pixels = (long long)dst.n * dst.h * dst.w;
+    const int G = (dst.c + 3) / 4;
+    return f4 ? ew_launch(ew_group_kernel<true, Op>, pixels * G, stream, op, pixels, G)
+              : ew_launch(ew_group_kernel<false, Op>, pixels * G, stream, op, pixels, G);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -668,14 +578,10 @@ __global__ void eigenspace_init_kernel(float* space, const float* eigvec9) {
     if (i < 3) reinterpret_cast<double*>(space + 26)[i] = 0.0;
 }
 __global__ void eigenspace_stats_kernel(T4 d, float* space) {
-    const long long total = (long long)d.n * d.h * d.w;
     const float* ev = space + 16;
     float mx_eig[3] = {0, 0, 0}, mx[3] = {0, 0, 0}, mn[3] = {FLT_MAX, FLT_MAX, FLT_MAX};
     double sum[3] = {0, 0, 0};
-    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
-        const int x = (int)(idx % d.w);
-        const int y = (int)((idx / d.w) % d.h);
-        const int n = (int)(idx / ((long long)d.w * d.h));
+    for_each_pixel(d.n, d.h, d.w, [&](int n, int y, int x) {
         float rgb[3];
         for (int c = 0; c < 3; c++) rgb[c] = d.p[d.off(n, c, y, x)];
         for (int c = 0; c < 3; c++) {
@@ -685,7 +591,7 @@ __global__ void eigenspace_stats_kernel(T4 d, float* space) {
             mn[c] = fminf(mn[c], rgb[c]);
             sum[c] += rgb[c];
         }
-    }
+    });
     for (int c = 0; c < 3; c++) {
         for (int o = 16; o > 0; o >>= 1) {
             mx_eig[c] = fmaxf(mx_eig[c], __shfl_xor_sync(0xffffffffu, mx_eig[c], o));
@@ -717,13 +623,9 @@ __global__ void eigenspace_finish_kernel(float* space, int num, int height, int 
     space[15] = sqrtf(max_abs_eig[0] * max_abs_eig[0] + max_abs_eig[1] * max_abs_eig[1] + max_abs_eig[2] * max_abs_eig[2]);
 }
 __global__ void chromatic_eigen_kernel(T4 d, const float* __restrict__ coeffs, const float* __restrict__ space, float max_multiplier) {
-    const long long total = (long long)d.n * d.h * d.w;
     const float* mean_eig = space, *mean_rgb = space + 3, *max_abs_eig = space + 6, *eigvec = space + 16;
     const float max_l = space[15];
-    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
-        const int x = (int)(idx % d.w);
-        const int y = (int)((idx / d.w) % d.h);
-        const int n = (int)(idx / ((long long)d.w * d.h));
+    for_each_pixel(d.n, d.h, d.w, [&](int n, int y, int x) {
         const float* ch = coeffs + 22 * n;
         float s, s1, l, l1 = 0.f;
         float rgb[3], eig[3];
@@ -779,14 +681,10 @@ __global__ void chromatic_eigen_kernel(T4 d, const float* __restrict__ coeffs, c
             v = fmaxf(v, 0.f);
             d.p[d.off(n, c, y, x)] = v;
         }
-    }
+    });
 }
 __global__ void apply_effects_kernel(T4 d, const float* __restrict__ effects, float max_multiplier) {
-    const long long total = (long long)d.n * d.h * d.w;
-    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
-        const int x = (int)(idx % d.w);
-        const int y = (int)((idx / d.w) % d.h);
-        const int n = (int)(idx / ((long long)d.w * d.h));
+    for_each_pixel(d.n, d.h, d.w, [&](int n, int y, int x) {
         const float* e = effects + 9 * n;
         const bool shadow = (x - d.w / 2) * e[4] + (y - d.h / 2) * e[5] - e[6] > 0;
         for (int c = 0; c < d.c; c++) {
@@ -794,7 +692,7 @@ __global__ void apply_effects_kernel(T4 d, const float* __restrict__ effects, fl
             if (shadow) sample -= e[7];
             d.p[d.off(n, c, y, x)] = clampf(sample, 0.f, max_multiplier);
         }
-    }
+    });
 }
 // counter-based generator (SplitMix64 of (seed, element index)) + Box-Muller.  The reference draws from cuRAND's default
 // generator with an unpinned seed/offset: the noise field is not reproducible there either, only its distribution.
@@ -805,22 +703,26 @@ __device__ __forceinline__ unsigned long long splitmix64(unsigned long long z) {
     return z ^ (z >> 31);
 }
 __global__ void gaussian_noise_kernel(T4 d, const float* __restrict__ effects, unsigned long long seed) {
-    const long long total = d.count();
-    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
-        const int x = (int)(idx % d.w);
-        long long r = idx / d.w;
-        const int y = (int)(r % d.h); r /= d.h;
-        const int c = (int)(r % d.c);
-        const int n = (int)(r / d.c);
-        const float sigma = effects[9 * n + 8];
-        if (!(sigma > 0)) continue;
+    for_each_element(d, [&](Idx4 e, long long idx) {
+        const float sigma = effects[9 * e.n + 8];
+        if (!(sigma > 0)) return;
         const unsigned long long h = splitmix64(seed ^ splitmix64((unsigned long long)idx));
         const float u1 = ((float)(h >> 40) + 1.0f) * (1.0f / 16777216.0f);                 // (0, 1]
         const float u2 = (float)((h >> 16) & 0xffffff) * (1.0f / 16777216.0f);
         const float g = sqrtf(-2.0f * logf(u1)) * cosf(6.28318530718f * u2);
-        d.p[d.off(n, c, y, x)] = d.p[d.off(n, c, y, x)] + sigma * g;
-    }
+        float* p = d.p + d.off(e.n, e.c, e.y, e.x);
+        *p = *p + sigma * g;
+    });
 }
+
+// 0xFFE00000, the reference GPU's NaN pattern (flow_warp_layer.cu:372-375), if fill_nan, else 0: FlowWarp's value outside the image
+static float warp_fill(int fill_nan) {
+    float fill = 0.f;
+    if (fill_nan) { unsigned u = 0xFFE00000u; memcpy(&fill, &u, 4); }
+    return fill;
+}
+// The F4 route of FlowWarp, ChannelNorm and the warp block: every pixel of t (c <= 4) is one 16-byte float4 group.
+static bool px_one_group(const T4& t) { return t.c <= 4 && t.px_float4_groups(); }
 
 }  // namespace fn2
 
@@ -836,14 +738,10 @@ int fn2_flow_warp_forward(const fn2_tensor* image, const fn2_tensor* flow, const
     FN2_CHECK_ARG(fl.n == img.n && fl.h == img.h && fl.w == img.w,
                   "flow_warp: flow dims must match image (flow_warp_layer.cpp:45-48)");
     FN2_CHECK_ARG(same_dims(img, out), "flow_warp: top must have the image's shape");
-    // 0xFFE00000 is the reference GPU NaN pattern (flow_warp_layer.cu:372-375)
-    float fill = 0.f;
-    if (fill_nan) { unsigned u = 0xFFE00000u; memcpy(&fill, &u, 4); }
+    const float fill = warp_fill(fill_nan);
     const long long total = (long long)out.n * out.h * out.w;
-    const int vec4 = img.c <= 4 && img.px_float4_groups();
-    flow_warp_fwd_kernel<<<ew_grid(total, 256), 256, 0, (cudaStream_t)stream>>>(img, fl, out, fill, vec4);
-    FN2_LAUNCH_CHECK();
-    return FN2_OK;
+    return px_one_group(img) ? ew_launch(flow_warp_fwd_kernel<true>, total, stream, img, fl, out, fill)
+                             : ew_launch(flow_warp_fwd_kernel<false>, total, stream, img, fl, out, fill);
 }
 
 int fn2_flow_warp_backward(const fn2_tensor* image, const fn2_tensor* flow,
@@ -856,10 +754,7 @@ int fn2_flow_warp_backward(const fn2_tensor* image, const fn2_tensor* flow,
                   "flow_warp_backward: shape mismatch");
     const int rc = fn2_fill(image_diff, 0.f, stream);
     if (rc) return rc;
-    const long long total = (long long)img.n * img.h * img.w;
-    flow_warp_bwd_kernel<<<ew_grid(total, 256), 256, 0, (cudaStream_t)stream>>>(img, fl, wd, id, fd);
-    FN2_LAUNCH_CHECK();
-    return FN2_OK;
+    return ew_launch(flow_warp_bwd_kernel, (long long)img.n * img.h * img.w, stream, img, fl, wd, id, fd);
 }
 
 int fn2_resample_forward(const fn2_tensor* bottom, const fn2_tensor* top, int type, int antialias,
@@ -872,14 +767,12 @@ int fn2_resample_forward(const fn2_tensor* bottom, const fn2_tensor* top, int ty
     const float fy = (float)in.h / (float)out.h;
     const int isDown = (fx > 1) || (fy > 1);
     const int aa = isDown && antialias;
-    const int grid = ew_grid((long long)out.n * out.h * out.w, 256);
-    cudaStream_t s = (cudaStream_t)stream;
-    if (type == 1) resample_kernel<1><<<grid, 256, 0, s>>>(in, out, fx, fy, aa);
-    else if (type == 2) resample_kernel<2><<<grid, 256, 0, s>>>(in, out, fx, fy, aa);
-    else if (type == 3) resample_kernel<3><<<grid, 256, 0, s>>>(in, out, fx, fy, aa);
-    else { set_error("resample: unsupported type %d (resample_layer.cu:204)", type); return FN2_ERR_INVALID; }
-    FN2_LAUNCH_CHECK();
-    return FN2_OK;
+    const long long total = (long long)out.n * out.h * out.w;
+    if (type == 1) return ew_launch(resample_kernel<1>, total, stream, in, out, fx, fy, aa);
+    if (type == 2) return ew_launch(resample_kernel<2>, total, stream, in, out, fx, fy, aa);
+    if (type == 3) return ew_launch(resample_kernel<3>, total, stream, in, out, fx, fy, aa);
+    set_error("resample: unsupported type %d (resample_layer.cu:204)", type);
+    return FN2_ERR_INVALID;
 }
 
 int fn2_warp_block_forward(const fn2_tensor* flow_in, const fn2_tensor* image0, const fn2_tensor* image1, const fn2_tensor* flow_full,
@@ -894,13 +787,10 @@ int fn2_warp_block_forward(const fn2_tensor* flow_in, const fn2_tensor* image0, 
                   en.n == i0.n && en.h == i0.h && en.w == i0.w && fin.n == ff.n, "warp_block: shape mismatch");
     const float fx = (float)fin.w / (float)ff.w, fy = (float)fin.h / (float)ff.h;
     FN2_CHECK_ARG(fx <= 1.f && fy <= 1.f, "warp_block: the flow must be up-sampled (use the layer chain otherwise)");
-    float fill = 0.f;
-    if (fill_nan) { unsigned u = 0xFFE00000u; memcpy(&fill, &u, 4); }
-    const int vec4 = i1.px_float4_groups();           // i1.c <= 4, checked above
+    const float fill = warp_fill(fill_nan);
     const long long total = (long long)ff.n * ff.h * ff.w;
-    warp_block_kernel<<<ew_grid(total, 256), 256, 0, (cudaStream_t)stream>>>(fin, i0, i1, ff, wp, er, en, fs, fx, fy, scale_coeff, fill, vec4);
-    FN2_LAUNCH_CHECK();
-    return FN2_OK;
+    return px_one_group(i1) ? ew_launch(warp_block_kernel<true>, total, stream, fin, i0, i1, ff, wp, er, en, fs, fx, fy, scale_coeff, fill)
+                            : ew_launch(warp_block_kernel<false>, total, stream, fin, i0, i1, ff, wp, er, en, fs, fx, fy, scale_coeff, fill);
 }
 
 int fn2_spatial_augmentation(const fn2_tensor* bottom, const fn2_tensor* top,
@@ -909,10 +799,7 @@ int fn2_spatial_augmentation(const fn2_tensor* bottom, const fn2_tensor* top,
     T4 in = view(bottom), out = view(top);
     FN2_CHECK_ARG(in.n == out.n && in.c == out.c, "spatial_augmentation: num/channels must match");
     FN2_CHECK_ARG(in.w >= 2 && in.h >= 2, "spatial_augmentation: bottom must be at least 2x2");
-    const long long total = (long long)out.n * out.h * out.w;
-    spatial_aug_kernel<<<ew_grid(total, 256), 256, 0, (cudaStream_t)stream>>>(in, out, trans_mats_dev);
-    FN2_LAUNCH_CHECK();
-    return FN2_OK;
+    return ew_launch(spatial_aug_kernel, (long long)out.n * out.h * out.w, stream, in, out, trans_mats_dev);
 }
 
 int fn2_color_contrast_augmentation(const fn2_tensor* data, const float* chroma_dev,
@@ -921,10 +808,7 @@ int fn2_color_contrast_augmentation(const fn2_tensor* data, const float* chroma_
     T4 d = view(data);
     FN2_CHECK_ARG(d.c == 3, "Chromatic augmentations only work with 3-channel input "
                             "(data_augmentation_layer.cu:561)");
-    const long long total = (long long)d.n * d.h * d.w;
-    color_contrast_kernel<<<ew_grid(total, 256), 256, 0, (cudaStream_t)stream>>>(d, chroma_dev, max_multiplier);
-    FN2_LAUNCH_CHECK();
-    return FN2_OK;
+    return ew_launch(color_contrast_kernel, (long long)d.n * d.h * d.w, stream, d, chroma_dev, max_multiplier);
 }
 
 int fn2_mean_update(const fn2_tensor* top, const fn2_tensor* mean_pp, float* mean_pc_dev,
@@ -933,9 +817,8 @@ int fn2_mean_update(const fn2_tensor* top, const fn2_tensor* mean_pp, float* mea
     T4 t = view(top), m = view(mean_pp);
     FN2_CHECK_ARG(m.n == 1 && m.c == t.c && m.h == t.h && m.w == t.w,
                   "mean_update: mean blob must be (1,C,H,W) (data_augmentation_layer.cu:603)");
-    const long long total = (long long)t.c * t.h * t.w;
-    mean_update_kernel<<<ew_grid(total, 256), 256, 0, (cudaStream_t)stream>>>(t, m, num_iter);
-    FN2_LAUNCH_CHECK();
+    const int rc = ew_launch(mean_update_kernel, (long long)t.c * t.h * t.w, stream, t, m, num_iter);
+    if (rc) return rc;
     mean_per_channel_kernel<<<t.c, 256, 0, (cudaStream_t)stream>>>(m, mean_pc_dev);
     FN2_LAUNCH_CHECK();
     return FN2_OK;
@@ -952,9 +835,7 @@ int fn2_mean_subtract(const fn2_tensor* top, const fn2_tensor* mean_pp, const fl
     } else {
         FN2_CHECK_ARG(mean_pc_dev, "mean_subtract: per-channel mean missing");
     }
-    mean_subtract_kernel<<<ew_grid(t.count(), 256), 256, 0, (cudaStream_t)stream>>>(t, m, mean_pc_dev, per_pixel);
-    FN2_LAUNCH_CHECK();
-    return FN2_OK;
+    return ew_launch(mean_subtract_kernel, t.count(), stream, t, m, mean_pc_dev, per_pixel);
 }
 
 int fn2_relu_forward(const fn2_tensor* bottom, const fn2_tensor* top, float negative_slope, void* stream) {
@@ -1003,10 +884,8 @@ int fn2_channel_norm_forward(const fn2_tensor* bottom, const fn2_tensor* top, vo
     FN2_CHECK_ARG(out.c == 1 && out.n == in.n && out.h == in.h && out.w == in.w,
                   "channel_norm: top must be (N,1,H,W) (channel_norm_layer.cpp:29)");
     const long long total = (long long)in.n * in.h * in.w;
-    const int vec4 = in.c <= 4 && in.px_float4_groups();
-    channel_norm_kernel<<<ew_grid(total, 256), 256, 0, (cudaStream_t)stream>>>(in, out, vec4);
-    FN2_LAUNCH_CHECK();
-    return FN2_OK;
+    return px_one_group(in) ? ew_launch(channel_norm_kernel<true>, total, stream, in, out)
+                            : ew_launch(channel_norm_kernel<false>, total, stream, in, out);
 }
 
 int fn2_copy(const fn2_tensor* src, const fn2_tensor* dst, void* stream) {
@@ -1034,9 +913,8 @@ int fn2_chromatic_eigenspace(const fn2_tensor* data, const float* eigvec9_dev, f
     cudaStream_t st = (cudaStream_t)stream;
     eigenspace_init_kernel<<<1, 32, 0, st>>>(space_dev, eigvec9_dev);
     FN2_LAUNCH_CHECK();
-    const long long total = (long long)d.n * d.h * d.w;
-    eigenspace_stats_kernel<<<ew_grid(total, 256), 256, 0, st>>>(d, space_dev);
-    FN2_LAUNCH_CHECK();
+    const int rc = ew_launch(eigenspace_stats_kernel, (long long)d.n * d.h * d.w, stream, d, space_dev);
+    if (rc) return rc;
     eigenspace_finish_kernel<<<1, 32, 0, st>>>(space_dev, d.n, d.h, d.w);
     FN2_LAUNCH_CHECK();
     return FN2_OK;
@@ -1047,10 +925,7 @@ int fn2_chromatic_eigen_augmentation(const fn2_tensor* data, const float* coeffs
     FN2_CHECK_ARG(valid(data) && coeffs_dev && space_dev, "chromatic_eigen: null argument");
     T4 d = view(data);
     FN2_CHECK_ARG(d.c == 3, "Chromatic-Eigen augmentations only work with 3-channel input (data_augmentation_layer.cu:551)");
-    const long long total = (long long)d.n * d.h * d.w;
-    chromatic_eigen_kernel<<<ew_grid(total, 256), 256, 0, (cudaStream_t)stream>>>(d, coeffs_dev, space_dev, max_multiplier);
-    FN2_LAUNCH_CHECK();
-    return FN2_OK;
+    return ew_launch(chromatic_eigen_kernel, (long long)d.n * d.h * d.w, stream, d, coeffs_dev, space_dev, max_multiplier);
 }
 
 int fn2_apply_effects(const fn2_tensor* data, const float* effects_dev, float max_multiplier, unsigned long long noise_seed,
@@ -1058,14 +933,9 @@ int fn2_apply_effects(const fn2_tensor* data, const float* effects_dev, float ma
     FN2_CHECK_ARG(valid(data) && effects_dev, "apply_effects: null argument");
     T4 d = view(data);
     FN2_CHECK_ARG(d.c == 3, "Effect augmentations only work with 3-channel input (data_augmentation_layer.cu:567)");
-    const long long total = (long long)d.n * d.h * d.w;
-    apply_effects_kernel<<<ew_grid(total, 256), 256, 0, (cudaStream_t)stream>>>(d, effects_dev, max_multiplier);
-    FN2_LAUNCH_CHECK();
-    if (add_noise) {
-        gaussian_noise_kernel<<<ew_grid(d.count(), 256), 256, 0, (cudaStream_t)stream>>>(d, effects_dev, noise_seed);
-        FN2_LAUNCH_CHECK();
-    }
-    return FN2_OK;
+    const int rc = ew_launch(apply_effects_kernel, (long long)d.n * d.h * d.w, stream, d, effects_dev, max_multiplier);
+    if (rc || !add_noise) return rc;
+    return ew_launch(gaussian_noise_kernel, d.count(), stream, d, effects_dev, noise_seed);
 }
 
 int fn2_fill(const fn2_tensor* dst, float value, void* stream) {

@@ -106,8 +106,9 @@ def correlation1d_backward(b0, b1, top_diff, pad, kernel_size, max_displacement,
     return g0, g1
 
 
-def flow_warp(image, flow, fill_nan=False):
-    out = torch.empty_like(image)
+def flow_warp(image, flow, fill_nan=False, out=None):
+    if out is None:
+        out = torch.empty_like(image)
     di, df, do = desc(image), desc(flow), desc(out)
     check(lib().fn2_flow_warp_forward(C.byref(di), C.byref(df), C.byref(do), 1 if fill_nan else 0, _stream()))
     return out
@@ -309,10 +310,32 @@ def eltwise_sum(bottoms, coeffs=None, out=None):
     return out
 
 
-def channel_norm(x):
-    out = torch.empty((x.shape[0], 1, x.shape[2], x.shape[3]), device=x.device, dtype=torch.float32)
+def channel_norm(x, out=None):
+    if out is None:
+        out = torch.empty((x.shape[0], 1, x.shape[2], x.shape[3]), device=x.device, dtype=torch.float32)
     dx, do = desc(x), desc(out)
     check(lib().fn2_channel_norm_forward(C.byref(dx), C.byref(do), _stream()))
+    return out
+
+
+def warp_block(flow, image0, image1, scale_coeff, fill_nan=False, out=None):
+    """The warp block between stacked networks in one pass: flow (N, 2, h, w) up-sampled to the images' size (LINEAR),
+    image1 warped by it, the error image0 - warped, its channel norm and the up-sampled flow times scale_coeff.
+    -> out = (flow_full, warped, err, err_norm, flow_scaled), new tensors if None."""
+    if out is None:
+        N, Cc, H, W = image0.shape
+        out = (_empty((N, 2, H, W), image0), torch.empty_like(image1), torch.empty_like(image0),
+               _empty((N, 1, H, W), image0, False), _empty((N, 2, H, W), image0))
+    ds = [desc(t) for t in (flow, image0, image1) + tuple(out)]
+    check(lib().fn2_warp_block_forward(*[C.byref(d) for d in ds], scale_coeff, 1 if fill_nan else 0, _stream()))
+    return out
+
+
+def downsample(x, top_h, top_w, out=None):
+    if out is None:
+        out = _empty((x.shape[0], x.shape[1], top_h, top_w), x)
+    dx, do = desc(x), desc(out)
+    check(lib().fn2_downsample_forward(C.byref(dx), C.byref(do), _stream()))
     return out
 
 

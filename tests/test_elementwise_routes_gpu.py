@@ -6,14 +6,13 @@ channels_last parent, like a concat child); the strided route runs otherwise (NC
 map, mixed layouts); copy between NCHW and channels_last with C >= 8 runs the transpose.  `test_elementwise_route_kernels`
 checks, with the CUDA profiler, that each case runs its route's kernel.
 """
-import time
 import zlib
 
 import numpy as np
 import pytest
 
 from oracle import oracle as O
-from tests.util import rng
+from tests.util import kernels_per_case, rng
 
 pytestmark = pytest.mark.gpu
 torch = pytest.importorskip("torch")
@@ -157,41 +156,6 @@ def test_axpby_every_coefficient(ops, li):
         got = host(ops.axpby(vx, alpha, vy, beta))
         assert np.array_equal(got, np.float32(alpha) * x + np.float32(beta) * y), (alpha, beta)
         assert outside_kept(parent, idx)
-
-
-def kernels_per_case(runs):
-    """Names of the kernels each of runs launches, from one profiler session.  Every run sits in a window of its own between
-    synchronisations, 2 ms from the next.  A kernel belongs to the window of its launch call (the profiler gives both the
-    same correlation id), else to the window its start falls in or is nearest to (a warm-up run of the first case before
-    the windows lands in that case's).  A session in which some window has no kernel at all (the profiler now and then
-    drops device activity) is taken again."""
-    cpu, cuda = torch.profiler.ProfilerActivity.CPU, torch.profiler.ProfilerActivity.CUDA
-    for _ in range(3):
-        torch.cuda.synchronize()
-        with torch.profiler.profile(activities=[cpu, cuda]) as prof:
-            runs[0]()                                   # the session's first kernels can go unrecorded
-            torch.cuda.synchronize()
-            time.sleep(0.002)
-            for i, run in enumerate(runs):
-                with torch.profiler.record_function("ew_case_%d" % i):
-                    run()
-                    torch.cuda.synchronize()
-                time.sleep(0.002)
-        events = prof.events()
-        win = {int(e.name[8:]): e.time_range for e in events if e.name.startswith("ew_case_")}
-
-        def window(t):
-            return min(win, key=lambda i: max(win[i].start - t, t - win[i].end, 0))
-
-        launch = {e.id: window(e.time_range.start) for e in events
-                  if e.device_type == torch.autograd.DeviceType.CPU and "LaunchKernel" in e.name}
-        names = [set() for _ in runs]
-        for e in events:
-            if e.device_type == torch.autograd.DeviceType.CUDA:
-                names[launch.get(e.id, window(e.time_range.start))].add(e.name)
-        if all(names):
-            break
-    return names
 
 
 def test_elementwise_route_kernels(ops):

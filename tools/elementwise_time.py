@@ -1,4 +1,5 @@
-"""Time the element-wise entry points (fn2_relu_backward, fn2_axpby, fn2_eltwise_sum, fn2_copy) at the shapes FlowNet2 gives them.
+"""Time the element-wise and streaming entry points (fn2_relu_backward, fn2_axpby, fn2_eltwise_sum, fn2_copy, FlowWarp, Resample,
+ChannelNorm, the warp block, Downsample and L1Loss) at the shapes FlowNet2 and its training step give them.
 
 Each case is warmed up, then `--launches` back-to-back calls are captured into one CUDA graph (so that the host's call
 overhead does not hide the kernel), and CUDA events bracket each replay; the median over `--reps` replays is reported per
@@ -9,6 +10,7 @@ FN2_LIB selects the library, so two builds can be compared by alternating runs. 
     python tools/elementwise_time.py [--launches 200] [--reps 5]
 """
 import argparse
+import ctypes as C
 import json
 import os
 import subprocess
@@ -65,6 +67,49 @@ def main():
     cases["copy_nchw_to_nhwc_c3_%dx%d" % (w, h)] = lambda: ops.copy(src3, dst3)
     src2, dst2 = blob(n, 2, h, w), nchw(n, 2, h, w)
     cases["copy_nhwc_to_nchw_c2_%dx%d" % (w, h)] = lambda: ops.copy(src2, dst2)
+    # the warp block between stacked networks and the layers it fuses: flow up-sampled x4 from 109x256, 3-channel images
+    img0, img1, flow = blob(n, 3, h, w), blob(n, 3, h, w), blob(n, 2, h, w)
+    flow.mul_(8.0)
+    small = blob(n, 2, 109, 256)
+    small.mul_(8.0)
+    warped, err, norm, full, scaled = blob(n, 3, h, w), blob(n, 3, h, w), blob(n, 1, h, w), blob(n, 2, h, w), blob(n, 2, h, w)
+    cases["flow_warp_c3_%dx%d" % (w, h)] = lambda: ops.flow_warp(img1, flow, out=warped)
+    cases["resample_flow_256x109_to_%dx%d" % (w, h)] = lambda: ops.resample(small, h, w, 2)
+    cases["resample_image_%dx%d_to_%dx448" % (w, h, w)] = lambda: ops.resample(img0, 448, w, 2)
+    cases["channel_norm_c3_%dx%d" % (w, h)] = lambda: ops.channel_norm(err, out=norm)
+    cases["warp_block_%dx%d" % (w, h)] = lambda: ops.warp_block(small, img0, img1, 0.05, out=(full, warped, err, norm, scaled))
+    # mean subtraction of the 3-channel input images (per pixel and per channel)
+    top, mpp, mpc = nchw(n, 3, h, w), nchw(1, 3, h, w), torch.rand(3, device="cuda", generator=g)
+    cases["mean_subtract_pp_c3_%dx%d" % (w, h)] = lambda: ops.mean_subtract(top, mpp, mpc, True)
+    cases["mean_subtract_pc_c3_%dx%d" % (w, h)] = lambda: ops.mean_subtract(top, None, mpc, False)
+    # FlowNet2-C training step at a 448x320 crop, batch 8: the ground truth's Downsample to each pyramid level, and the
+    # end-point-error L1Loss forward + backward there
+    gt = blob(8, 2, 320, 448)
+    lib = F.lib()
+
+    class L1Desc(C.Structure):
+        _fields_ = [("l2_per_location", C.c_int32), ("l2_prescale_by_channels", C.c_int32), ("normalize_by_num_entries", C.c_int32),
+                    ("epsilon", C.c_float), ("plateau", C.c_float)]
+    epe = L1Desc(1, 0, 0, 0.0, 0.0)
+
+    def l1loss(pred, gtl, diff, ws, nbytes, state, one):
+        dp, dg, dd = ops.desc(pred), ops.desc(gtl), ops.desc(diff)
+        st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+        F.check(lib.fn2_l1loss_forward(C.byref(dp), C.byref(dg), C.byref(epe), C.c_void_p(state.data_ptr()), None,
+                                       C.c_void_p(ws.data_ptr()), C.c_size_t(nbytes), st))
+        F.check(lib.fn2_l1loss_backward(C.byref(dp), C.byref(dg), C.byref(epe), C.c_void_p(state.data_ptr()), C.c_void_p(one.data_ptr()),
+                                        C.byref(dd), None, 0, 0, st))
+
+    for s in (4, 8, 16, 32, 64):
+        th, tw = 320 // s, 448 // s
+        lvl = blob(8, 2, th, tw)
+        cases["downsample_448x320_to_%dx%d" % (tw, th)] = lambda lvl=lvl, th=th, tw=tw: ops.downsample(gt, th, tw, out=lvl)
+        pred, diff = blob(8, 2, th, tw), blob(8, 2, th, tw)
+        nb = C.c_size_t()
+        F.check(lib.fn2_l1loss_workspace_bytes(8, th, tw, C.byref(nb)))
+        ws, state, one = torch.zeros(nb.value, dtype=torch.uint8, device="cuda"), torch.zeros(4, device="cuda"), torch.ones(1, device="cuda")
+        cases["l1loss_epe_fwd_bwd_%dx%d" % (tw, th)] = (lambda pred=pred, lvl=lvl, diff=diff, ws=ws, nb=nb.value, state=state, one=one:
+                                                       l1loss(pred, lvl, diff, ws, nb, state, one))
 
     name, watts = card(torch.cuda.current_device())
     res = {"card": name, "power_limit_w": watts, "lib": F.lib_path(), "launches": args.launches, "us": {}}
