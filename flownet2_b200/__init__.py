@@ -52,6 +52,8 @@ def lib():
         l.fn2_last_error.restype = C.c_char_p
         l.fn2_version.restype = C.c_char_p
         l.fn2_launch_count.restype = C.c_uint64
+        l.fn2_device_allocations.restype = C.c_uint64
+        l.fn2_device_allocations.argtypes = [C.POINTER(C.c_uint64)]
         for name in ("fn2_net_input_name", "fn2_net_output_name", "fn2_net_blob_name", "fn2_net_layer_name",
                      "fn2_net_layer_type"):
             getattr(l, name).restype = C.c_char_p
@@ -130,6 +132,13 @@ def check(rc):
 
 def launch_count():
     return int(lib().fn2_launch_count())
+
+
+def device_allocations():
+    """(allocations made so far, bytes held now) by the net host's device and pinned-host buffers."""
+    live = C.c_uint64()
+    n = lib().fn2_device_allocations(C.byref(live))
+    return int(n), int(live.value)
 
 
 # ------------------------------------------------------------------------------------------------

@@ -1,13 +1,62 @@
 #include "blob.hpp"
 
+#include <algorithm>
+#include <atomic>
 #include <cstring>
 
 namespace caffe {
 
-template <typename Dtype>
-Blob<Dtype>::~Blob() {
-    if (own_dev_ && dev_) cudaFree(dev_ - kGuardFloats);
-    if (ddev_ && own_ddev_) cudaFree(ddev_ - kGuardFloats);
+// ---- DeviceBuffer -----------------------------------------------------------------------------------------------------
+static std::atomic<uint64_t> g_allocations{0}, g_live_bytes{0};
+
+DeviceBuffer& DeviceBuffer::operator=(DeviceBuffer&& o) noexcept {
+    if (this != &o) {
+        release();
+        p_ = o.p_; bytes_ = o.bytes_; pinned_ = o.pinned_;
+        o.p_ = nullptr; o.bytes_ = 0;
+    }
+    return *this;
+}
+
+void DeviceBuffer::release() noexcept {
+    if (!p_) return;
+    if (pinned_) cudaFreeHost(p_);
+    else cudaFree(p_);
+    g_live_bytes -= bytes_;
+    p_ = nullptr; bytes_ = 0;
+}
+
+void DeviceBuffer::reserve(size_t bytes) {
+    if (bytes <= bytes_) return;
+    release();
+    void* p = nullptr;
+    const cudaError_t e = pinned_ ? cudaMallocHost(&p, bytes) : cudaMalloc(&p, bytes);
+    CHECK(e == cudaSuccess) << (pinned_ ? "cudaMallocHost" : "cudaMalloc") << " of " << bytes << " bytes: " << cudaGetErrorString(e);
+    p_ = p; bytes_ = bytes;
+    g_allocations++; g_live_bytes += bytes;
+}
+
+void DeviceBuffer::reserve(size_t bytes, cudaStream_t zero_on) {
+    if (bytes <= bytes_) return;
+    reserve(bytes);
+    CUDA_CHECK(cudaMemsetAsync(p_, 0, bytes, zero_on));
+    CUDA_CHECK(cudaStreamSynchronize(zero_on));
+}
+
+// Copies between a device view and a dense host NCHW array through a dense device temporary (fn2_copy changes the layout).
+static void copy_nchw(const fn2_tensor& view, float* host, cudaMemcpyKind dir, cudaStream_t st) {
+    const size_t bytes = (size_t)view.n * view.c * view.h * view.w * sizeof(float);
+    DeviceBuffer tmp;
+    tmp.reserve(bytes);
+    const fn2_tensor dense = nchw_view(tmp.as<float>(), view.n, view.c, view.h, view.w);
+    if (dir == cudaMemcpyDeviceToHost) {
+        FN2_CALL(fn2_copy(&view, &dense, st));
+        CUDA_CHECK(cudaMemcpyAsync(host, tmp.get(), bytes, dir, st));
+    } else {
+        CUDA_CHECK(cudaMemcpyAsync(tmp.get(), host, bytes, dir, st));
+        FN2_CALL(fn2_copy(&dense, &view, st));
+    }
+    CUDA_CHECK(cudaStreamSynchronize(st));
 }
 
 // ---- gradient storage -------------------------------------------------------------------------------------------------
@@ -17,16 +66,10 @@ fn2_tensor Blob<Dtype>::diff_tensor(int c0, int cn) {
         fn2_tensor pt = parent_->diff_tensor(parent_c0_ + c0, cn < 0 ? channels() - c0 : cn);
         return pt;
     }
-    if (!ddev_ || (own_ddev_ && storage_floats() > ddev_floats_)) {
-        if (ddev_) cudaFree(ddev_ - kGuardFloats);
-        size_t n = storage_floats();
-        if (n == 0) n = 1;
-        ddev_floats_ = n; own_ddev_ = true;
-        Dtype* base = nullptr;
-        CUDA_CHECK(cudaMalloc(&base, (n + 2 * kGuardFloats) * sizeof(Dtype)));
-        CUDA_CHECK(cudaMemsetAsync(base, 0, (n + 2 * kGuardFloats) * sizeof(Dtype), Caffe::stream()));
-        CUDA_CHECK(cudaStreamSynchronize(Caffe::stream()));
-        ddev_ = base + kGuardFloats;
+    if (!ddev_ || !diff_.empty()) {                           // owned storage grows with the blob
+        ddev_ = nullptr;
+        diff_.reserve((std::max<size_t>(storage_floats(), 1) + 2 * kGuardFloats) * sizeof(Dtype), Caffe::stream());
+        ddev_ = diff_.as<Dtype>() + kGuardFloats;
     }
     mutable_gpu_data();                                       // make sure the data view (strides) exists
     Head h = head_;
@@ -39,8 +82,8 @@ fn2_tensor Blob<Dtype>::diff_tensor(int c0, int cn) {
 template <typename Dtype>
 void Blob<Dtype>::BindExternalDiff(Dtype* dev) {
     CHECK(layout_ == PLAIN && !parent_) << "only PLAIN blobs can be bound to the gradient arena";
-    if (ddev_ && own_ddev_) cudaFree(ddev_ - kGuardFloats);
-    ddev_ = dev; own_ddev_ = false; ddev_floats_ = storage_floats();
+    diff_.release();
+    ddev_ = dev;
 }
 
 template <typename Dtype>
@@ -54,36 +97,14 @@ template <typename Dtype>
 const Dtype* Blob<Dtype>::cpu_diff() {
     dhost_.resize((size_t)count_);
     if (count_ == 0) return dhost_.data();
-    cudaStream_t st = Caffe::stream();
-    fn2_tensor src = diff_tensor();
-    Dtype* tmp = nullptr;
-    CUDA_CHECK(cudaMalloc(&tmp, (size_t)count_ * sizeof(Dtype)));
-    fn2_tensor dst = src;
-    dst.data = tmp; dst.sw = 1; dst.sh = width(); dst.sc = (int64_t)height() * width(); dst.sn = (int64_t)channels() * height() * width();
-    int rc = fn2_copy(&src, &dst, st);
-    if (rc == 0) {
-        cudaMemcpyAsync(dhost_.data(), tmp, (size_t)count_ * sizeof(Dtype), cudaMemcpyDeviceToHost, st);
-        cudaStreamSynchronize(st);
-    }
-    cudaFree(tmp);
-    CHECK(rc == 0) << "fn2_copy: " << fn2_last_error();
+    copy_nchw(diff_tensor(), dhost_.data(), cudaMemcpyDeviceToHost, Caffe::stream());
     return dhost_.data();
 }
 
 template <typename Dtype>
 void Blob<Dtype>::set_cpu_diff(const Dtype* host_nchw) {
     if (count_ == 0) return;
-    cudaStream_t st = Caffe::stream();
-    fn2_tensor dst = diff_tensor();
-    Dtype* tmp = nullptr;
-    CUDA_CHECK(cudaMalloc(&tmp, (size_t)count_ * sizeof(Dtype)));
-    cudaMemcpyAsync(tmp, host_nchw, (size_t)count_ * sizeof(Dtype), cudaMemcpyHostToDevice, st);
-    fn2_tensor src = dst;
-    src.data = tmp; src.sw = 1; src.sh = width(); src.sc = (int64_t)height() * width(); src.sn = (int64_t)channels() * height() * width();
-    int rc = fn2_copy(&src, &dst, st);
-    cudaStreamSynchronize(st);
-    cudaFree(tmp);
-    CHECK(rc == 0) << "fn2_copy: " << fn2_last_error();
+    copy_nchw(diff_tensor(), const_cast<Dtype*>(host_nchw), cudaMemcpyHostToDevice, Caffe::stream());
 }
 
 template <typename Dtype>
@@ -104,13 +125,12 @@ void Blob<Dtype>::Reshape(const vector<int>& shape) {
     if (shape == shape_ && count_ == (int)cnt) return;
     CHECK(!parent_) << "cannot reshape an aliased blob";
     // externally bound storage (a slot of the Net's parameter arena, or another blob's buffer) has a fixed size
-    CHECK(own_dev_ || !dev_ || (long long)count_ == cnt)
+    CHECK(!data_.empty() || !dev_ || (long long)count_ == cnt)
         << "cannot reshape a blob bound to external storage to a different count (" << count_ << " -> " << cnt << ")";
     shape_ = shape;
     count_ = (int)cnt;
     cstride_ = compute_cstride();
-    if (own_dev_ && dev_) { cudaFree(dev_ - kGuardFloats); }
-    if (own_dev_ || !dev_) { dev_ = nullptr; own_dev_ = false; }
+    if (!data_.empty()) { data_.release(); dev_ = nullptr; }
     host_.clear();
     head_ = UNINIT;
 }
@@ -145,20 +165,13 @@ void Blob<Dtype>::alloc_device() {
         return;
     }
     if (dev_) return;
-    size_t n = storage_floats();
-    if (n == 0) n = 1;
     // kGuardFloats readable floats on both sides: the small-Ci tensor-core convolution fetches whole kernel rows and
-    // reaches a few pixels outside the tensor at the image corners (those values are masked, never used)
-    Dtype* base = nullptr;
-    CUDA_CHECK(cudaMalloc(&base, (n + 2 * kGuardFloats) * sizeof(Dtype)));
-    // channel padding must read as zero forever (weights for padded channels are zero, but
-    // 0 * NaN would poison the tensor-core path)
-    // stream-ordered: the nets run on non-blocking streams, a legacy-stream memset could land AFTER the first kernel
-    // that writes the blob
-    CUDA_CHECK(cudaMemsetAsync(base, 0, (n + 2 * kGuardFloats) * sizeof(Dtype), Caffe::stream()));
-    CUDA_CHECK(cudaStreamSynchronize(Caffe::stream()));
-    dev_ = base + kGuardFloats;
-    own_dev_ = true;
+    // reaches a few pixels outside the tensor at the image corners (those values are masked, never used).
+    // Zeroed because channel padding must read as zero forever (weights for padded channels are zero, but 0 * NaN would
+    // poison the tensor-core path); stream-ordered, because the nets run on non-blocking streams and a legacy-stream memset
+    // could land AFTER the first kernel that writes the blob
+    data_.reserve((std::max<size_t>(storage_floats(), 1) + 2 * kGuardFloats) * sizeof(Dtype), Caffe::stream());
+    dev_ = data_.as<Dtype>() + kGuardFloats;
 }
 
 template <typename Dtype>
@@ -203,21 +216,10 @@ void Blob<Dtype>::to_cpu() {
         CUDA_CHECK(cudaMemcpyAsync(host_.data(), dev_, (size_t)count_ * sizeof(Dtype), cudaMemcpyDeviceToHost, st));
         CUDA_CHECK(cudaStreamSynchronize(st));
     } else {
-        Dtype* tmp = nullptr;
-        CUDA_CHECK(cudaMalloc(&tmp, (size_t)count_ * sizeof(Dtype)));
         Head h = head_;
         fn2_tensor src = mutable_tensor();
         head_ = h;
-        fn2_tensor dst = src;
-        dst.data = tmp; dst.sw = 1; dst.sh = width(); dst.sc = (int64_t)height() * width();
-        dst.sn = (int64_t)channels() * height() * width();
-        int rc = fn2_copy(&src, &dst, st);
-        if (rc == 0) {
-            cudaMemcpyAsync(host_.data(), tmp, (size_t)count_ * sizeof(Dtype), cudaMemcpyDeviceToHost, st);
-            cudaStreamSynchronize(st);
-        }
-        cudaFree(tmp);
-        CHECK(rc == 0) << "fn2_copy: " << fn2_last_error();
+        copy_nchw(src, host_.data(), cudaMemcpyDeviceToHost, st);
     }
     head_ = SYNCED;
 }
@@ -226,9 +228,6 @@ template <typename Dtype>
 void Blob<Dtype>::to_gpu() {
     if (head_ == UNINIT) {
         alloc_device();
-        if (parent_ || !own_dev_) {
-            // aliased / externally bound storage is not zeroed by alloc_device
-        }
         head_ = AT_GPU;
         return;
     }
@@ -240,18 +239,8 @@ void Blob<Dtype>::to_gpu() {
         CUDA_CHECK(cudaMemcpyAsync(dev_, host_.data(), (size_t)count_ * sizeof(Dtype), cudaMemcpyHostToDevice, st));
         CUDA_CHECK(cudaStreamSynchronize(st));
     } else {
-        Dtype* tmp = nullptr;
-        CUDA_CHECK(cudaMalloc(&tmp, (size_t)count_ * sizeof(Dtype)));
-        cudaMemcpyAsync(tmp, host_.data(), (size_t)count_ * sizeof(Dtype), cudaMemcpyHostToDevice, st);
         head_ = SYNCED;
-        fn2_tensor dst = mutable_tensor();
-        fn2_tensor src = dst;
-        src.data = tmp; src.sw = 1; src.sh = width(); src.sc = (int64_t)height() * width();
-        src.sn = (int64_t)channels() * height() * width();
-        int rc = fn2_copy(&src, &dst, st);
-        cudaStreamSynchronize(st);
-        cudaFree(tmp);
-        CHECK(rc == 0) << "fn2_copy: " << fn2_last_error();
+        copy_nchw(mutable_tensor(), host_.data(), cudaMemcpyHostToDevice, st);
     }
     head_ = SYNCED;
 }
@@ -283,11 +272,11 @@ Dtype* Blob<Dtype>::mutable_gpu_data() {
 template <typename Dtype>
 void Blob<Dtype>::AliasInto(Blob* parent, int c0) {
     CHECK(parent && parent->layout_ == NHWC && layout_ == NHWC) << "aliasing needs NHWC blobs";
-    CHECK(!dev_ || !own_dev_ || head_ == UNINIT) << "blob already has device data";
+    CHECK(data_.empty() || head_ == UNINIT) << "blob already has device data";
     CHECK(num() == parent->num() && height() == parent->height() && width() == parent->width());
     CHECK(c0 >= 0 && c0 + channels() <= parent->channels());
-    if (own_dev_ && dev_) cudaFree(dev_ - kGuardFloats);
-    dev_ = nullptr; own_dev_ = false;
+    data_.release();
+    dev_ = nullptr;
     parent_ = parent;
     parent_c0_ = c0;
     cstride_ = parent->cstride_;
@@ -297,8 +286,8 @@ template <typename Dtype>
 void Blob<Dtype>::BindExternal(Dtype* dev) {
     CHECK(layout_ == PLAIN && !parent_) << "only PLAIN blobs can be bound to the parameter arena";
     const Dtype* h = cpu_data();           // bring current contents to the host
-    if (own_dev_ && dev_) cudaFree(dev_ - kGuardFloats);
-    dev_ = dev; own_dev_ = false;
+    data_.release();
+    dev_ = dev;
     if (count_) CUDA_CHECK(cudaMemcpy(dev_, h, (size_t)count_ * sizeof(Dtype), cudaMemcpyHostToDevice));
     head_ = SYNCED;
 }
@@ -313,8 +302,8 @@ void Blob<Dtype>::ShareData(Blob& other) {
     CHECK_EQ(count_, other.count_);
     CHECK(layout_ == other.layout_);
     other.gpu_data();
-    if (own_dev_ && dev_) cudaFree(dev_ - kGuardFloats);
-    dev_ = other.dev_; own_dev_ = false;
+    data_.release();
+    dev_ = other.dev_;
     cstride_ = other.cstride_;
     head_ = AT_GPU;
 }
@@ -346,3 +335,8 @@ void Blob<Dtype>::ToProto(BlobProtoData* p) {
 template class Blob<float>;
 
 }  // namespace caffe
+
+uint64_t fn2_device_allocations(uint64_t* live_bytes) {
+    if (live_bytes) *live_bytes = caffe::g_live_bytes;
+    return caffe::g_allocations;
+}

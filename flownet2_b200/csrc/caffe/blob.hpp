@@ -19,7 +19,6 @@ class Blob {
     enum Layout { PLAIN = 0, NHWC = 1 };
     Blob() {}
     explicit Blob(int n, int c, int h, int w) { Reshape(n, c, h, w); }
-    ~Blob();
     Blob(const Blob&) = delete;
     Blob& operator=(const Blob&) = delete;
 
@@ -92,11 +91,12 @@ class Blob {
     int cstride_ = 0;             // pixel stride (floats) for NHWC
     Head head_ = UNINIT;
     vector<Dtype> host_;
+    // dev_ / ddev_ point kGuardFloats into data_ / diff_ while those own the storage (non-empty); aliased, arena-bound and
+    // shared storage is a plain pointer with the buffer empty
     Dtype* dev_ = nullptr;
-    bool own_dev_ = false;
-    Dtype* ddev_ = nullptr;       // gradient storage (owned unless aliased or bound to the gradient arena)
-    bool own_ddev_ = false;
-    size_t ddev_floats_ = 0;
+    DeviceBuffer data_;
+    Dtype* ddev_ = nullptr;       // gradient storage
+    DeviceBuffer diff_;
     vector<Dtype> dhost_;
     Blob* parent_ = nullptr;      // alias target
     int parent_c0_ = 0;

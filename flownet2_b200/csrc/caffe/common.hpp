@@ -58,4 +58,39 @@ class Caffe {
     static uint64_t& seed() { static thread_local uint64_t s = 1701; return s; }
 };
 
+// The one owner of host-side CUDA allocations: a cudaMalloc block (or a pinned cudaMallocHost block), freed with the
+// object.  reserve() only grows, and frees the old block before it allocates the new one, so peak memory never holds both;
+// a failed allocation leaves the buffer empty.  Every allocation is counted process-wide (fn2_device_allocations).
+class DeviceBuffer {
+ public:
+    enum Memory { DEVICE, PINNED_HOST };
+    explicit DeviceBuffer(Memory m = DEVICE) : pinned_(m == PINNED_HOST) {}
+    ~DeviceBuffer() { release(); }
+    DeviceBuffer(DeviceBuffer&& o) noexcept : p_(o.p_), bytes_(o.bytes_), pinned_(o.pinned_) { o.p_ = nullptr; o.bytes_ = 0; }
+    DeviceBuffer& operator=(DeviceBuffer&& o) noexcept;
+    DeviceBuffer(const DeviceBuffer&) = delete;
+    DeviceBuffer& operator=(const DeviceBuffer&) = delete;
+
+    void reserve(size_t bytes);
+    void reserve(size_t bytes, cudaStream_t zero_on);   // a new block is cleared on `zero_on`, which is then synchronised
+    void release() noexcept;
+    void* get() const { return p_; }
+    template <typename T> T* as() const { return static_cast<T*>(p_); }
+    size_t bytes() const { return bytes_; }
+    bool empty() const { return p_ == nullptr; }
+
+ private:
+    void* p_ = nullptr;
+    size_t bytes_ = 0;
+    bool pinned_;
+};
+
+// Dense NCHW view of n x c x h x w floats at p
+inline fn2_tensor nchw_view(float* p, int n, int c, int h, int w) {
+    fn2_tensor t;
+    t.data = p; t.n = n; t.c = c; t.h = h; t.w = w;
+    t.sw = 1; t.sh = w; t.sc = (int64_t)h * w; t.sn = (int64_t)c * h * w;
+    return t;
+}
+
 }  // namespace caffe

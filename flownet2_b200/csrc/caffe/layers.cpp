@@ -17,6 +17,29 @@ typedef Blob<float> BlobF;
 
 static cudaStream_t S() { return Caffe::stream(); }
 
+// A kernel that overwrites its output cannot write into a bottom diff that already holds another consumer's contribution
+// (Net::PlanBackward's accumulate flag): such a bottom gets a scratch diff blob, which is then added in.
+template <typename Dtype>
+class ScratchDiff {
+ public:
+    // The blob whose diff the kernel writes: `bottom`, or with `use_scratch` a blob of bottom's layout with `channels` channels
+    Blob<Dtype>* target(Blob<Dtype>* bottom, bool use_scratch, int channels) {
+        if (!use_scratch) return bottom;
+        if (!blob_) blob_.reset(new Blob<Dtype>());
+        blob_->set_layout(bottom->layout(), -1);
+        blob_->Reshape(bottom->num(), channels, bottom->height(), bottom->width());
+        return blob_.get();
+    }
+    // After the kernel: a scratch target's first bottom->channels() channels go to the bottom's diff, added when it accumulates
+    void finish(Blob<Dtype>* target, Blob<Dtype>* bottom, bool accumulate, cudaStream_t st) {
+        if (target == bottom) return;
+        fn2_tensor s = target->diff_tensor(0, bottom->channels()), d = bottom->diff_tensor();
+        FN2_CALL(fn2_axpby(&s, 1.f, &d, accumulate ? 1.f : 0.f, st));
+    }
+ private:
+    shared_ptr<Blob<Dtype> > blob_;
+};
+
 // ---------------------------------------------------------------------------------------------
 // Fillers (include/caffe/filler.hpp).  Deterministic host RNG (the reference draws from boost
 // mt19937, util/rng.hpp:16-20; bit-matching boost is out of scope -- weights come from a
@@ -401,87 +424,83 @@ REGISTER_LAYER_CLASS(Resample);
 // ---------------------------------------------------------------------------------------------
 // Correlation (correlation_layer.cpp:13-84, .cu:431-504)
 // ---------------------------------------------------------------------------------------------
+// correlation_param of Correlation and Correlation1D (correlation_layer.cpp:13-35, correlation_layer1d.cpp:13-37)
+struct CorrParams {
+    int kernel_size = 0, max_displacement = 0, pad = 0, stride1 = 1, stride2 = 1, corr_type = 0, single_direction = 0;
+    static CorrParams Parse(const CorrelationParameter& cp) {
+        CorrParams p;
+        CHECK(cp.has_kernel_size()) << "Filter kernel_size is not set";
+        CHECK(cp.has_max_displacement()) << "Max displacement is required.";
+        p.kernel_size = cp.kernel_size();
+        CHECK(p.kernel_size % 2 == 1) << "Odd kernel size required";
+        p.max_displacement = cp.max_displacement();
+        p.pad = cp.pad();
+        p.stride1 = cp.stride_1();
+        p.stride2 = cp.stride_2();
+        p.single_direction = cp.single_direction();             // Correlation1D only
+        p.corr_type = cp.correlation_type();                     // do_abs is parsed and unused in the reference too
+        return p;
+    }
+    // SURVEY 8(d): bytes = read both maps once + write top once; flops = 2*D^2*k^2*C per output pixel
+    template <typename Dtype>
+    void WorkEstimate(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top, double* flops, double* bytes) const {
+        *bytes = 4.0 * (bottom[0]->count() + bottom[1]->count() + top[0]->count());
+        *flops = 2.0 * top[0]->count() * (double)kernel_size * kernel_size * bottom[0]->channels();
+    }
+};
+
 template <typename Dtype>
 class CorrelationLayer : public Layer<Dtype> {
  public:
     explicit CorrelationLayer(const LayerParameter& p) : Layer<Dtype>(p) {}
-    ~CorrelationLayer() override { if (ws_) cudaFree(ws_); if (bws_) cudaFree(bws_); }
     const char* type() const override { return "Correlation"; }
     int ExactNumBottomBlobs() const override { return 2; }
     int ExactNumTopBlobs() const override { return 1; }
     void LayerSetUp(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) override {
-        CorrelationParameter cp = this->layer_param_.correlation_param();
-        CHECK(cp.has_kernel_size()) << "Filter kernel_size is not set";
-        CHECK(cp.has_max_displacement()) << "Max displacement is required.";
-        kernel_size_ = cp.kernel_size();
-        CHECK(kernel_size_ % 2 == 1) << "Odd kernel size required";
-        max_displacement_ = cp.max_displacement();
-        pad_size_ = cp.pad();
-        stride1_ = cp.stride_1();
-        stride2_ = cp.stride_2();
-        corr_type_ = cp.correlation_type();      // do_abs is parsed and unused in the reference too
+        p_ = CorrParams::Parse(this->layer_param_.correlation_param());
     }
     void Reshape(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) override {
         CHECK_EQ(bottom[0]->width(), bottom[1]->width()) << "Both bottom blobs must have same width";
         CHECK_EQ(bottom[0]->height(), bottom[1]->height()) << "Both bottom blobs must have same height";
         CHECK_EQ(bottom[0]->channels(), bottom[1]->channels()) << "Both bottom blobs must have same height";
         int tc, th, tw;
-        FN2_CALL(fn2_correlation_shape(bottom[0]->height(), bottom[0]->width(), pad_size_, kernel_size_,
-                                       max_displacement_, stride1_, stride2_, &tc, &th, &tw));
+        FN2_CALL(fn2_correlation_shape(bottom[0]->height(), bottom[0]->width(), p_.pad, p_.kernel_size,
+                                       p_.max_displacement, p_.stride1, p_.stride2, &tc, &th, &tw));
         top[0]->Reshape(bottom[0]->num(), tc, th, tw);
         size_t need = 0;
         FN2_CALL(fn2_correlation_workspace_bytes(bottom[0]->num(), bottom[0]->channels(), bottom[0]->height(),
-                                                 bottom[0]->width(), pad_size_, kernel_size_, max_displacement_,
-                                                 stride1_, stride2_, corr_type_, &need));
-        if (need > ws_bytes_) {
-            if (ws_) cudaFree(ws_);
-            CUDA_CHECK(cudaMalloc(&ws_, need));
-            CUDA_CHECK(cudaMemsetAsync(ws_, 0, need, S()));
-            CUDA_CHECK(cudaStreamSynchronize(S()));
-            ws_bytes_ = need;
-        }
+                                                 bottom[0]->width(), p_.pad, p_.kernel_size, p_.max_displacement,
+                                                 p_.stride1, p_.stride2, p_.corr_type, &need));
+        ws_.reserve(need, S());
     }
  protected:
     void Forward_gpu(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) override {
         fn2_tensor b0 = bottom[0]->tensor(), b1 = bottom[1]->tensor(), t = top[0]->mutable_tensor();
-        FN2_CALL(fn2_correlation_forward(&b0, &b1, &t, pad_size_, kernel_size_, max_displacement_, stride1_,
-                                         stride2_, corr_type_, ws_, ws_bytes_, S()));
+        FN2_CALL(fn2_correlation_forward(&b0, &b1, &t, p_.pad, p_.kernel_size, p_.max_displacement, p_.stride1,
+                                         p_.stride2, p_.corr_type, ws_.get(), ws_.bytes(), S()));
     }
-    // correlation_layer.cu:508-600
+    // correlation_layer.cu:508-600.  The kernels overwrite both bottom diffs.
     void Backward_gpu(const vector<Blob<Dtype>*>& top, const vector<bool>& propagate_down, const vector<Blob<Dtype>*>& bottom) override {
         if (!propagate_down[0] && !propagate_down[1]) return;
         size_t need = 0;
         FN2_CALL(fn2_correlation_backward_workspace_bytes(bottom[0]->num(), bottom[0]->channels(), bottom[0]->height(), bottom[0]->width(),
-                                                          pad_size_, kernel_size_, max_displacement_, stride1_, stride2_, corr_type_, &need));
-        if (need > bws_bytes_) { if (bws_) cudaFree(bws_); CUDA_CHECK(cudaMalloc(&bws_, need)); bws_bytes_ = need; }
-        // the kernels overwrite: a bottom that already holds a contribution gets this one through a scratch blob
+                                                          p_.pad, p_.kernel_size, p_.max_displacement, p_.stride1, p_.stride2, p_.corr_type, &need));
+        bws_.reserve(need);
         Blob<Dtype>* tgt[2];
-        for (int i = 0; i < 2; i++) {
-            tgt[i] = bottom[i];
-            if (this->bottom_accumulate_[i]) { if (!scratch_[i]) scratch_[i].reset(new Blob<Dtype>()); scratch_[i]->set_layout(bottom[i]->layout(), -1); scratch_[i]->ReshapeLike(*bottom[i]); tgt[i] = scratch_[i].get(); }
-        }
+        for (int i = 0; i < 2; i++) tgt[i] = scratch_[i].target(bottom[i], this->bottom_accumulate_[i], bottom[i]->channels());
         fn2_tensor b0 = bottom[0]->tensor(), b1 = bottom[1]->tensor(), dy = top[0]->diff_tensor();
         fn2_tensor d0 = tgt[0]->diff_tensor(), d1 = tgt[1]->diff_tensor();
-        FN2_CALL(fn2_correlation_backward(&b0, &b1, &dy, &d0, &d1, pad_size_, kernel_size_, max_displacement_, stride1_, stride2_,
-                                          corr_type_, bws_, bws_bytes_, S()));
-        for (int i = 0; i < 2; i++)
-            if (this->bottom_accumulate_[i]) {
-                fn2_tensor s = tgt[i]->diff_tensor(), d = bottom[i]->diff_tensor();
-                FN2_CALL(fn2_axpby(&s, 1.f, &d, 1.f, S()));
-            }
+        FN2_CALL(fn2_correlation_backward(&b0, &b1, &dy, &d0, &d1, p_.pad, p_.kernel_size, p_.max_displacement, p_.stride1, p_.stride2,
+                                          p_.corr_type, bws_.get(), bws_.bytes(), S()));
+        for (int i = 0; i < 2; i++) scratch_[i].finish(tgt[i], bottom[i], this->bottom_accumulate_[i], S());
     }
     void WorkEstimate(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top, double* flops,
                       double* bytes) const override {
-        // SURVEY 8(d): bytes = read both maps once + write top once; flops = 2*D^2*k^2*C per output pixel
-        *bytes = 4.0 * (bottom[0]->count() + bottom[1]->count() + top[0]->count());
-        *flops = 2.0 * top[0]->count() * (double)kernel_size_ * kernel_size_ * bottom[0]->channels();
+        p_.WorkEstimate(bottom, top, flops, bytes);
     }
-    int kernel_size_ = 0, max_displacement_ = 0, pad_size_ = 0, stride1_ = 1, stride2_ = 1, corr_type_ = 0;
-    void* ws_ = nullptr;
-    size_t ws_bytes_ = 0;
-    void* bws_ = nullptr;
-    size_t bws_bytes_ = 0;
-    shared_ptr<Blob<Dtype> > scratch_[2];
+    CorrParams p_;
+    DeviceBuffer ws_, bws_;
+    ScratchDiff<Dtype> scratch_[2];
 };
 REGISTER_LAYER_CLASS(Correlation);
 
@@ -494,40 +513,29 @@ class Correlation1DLayer : public Layer<Dtype> {
     int ExactNumBottomBlobs() const override { return 2; }
     int ExactNumTopBlobs() const override { return 1; }
     void LayerSetUp(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) override {
-        CorrelationParameter cp = this->layer_param_.correlation_param();
-        CHECK(cp.has_kernel_size()) << "Filter kernel_size is not set";
-        CHECK(cp.has_max_displacement()) << "Max displacement is required.";
-        kernel_size_ = cp.kernel_size();
-        CHECK(kernel_size_ % 2 == 1) << "Odd kernel size required";
-        max_displacement_ = cp.max_displacement();
-        pad_size_ = cp.pad();
-        stride1_ = cp.stride_1();
-        stride2_ = cp.stride_2();
-        single_direction_ = cp.single_direction();
-        CHECK(single_direction_ >= -1 && single_direction_ <= 1) << "single_direction must be -1 (left), 0 (off), or 1 (right)";
-        corr_type_ = cp.correlation_type();
+        p_ = CorrParams::Parse(this->layer_param_.correlation_param());
+        CHECK(p_.single_direction >= -1 && p_.single_direction <= 1) << "single_direction must be -1 (left), 0 (off), or 1 (right)";
     }
     void Reshape(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) override {
         CHECK_EQ(bottom[0]->width(), bottom[1]->width()) << "Both bottom blobs must have same width";
         CHECK_EQ(bottom[0]->height(), bottom[1]->height()) << "Both bottom blobs must have same height";
         CHECK_EQ(bottom[0]->channels(), bottom[1]->channels()) << "Both bottom blobs must have same number of channels";
         int tc, th, tw;
-        FN2_CALL(fn2_correlation1d_shape(bottom[0]->height(), bottom[0]->width(), pad_size_, kernel_size_, max_displacement_,
-                                         stride1_, stride2_, single_direction_, &tc, &th, &tw));
+        FN2_CALL(fn2_correlation1d_shape(bottom[0]->height(), bottom[0]->width(), p_.pad, p_.kernel_size, p_.max_displacement,
+                                         p_.stride1, p_.stride2, p_.single_direction, &tc, &th, &tw));
         top[0]->Reshape(bottom[0]->num(), tc, th, tw);
     }
  protected:
     void Forward_gpu(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) override {
         fn2_tensor b0 = bottom[0]->tensor(), b1 = bottom[1]->tensor(), t = top[0]->mutable_tensor();
-        FN2_CALL(fn2_correlation1d_forward(&b0, &b1, &t, pad_size_, kernel_size_, max_displacement_, stride1_, stride2_,
-                                           single_direction_, corr_type_, S()));
+        FN2_CALL(fn2_correlation1d_forward(&b0, &b1, &t, p_.pad, p_.kernel_size, p_.max_displacement, p_.stride1, p_.stride2,
+                                           p_.single_direction, p_.corr_type, S()));
     }
     void WorkEstimate(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top, double* flops,
                       double* bytes) const override {
-        *bytes = 4.0 * (bottom[0]->count() + bottom[1]->count() + top[0]->count());
-        *flops = 2.0 * top[0]->count() * (double)kernel_size_ * kernel_size_ * bottom[0]->channels();
+        p_.WorkEstimate(bottom, top, flops, bytes);
     }
-    int kernel_size_ = 0, max_displacement_ = 0, pad_size_ = 0, stride1_ = 1, stride2_ = 1, corr_type_ = 0, single_direction_ = 0;
+    CorrParams p_;
 };
 REGISTER_LAYER_CLASS(Correlation1D);
 
@@ -538,15 +546,12 @@ REGISTER_LAYER_CLASS(Correlation1D);
 // engine CAFFE -> exact FP32 SIMT kernel, DEFAULT/CUDNN -> wgmma tensor-core kernel when the
 // shape is eligible.
 // ---------------------------------------------------------------------------------------------
+struct PackedWeights { DeviceBuffer buf; int gen = -1; };   // fn2_conv_pack_weights output of one ParamsChanged generation
+
 template <typename Dtype>
 class BaseConvolutionLayer : public Layer<Dtype> {
  public:
     explicit BaseConvolutionLayer(const LayerParameter& p, bool deconv) : Layer<Dtype>(p), deconv_(deconv) {}
-    ~BaseConvolutionLayer() override {
-        for (auto& kv : packed_) if (kv.second.p) cudaFree(kv.second.p);
-        for (auto& kv : bpacked_) if (kv.second.p) cudaFree(kv.second.p);
-        if (ws_) cudaFree(ws_); if (pws_) cudaFree(pws_); if (bws_) cudaFree(bws_); if (flipped_) cudaFree(flipped_);
-    }
     int MinBottomBlobs() const override { return 1; }
     int MinTopBlobs() const override { return 1; }
     bool EqualNumBottomTopBlobs() const override { return true; }
@@ -592,11 +597,7 @@ class BaseConvolutionLayer : public Layer<Dtype> {
         bottoms_.assign(bottom.begin(), bottom.end());
         size_t need = 0;
         FN2_CALL(fn2_conv_workspace_bytes(&d_, bottom[0]->num(), bottom[0]->height(), bottom[0]->width(), &need));
-        if (need > ws_bytes_) {
-            if (ws_) cudaFree(ws_);
-            CUDA_CHECK(cudaMalloc(&ws_, need));
-            ws_bytes_ = need;
-        }
+        ws_.reserve(need);
     }
     void FillParams(uint64_t seed) override {
         ConvolutionParameter cp = this->layer_param_.convolution_param();
@@ -613,13 +614,9 @@ class BaseConvolutionLayer : public Layer<Dtype> {
         for (int cis : strides) {
             size_t floats = 0;
             FN2_CALL(fn2_conv_packed_floats(&d_, cis, &floats));
-            Packed& pk = packed_[cis];
-            if (floats > pk.floats) {
-                if (pk.p) cudaFree(pk.p);
-                CUDA_CHECK(cudaMalloc(&pk.p, floats * sizeof(float)));
-                pk.floats = floats;
-            }
-            FN2_CALL(fn2_conv_pack_weights(&d_, cis, this->blobs_[0]->gpu_data(), pk.p, S()));
+            DeviceBuffer& pk = packed_[cis].buf;
+            pk.reserve(floats * sizeof(float));
+            FN2_CALL(fn2_conv_pack_weights(&d_, cis, this->blobs_[0]->gpu_data(), pk.as<float>(), S()));
         }
     }
     void WorkEstimate(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top, double* flops,
@@ -649,10 +646,10 @@ class BaseConvolutionLayer : public Layer<Dtype> {
             CHECK(!(!deconv_ && bottom[i]->is_alias() && d_.ci <= 16 && d_.input_guard_bytes > 0))
                 << "a zero-copy concat child must not feed a convolution with <= 16 input channels (layer " << this->layer_param_.name() << ")";
             auto it = packed_.find(bottom[i]->channel_stride() > 0 ? bottom[i]->channel_stride() : d_.ci);
-            CHECK(it != packed_.end() && it->second.p) << "convolution weights were never packed for this bottom layout";
-            const float* packed = it->second.p;
-            FN2_CALL(fn2_conv_forward(&d, &b, packed, d_.has_bias ? this->blobs_[1]->gpu_data() : nullptr, &t, ws_,
-                                      ws_bytes_, S()));
+            CHECK(it != packed_.end() && !it->second.buf.empty()) << "convolution weights were never packed for this bottom layout";
+            const DeviceBuffer& packed = it->second.buf;
+            FN2_CALL(fn2_conv_forward(&d, &b, packed.as<float>(), d_.has_bias ? this->blobs_[1]->gpu_data() : nullptr, &t,
+                                      ws_.get(), ws_.bytes(), S()));
         }
     }
     // conv_layer.cu:26-58 / deconv_layer.cu:26-55.  Weight and bias gradients: fn2_conv_backward_params (ADDED to the parameter
@@ -663,7 +660,7 @@ class BaseConvolutionLayer : public Layer<Dtype> {
         cudaStream_t st = S();
         size_t need = 0;
         FN2_CALL(fn2_conv_backward_params_workspace_bytes(&d_, bottom[0]->num(), bottom[0]->height(), bottom[0]->width(), &need));
-        if (need > pws_bytes_) { if (pws_) cudaFree(pws_); CUDA_CHECK(cudaMalloc(&pws_, need)); pws_bytes_ = need; }
+        pws_.reserve(need);
         fn2_tensor wd = this->blobs_[0]->diff_tensor();
         float* bd = d_.has_bias ? this->blobs_[1]->diff_tensor().data : nullptr;
         for (size_t i = 0; i < bottom.size(); ++i) {
@@ -673,7 +670,7 @@ class BaseConvolutionLayer : public Layer<Dtype> {
                 FN2_CALL(fn2_relu_backward(&y, &dy, &dy, slope_[i], 0, st));
             }
             fn2_tensor x = bottom[i]->tensor();
-            FN2_CALL(fn2_conv_backward_params(&d_, &x, &dy, wd.data, bd, 1, pws_, pws_bytes_, st));
+            FN2_CALL(fn2_conv_backward_params(&d_, &x, &dy, wd.data, bd, 1, pws_.get(), pws_.bytes(), st));
             if (!propagate_down[i]) continue;
             BackwardData(top[i], bottom[i], this->bottom_accumulate_[i], st);
         }
@@ -684,9 +681,7 @@ class BaseConvolutionLayer : public Layer<Dtype> {
         FN2_CALL(fn2_conv_backward_data_desc(&d_, bottom->height(), bottom->width(), &bd, &flip));
         fn2_tensor dy = top->diff_tensor();
         // The tensor-core engine wants output channels in multiples of 16; concat-sized bottoms (1026, 770, 386, 473 channels)
-        // are not.  Their adjoint convolution runs with zero weight rows appended, into a scratch blob whose first channels are
-        // then copied / added to the bottom diff.
-        const int co_real = bd.co;
+        // are not.  Their adjoint convolution runs with zero weight rows appended, into the scratch diff blob.
         const bool pad_co = !bd.deconv && bd.co > 16 && bd.co % 16 != 0;
         if (pad_co) {
             // wide tiles: a multiple of 128 when that costs <= 1/8 more channels, else of 64 (of 16 for narrow outputs)
@@ -695,59 +690,46 @@ class BaseConvolutionLayer : public Layer<Dtype> {
         }
         // packed weights of the adjoint operator for this top layout (derived once per ParamsChanged generation)
         const int cis = top->channel_stride() > 0 ? top->channel_stride() : d_.co;
-        Packed& pk = bpacked_[cis];
+        PackedWeights& pk = bpacked_[cis];
         if (pk.gen != params_gen_) {
             const float* w = this->blobs_[0]->gpu_data();
             if (flip || pad_co) {
                 const size_t wn = (size_t)bd.co * bd.ci * bd.kh * bd.kw, wreal = (size_t)this->blobs_[0]->count();
-                if (wn > flipped_floats_) { if (flipped_) cudaFree(flipped_); CUDA_CHECK(cudaMalloc(&flipped_, wn * sizeof(float))); flipped_floats_ = wn; }
-                if (flip) FN2_CALL(fn2_conv_flip_transpose_weights(&d_, w, flipped_, st));
-                else CUDA_CHECK(cudaMemcpyAsync(flipped_, w, wreal * sizeof(float), cudaMemcpyDeviceToDevice, st));
-                if (wn > wreal) CUDA_CHECK(cudaMemsetAsync(flipped_ + wreal, 0, (wn - wreal) * sizeof(float), st));
-                w = flipped_;
+                flipped_.reserve(wn * sizeof(float));
+                float* fw = flipped_.as<float>();
+                if (flip) FN2_CALL(fn2_conv_flip_transpose_weights(&d_, w, fw, st));
+                else CUDA_CHECK(cudaMemcpyAsync(fw, w, wreal * sizeof(float), cudaMemcpyDeviceToDevice, st));
+                if (wn > wreal) CUDA_CHECK(cudaMemsetAsync(fw + wreal, 0, (wn - wreal) * sizeof(float), st));
+                w = fw;
             }
             size_t floats = 0;
             FN2_CALL(fn2_conv_packed_floats(&bd, cis, &floats));
-            if (floats > pk.floats) { if (pk.p) cudaFree(pk.p); CUDA_CHECK(cudaMalloc(&pk.p, floats * sizeof(float))); pk.floats = floats; }
-            FN2_CALL(fn2_conv_pack_weights(&bd, cis, w, pk.p, st));
+            pk.buf.reserve(floats * sizeof(float));
+            FN2_CALL(fn2_conv_pack_weights(&bd, cis, w, pk.buf.as<float>(), st));
             pk.gen = params_gen_;
         }
         int Hb, Wb;
         FN2_CALL(fn2_conv_out_shape(&bd, top->height(), top->width(), &Hb, &Wb));
         CHECK(Hb == bottom->height() && Wb == bottom->width()) << "conv backward: adjoint output " << Hb << "x" << Wb << " != bottom";
-        Blob<Dtype>* tgt = bottom;
-        if (accumulate || pad_co) {
-            if (!bscratch_) bscratch_.reset(new Blob<Dtype>());
-            bscratch_->set_layout(bottom->layout(), -1);
-            bscratch_->Reshape(bottom->num(), bd.co, bottom->height(), bottom->width());
-            tgt = bscratch_.get();
-        }
+        Blob<Dtype>* tgt = bscratch_.target(bottom, accumulate || pad_co, bd.co);
         fn2_tensor dx = tgt->diff_tensor();
         size_t wsn = 0;
         FN2_CALL(fn2_conv_workspace_bytes(&bd, top->num(), top->height(), top->width(), &wsn));
-        if (wsn > bws_bytes_) { if (bws_) cudaFree(bws_); CUDA_CHECK(cudaMalloc(&bws_, wsn)); bws_bytes_ = wsn; }
-        FN2_CALL(fn2_conv_forward(&bd, &dy, pk.p, nullptr, &dx, bws_, bws_bytes_, st));
-        if (tgt != bottom) {
-            fn2_tensor s = tgt->diff_tensor(0, co_real), d = bottom->diff_tensor();
-            FN2_CALL(fn2_axpby(&s, 1.f, &d, accumulate ? 1.f : 0.f, st));
-        }
+        bws_.reserve(wsn);
+        FN2_CALL(fn2_conv_forward(&bd, &dy, pk.buf.as<float>(), nullptr, &dx, bws_.get(), bws_.bytes(), st));
+        bscratch_.finish(tgt, bottom, accumulate, st);
     }
     bool deconv_;
     fn2_conv_desc d_;
     vector<int> relu_;
     vector<float> slope_;
-    struct Packed { float* p = nullptr; size_t floats = 0; int gen = -1; };
-    std::map<int, Packed> packed_;        // by bottom pixel stride
-    std::map<int, Packed> bpacked_;       // adjoint operator's packed weights, by top pixel stride
+    std::map<int, PackedWeights> packed_;        // by bottom pixel stride
+    std::map<int, PackedWeights> bpacked_;       // adjoint operator's packed weights, by top pixel stride
     int params_gen_ = 0;                  // bumped by ParamsChanged
-    float* flipped_ = nullptr;
-    size_t flipped_floats_ = 0;
-    void* pws_ = nullptr; size_t pws_bytes_ = 0;
-    void* bws_ = nullptr; size_t bws_bytes_ = 0;
-    shared_ptr<Blob<Dtype> > bscratch_;
+    DeviceBuffer flipped_;                // flipped and / or Co-padded weights the adjoint packs from
+    DeviceBuffer ws_, pws_, bws_;         // forward, parameter-gradient and adjoint workspaces
+    ScratchDiff<Dtype> bscratch_;
     vector<const Blob<Dtype>*> bottoms_;
-    void* ws_ = nullptr;
-    size_t ws_bytes_ = 0;
 };
 
 template <typename Dtype>
@@ -816,6 +798,49 @@ struct AugCoeff {
         for (int f = 0; f < N; f++) if (std::fabs(def(f) - v[f]) < 1e-3) clear(f);
     }
 };
+
+// tTransMat::fromCoeff (augmentation_layer_base.cpp:38-48): crop (cw x ch) -> bottom (bw x bh) coordinates; each factor is
+// applied when its coefficient is set
+static TransMat TransMatFromCoeff(const AugCoeff& c, int cw, int ch, int bw, int bh) {
+    TransMat t; t.toIdentity();
+    if (c.get(AugCoeff::MIRROR)) t.leftMultiply(-1, 0, 0, 1, .5f * (float)cw, -.5f * (float)ch);
+    else                         t.leftMultiply(1, 0, 0, 1, -.5f * (float)cw, -.5f * (float)ch);
+    if (c.has[AugCoeff::ANGLE]) {
+        const float a = c.get(AugCoeff::ANGLE);
+        t.leftMultiply(std::cos(a), std::sin(a), -std::sin(a), std::cos(a), 0, 0);
+    }
+    if (c.has[AugCoeff::DX] || c.has[AugCoeff::DY])
+        t.leftMultiply(1, 0, 0, 1, c.get(AugCoeff::DX) * (float)cw, c.get(AugCoeff::DY) * (float)ch);
+    if (c.has[AugCoeff::ZOOM_X] || c.has[AugCoeff::ZOOM_Y])
+        t.leftMultiply((float)(1.0 / c.get(AugCoeff::ZOOM_X)), 0, 0, (float)(1.0 / c.get(AugCoeff::ZOOM_Y)), 0, 0);
+    t.leftMultiply(1, 0, 0, 1, .5f * (float)bw, .5f * (float)bh);
+    return t;
+}
+
+// Which coefficient groups an augmentation_param samples: decided by the presence of their generators
+// (data_augmentation_layer.cu:383-396)
+struct AugGroups { bool spatial, chromatic, eigen, effect; };
+static AugGroups SampledGroups(const AugmentationParameter& aug) {
+    AugGroups g;
+    g.spatial = aug.has("mirror") || aug.has("rotate") || aug.has("zoom") || aug.has("translate") || aug.has("squeeze") ||
+                aug.has("translate_x") || aug.has("translate_y");
+    g.chromatic = aug.has("brightness") || aug.has("gamma") || aug.has("contrast") || aug.has("color");
+    g.effect = aug.has("fog_size") || aug.has("fog_amount") || aug.has("motion_blur_angle") || aug.has("motion_blur_size") ||
+               aug.has("shadow_angle") || aug.has("shadow_distance") || aug.has("shadow_strength") || aug.has("noise");
+    g.eigen = aug.has("lmult_pow") || aug.has("lmult_mult") || aug.has("lmult_add") || aug.has("sat_pow") || aug.has("sat_mult") ||
+              aug.has("sat_add") || aug.has("col_pow") || aug.has("col_mult") || aug.has("col_add") || aug.has("ladd_pow") ||
+              aug.has("ladd_mult") || aug.has("ladd_add") || aug.has("col_rotate");
+    return g;
+}
+
+// Seed of a layer's coefficient sampler: FN2_SEED (default 1701, the reference tests' seed, test_gradient_check_util.hpp:25)
+// hashed with the layer name
+static uint32_t seed_of(const std::string& name) {
+    uint32_t h = 1701u;
+    if (const char* e = getenv("FN2_SEED")) h = (uint32_t)strtoul(e, nullptr, 10);
+    for (char c : name) h = h * 16777619u ^ (unsigned char)c;
+    return h;
+}
 
 // caffe_rng_generate, util/rng.cpp:8-114.  The reference draws from boost::mt19937 through boost's uniform_real /
 // normal_distribution / bernoulli_distribution of an unpinned boost version: the random STREAM is unpinned, the
@@ -965,23 +990,14 @@ struct AugSampler {
         }
         if (aug.has("noise")) c.set(AugCoeff::NOISE, rng.generate(aug.gen("noise"), dc, NAN));
     }
-    // one item: which groups are sampled is decided by the presence of their generators (:383-396)
+    // one item
     void sample(const AugmentationParameter& aug, float dc, int width, int height, int cw, int ch, AugCoeff& c) {
-        const bool spatial = aug.has("mirror") || aug.has("rotate") || aug.has("zoom") || aug.has("translate") ||
-                             aug.has("squeeze") || aug.has("translate_x") || aug.has("translate_y");
-        const bool chromatic = aug.has("brightness") || aug.has("gamma") || aug.has("contrast") || aug.has("color");
-        const bool effect = aug.has("fog_size") || aug.has("fog_amount") || aug.has("motion_blur_angle") ||
-                            aug.has("motion_blur_size") || aug.has("shadow_angle") || aug.has("shadow_distance") ||
-                            aug.has("shadow_strength") || aug.has("noise");
-        const bool eigen = aug.has("lmult_pow") || aug.has("lmult_mult") || aug.has("lmult_add") || aug.has("sat_pow") ||
-                           aug.has("sat_mult") || aug.has("sat_add") || aug.has("col_pow") || aug.has("col_mult") ||
-                           aug.has("col_add") || aug.has("ladd_pow") || aug.has("ladd_mult") || aug.has("ladd_add") ||
-                           aug.has("col_rotate");
+        const AugGroups g = SampledGroups(aug);
         c.clear_all();
-        if (spatial) generate_valid_spatial(aug, c, dc, width, height, cw, ch);
-        if (chromatic) generate_chromatic(aug, c, dc);
-        if (eigen) generate_chromatic_eigen(aug, c, dc);
-        if (effect) generate_effect(aug, c, dc);
+        if (g.spatial) generate_valid_spatial(aug, c, dc, width, height, cw, ch);
+        if (g.chromatic) generate_chromatic(aug, c, dc);
+        if (g.eigen) generate_chromatic_eigen(aug, c, dc);
+        if (g.effect) generate_effect(aug, c, dc);
     }
     // discount schedule, data_augmentation_layer.cu:372-374
     static float discount(const LayerParameter& lp, float num_iter) {
@@ -1007,11 +1023,6 @@ template <typename Dtype>
 class DataAugmentationLayer : public Layer<Dtype> {
  public:
     explicit DataAugmentationLayer(const LayerParameter& p) : Layer<Dtype>(p), sampler_(seed_of(p.name())) {}
-    ~DataAugmentationLayer() override {
-        if (coef_dev_) cudaFree(coef_dev_);
-        if (fixed_mean_dev_) cudaFree(fixed_mean_dev_);
-        if (coef_host_) cudaFreeHost(coef_host_);
-    }
     const char* type() const override { return "DataAugmentation"; }
     bool AllowBackward() const override { return false; }              // data_augmentation_layer.hpp:29
     bool DoesUseCustomCopyBlobs() const override { return true; }      // data_augmentation_layer.hpp:43-46
@@ -1053,24 +1064,22 @@ class DataAugmentationLayer : public Layer<Dtype> {
         //   [N x 6 matrices][N x 6 chromatic][N x 22 chromatic-eigen][N x 9 effects][9 eigvec][pad][32 eigenspace]
         off_mat_ = 0; off_chroma_ = off_mat_ + 6 * num; off_eigen_ = off_chroma_ + 6 * num; off_effect_ = off_eigen_ + 22 * num;
         off_eigvec_ = off_effect_ + 9 * num; off_space_ = (off_eigvec_ + 9 + 1) / 2 * 2; coef_floats_ = off_space_ + 32;
-        if (coef_dev_) cudaFree(coef_dev_);
-        if (coef_host_) cudaFreeHost(coef_host_);
-        CUDA_CHECK(cudaMalloc(&coef_dev_, coef_floats_ * sizeof(float)));
-        CUDA_CHECK(cudaMallocHost(&coef_host_, coef_floats_ * sizeof(float)));
-        memset(coef_host_, 0, coef_floats_ * sizeof(float));
-        for (int i = 0; i < 9 && i < aug.chromatic_eigvec_size(); i++) coef_host_[off_eigvec_ + i] = aug.chromatic_eigvec(i);
+        coef_dev_.reserve(coef_floats_ * sizeof(float));
+        coef_host_.reserve(coef_floats_ * sizeof(float));
+        memset(coef_host_.get(), 0, coef_floats_ * sizeof(float));
+        for (int i = 0; i < 9 && i < aug.chromatic_eigvec_size(); i++) coef_host_.as<float>()[off_eigvec_ + i] = aug.chromatic_eigvec(i);
         gen_active_ = do_cropping_ && !input_params_ && aug.has_any_generator() && (this->phase_ == TRAIN || aug.augment_during_test());
         // default coefficients -> one matrix per sample (data_augmentation_layer.cu:462-468); constant unless coefficients
         // are generated or received
         prepare_records(width, height);
-        CUDA_CHECK(cudaMemcpy(coef_dev_, coef_host_, coef_floats_ * sizeof(float), cudaMemcpyHostToDevice));
+        CUDA_CHECK(cudaMemcpy(coef_dev_.get(), coef_host_.get(), coef_floats_ * sizeof(float), cudaMemcpyHostToDevice));
         if (aug.recompute_mean()) {
             this->blobs_[1]->Reshape(1, channels, cropped_height_, cropped_width_);
             this->blobs_[2]->Reshape(1, channels, 1, 1);
         } else if (aug.mean_size() == 3 && !aug.mean_per_pixel()) {
             float mv[3] = {aug.mean(0), aug.mean(1), aug.mean(2)};
-            if (!fixed_mean_dev_) CUDA_CHECK(cudaMalloc(&fixed_mean_dev_, 3 * sizeof(float)));
-            CUDA_CHECK(cudaMemcpy(fixed_mean_dev_, mv, sizeof(mv), cudaMemcpyHostToDevice));
+            fixed_mean_dev_.reserve(sizeof(mv));
+            CUDA_CHECK(cudaMemcpy(fixed_mean_dev_.get(), mv, sizeof(mv), cudaMemcpyHostToDevice));
         }
         *(this->blobs_[0]->mutable_cpu_data()) = 0;                    // data_augmentation_layer.cpp:155
     }
@@ -1103,12 +1112,6 @@ class DataAugmentationLayer : public Layer<Dtype> {
     }
 
  protected:
-    static uint32_t seed_of(const std::string& name) {
-        uint32_t h = 1701u;                                             // the reference tests' seed (test_gradient_check_util.hpp:25)
-        if (const char* e = getenv("FN2_SEED")) h = (uint32_t)strtoul(e, nullptr, 10);
-        for (char c : name) h = h * 16777619u ^ (unsigned char)c;
-        return h;
-    }
     // all_coeffs_ (N x 42 array form) -> matrices / chromatic / eigen / effect records in coef_host_
     // (data_augmentation_layer.cu:452-477; tTransMat::fromCoeff augmentation_layer_base.cpp:38-48)
     void prepare_records(int bottomwidth, int bottomheight) {
@@ -1118,30 +1121,20 @@ class DataAugmentationLayer : public Layer<Dtype> {
             AugCoeff c;
             c.from_array(&all_coeffs_[(size_t)n * AugCoeff::N]);
             c.clear_defaults();
-            TransMat t; t.toIdentity();
-            if (c.get(AugCoeff::MIRROR)) t.leftMultiply(-1, 0, 0, 1, .5f * (float)cropped_width_, -.5f * (float)cropped_height_);
-            else                         t.leftMultiply(1, 0, 0, 1, -.5f * (float)cropped_width_, -.5f * (float)cropped_height_);
-            if (c.has[AugCoeff::ANGLE]) {
-                const float a = c.get(AugCoeff::ANGLE);
-                t.leftMultiply(std::cos(a), std::sin(a), -std::sin(a), std::cos(a), 0, 0);
-            }
-            if (c.has[AugCoeff::DX] || c.has[AugCoeff::DY])
-                t.leftMultiply(1, 0, 0, 1, c.get(AugCoeff::DX) * (float)cropped_width_, c.get(AugCoeff::DY) * (float)cropped_height_);
-            if (c.has[AugCoeff::ZOOM_X] || c.has[AugCoeff::ZOOM_Y])
-                t.leftMultiply((float)(1.0 / c.get(AugCoeff::ZOOM_X)), 0, 0, (float)(1.0 / c.get(AugCoeff::ZOOM_Y)), 0, 0);
-            t.leftMultiply(1, 0, 0, 1, .5f * (float)bottomwidth, .5f * (float)bottomheight);
-            float* m = coef_host_ + off_mat_ + 6 * n;
+            const TransMat t = TransMatFromCoeff(c, cropped_width_, cropped_height_, bottomwidth, bottomheight);
+            float* const rec = coef_host_.as<float>();
+            float* m = rec + off_mat_ + 6 * n;
             m[0] = t.t0; m[1] = t.t1; m[2] = t.t2; m[3] = t.t3; m[4] = t.t4; m[5] = t.t5;
-            float* ch = coef_host_ + off_chroma_ + 6 * n;          // tChromaticCoeffs: gamma, brightness, contrast, color[3]
+            float* ch = rec + off_chroma_ + 6 * n;          // tChromaticCoeffs: gamma, brightness, contrast, color[3]
             ch[0] = c.get(AugCoeff::GAMMA); ch[1] = c.get(AugCoeff::BRIGHTNESS); ch[2] = c.get(AugCoeff::CONTRAST);
             for (int k = 0; k < 3; k++) ch[3 + k] = c.get(AugCoeff::COLOR1 + k);
             if (ch[0] != 1 || ch[1] != 0 || ch[2] != 1 || ch[3] != 1 || ch[4] != 1 || ch[5] != 1) has_chromatic_ = true;
-            float* eg = coef_host_ + off_eigen_ + 22 * n;          // tChromaticEigenCoeffs
+            float* eg = rec + off_eigen_ + 22 * n;          // tChromaticEigenCoeffs
             for (int k = 0; k < 22; k++) {
                 eg[k] = c.get(AugCoeff::POW_NOMEAN0 + k);
                 if (eg[k] != AugCoeff::def(AugCoeff::POW_NOMEAN0 + k)) has_eigen_ = true;
             }
-            float* ef = coef_host_ + off_effect_ + 9 * n;          // tEffectCoeffs
+            float* ef = rec + off_effect_ + 9 * n;          // tEffectCoeffs
             ef[0] = c.get(AugCoeff::FOG_AMOUNT); ef[1] = c.get(AugCoeff::FOG_SIZE);
             ef[2] = c.get(AugCoeff::MOTION_BLUR_ANGLE); ef[3] = c.get(AugCoeff::MOTION_BLUR_SIZE);
             ef[4] = std::cos(c.get(AugCoeff::SHADOW_ANGLE)); ef[5] = std::sin(c.get(AugCoeff::SHADOW_ANGLE));
@@ -1155,6 +1148,7 @@ class DataAugmentationLayer : public Layer<Dtype> {
         AugmentationParameter aug = this->layer_param_.augmentation_param();
         fn2_tensor b = bottom[0]->tensor(), t = top[0]->mutable_tensor();
         const int num = bottom[0]->num();
+        float* coef = coef_dev_.as<float>();
         if (do_cropping_) {
             if (gen_active_ || input_params_) {
                 if (input_params_) {
@@ -1169,23 +1163,23 @@ class DataAugmentationLayer : public Layer<Dtype> {
                     }
                 }
                 prepare_records(bottom[0]->width(), bottom[0]->height());
-                CUDA_CHECK(cudaMemcpyAsync(coef_dev_, coef_host_, (size_t)off_eigvec_ * sizeof(float), cudaMemcpyHostToDevice, S()));
+                CUDA_CHECK(cudaMemcpyAsync(coef_dev_.get(), coef_host_.get(), (size_t)off_eigvec_ * sizeof(float), cudaMemcpyHostToDevice, S()));
             }
             if (output_params_) memcpy(top[1]->mutable_cpu_data(), all_coeffs_.data(), all_coeffs_.size() * sizeof(float));
             if (has_eigen_) {
                 CHECK_EQ(bottom[0]->channels(), 3) << "Chromatic-Eigen augmentations only work with 3-channel input";
                 CHECK_EQ(aug.chromatic_eigvec_size(), 9) << "You need to specify chromatic eigenvectors for Chromatic-Eigen augmentation";
-                FN2_CALL(fn2_chromatic_eigenspace(&b, coef_dev_ + off_eigvec_, coef_dev_ + off_space_, S()));
+                FN2_CALL(fn2_chromatic_eigenspace(&b, coef + off_eigvec_, coef + off_space_, S()));
             }
-            FN2_CALL(fn2_spatial_augmentation(&b, &t, coef_dev_ + off_mat_, S()));
-            if (has_eigen_) FN2_CALL(fn2_chromatic_eigen_augmentation(&t, coef_dev_ + off_eigen_, coef_dev_ + off_space_, aug.max_multiplier(), S()));
+            FN2_CALL(fn2_spatial_augmentation(&b, &t, coef + off_mat_, S()));
+            if (has_eigen_) FN2_CALL(fn2_chromatic_eigen_augmentation(&t, coef + off_eigen_, coef + off_space_, aug.max_multiplier(), S()));
             if (has_chromatic_) {
                 CHECK_EQ(bottom[0]->channels(), 3) << "Chromatic augmentations only work with 3-channel input";
-                FN2_CALL(fn2_color_contrast_augmentation(&t, coef_dev_ + off_chroma_, aug.max_multiplier(), S()));
+                FN2_CALL(fn2_color_contrast_augmentation(&t, coef + off_chroma_, aug.max_multiplier(), S()));
             }
             if (has_effect_) {
                 CHECK_EQ(bottom[0]->channels(), 3) << "Effect augmentations only work with 3-channel input";
-                FN2_CALL(fn2_apply_effects(&t, coef_dev_ + off_effect_, aug.max_multiplier(), (unsigned long long)sampler_.rng.gen() << 32 | sampler_.rng.gen(),
+                FN2_CALL(fn2_apply_effects(&t, coef + off_effect_, aug.max_multiplier(), (unsigned long long)sampler_.rng.gen() << 32 | sampler_.rng.gen(),
                                            has_noise_ ? 1 : 0, S()));
             }
             if (gen_active_ || input_params_) CUDA_CHECK(cudaStreamSynchronize(S()));   // coef_host_ is rewritten next call
@@ -1198,7 +1192,7 @@ class DataAugmentationLayer : public Layer<Dtype> {
             if (num_iter_ <= (float)aug.recompute_mean()) FN2_CALL(fn2_mean_update(&t, &mpp, mpc, num_iter_, S()));
             FN2_CALL(fn2_mean_subtract(&t, &mpp, mpc, aug.mean_per_pixel() ? 1 : 0, S()));
         } else if (aug.mean_size() == 3 && !aug.mean_per_pixel()) {
-            FN2_CALL(fn2_mean_subtract(&t, nullptr, fixed_mean_dev_, 0, S()));
+            FN2_CALL(fn2_mean_subtract(&t, nullptr, fixed_mean_dev_.as<float>(), 0, S()));
         }
     }
 
@@ -1237,11 +1231,11 @@ class DataAugmentationLayer : public Layer<Dtype> {
     int cropped_width_ = 0, cropped_height_ = 0;
     float num_iter_ = 0;
     vector<float> all_coeffs_;                   // N x 42, array form (coeff_to_array)
-    float* coef_host_ = nullptr;                 // pinned
-    float* coef_dev_ = nullptr;
+    DeviceBuffer coef_host_{DeviceBuffer::PINNED_HOST};   // uploaded asynchronously
+    DeviceBuffer coef_dev_;
     size_t coef_floats_ = 0;
     int off_mat_ = 0, off_chroma_ = 0, off_eigen_ = 0, off_effect_ = 0, off_eigvec_ = 0, off_space_ = 0;
-    float* fixed_mean_dev_ = nullptr;
+    DeviceBuffer fixed_mean_dev_;
     AugSampler sampler_;
 };
 REGISTER_LAYER_CLASS(DataAugmentation);
@@ -1249,19 +1243,11 @@ REGISTER_LAYER_CLASS(DataAugmentation);
 // ---------------------------------------------------------------------------------------------
 // Training-side layers next to the FlowNet2-C training step (SURVEY.md 8 "next" row 2)
 // ---------------------------------------------------------------------------------------------
+// array_to_coeff sets every field (augmentation_layer_base.cpp:368-379), so fromCoeff applies every factor
 static TransMat TransMatFromArray(const float* arr, int cw, int ch, int bw, int bh) {
-    // array_to_coeff sets every field (augmentation_layer_base.cpp:368-379), so fromCoeff applies every factor (:38-48)
     AugCoeff c;
     c.from_array(arr);
-    TransMat t; t.toIdentity();
-    if (c.get(AugCoeff::MIRROR)) t.leftMultiply(-1, 0, 0, 1, .5f * (float)cw, -.5f * (float)ch);
-    else                         t.leftMultiply(1, 0, 0, 1, -.5f * (float)cw, -.5f * (float)ch);
-    const float a = c.get(AugCoeff::ANGLE);
-    t.leftMultiply(std::cos(a), std::sin(a), -std::sin(a), std::cos(a), 0, 0);
-    t.leftMultiply(1, 0, 0, 1, c.get(AugCoeff::DX) * (float)cw, c.get(AugCoeff::DY) * (float)ch);
-    t.leftMultiply((float)(1.0 / c.get(AugCoeff::ZOOM_X)), 0, 0, (float)(1.0 / c.get(AugCoeff::ZOOM_Y)), 0, 0);
-    t.leftMultiply(1, 0, 0, 1, .5f * (float)bw, .5f * (float)bh);
-    return t;
+    return TransMatFromCoeff(c, cw, ch, bw, bh);
 }
 static TransMat TransMatInverse(const TransMat& m) {              // augmentation_layer_base.cpp:51-68
     const float a = m.t0, c = m.t2, e = m.t4, b = m.t1, d = m.t3, f = m.t5;
@@ -1277,7 +1263,6 @@ template <typename Dtype>
 class L1LossLayer : public Layer<Dtype> {
  public:
     explicit L1LossLayer(const LayerParameter& p) : Layer<Dtype>(p) {}
-    ~L1LossLayer() override { if (state_) cudaFree(state_); if (ws_) cudaFree(ws_); }
     const char* type() const override { return "L1Loss"; }
     bool IsLossLayer() const override { return true; }
     typename Blob<Dtype>::Layout TopLayout() const override { return Blob<Dtype>::PLAIN; }
@@ -1289,8 +1274,7 @@ class L1LossLayer : public Layer<Dtype> {
         d_.normalize_by_num_entries = lp.b("normalize_by_num_entries", false) ? 1 : 0;
         d_.epsilon = lp.f("epsilon", 1e-2f);
         d_.plateau = lp.f("plateau", 0.f);
-        CUDA_CHECK(cudaMalloc(&state_, 4 * sizeof(float)));
-        CUDA_CHECK(cudaMemset(state_, 0, 4 * sizeof(float)));
+        state_.reserve(4 * sizeof(float), S());
     }
     void Reshape(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) override {
         if (bottom.size() > 1) CHECK(bottom[0]->shape() == bottom[1]->shape()) << "L1Loss: bottoms must have the same shape";
@@ -1298,12 +1282,13 @@ class L1LossLayer : public Layer<Dtype> {
         top[0]->Reshape(vector<int>());                               // loss layers output a scalar (l1loss_layer.cpp:69-70)
         size_t need = 0;
         FN2_CALL(fn2_l1loss_workspace_bytes(bottom[0]->num(), bottom[0]->height(), bottom[0]->width(), &need));
-        if (need > ws_bytes_) { if (ws_) cudaFree(ws_); CUDA_CHECK(cudaMalloc(&ws_, need)); ws_bytes_ = need; }
+        ws_.reserve(need);
     }
     void Forward_gpu(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) override {
         fn2_tensor b0 = bottom[0]->tensor(), b1 = b0;
         if (bottom.size() > 1) b1 = bottom[1]->tensor();
-        FN2_CALL(fn2_l1loss_forward(&b0, bottom.size() > 1 ? &b1 : nullptr, &d_, state_, top[0]->mutable_gpu_data(), ws_, ws_bytes_, S()));
+        FN2_CALL(fn2_l1loss_forward(&b0, bottom.size() > 1 ? &b1 : nullptr, &d_, state_.as<float>(), top[0]->mutable_gpu_data(), ws_.get(),
+                                    ws_.bytes(), S()));
     }
     void Backward_gpu(const vector<Blob<Dtype>*>& top, const vector<bool>& propagate_down, const vector<Blob<Dtype>*>& bottom) override {
         const bool p0 = propagate_down[0], p1 = bottom.size() > 1 && propagate_down[1];
@@ -1313,14 +1298,12 @@ class L1LossLayer : public Layer<Dtype> {
         if (p0) d0 = bottom[0]->diff_tensor();
         if (p1) d1 = bottom[1]->diff_tensor();
         fn2_tensor td = top[0]->diff_tensor();
-        FN2_CALL(fn2_l1loss_backward(&b0, bottom.size() > 1 ? &b1 : nullptr, &d_, state_, td.data, p0 ? &d0 : nullptr, p1 ? &d1 : nullptr,
+        FN2_CALL(fn2_l1loss_backward(&b0, bottom.size() > 1 ? &b1 : nullptr, &d_, state_.as<float>(), td.data, p0 ? &d0 : nullptr, p1 ? &d1 : nullptr,
                                      this->bottom_accumulate_[0] ? 1 : 0, bottom.size() > 1 && this->bottom_accumulate_[1] ? 1 : 0, S()));
     }
  protected:
     fn2_l1loss_desc d_;
-    float* state_ = nullptr;
-    void* ws_ = nullptr;
-    size_t ws_bytes_ = 0;
+    DeviceBuffer state_, ws_;
 };
 REGISTER_LAYER_CLASS(L1Loss);
 
@@ -1357,7 +1340,6 @@ template <typename Dtype>
 class FlowAugmentationLayer : public Layer<Dtype> {
  public:
     explicit FlowAugmentationLayer(const LayerParameter& p) : Layer<Dtype>(p) {}
-    ~FlowAugmentationLayer() override { if (mats_dev_) cudaFree(mats_dev_); if (mats_host_) cudaFreeHost(mats_host_); }
     const char* type() const override { return "FlowAugmentation"; }
     bool AllowBackward() const override { return false; }             // flow_augmentation_layer.hpp
     bool GraphSafe() const override { return false; }                 // the matrices come from host blobs every pass
@@ -1376,13 +1358,8 @@ class FlowAugmentationLayer : public Layer<Dtype> {
         cw_ = aug.crop_width(); ch_ = aug.crop_height();
         const int num = bottom[0]->num();
         top[0]->Reshape(num, 2, ch_, cw_);
-        if (num > cap_) {
-            if (mats_dev_) cudaFree(mats_dev_);
-            if (mats_host_) cudaFreeHost(mats_host_);
-            CUDA_CHECK(cudaMalloc(&mats_dev_, (size_t)num * 12 * sizeof(float)));
-            CUDA_CHECK(cudaMallocHost(&mats_host_, (size_t)num * 12 * sizeof(float)));
-            cap_ = num;
-        }
+        mats_dev_.reserve((size_t)num * 12 * sizeof(float));
+        mats_host_.reserve((size_t)num * 12 * sizeof(float));
     }
     void Forward_gpu(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) override {
         const int num = bottom[0]->num();
@@ -1394,19 +1371,19 @@ class FlowAugmentationLayer : public Layer<Dtype> {
         for (int n = 0; n < num; n++) {
             const TransMat m1 = TransMatFromArray(p1 + (size_t)n * AugCoeff::N, cw_, ch_, bottom[0]->width(), bottom[0]->height());
             const TransMat m2 = TransMatInverse(TransMatFromArray(p2 + (size_t)n * AugCoeff::N, cw_, ch_, bottom[0]->width(), bottom[0]->height()));
-            float* a = mats_host_ + 6 * n;
-            float* b = mats_host_ + 6 * num + 6 * n;
+            float* a = mats_host_.as<float>() + 6 * n;
+            float* b = mats_host_.as<float>() + 6 * num + 6 * n;
             a[0] = m1.t0; a[1] = m1.t1; a[2] = m1.t2; a[3] = m1.t3; a[4] = m1.t4; a[5] = m1.t5;
             b[0] = m2.t0; b[1] = m2.t1; b[2] = m2.t2; b[3] = m2.t3; b[4] = m2.t4; b[5] = m2.t5;
         }
-        CUDA_CHECK(cudaMemcpyAsync(mats_dev_, mats_host_, (size_t)num * 12 * sizeof(float), cudaMemcpyHostToDevice, S()));
+        CUDA_CHECK(cudaMemcpyAsync(mats_dev_.get(), mats_host_.get(), (size_t)num * 12 * sizeof(float), cudaMemcpyHostToDevice, S()));
         fn2_tensor b = bottom[0]->tensor(), t = top[0]->mutable_tensor();
-        FN2_CALL(fn2_flow_augmentation(&b, &t, mats_dev_, mats_dev_ + 6 * num, S()));
+        FN2_CALL(fn2_flow_augmentation(&b, &t, mats_dev_.as<float>(), mats_dev_.as<float>() + 6 * num, S()));
     }
  protected:
-    int cw_ = 0, ch_ = 0, cap_ = 0;
-    float* mats_dev_ = nullptr;
-    float* mats_host_ = nullptr;
+    int cw_ = 0, ch_ = 0;
+    DeviceBuffer mats_dev_;
+    DeviceBuffer mats_host_{DeviceBuffer::PINNED_HOST};   // uploaded asynchronously
 };
 REGISTER_LAYER_CLASS(FlowAugmentation);
 
@@ -1451,18 +1428,9 @@ class GenerateAugmentationParametersLayer : public Layer<Dtype> {
         AugmentationParameter aug = this->layer_param_.augmentation_param();
         num_iter_++;
         const float dc = AugSampler::discount(this->layer_param_, (float)num_iter_);
-        bool spatial = false, chromatic = false, effect = false, eigen = false;
-        if (this->phase_ == TRAIN || aug.augment_during_test()) {
-            spatial = aug.has("mirror") || aug.has("rotate") || aug.has("zoom") || aug.has("translate") || aug.has("squeeze") ||
-                      aug.has("translate_x") || aug.has("translate_y");
-            chromatic = aug.has("brightness") || aug.has("gamma") || aug.has("contrast") || aug.has("color");
-            effect = aug.has("fog_size") || aug.has("fog_amount") || aug.has("motion_blur_angle") || aug.has("motion_blur_size") ||
-                     aug.has("shadow_angle") || aug.has("shadow_distance") || aug.has("shadow_strength") || aug.has("noise");
-            eigen = aug.has("lmult_pow") || aug.has("lmult_mult") || aug.has("lmult_add") || aug.has("sat_pow") || aug.has("sat_mult") ||
-                    aug.has("sat_add") || aug.has("col_pow") || aug.has("col_mult") || aug.has("col_add") || aug.has("ladd_pow") ||
-                    aug.has("ladd_mult") || aug.has("ladd_add") || aug.has("col_rotate");
-        }
-        if (spatial) CHECK(cw_ >= 1 && ch_ >= 1 && bw_ >= 1 && bh_ >= 1) << "Must provide crop and bottom sizes to do spatial augmentations";
+        AugGroups g = {false, false, false, false};
+        if (this->phase_ == TRAIN || aug.augment_during_test()) g = SampledGroups(aug);
+        if (g.spatial) CHECK(cw_ >= 1 && ch_ >= 1 && bw_ >= 1 && bh_ >= 1) << "Must provide crop and bottom sizes to do spatial augmentations";
         const bool use_in = mode_ == "add" || mode_ == "replace";
         const float* in = use_in ? bottom[0]->cpu_data() : nullptr;
         float* out = top[0]->mutable_cpu_data();
@@ -1470,7 +1438,7 @@ class GenerateAugmentationParametersLayer : public Layer<Dtype> {
         for (int n = 0; n < num_; n++) {
             AugCoeff c;
             if (use_in) c.from_array(in + (size_t)n * AugCoeff::N);
-            if (spatial) {
+            if (g.spatial) {
                 if (mode_ == "replace") for (int f = AugCoeff::MIRROR; f <= AugCoeff::ZOOM_Y; f++) c.clear(f);     // clear_spatial_coeffs
                 sampler_.generate_valid_spatial(aug, c, dc, bw_, bh_, cw_, ch_, 50);
             }
@@ -1489,18 +1457,12 @@ class GenerateAugmentationParametersLayer : public Layer<Dtype> {
                     for (int f = 0; f < AugCoeff::N; f++) o[f] += arr[f];
                 }
             };
-            group(chromatic, &AugSampler::generate_chromatic);
-            group(eigen, &AugSampler::generate_chromatic_eigen);
-            group(effect, &AugSampler::generate_effect);
+            group(g.chromatic, &AugSampler::generate_chromatic);
+            group(g.eigen, &AugSampler::generate_chromatic_eigen);
+            group(g.effect, &AugSampler::generate_effect);
         }
     }
  protected:
-    static uint32_t seed_of(const std::string& name) {
-        uint32_t h = 1701u;
-        if (const char* e = getenv("FN2_SEED")) h = (uint32_t)strtoul(e, nullptr, 10);
-        for (char c : name) h = h * 16777619u ^ (unsigned char)c;
-        return h;
-    }
     std::string mode_;
     int num_ = 0, cw_ = 0, ch_ = 0, bw_ = 0, bh_ = 0, num_iter_ = 0;
     AugSampler sampler_;

@@ -25,9 +25,6 @@ Net<Dtype>::~Net() {
     if (graph_) cudaGraphDestroy(graph_);
     layers_.clear();
     blobs_.clear();
-    for (auto& kv : staging_) if (kv.second.first) cudaFree(kv.second.first);
-    if (arena_) cudaFree(arena_);
-    if (diff_arena_) cudaFree(diff_arena_);
     for (cudaEvent_t e : layer_event_) if (e) cudaEventDestroy(e);
     if (fork_event_) cudaEventDestroy(fork_event_);
     if (join_event_) cudaEventDestroy(join_event_);
@@ -258,21 +255,23 @@ void Net<Dtype>::AliasConcats() {
     }
 }
 
+// Floats a parameter blob takes in the parameter and gradient arenas: every slot starts 256-byte aligned
+template <typename Dtype>
+static size_t arena_slot(const Blob<Dtype>& b) { return ((size_t)b.count() + 63) / 64 * 64; }
+
 template <typename Dtype>
 void Net<Dtype>::BuildArena() {
     size_t total = 0;
     for (auto& l : layers_)
-        for (auto& b : l->blobs()) total += ((size_t)b->count() + 63) / 64 * 64;
+        for (auto& b : l->blobs()) total += arena_slot(*b);
     arena_floats_ = total;
     if (!total) return;
-    CUDA_CHECK(cudaMalloc(&arena_, total * sizeof(Dtype)));
-    CUDA_CHECK(cudaMemset(arena_, 0, total * sizeof(Dtype)));
-    CUDA_CHECK(cudaDeviceSynchronize());
+    arena_.reserve(total * sizeof(Dtype), stream_);
     size_t off = 0;
     for (auto& l : layers_)
         for (auto& b : l->blobs()) {
-            b->BindExternal(arena_ + off);
-            off += ((size_t)b->count() + 63) / 64 * 64;
+            b->BindExternal(arena_.as<Dtype>() + off);
+            off += arena_slot(*b);
         }
 }
 
@@ -663,21 +662,20 @@ void Net<Dtype>::PlanBackward() {
 
 template <typename Dtype>
 void Net<Dtype>::BuildDiffArena() {
-    if (diff_arena_ || !arena_floats_) return;
-    CUDA_CHECK(cudaMalloc(&diff_arena_, arena_floats_ * sizeof(Dtype)));
-    CUDA_CHECK(cudaMemset(diff_arena_, 0, arena_floats_ * sizeof(Dtype)));
+    if (!diff_arena_.empty() || !arena_floats_) return;
+    diff_arena_.reserve(arena_floats_ * sizeof(Dtype), stream_);
     size_t off = 0;
     for (auto& l : layers_)
         for (auto& b : l->blobs()) {
-            b->BindExternalDiff(diff_arena_ + off);
-            off += ((size_t)b->count() + 63) / 64 * 64;
+            b->BindExternalDiff(diff_arena_.as<Dtype>() + off);
+            off += arena_slot(*b);
         }
 }
 
 template <typename Dtype>
 void Net<Dtype>::ParamDiffArena(void** dev, size_t* bytes) {
     BuildDiffArena();
-    *dev = diff_arena_; *bytes = arena_floats_ * sizeof(Dtype);
+    *dev = diff_arena_.get(); *bytes = arena_floats_ * sizeof(Dtype);
 }
 
 // Parameters the backward pass writes (lr_mult != 0 in a layer that needs backward) as one range of the gradient arena: a
@@ -690,18 +688,18 @@ void Net<Dtype>::TrainableDiffSpan(void** dev, size_t* bytes) {
     size_t off = 0, lo = arena_floats_, hi = 0;
     for (size_t i = 0; i < layers_.size(); i++)
         for (size_t pi = 0; pi < layers_[i]->blobs().size(); pi++) {
-            const size_t padded = ((size_t)layers_[i]->blobs()[pi]->count() + 63) / 64 * 64;
+            const size_t padded = arena_slot(*layers_[i]->blobs()[pi]);
             if (layer_need[i] && lr_mult((int)i, (int)pi) != 0.f) { lo = std::min(lo, off); hi = off + padded; }
             off += padded;
         }
     if (hi == 0) lo = 0;
-    *dev = diff_arena_ + lo; *bytes = (hi - lo) * sizeof(Dtype);
+    *dev = diff_arena_.as<Dtype>() + lo; *bytes = (hi - lo) * sizeof(Dtype);
 }
 
 template <typename Dtype>
 void Net<Dtype>::ClearParamDiffs() {
     BuildDiffArena();
-    if (diff_arena_) CUDA_CHECK(cudaMemsetAsync(diff_arena_, 0, arena_floats_ * sizeof(Dtype), stream_));
+    if (!diff_arena_.empty()) CUDA_CHECK(cudaMemsetAsync(diff_arena_.get(), 0, arena_floats_ * sizeof(Dtype), stream_));
 }
 
 template <typename Dtype>
@@ -757,20 +755,9 @@ void Net<Dtype>::Sync() {
 
 template <typename Dtype>
 Dtype* Net<Dtype>::staging(const string& blob, size_t floats) {
-    auto& s = staging_[blob];
-    if (s.second < floats) {
-        if (s.first) cudaFree(s.first);
-        CUDA_CHECK(cudaMalloc(&s.first, floats * sizeof(Dtype)));
-        s.second = floats;
-    }
-    return s.first;
-}
-
-static fn2_tensor nchw_view(float* p, int n, int c, int h, int w) {
-    fn2_tensor t;
-    t.data = p; t.n = n; t.c = c; t.h = h; t.w = w;
-    t.sw = 1; t.sh = w; t.sc = (int64_t)h * w; t.sn = (int64_t)c * h * w;
-    return t;
+    DeviceBuffer& s = staging_[blob];
+    s.reserve(floats * sizeof(Dtype));
+    return s.as<Dtype>();
 }
 
 template <typename Dtype>

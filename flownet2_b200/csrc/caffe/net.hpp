@@ -39,7 +39,7 @@ class Net {
     void FillParams(uint64_t seed);
     void ParamsChanged();
     void ArenaWritten();                               // device arena overwritten externally (broadcast)
-    void ParamArena(void** dev, size_t* bytes) { *dev = arena_; *bytes = arena_floats_ * sizeof(Dtype); }
+    void ParamArena(void** dev, size_t* bytes) { *dev = arena_.get(); *bytes = arena_floats_ * sizeof(Dtype); }
 
     const vector<string>& layer_names() const { return layer_names_; }
     const vector<shared_ptr<Layer<Dtype> > >& layers() const { return layers_; }
@@ -89,7 +89,7 @@ class Net {
     vector<vector<bool> > bw_propagate_, bw_accumulate_;
     vector<int> bw_zero_;
     std::set<int> bw_seeds_;
-    Dtype* diff_arena_ = nullptr;
+    DeviceBuffer diff_arena_;
     int launches_per_backward_ = 0;
 
     Phase phase_;
@@ -102,7 +102,7 @@ class Net {
     vector<string> blob_names_;
     std::map<string, int> blob_names_index_;
     vector<int> net_input_blob_indices_, net_output_blob_indices_;
-    Dtype* arena_ = nullptr;
+    DeviceBuffer arena_;
     size_t arena_floats_ = 0;
     cudaStream_t stream_ = nullptr;
     // second stream for layers off the critical path (FlowNet2: the FlowNet-SD branch next to the C-S-S chain), so that
@@ -119,7 +119,7 @@ class Net {
     bool graph_disabled_ = false;
     bool params_ready_ = false;
     int launches_per_forward_ = 0;
-    std::map<string, std::pair<Dtype*, size_t> > staging_;
+    std::map<string, DeviceBuffer> staging_;
 };
 
 }  // namespace caffe

@@ -49,6 +49,9 @@ FN2_API const char* fn2_version(void);
 /* Number of kernels launched by this library on the calling thread since process start
  * (bench.py's gpu_launches). */
 FN2_API uint64_t fn2_launch_count(void);
+/* Allocations the Caffe-surface host has made since process start (device and pinned host blocks); *live_bytes (if not
+ * NULL) receives the bytes it holds now.  For tests of steady-state allocation and leaks. */
+FN2_API uint64_t fn2_device_allocations(uint64_t* live_bytes);
 
 /* ------------------------------------------------------------------------------------ */
 /* Correlation -- replaces CorrelationLayer::Forward_gpu / Backward_gpu                  */
