@@ -1012,15 +1012,22 @@ __global__ void wg_reduce_kernel(const float* __restrict__ part, float* __restri
     }
 }
 
+// the layer shapes the weight-gradient engine takes (engine 1 = `engine: CAFFE`: exact-FP32 SIMT everywhere)
+int conv_tc_wgrad_takes(const fn2_conv_desc* d) {
+    return d->engine != 1 && d->kh * d->kw <= 49 && d->stride_w <= 8 && d->stride_h <= 8;
+}
 int conv_tc_wgrad_eligible(const fn2_conv_desc* d) {
-    if (!tc_enabled() || d->engine == 1) return 0;      // engine 1 = `engine: CAFFE`: exact-FP32 SIMT everywhere
-    if (d->kh * d->kw > 49 || d->stride_w > 8 || d->stride_h > 8) return 0;
-    if (!tc_encode_fn()) return 0;
-    return 1;
+    return tc_enabled() && conv_tc_wgrad_takes(d) && tc_encode_fn() ? 1 : 0;
 }
 size_t conv_tc_wgrad_workspace_floats(const fn2_conv_desc* d, int N, int H, int W) {
     const WgPlan g = wg_plan(d, N, H, W);
     return g.big_floats + g.small_floats + g.part_floats + g.bias_floats + 64;
+}
+// plan8 of fn2_conv_wgrad_plan for the tensor-core route: {2, NT, G, TG, BT, ST, S, bias blocks (0 without a bias)}
+void conv_tc_wgrad_plan(const fn2_conv_desc* d, int N, int H, int W, int32_t* out8) {
+    const WgPlan g = wg_plan(d, N, H, W);
+    out8[0] = 2; out8[1] = g.NT; out8[2] = g.G; out8[3] = g.TG; out8[4] = g.BT; out8[5] = g.ST; out8[6] = g.S;
+    out8[7] = d->has_bias ? g.bias_blocks : 0;
 }
 
 int conv_tc_wgrad(const fn2_conv_desc* d, const T4& bottom, const T4& top_diff, float* dw, float* db, int accumulate, float* ws,

@@ -10,8 +10,10 @@
 namespace fn2 {
 
 // fn2_conv_tc.cu: weight gradient on the wgmma pipeline
+int conv_tc_wgrad_takes(const fn2_conv_desc* d);
 int conv_tc_wgrad_eligible(const fn2_conv_desc* d);
 size_t conv_tc_wgrad_workspace_floats(const fn2_conv_desc* d, int N, int H, int W);
+void conv_tc_wgrad_plan(const fn2_conv_desc* d, int N, int H, int W, int32_t* out8);
 int conv_tc_wgrad(const fn2_conv_desc* d, const T4& bottom, const T4& top_diff, float* dw, float* db, int accumulate, float* ws,
                   size_t ws_floats, cudaStream_t st);
 
@@ -70,6 +72,16 @@ struct WgP {
 };
 constexpr int WG_T = 64, WG_PX = 16;
 constexpr int BIAS_CHUNKS = 296;                   // two blocks per SM
+
+// pixel ranges of the SIMT weight gradient: about 4 CTAs per SM over the (a, b, tap) tiles, at most 64, >= 256 pixels each
+int simt_wgrad_splits(const fn2_conv_desc* d, int N, int Hs, int Ws) {
+    const long long P = (long long)N * Hs * Ws;
+    const int A = d->deconv ? d->ci : d->co, Bc = d->deconv ? d->co : d->ci;
+    const int tiles = ((A + WG_T - 1) / WG_T) * ((Bc + WG_T - 1) / WG_T) * d->kh * d->kw;
+    int splits = (int)max(1LL, min((long long)64, (long long)(num_sms() * 4) / max(1, tiles)));
+    splits = (int)min((long long)splits, (P + 255) / 256);
+    return max(splits, 1);
+}
 
 __global__ void __launch_bounds__(256) weight_grad_kernel(T4 S, T4 B, float* __restrict__ ws, WgP p) {
     __shared__ float sS[WG_PX][WG_T + 4], sB[WG_PX][WG_T + 4];
@@ -159,17 +171,27 @@ int fn2_conv_backward_params_workspace_bytes(const fn2_conv_desc* d, int N, int 
     int Ho, Wo;
     int rc = fn2_conv_out_shape(d, H, W, &Ho, &Wo);
     if (rc) return rc;
-    const int Hs = d->deconv ? H : Ho, Ws = d->deconv ? W : Wo;
-    const long long P = (long long)N * Hs * Ws;
-    const int A = d->deconv ? d->ci : d->co, Bc = d->deconv ? d->co : d->ci;
-    const int tiles = ((A + WG_T - 1) / WG_T) * ((Bc + WG_T - 1) / WG_T) * d->kh * d->kw;
-    int splits = (int)max(1LL, min((long long)64, (long long)(num_sms() * 4) / max(1, tiles)));
-    splits = (int)min((long long)splits, (P + 255) / 256);
-    if (splits < 1) splits = 1;
+    const int splits = simt_wgrad_splits(d, N, d->deconv ? H : Ho, d->deconv ? W : Wo);
     size_t wfloats = (size_t)splits * d->ci * d->co * d->kh * d->kw;
     if (conv_tc_wgrad_eligible(d)) wfloats = max(wfloats, conv_tc_wgrad_workspace_floats(d, N, H, W));
     const size_t bfloats = (size_t)BIAS_CHUNKS * d->co;
     *bytes = (wfloats + bfloats + 64) * sizeof(float);
+    return FN2_OK;
+}
+
+int fn2_conv_wgrad_plan(const fn2_conv_desc* d, int N, int H, int W, int32_t* plan8) {
+    FN2_CHECK_ARG(d && plan8, "conv_wgrad_plan: null argument");
+    int Ho, Wo;
+    int rc = fn2_conv_out_shape(d, H, W, &Ho, &Wo);
+    if (rc) return rc;
+    for (int i = 0; i < 8; i++) plan8[i] = 0;
+    if (conv_tc_wgrad_takes(d)) {
+        conv_tc_wgrad_plan(d, N, H, W, plan8);
+    } else {
+        plan8[0] = 1;
+        plan8[6] = simt_wgrad_splits(d, N, d->deconv ? H : Ho, d->deconv ? W : Wo);
+        plan8[7] = d->has_bias ? BIAS_CHUNKS : 0;
+    }
     return FN2_OK;
 }
 
@@ -193,9 +215,7 @@ int fn2_conv_backward_params(const fn2_conv_desc* d, const fn2_tensor* bottom, c
     p.Hs = S.h; p.Ws = S.w; p.Hb = B.h; p.Wb = B.w; p.N = x.n;
     const long long P = (long long)p.N * p.Hs * p.Ws;
     const int tiles = ((p.A + WG_T - 1) / WG_T) * ((p.Bc + WG_T - 1) / WG_T);
-    int splits = (int)max(1LL, min((long long)64, (long long)(num_sms() * 4) / max(1, tiles * d->kh * d->kw)));
-    splits = (int)min((long long)splits, (P + 255) / 256);
-    if (splits < 1) splits = 1;
+    const int splits = simt_wgrad_splits(d, p.N, p.Hs, p.Ws);
     p.splits = splits;
     p.per = ((P + splits - 1) / splits + WG_PX - 1) / WG_PX * WG_PX;
     float* ws = (float*)workspace;

@@ -236,20 +236,42 @@ def _conv_desc(weight, stride, pad, deconv, bias, engine=0):
     return fn2_conv_desc(ci, co, kh, kw, sh, sw, ph, pw, 1 if deconv else 0, 1 if bias else 0, 0, 0.0, engine, 0)
 
 
-def conv2d_backward(x, weight, top_diff, stride=1, pad=0, deconv=False, bias=True, need_input_grad=True, engine=0):
+def wgrad_plan(ci, co, k, stride, pad, deconv, n, h, w, engine=0, bias=True):
+    """fn2_conv_wgrad_plan: the weight-gradient route a layer shape takes (8 ints, see include/fn2.h): route (1 SIMT, 2 tensor
+    cores), NT, G, TG, BT, ST, S (SIMT: pixel splits), bias blocks.  k, stride, pad: an int or (h, w)."""
+    kh, kw = (k, k) if isinstance(k, int) else k
+    sh, sw = (stride, stride) if isinstance(stride, int) else stride
+    ph, pw = (pad, pad) if isinstance(pad, int) else pad
+    d = fn2_conv_desc(ci, co, kh, kw, sh, sw, ph, pw, 1 if deconv else 0, 1 if bias else 0, 0, 0.0, engine, 0)
+    plan = (C.c_int32 * 8)()
+    check(lib().fn2_conv_wgrad_plan(C.byref(d), n, h, w, plan))
+    return list(plan)
+
+
+def conv2d_backward(x, weight, top_diff, stride=1, pad=0, deconv=False, bias=True, need_input_grad=True, engine=0,
+                    accumulate=False, out=None, workspace=None):
     """ConvolutionLayer / DeconvolutionLayer::Backward_gpu (conv_layer.cu:26-58, deconv_layer.cu:26-55) through the C-ABI:
-    -> (bottom_diff or None, weight_diff, bias_diff or None)."""
+    -> (bottom_diff or None, weight_diff, bias_diff or None).
+    out=(weight_diff, bias_diff): write (accumulate: add) the parameter gradients there; a None bias_diff passes a null bias
+    pointer.  workspace: a uint8 CUDA tensor whose bytes are the workspace (default: one of the reported size)."""
     l = lib()
     d = _conv_desc(weight, stride, pad, deconv, bias, engine)
     weight = weight.contiguous()
-    wd = torch.zeros_like(weight)
-    bd = torch.zeros(d.co, dtype=torch.float32, device=x.device) if bias else None
-    nb = C.c_size_t()
-    check(l.fn2_conv_backward_params_workspace_bytes(C.byref(d), x.shape[0], x.shape[2], x.shape[3], C.byref(nb)))
-    ws = _ws(max(nb.value, 4), x.device)
+    if out is None:
+        wd = torch.zeros_like(weight)
+        bd = torch.zeros(d.co, dtype=torch.float32, device=x.device) if bias else None
+    else:
+        wd, bd = out
+        assert wd.is_contiguous() and wd.shape == weight.shape and (bd is None or bd.is_contiguous())
+    if workspace is None:
+        nb = C.c_size_t()
+        check(l.fn2_conv_backward_params_workspace_bytes(C.byref(d), x.shape[0], x.shape[2], x.shape[3], C.byref(nb)))
+        workspace = _ws(max(nb.value, 4), x.device)
+    assert workspace.dtype == torch.uint8 and workspace.is_contiguous()
     tx, tdy = desc(x), desc(top_diff)
     check(l.fn2_conv_backward_params(C.byref(d), C.byref(tx), C.byref(tdy), C.c_void_p(wd.data_ptr()),
-                                     C.c_void_p(bd.data_ptr()) if bias else None, 0, C.c_void_p(ws.data_ptr()), nb.value, _stream()))
+                                     C.c_void_p(bd.data_ptr()) if bd is not None else None, 1 if accumulate else 0,
+                                     C.c_void_p(workspace.data_ptr()), workspace.numel(), _stream()))
     dx = None
     if need_input_grad:
         bdsc, flip = fn2_conv_desc(), C.c_int()

@@ -211,6 +211,12 @@ FN2_API int fn2_conv_forward(const fn2_conv_desc* d, const fn2_tensor* bottom,
  *                              convolution's last window does not start at but still covers) and vice versa; run it with
  *                              fn2_conv_forward on the top diff: the result has exactly the bottom's shape. */
 FN2_API int fn2_conv_backward_params_workspace_bytes(const fn2_conv_desc* d, int N, int H, int W, size_t* bytes);
+/* Host-side plan of fn2_conv_backward_params for a layer shape (introspection; needs no GPU).  It reports the choice the layer
+ * shape makes, not whether this process can run the tensor cores.  "Small" is the top diff of a convolution and the bottom of
+ * a deconvolution, "big" the other map.  plan8 = {route (1 SIMT, 2 tensor cores), small channels per tile NT, big-map rows
+ * per tap G, tap groups TG, big-channel tiles BT, small-channel tiles ST, K ranges per tile S (SIMT: pixel splits), bias
+ * blocks (0 without a bias)}; the SIMT route leaves slots 1-5 at 0. */
+FN2_API int fn2_conv_wgrad_plan(const fn2_conv_desc* d, int N, int H, int W, int32_t* plan8);
 FN2_API int fn2_conv_backward_params(const fn2_conv_desc* d, const fn2_tensor* bottom, const fn2_tensor* top_diff,
                                      float* weight_diff_dev, float* bias_diff_dev, int accumulate, void* workspace,
                                      size_t workspace_bytes, void* stream);

@@ -229,6 +229,38 @@ def test_tensor_core_engine_split_plan_for_flownet2_shapes(fn2):
     assert pl == [0] * 8
 
 
+def test_weight_gradient_plan_for_flownet2_c_training_shapes(fn2):
+    """fn2_conv_wgrad_plan (no GPU needed) at the FlowNet2-C training shapes, 448x320 crops: {route (2 tensor cores, 1 SIMT),
+    small channels per tile NT, big-map rows per tap G, tap groups, big / small channel tiles, K ranges S, bias blocks}.  S
+    assumes the H100's 132 SMs (the count without a device)."""
+    from flownet2_b200 import ops
+
+    def plan(ci, co, k, s, p, H, W, deconv=False, N=1, engine=0, bias=True):
+        return ops.wgrad_plan(ci, co, k, s, p, deconv, N, H, W, engine, bias)
+
+    # conv1: 3 big channels -> 8 rows per tap, 16 taps per tile, 49 taps in 4 groups; the 224-wide top diff gives 2 bias column
+    # tiles per row; the reduction over 160 x 224 pixels runs in 99 K ranges, at batch 8 too
+    assert plan(3, 64, 7, 2, 3, 320, 448) == [2, 64, 8, 4, 1, 1, 99, 2 * 160]
+    assert plan(3, 64, 7, 2, 3, 320, 448, N=8) == [2, 64, 8, 4, 1, 1, 99, 2 * 160 * 8]
+    assert plan(3, 64, 7, 2, 3, 320, 448, bias=False)[7] == 0
+    # conv2 (64 -> 128, 5x5): two taps per 128-row tile
+    assert plan(64, 128, 5, 2, 2, 160, 224) == [2, 128, 64, 13, 1, 1, 31, 80]
+    # conv3_1 (473 -> 256): 4 big-channel tiles (the last with 89 rows), 2 small-channel tiles
+    assert plan(473, 256, 3, 1, 1, 40, 56) == [2, 128, 128, 9, 4, 2, 6, 40]
+    # conv6_1 (1024 -> 1024 on 5 x 7): 576 tile units fill the GPU, one K range
+    assert plan(1024, 1024, 3, 1, 1, 5, 7) == [2, 128, 128, 9, 8, 8, 1, 5]
+    # deconv2 (386 -> 64, 4x4 stride 2): the small map is the 386-channel bottom; the bias comes from the 112-wide top diff's
+    # two parity planes per row
+    assert plan(386, 64, 4, 2, 1, 40, 56, deconv=True) == [2, 128, 64, 8, 1, 4, 10, 160]
+    # predict_flow2 (194 -> 2): NT 16
+    assert plan(194, 2, 3, 1, 1, 80, 112)[:6] == [2, 16, 128, 9, 2, 1]
+    # the SIMT route: `engine: CAFFE` (49 tiles of 64 x 64 (a, b) pairs, one per tap: 528 // 49 = 10 pixel ranges), more than
+    # 49 taps, a stride above 8
+    assert plan(3, 64, 7, 2, 3, 320, 448, engine=1) == [1, 0, 0, 0, 0, 0, 10, 296]
+    assert plan(16, 32, 9, 1, 4, 24, 40)[0] == 1 and plan(8, 16, 3, 9, 1, 30, 50)[0] == 1
+    assert plan(16, 32, 9, 1, 4, 24, 40)[6] == 4
+
+
 def test_tensor_core_engine_plan_golden(fn2):
     """fn2_conv_plan over a sweep of conv / deconv descriptors (tests/golden/make_conv_plan_golden.py): engine, NT, tiles, K
     steps, small-Ci mode and K split unchanged.  The workspace is unchanged too, except for layers that split every tile: their

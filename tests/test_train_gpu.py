@@ -82,22 +82,13 @@ def test_conv_backward_simt_engine(fn2, case):
 
 
 def test_conv_backward_params_accumulates(fn2):
-    import ctypes as C
     r = rng(5)
     x = r.standard_normal((2, 8, 10, 12)).astype(np.float32)
     w = r.standard_normal((16, 8, 3, 3)).astype(np.float32)
     dy = r.standard_normal((2, 16, 10, 12)).astype(np.float32)
     _, gw, gb = OPS.conv2d_backward(dev(x, True), dev(w), dev(dy, True), 1, 1, False, need_input_grad=False)
-    l = fn2.lib()
-    d = OPS._conv_desc(dev(w), 1, 1, False, True)
-    nb = C.c_size_t()
-    fn2.check(l.fn2_conv_backward_params_workspace_bytes(C.byref(d), 2, 10, 12, C.byref(nb)))
-    ws = torch.empty(max(nb.value, 4), dtype=torch.uint8, device="cuda")
     gw2, gb2 = gw.clone(), gb.clone()
-    xx, dd = dev(x, True), dev(dy, True)
-    tx, tdy = OPS.desc(xx), OPS.desc(dd)
-    fn2.check(l.fn2_conv_backward_params(C.byref(d), C.byref(tx), C.byref(tdy), C.c_void_p(gw2.data_ptr()), C.c_void_p(gb2.data_ptr()),
-                                         1, C.c_void_p(ws.data_ptr()), nb.value, None))
+    OPS.conv2d_backward(dev(x, True), dev(w), dev(dy, True), 1, 1, False, need_input_grad=False, accumulate=True, out=(gw2, gb2))
     torch.cuda.synchronize()
     assert rel(gw2.cpu().numpy(), 2 * gw.cpu().numpy()) <= 1e-6
     assert rel(gb2.cpu().numpy(), 2 * gb.cpu().numpy()) <= 1e-6
