@@ -11,29 +11,22 @@ any compute call without the built library or without a GPU raises.
 import ctypes as C
 import math
 import os
-import re
 
 import numpy as np
+
+from ._abi import read_header
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB = None
 TRAIN, TEST = 0, 1
 
+with open(os.path.join(os.path.dirname(_HERE), "include", "fn2.h")) as _f:
+    _STRUCTS, _PROTOTYPES = read_header(_f.read())
+fn2_tensor, fn2_conv_desc, fn2_l1loss_desc = (_STRUCTS[n] for n in ("fn2_tensor", "fn2_conv_desc", "fn2_l1loss_desc"))
+
 
 class Fn2Error(RuntimeError):
     pass
-
-
-class fn2_tensor(C.Structure):
-    _fields_ = [("data", C.c_void_p), ("n", C.c_int32), ("c", C.c_int32), ("h", C.c_int32), ("w", C.c_int32),
-                ("sn", C.c_int64), ("sc", C.c_int64), ("sh", C.c_int64), ("sw", C.c_int64)]
-
-
-class fn2_conv_desc(C.Structure):
-    _fields_ = [("ci", C.c_int32), ("co", C.c_int32), ("kh", C.c_int32), ("kw", C.c_int32),
-                ("stride_h", C.c_int32), ("stride_w", C.c_int32), ("pad_h", C.c_int32), ("pad_w", C.c_int32),
-                ("deconv", C.c_int32), ("has_bias", C.c_int32), ("relu", C.c_int32), ("negative_slope", C.c_float),
-                ("engine", C.c_int32), ("input_guard_bytes", C.c_int32), ("out_pad_h", C.c_int32), ("out_pad_w", C.c_int32)]
 
 
 def lib_path():
@@ -49,78 +42,9 @@ def lib():
             raise Fn2Error("libfn2.so is not built (%s); run `python -m flownet2_b200.build` -- there is no "
                            "CPU/PyTorch fallback" % p)
         l = C.CDLL(p)
-        l.fn2_last_error.restype = C.c_char_p
-        l.fn2_version.restype = C.c_char_p
-        l.fn2_launch_count.restype = C.c_uint64
-        l.fn2_device_allocations.restype = C.c_uint64
-        l.fn2_device_allocations.argtypes = [C.POINTER(C.c_uint64)]
-        for name in ("fn2_net_input_name", "fn2_net_output_name", "fn2_net_blob_name", "fn2_net_layer_name",
-                     "fn2_net_layer_type"):
-            getattr(l, name).restype = C.c_char_p
-            getattr(l, name).argtypes = [C.c_void_p, C.c_int]
-        l.fn2_net_stream.restype = C.c_void_p
-        l.fn2_net_stream.argtypes = [C.c_void_p]
-        l.fn2_net_create_batch.argtypes = [C.c_char_p, C.c_int, C.c_int, C.POINTER(C.c_void_p)]
-        l.fn2_net_destroy.argtypes = [C.c_void_p]
-        l.fn2_net_destroy.restype = None
-        for name in ("fn2_net_num_inputs", "fn2_net_num_outputs", "fn2_net_num_blobs", "fn2_net_num_layers",
-                     "fn2_net_forward", "fn2_net_sync", "fn2_net_params_changed", "fn2_net_launches_per_forward",
-                     "fn2_net_graph_active", "fn2_net_backward", "fn2_net_clear_param_diffs", "fn2_net_launches_per_backward"):
-            getattr(l, name).argtypes = [C.c_void_p]
-        l.fn2_net_param_diff_arena.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t)]
-        l.fn2_net_trainable_diff_span.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t)]
-        l.fn2_net_set_diff.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p]
-        l.fn2_net_get_diff.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p]
-        l.fn2_net_param_shape.argtypes = [C.c_void_p, C.c_char_p, C.c_int, C.POINTER(C.c_int)]
-        l.fn2_net_get_param.argtypes = [C.c_void_p, C.c_char_p, C.c_int, C.c_int, C.c_void_p]
-        l.fn2_net_layer_need_backward.argtypes = [C.c_void_p, C.c_int]
-        l.fn2_net_copy_trained_layers.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
-        l.fn2_net_copy_trained_layers_prefixed.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_char_p]
-        l.fn2_net_to_caffemodel.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_size_t)]
-        l.fn2_net_to_hdf5.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_size_t)]
-        l.fn2_caffemodel_to_hdf5.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_size_t)]
-        l.fn2_hdf5_summary.argtypes = [C.c_void_p, C.c_size_t, C.c_char_p, C.POINTER(C.c_size_t)]
-        l.fn2_net_fill_params.argtypes = [C.c_void_p, C.c_uint64]
-        l.fn2_net_param_arena.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t)]
-        l.fn2_net_blob_shape.argtypes = [C.c_void_p, C.c_char_p, C.POINTER(C.c_int)]
-        for name in ("fn2_net_set_input", "fn2_net_get_blob", "fn2_net_set_input_device", "fn2_net_get_blob_device"):
-            getattr(l, name).argtypes = [C.c_void_p, C.c_char_p, C.c_void_p]
-        l.fn2_net_time_layers.argtypes = [C.c_void_p, C.c_void_p]
-        l.fn2_net_layer_work.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double)]
-        T = C.POINTER(fn2_tensor)
-        l.fn2_correlation_forward.argtypes = [T, T, T, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
-                                              C.c_void_p, C.c_size_t, C.c_void_p]
-        l.fn2_correlation_backward.argtypes = [T, T, T, T, T, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
-        l.fn2_correlation_workspace_bytes.argtypes = [C.c_int] * 10 + [C.POINTER(C.c_size_t)]
-        l.fn2_correlation_shape.argtypes = [C.c_int] * 7 + [C.POINTER(C.c_int)] * 3
-        l.fn2_flow_warp_forward.argtypes = [T, T, T, C.c_int, C.c_void_p]
-        l.fn2_flow_warp_backward.argtypes = [T, T, T, T, T, C.c_void_p]
-        l.fn2_resample_forward.argtypes = [T, T, C.c_int, C.c_int, C.c_void_p]
-        l.fn2_spatial_augmentation.argtypes = [T, T, C.c_void_p, C.c_void_p]
-        l.fn2_color_contrast_augmentation.argtypes = [T, C.c_void_p, C.c_float, C.c_void_p]
-        l.fn2_mean_update.argtypes = [T, T, C.c_void_p, C.c_float, C.c_void_p]
-        l.fn2_mean_subtract.argtypes = [T, T, C.c_void_p, C.c_int, C.c_void_p]
-        D = C.POINTER(fn2_conv_desc)
-        l.fn2_conv_packed_floats.argtypes = [D, C.c_int, C.POINTER(C.c_size_t)]
-        l.fn2_conv_pack_weights.argtypes = [D, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
-        l.fn2_conv_out_shape.argtypes = [D, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
-        l.fn2_conv_forward.argtypes = [D, T, C.c_void_p, C.c_void_p, T, C.c_void_p, C.c_size_t, C.c_void_p]
-        l.fn2_conv_workspace_bytes.argtypes = [D, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t)]
-        l.fn2_relu_forward.argtypes = [T, T, C.c_float, C.c_void_p]
-        l.fn2_relu_backward.argtypes = [T, T, T, C.c_float, C.c_int, C.c_void_p]
-        l.fn2_axpby.argtypes = [T, C.c_float, T, C.c_float, C.c_void_p]
-        l.fn2_conv_backward_params_workspace_bytes.argtypes = [D, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t)]
-        l.fn2_conv_backward_params.argtypes = [D, T, T, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]
-        l.fn2_conv_backward_data_desc.argtypes = [D, C.c_int, C.c_int, D, C.POINTER(C.c_int)]
-        l.fn2_conv_flip_transpose_weights.argtypes = [D, C.c_void_p, C.c_void_p, C.c_void_p]
-        l.fn2_eltwise_sum.argtypes = [C.POINTER(T), C.POINTER(C.c_float), C.c_int, T, C.c_void_p]
-        l.fn2_channel_norm_forward.argtypes = [T, T, C.c_void_p]
-        l.fn2_warp_block_forward.argtypes = [T] * 8 + [C.c_float, C.c_int, C.c_void_p]
-        l.fn2_downsample_forward.argtypes = [T, T, C.c_void_p]
-        l.fn2_copy.argtypes = [T, T, C.c_void_p]
-        l.fn2_fill.argtypes = [T, C.c_float, C.c_void_p]
-        l.fn2_write_flo.argtypes = [C.c_char_p, C.c_void_p, C.c_int, C.c_int]
-        l.fn2_read_flo.argtypes = [C.c_char_p, C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_size_t]
+        for name, (restype, argtypes) in _PROTOTYPES.items():
+            f = getattr(l, name)
+            f.restype, f.argtypes = restype, argtypes
         _LIB = l
     return _LIB
 
@@ -128,6 +52,23 @@ def lib():
 def check(rc):
     if rc != 0:
         raise Fn2Error("fn2 error %d: %s" % (rc, lib().fn2_last_error().decode("utf-8", "replace")))
+
+
+def sized_output(fn, *args):
+    """The size-query convention: fn(*args, NULL, &bytes) reports the size, fn(*args, buf, &bytes) fills buf -> its bytes
+    (a text output's bytes include the terminating NUL)."""
+    n = C.c_size_t(0)
+    check(fn(*args, None, C.byref(n)))
+    buf = C.create_string_buffer(n.value)
+    check(fn(*args, buf, C.byref(n)))
+    return buf.raw[:n.value]
+
+
+def out_span(fn, *args):
+    """fn(*args, &dev_ptr, &bytes) -> (dev_ptr, bytes): the parameter and gradient arenas."""
+    p, n = C.c_void_p(), C.c_size_t()
+    check(fn(*args, C.byref(p), C.byref(n)))
+    return p.value, n.value
 
 
 def launch_count():
@@ -264,24 +205,14 @@ class Net(object):
         check(lib().fn2_net_fill_params(self._h, int(seed)))
 
     def to_caffemodel(self):
-        n = C.c_size_t(0)
-        check(lib().fn2_net_to_caffemodel(self._h, None, C.byref(n)))
-        buf = (C.c_char * n.value)()
-        check(lib().fn2_net_to_caffemodel(self._h, buf, C.byref(n)))
-        return bytes(buf[:n.value])
+        return sized_output(lib().fn2_net_to_caffemodel, self._h)
 
     def to_hdf5(self):
         """Net::ToHDF5 (net.cpp:905-960): the weights as the bytes of a .caffemodel.h5 file."""
-        n = C.c_size_t(0)
-        check(lib().fn2_net_to_hdf5(self._h, None, C.byref(n)))
-        buf = (C.c_char * n.value)()
-        check(lib().fn2_net_to_hdf5(self._h, buf, C.byref(n)))
-        return bytes(buf[:n.value])
+        return sized_output(lib().fn2_net_to_hdf5, self._h)
 
     def param_arena(self):
-        p, n = C.c_void_p(), C.c_size_t()
-        check(lib().fn2_net_param_arena(self._h, C.byref(p), C.byref(n)))
-        return p.value, n.value
+        return out_span(lib().fn2_net_param_arena, self._h)
 
     def params_changed(self):
         check(lib().fn2_net_params_changed(self._h))
@@ -345,15 +276,11 @@ class Net(object):
         return out
 
     def param_diff_arena(self):
-        p, n = C.c_void_p(), C.c_size_t()
-        check(lib().fn2_net_param_diff_arena(self._h, C.byref(p), C.byref(n)))
-        return p.value, n.value
+        return out_span(lib().fn2_net_param_diff_arena, self._h)
 
     def trainable_diff_span(self):
         """(device pointer, bytes): the range of param_diff_arena() that holds every gradient the backward pass writes."""
-        p, n = C.c_void_p(), C.c_size_t()
-        check(lib().fn2_net_trainable_diff_span(self._h, C.byref(p), C.byref(n)))
-        return p.value, n.value
+        return out_span(lib().fn2_net_trainable_diff_span, self._h)
 
     def layer_need_backward(self):
         return [bool(lib().fn2_net_layer_need_backward(self._h, i)) for i in range(len(self.layer_names))]

@@ -1,5 +1,6 @@
 // extern "C" net-level entry points of include/fn2.h over caffe::Net<float>.
 #include <cstring>
+#include <type_traits>
 
 #include "net.hpp"
 #include "hdf5_min.hpp"
@@ -22,6 +23,29 @@ struct fn2_net {
         return strstr(e.what(), "Unknown") ? FN2_ERR_NOTFOUND : FN2_ERR_INVALID; \
     }
 
+// A status-returning net entry point: FN2_ERR_INVALID if an argument is null, else f() (FN2_OK if it returns nothing) with
+// its exceptions mapped to a status, so none crosses the extern "C" boundary.
+template <class F>
+static int net_call(const char* what, bool args_ok, F&& f) {
+    if (!args_ok) { fn2::set_error("%s: null argument", what); return FN2_ERR_INVALID; }
+    FN2_TRY
+        if constexpr (std::is_void<decltype(f())>::value) { f(); return FN2_OK; }
+        else return f();
+    FN2_CATCH
+}
+
+// The size-query convention: out == NULL reports the size in *bytes; otherwise out receives the output if *bytes holds it.
+// A text output includes its terminating NUL.
+static int emit(const char* what, const std::string& s, bool text, void* out, size_t* bytes) {
+    if (!bytes) { fn2::set_error("%s: null size pointer", what); return FN2_ERR_INVALID; }
+    const size_t n = s.size() + (text ? 1 : 0);
+    if (!out) { *bytes = n; return FN2_OK; }
+    if (*bytes < n) { fn2::set_error("%s: buffer too small", what); return FN2_ERR_INVALID; }
+    memcpy(out, s.c_str(), n);
+    *bytes = n;
+    return FN2_OK;
+}
+
 namespace caffe { void SampleAugmentationCoeffs(const LayerParameter& lp, uint32_t seed, int num, int width, int height, float num_iter, float* out); }
 
 extern "C" {
@@ -31,9 +55,8 @@ int fn2_net_create(const char* prototxt_text, int phase, fn2_net** out) {
 }
 
 int fn2_net_create_batch(const char* prototxt_text, int phase, int batch, fn2_net** out) {
-    if (!prototxt_text || !out) { fn2::set_error("net_create: null argument"); return FN2_ERR_INVALID; }
-    *out = nullptr;
-    FN2_TRY
+    return net_call("net_create", prototxt_text && out, [&] {
+        *out = nullptr;
         caffe::NetParameter np = caffe::NetParameter::FromText(prototxt_text);
         if (batch > 0) {
             for (auto& lp : np.layers) {
@@ -50,62 +73,41 @@ int fn2_net_create_batch(const char* prototxt_text, int phase, int batch, fn2_ne
         for (int i : h->net->input_blob_indices()) h->input_names.push_back(h->net->blob_names()[i]);
         for (int i : h->net->output_blob_indices()) h->output_names.push_back(h->net->blob_names()[i]);
         *out = h.release();
-        return FN2_OK;
-    FN2_CATCH
+    });
 }
 
 void fn2_net_destroy(fn2_net* net) { delete net; }
 
 int fn2_net_copy_trained_layers(fn2_net* net, const void* caffemodel, size_t bytes) {
-    if (!net || !caffemodel) { fn2::set_error("copy_trained_layers: null argument"); return FN2_ERR_INVALID; }
-    FN2_TRY
-        net->net->CopyTrainedLayersFrom(caffemodel, bytes);
-        return FN2_OK;
-    FN2_CATCH
+    return net_call("copy_trained_layers", net && caffemodel, [&] { net->net->CopyTrainedLayersFrom(caffemodel, bytes); });
 }
 
 int fn2_net_copy_trained_layers_prefixed(fn2_net* net, const void* caffemodel, size_t bytes, const char* prefix) {
-    if (!net || !caffemodel || !prefix) { fn2::set_error("copy_trained_layers_prefixed: null argument"); return FN2_ERR_INVALID; }
-    FN2_TRY
-        net->net->CopyTrainedLayersFrom(caffemodel, bytes, prefix);
-        return FN2_OK;
-    FN2_CATCH
+    return net_call("copy_trained_layers_prefixed", net && caffemodel && prefix,
+                    [&] { net->net->CopyTrainedLayersFrom(caffemodel, bytes, prefix); });
 }
 
 int fn2_net_to_caffemodel(fn2_net* net, void* buf, size_t* bytes) {
-    if (!net || !bytes) { fn2::set_error("to_caffemodel: null argument"); return FN2_ERR_INVALID; }
-    FN2_TRY
-        if (!buf || net->caffemodel_cache.empty()) net->caffemodel_cache = net->net->ToCaffemodel();
-        if (!buf) { *bytes = net->caffemodel_cache.size(); return FN2_OK; }
-        if (*bytes < net->caffemodel_cache.size()) { fn2::set_error("to_caffemodel: buffer too small"); return FN2_ERR_INVALID; }
-        memcpy(buf, net->caffemodel_cache.data(), net->caffemodel_cache.size());
-        *bytes = net->caffemodel_cache.size();
-        net->caffemodel_cache.clear();
-        net->caffemodel_cache.shrink_to_fit();
-        return FN2_OK;
-    FN2_CATCH
+    return net_call("to_caffemodel", net && bytes, [&] {
+        std::string& cache = net->caffemodel_cache;        // serialised once for the query and the fill call
+        if (!buf || cache.empty()) cache = net->net->ToCaffemodel();
+        const int rc = emit("to_caffemodel", cache, false, buf, bytes);
+        if (buf && rc == FN2_OK) { cache.clear(); cache.shrink_to_fit(); }
+        return rc;
+    });
 }
 
 int fn2_net_fill_params(fn2_net* net, uint64_t seed) {
-    if (!net) { fn2::set_error("fill_params: null net"); return FN2_ERR_INVALID; }
-    FN2_TRY
-        net->net->FillParams(seed);
-        return FN2_OK;
-    FN2_CATCH
+    return net_call("fill_params", net, [&] { net->net->FillParams(seed); });
 }
 
 int fn2_net_param_arena(fn2_net* net, void** dev_ptr, size_t* bytes) {
-    if (!net || !dev_ptr || !bytes) { fn2::set_error("param_arena: null argument"); return FN2_ERR_INVALID; }
-    net->net->ParamArena(dev_ptr, bytes);
-    return FN2_OK;
+    return net_call("param_arena", net && dev_ptr && bytes, [&] { net->net->ParamArena(dev_ptr, bytes); });
 }
 
 int fn2_net_params_changed(fn2_net* net) {
-    if (!net) { fn2::set_error("params_changed: null net"); return FN2_ERR_INVALID; }
-    FN2_TRY
-        net->net->ArenaWritten();      // the caller wrote the DEVICE arena: host caches of every param blob are stale
-        return FN2_OK;
-    FN2_CATCH
+    // the caller wrote the DEVICE arena: host caches of every param blob are stale
+    return net_call("params_changed", net, [&] { net->net->ArenaWritten(); });
 }
 
 int fn2_net_num_inputs(fn2_net* net) { return net ? (int)net->input_names.size() : 0; }
@@ -129,91 +131,39 @@ const char* fn2_net_layer_type(fn2_net* net, int i) {
 }
 
 int fn2_net_blob_shape(fn2_net* net, const char* blob, int shape[4]) {
-    if (!net || !blob || !shape) { fn2::set_error("blob_shape: null argument"); return FN2_ERR_INVALID; }
-    FN2_TRY
+    return net_call("blob_shape", net && blob && shape, [&] {
         auto b = net->net->blob_by_name(blob);
         for (int i = 0; i < 4; i++) shape[i] = b->shape(i);
-        return FN2_OK;
-    FN2_CATCH
+    });
 }
 
 int fn2_net_set_input(fn2_net* net, const char* blob, const float* host_nchw) {
-    if (!net || !blob || !host_nchw) { fn2::set_error("set_input: null argument"); return FN2_ERR_INVALID; }
-    FN2_TRY
-        net->net->SetInput(blob, host_nchw);
-        return FN2_OK;
-    FN2_CATCH
+    return net_call("set_input", net && blob && host_nchw, [&] { net->net->SetInput(blob, host_nchw); });
 }
 int fn2_net_set_input_device(fn2_net* net, const char* blob, const float* dev_nchw) {
-    if (!net || !blob || !dev_nchw) { fn2::set_error("set_input_device: null argument"); return FN2_ERR_INVALID; }
-    FN2_TRY
-        net->net->SetInputDevice(blob, dev_nchw);
-        return FN2_OK;
-    FN2_CATCH
+    return net_call("set_input_device", net && blob && dev_nchw, [&] { net->net->SetInputDevice(blob, dev_nchw); });
 }
 int fn2_net_get_blob(fn2_net* net, const char* blob, float* host_nchw) {
-    if (!net || !blob || !host_nchw) { fn2::set_error("get_blob: null argument"); return FN2_ERR_INVALID; }
-    FN2_TRY
-        net->net->GetBlob(blob, host_nchw);
-        return FN2_OK;
-    FN2_CATCH
+    return net_call("get_blob", net && blob && host_nchw, [&] { net->net->GetBlob(blob, host_nchw); });
 }
 int fn2_net_get_blob_device(fn2_net* net, const char* blob, float* dev_nchw) {
-    if (!net || !blob || !dev_nchw) { fn2::set_error("get_blob_device: null argument"); return FN2_ERR_INVALID; }
-    FN2_TRY
-        net->net->GetBlobDevice(blob, dev_nchw);
-        return FN2_OK;
-    FN2_CATCH
+    return net_call("get_blob_device", net && blob && dev_nchw, [&] { net->net->GetBlobDevice(blob, dev_nchw); });
 }
 
-int fn2_net_forward(fn2_net* net) {
-    if (!net) { fn2::set_error("forward: null net"); return FN2_ERR_INVALID; }
-    FN2_TRY
-        net->net->Forward();
-        return FN2_OK;
-    FN2_CATCH
-}
-int fn2_net_backward(fn2_net* net) {
-    if (!net) { fn2::set_error("backward: null net"); return FN2_ERR_INVALID; }
-    FN2_TRY
-        net->net->Backward();
-        return FN2_OK;
-    FN2_CATCH
-}
-int fn2_net_clear_param_diffs(fn2_net* net) {
-    if (!net) { fn2::set_error("clear_param_diffs: null net"); return FN2_ERR_INVALID; }
-    FN2_TRY
-        net->net->ClearParamDiffs();
-        return FN2_OK;
-    FN2_CATCH
-}
+int fn2_net_forward(fn2_net* net) { return net_call("forward", net, [&] { net->net->Forward(); }); }
+int fn2_net_backward(fn2_net* net) { return net_call("backward", net, [&] { net->net->Backward(); }); }
+int fn2_net_clear_param_diffs(fn2_net* net) { return net_call("clear_param_diffs", net, [&] { net->net->ClearParamDiffs(); }); }
 int fn2_net_set_diff(fn2_net* net, const char* blob, const float* host_nchw) {
-    if (!net || !blob || !host_nchw) { fn2::set_error("set_diff: null argument"); return FN2_ERR_INVALID; }
-    FN2_TRY
-        net->net->SetDiff(blob, host_nchw);
-        return FN2_OK;
-    FN2_CATCH
+    return net_call("set_diff", net && blob && host_nchw, [&] { net->net->SetDiff(blob, host_nchw); });
 }
 int fn2_net_get_diff(fn2_net* net, const char* blob, float* host_nchw) {
-    if (!net || !blob || !host_nchw) { fn2::set_error("get_diff: null argument"); return FN2_ERR_INVALID; }
-    FN2_TRY
-        net->net->GetDiff(blob, host_nchw);
-        return FN2_OK;
-    FN2_CATCH
+    return net_call("get_diff", net && blob && host_nchw, [&] { net->net->GetDiff(blob, host_nchw); });
 }
 int fn2_net_param_diff_arena(fn2_net* net, void** dev_ptr, size_t* bytes) {
-    if (!net || !dev_ptr || !bytes) { fn2::set_error("param_diff_arena: null argument"); return FN2_ERR_INVALID; }
-    FN2_TRY
-        net->net->ParamDiffArena(dev_ptr, bytes);
-        return FN2_OK;
-    FN2_CATCH
+    return net_call("param_diff_arena", net && dev_ptr && bytes, [&] { net->net->ParamDiffArena(dev_ptr, bytes); });
 }
 int fn2_net_trainable_diff_span(fn2_net* net, void** dev_ptr, size_t* bytes) {
-    if (!net || !dev_ptr || !bytes) { fn2::set_error("trainable_diff_span: null argument"); return FN2_ERR_INVALID; }
-    FN2_TRY
-        net->net->TrainableDiffSpan(dev_ptr, bytes);
-        return FN2_OK;
-    FN2_CATCH
+    return net_call("trainable_diff_span", net && dev_ptr && bytes, [&] { net->net->TrainableDiffSpan(dev_ptr, bytes); });
 }
 static caffe::Blob<float>* find_param(fn2_net* net, const char* layer, int index) {
     const auto& names = net->net->layer_names();
@@ -226,17 +176,15 @@ static caffe::Blob<float>* find_param(fn2_net* net, const char* layer, int index
     return nullptr;
 }
 int fn2_net_param_shape(fn2_net* net, const char* layer, int index, int shape[4]) {
-    if (!net || !layer || !shape) { fn2::set_error("param_shape: null argument"); return FN2_ERR_INVALID; }
-    FN2_TRY
+    return net_call("param_shape", net && layer && shape, [&] {
         caffe::Blob<float>* b = find_param(net, layer, index);
         if (!b) { fn2::set_error("param_shape: no parameter blob %s[%d]", layer, index); return FN2_ERR_INVALID; }
         for (int i = 0; i < 4; i++) shape[i] = b->shape(i);
         return FN2_OK;
-    FN2_CATCH
+    });
 }
 int fn2_net_get_param(fn2_net* net, const char* layer, int index, int diff, float* host) {
-    if (!net || !layer || !host) { fn2::set_error("get_param: null argument"); return FN2_ERR_INVALID; }
-    FN2_TRY
+    return net_call("get_param", net && layer && host, [&] {
         caffe::Blob<float>* b = find_param(net, layer, index);
         if (!b) { fn2::set_error("get_param: no parameter blob %s[%d]", layer, index); return FN2_ERR_INVALID; }
         caffe::Caffe::stream() = net->net->stream();
@@ -245,7 +193,7 @@ int fn2_net_get_param(fn2_net* net, const char* layer, int index, int diff, floa
         const float* p = diff ? b->cpu_diff() : b->cpu_data();
         memcpy(host, p, (size_t)b->count() * sizeof(float));
         return FN2_OK;
-    FN2_CATCH
+    });
 }
 int fn2_net_launches_per_backward(fn2_net* net) { return net ? net->net->launches_per_backward() : 0; }
 int fn2_net_layer_need_backward(fn2_net* net, int layer) {
@@ -255,41 +203,21 @@ int fn2_net_layer_need_backward(fn2_net* net, int layer) {
     } catch (...) { return -1; }
 }
 
-int fn2_net_sync(fn2_net* net) {
-    if (!net) { fn2::set_error("sync: null net"); return FN2_ERR_INVALID; }
-    FN2_TRY
-        net->net->Sync();
-        return FN2_OK;
-    FN2_CATCH
-}
+int fn2_net_sync(fn2_net* net) { return net_call("sync", net, [&] { net->net->Sync(); }); }
 void* fn2_net_stream(fn2_net* net) { return net ? (void*)net->net->stream() : nullptr; }
 
 int fn2_net_time_layers(fn2_net* net, float* ms) {
-    if (!net || !ms) { fn2::set_error("time_layers: null argument"); return FN2_ERR_INVALID; }
-    FN2_TRY
-        net->net->TimeLayers(ms);
-        return FN2_OK;
-    FN2_CATCH
+    return net_call("time_layers", net && ms, [&] { net->net->TimeLayers(ms); });
 }
 int fn2_net_launches_per_forward(fn2_net* net) { return net ? net->net->launches_per_forward() : 0; }
 int fn2_net_graph_active(fn2_net* net) { return net && net->net->graph_active() ? 1 : 0; }
 
 int fn2_net_layer_work(fn2_net* net, int layer, double* flops, double* bytes) {
-    if (!net || !flops || !bytes || layer < 0 || layer >= (int)net->net->layers().size()) {
-        fn2::set_error("layer_work: bad argument");
-        return FN2_ERR_INVALID;
-    }
-    net->net->LayerWork(layer, flops, bytes);
-    return FN2_OK;
-}
-
-static int emit_string(const std::string& s, char* out, size_t* bytes) {
-    if (!bytes) { fn2::set_error("null size pointer"); return FN2_ERR_INVALID; }
-    if (!out) { *bytes = s.size() + 1; return FN2_OK; }
-    if (*bytes < s.size() + 1) { fn2::set_error("buffer too small"); return FN2_ERR_INVALID; }
-    memcpy(out, s.c_str(), s.size() + 1);
-    *bytes = s.size() + 1;
-    return FN2_OK;
+    return net_call("layer_work", net && flops && bytes, [&] {
+        if (layer < 0 || layer >= (int)net->net->layers().size()) { fn2::set_error("layer_work: bad argument"); return FN2_ERR_INVALID; }
+        net->net->LayerWork(layer, flops, bytes);
+        return FN2_OK;
+    });
 }
 
 int fn2_proto_canonical(const char* prototxt_text, char* out, size_t* bytes) {
@@ -299,7 +227,7 @@ int fn2_proto_canonical(const char* prototxt_text, char* out, size_t* bytes) {
         std::string s;
         if (!np.name.empty()) s += "name: \"" + np.name + "\"\n";
         for (const auto& l : np.layers) s += "layer {\n" + caffe::PrintTextFormat(*l.m, 1) + "}\n";
-        return emit_string(s, out, bytes);
+        return emit("proto_canonical", s, true, out, bytes);
     FN2_CATCH
 }
 
@@ -330,12 +258,7 @@ static std::string caffemodel_to_h5(const void* caffemodel, size_t n) {
 int fn2_caffemodel_to_hdf5(const void* caffemodel, size_t n, void* out, size_t* bytes) {
     if (!caffemodel || !bytes) { fn2::set_error("caffemodel_to_hdf5: null argument"); return FN2_ERR_INVALID; }
     try {
-        const std::string h5 = caffemodel_to_h5(caffemodel, n);
-        if (!out) { *bytes = h5.size(); return FN2_OK; }
-        if (*bytes < h5.size()) { fn2::set_error("caffemodel_to_hdf5: buffer too small"); return FN2_ERR_INVALID; }
-        memcpy(out, h5.data(), h5.size());
-        *bytes = h5.size();
-        return FN2_OK;
+        return emit("caffemodel_to_hdf5", caffemodel_to_h5(caffemodel, n), false, out, bytes);
     } catch (const std::exception& e) {
         fn2::set_error("%s", e.what());
         return FN2_ERR_PARSE;
@@ -343,16 +266,10 @@ int fn2_caffemodel_to_hdf5(const void* caffemodel, size_t n, void* out, size_t* 
 }
 
 int fn2_net_to_hdf5(fn2_net* net, void* buf, size_t* bytes) {
-    if (!net || !bytes) { fn2::set_error("to_hdf5: null argument"); return FN2_ERR_INVALID; }
-    FN2_TRY
+    return net_call("to_hdf5", net && bytes, [&] {
         const std::string cm = net->net->ToCaffemodel();
-        const std::string h5 = caffemodel_to_h5(cm.data(), cm.size());
-        if (!buf) { *bytes = h5.size(); return FN2_OK; }
-        if (*bytes < h5.size()) { fn2::set_error("to_hdf5: buffer too small"); return FN2_ERR_INVALID; }
-        memcpy(buf, h5.data(), h5.size());
-        *bytes = h5.size();
-        return FN2_OK;
-    FN2_CATCH
+        return emit("to_hdf5", caffemodel_to_h5(cm.data(), cm.size()), false, buf, bytes);
+    });
 }
 
 int fn2_hdf5_summary(const void* h5, size_t n, char* out, size_t* bytes) {
@@ -371,7 +288,7 @@ int fn2_hdf5_summary(const void* h5, size_t n, char* out, size_t* bytes) {
             s += buf;
             s += "\n";
         }
-        return emit_string(s, out, bytes);
+        return emit("hdf5_summary", s, true, out, bytes);
     } catch (const std::exception& e) {
         fn2::set_error("%s", e.what());
         return FN2_ERR_PARSE;
@@ -396,7 +313,7 @@ int fn2_caffemodel_summary(const void* caffemodel, size_t n, char* out, size_t* 
             }
             s += "\n";
         }
-        return emit_string(s, out, bytes);
+        return emit("caffemodel_summary", s, true, out, bytes);
     FN2_CATCH
 }
 

@@ -38,14 +38,11 @@ def test_library_is_sm90a_only():
 
 
 def canonical(fn2, text):
-    lib = fn2.lib()
-    n = C.c_size_t()
-    rc = lib.fn2_proto_canonical(text.encode(), None, C.byref(n))
-    if rc:
-        raise fn2.Fn2Error(lib.fn2_last_error().decode())
-    buf = C.create_string_buffer(n.value)
-    assert lib.fn2_proto_canonical(text.encode(), buf, C.byref(n)) == 0
-    return buf.value.decode()
+    return fn2.sized_output(fn2.lib().fn2_proto_canonical, text.encode()).rstrip(b"\0").decode()
+
+
+def summary_lines(fn2, fn, data):
+    return fn2.sized_output(fn, data, len(data)).rstrip(b"\0").decode().strip().splitlines()
 
 
 @pytest.mark.parametrize("model", ["FlowNet2-S", "FlowNet2-C", "FlowNet2-CSS", "FlowNet2-SD", "FlowNet2"])
@@ -108,12 +105,7 @@ def test_prototxt_text_format_quirks(fn2):
 def test_caffemodel_reader_matches_reference_protobuf(fn2):
     raw = open(os.path.join(GOLD, "ref_pb2_caffemodel.bin"), "rb").read()
     want = json.load(open(os.path.join(GOLD, "ref_pb2_caffemodel.json")))
-    lib = fn2.lib()
-    n = C.c_size_t()
-    assert lib.fn2_caffemodel_summary(raw, len(raw), None, C.byref(n)) == 0
-    buf = C.create_string_buffer(n.value)
-    assert lib.fn2_caffemodel_summary(raw, len(raw), buf, C.byref(n)) == 0
-    lines = buf.value.decode().strip().split("\n")
+    lines = summary_lines(fn2, fn2.lib().fn2_caffemodel_summary, raw)
     assert len(lines) == len(want)
     for line, w in zip(lines, want):
         parts = line.split(" ")
@@ -452,15 +444,7 @@ def test_train_prototxt_parser_matches_reference_protobuf(fn2):
 
 
 def _h5_summary(fn2, data):
-    lib = fn2.lib()
-    lib.fn2_hdf5_summary.argtypes = [C.c_void_p, C.c_size_t, C.c_char_p, C.POINTER(C.c_size_t)]
-    buf = (C.c_char * len(data)).from_buffer_copy(data)
-    n = C.c_size_t()
-    if lib.fn2_hdf5_summary(buf, len(data), None, C.byref(n)):
-        raise fn2.Fn2Error(lib.fn2_last_error().decode())
-    out = C.create_string_buffer(n.value)
-    assert lib.fn2_hdf5_summary(buf, len(data), out, C.byref(n)) == 0
-    return out.value.decode().strip().splitlines()
+    return summary_lines(fn2, fn2.lib().fn2_hdf5_summary, data)
 
 
 def test_hdf5_reader_on_files_written_by_the_real_library(fn2):
@@ -502,16 +486,9 @@ def test_hdf5_reader_nested_caffemodel_layout(fn2):
 def test_caffemodel_to_hdf5_round_trip(fn2):
     """fn2_caffemodel_to_hdf5 (the host half of Net::ToHDF5): a binary caffemodel -- here the fixture the reference's caffe_pb2 wrote --
     converted to HDF5 and read back by the reader that is pinned on real libhdf5 files: same layers, shapes and values."""
-    lib = fn2.lib()
-    lib.fn2_caffemodel_to_hdf5.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_size_t)]
     data = open(os.path.join(GOLD, "ref_pb2_caffemodel.bin"), "rb").read()
     desc = json.load(open(os.path.join(GOLD, "ref_pb2_caffemodel.json")))
-    buf = (C.c_char * len(data)).from_buffer_copy(data)
-    n = C.c_size_t()
-    assert lib.fn2_caffemodel_to_hdf5(buf, len(data), None, C.byref(n)) == 0
-    out = (C.c_char * n.value)()
-    assert lib.fn2_caffemodel_to_hdf5(buf, len(data), out, C.byref(n)) == 0
-    lines = _h5_summary(fn2, bytes(out[:n.value]))
+    lines = _h5_summary(fn2, fn2.sized_output(fn2.lib().fn2_caffemodel_to_hdf5, data, len(data)))
     want = {}
     for l in desc:
         for i, b in enumerate(l["blobs"]):

@@ -37,7 +37,7 @@ def kernels_per_case(runs):
     synchronisations, 2 ms from the next.  A kernel belongs to the window of its launch call (the profiler gives both the
     same correlation id), else to the window its start falls in or is nearest to (a warm-up run of the first case before
     the windows lands in that case's).  A session in which some window has no kernel at all (the profiler now and then
-    drops device activity) is taken again."""
+    drops device activity) is taken again; the windows' own annotations on the device timeline do not count as kernels."""
     import torch
     cpu, cuda = torch.profiler.ProfilerActivity.CPU, torch.profiler.ProfilerActivity.CUDA
     for _ in range(3):
@@ -60,8 +60,8 @@ def kernels_per_case(runs):
         launch = {e.id: window(e.time_range.start) for e in events
                   if e.device_type == torch.autograd.DeviceType.CPU and "LaunchKernel" in e.name}
         names = [set() for _ in runs]
-        for e in events:
-            if e.device_type == torch.autograd.DeviceType.CUDA:
+        for e in events:     # the device timeline also carries the ew_case_ ranges: not kernels, so a window with one only is empty
+            if e.device_type == torch.autograd.DeviceType.CUDA and not e.name.startswith("ew_case_"):
                 names[launch.get(e.id, window(e.time_range.start))].add(e.name)
         if all(names):
             break

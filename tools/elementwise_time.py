@@ -86,11 +86,7 @@ def main():
     # end-point-error L1Loss forward + backward there
     gt = blob(8, 2, 320, 448)
     lib = F.lib()
-
-    class L1Desc(C.Structure):
-        _fields_ = [("l2_per_location", C.c_int32), ("l2_prescale_by_channels", C.c_int32), ("normalize_by_num_entries", C.c_int32),
-                    ("epsilon", C.c_float), ("plateau", C.c_float)]
-    epe = L1Desc(1, 0, 0, 0.0, 0.0)
+    epe = F.fn2_l1loss_desc(1, 0, 0, 0.0, 0.0)
 
     def l1loss(pred, gtl, diff, ws, nbytes, state, one):
         dp, dg, dd = ops.desc(pred), ops.desc(gtl), ops.desc(diff)
