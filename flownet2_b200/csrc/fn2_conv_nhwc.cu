@@ -268,18 +268,22 @@ static int plan_splits(long long M, int co, int ci, int ntaps) {
 }
 
 // Workspace (floats) the split-K path may need for this shape; 0 = never splits.
+// The partials are written as float4: a caller's workspace may start anywhere 4-byte aligned, and the 4 floats of slack on top
+// of them are the room to move it to a 16-byte boundary.
+constexpr size_t NHWC_WS_SLACK = 4;
+
 size_t conv_nhwc_workspace_floats(const fn2_conv_desc* d, int N, int Ho, int Wo) {
     if (!d->deconv) {
         const long long M = (long long)N * Ho * Wo;
         const int z = plan_splits(M, d->co, d->ci, d->kh * d->kw);
-        return z > 1 ? (size_t)z * M * d->co : 0;
+        return z > 1 ? (size_t)z * M * d->co + NHWC_WS_SLACK : 0;
     }
     // deconvolution: per parity class; the largest class decides
     const int sh = d->stride_h, sw = d->stride_w;
     const long long M = (long long)N * ((Ho + sh - 1) / sh) * ((Wo + sw - 1) / sw);
     const int taps = ((d->kh + sh - 1) / sh) * ((d->kw + sw - 1) / sw);
     const int z = plan_splits(M, d->co, d->ci, taps);
-    return z > 1 ? (size_t)(z + 1) * M * d->co : 0;
+    return z > 1 ? (size_t)(z + 1) * M * d->co + NHWC_WS_SLACK : 0;
 }
 
 int conv_nhwc_forward(const fn2_conv_desc* d, const T4& in, const float* wp, const float* bias, const T4& out,
@@ -291,6 +295,8 @@ int conv_nhwc_forward(const fn2_conv_desc* d, const T4& in, const float* wp, con
     p.relu = d->relu; p.has_bias = d->has_bias; p.slope = d->negative_slope;
     p.vec_in = in.px_float4();          // both views are channel-fast (conv_nhwc_eligible)
     p.vec_out = out.px_float4();
+    ws_floats = ws && ws_floats > NHWC_WS_SLACK ? ws_floats - NHWC_WS_SLACK : 0;
+    ws = reinterpret_cast<float*>(((uintptr_t)ws + 15) & ~(uintptr_t)15);
     const int bn = pick_bn(d->co);
     auto launch = [&](dim3 grid, float* partial) {
         if (bn == 128) conv_nhwc_kernel<128><<<grid, 256, 0, st>>>(in.p, wp, bias, out.p, partial, p);

@@ -340,7 +340,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                     else if (p.gcs == 12) gather_taps<12>(st, r0, r1, t, nt, ah, al);
                     else gather_taps<16>(st, r0, r1, t, nt, ah, al);
                 } else if constexpr (MODE == TC_ROW) {
-                    // row mode: taps that fall outside the image row (and the K padding) hold whatever follows in memory
+                    // row mode: taps that fall outside the image row (and the K padding) hold whatever follows in memory; the
+                    // padding channels of the pixels inside the row meet zero weights (fn2.h: they must be finite)
                     const int kb32 = (i % p.rblocks) * 32;
                     int klo[2], khi[2];
 #pragma unroll
@@ -709,11 +710,15 @@ static bool tc_plan(const fn2_conv_desc* d, int N, int W, int Ho, int Wo, int ci
     return true;
 }
 
+// The partial tiles of a K split are written as float4: a caller's workspace may start anywhere 4-byte aligned, and the 4 floats
+// of slack on top of the partials are the room to move it to a 16-byte boundary.
+constexpr size_t TC_WS_SLACK = 4;
+
 // workspace of the layer's K split; the pixel stride does not matter: only the small-Ci modes depend on it, and they never split
 size_t conv_tc_workspace_floats(const fn2_conv_desc* d, int N, int W, int Ho, int Wo) {
     TcPlan pl;
     if (!tc_plan(d, N, W, Ho, Wo, d->ci, SIZE_MAX, &pl) || pl.p.split_z == 1) return 0;
-    return (size_t)(pl.p.ntotal - pl.p.split_first) * pl.p.split_z * 128 * pl.NT;
+    return (size_t)(pl.p.ntotal - pl.p.split_first) * pl.p.split_z * 128 * pl.NT + TC_WS_SLACK;
 }
 
 // plan8 (fn2_conv_plan): {NT, tile units, K steps per tile, small-Ci mode (0 plain, 1 tap groups, 2 kernel rows), first split
@@ -725,6 +730,8 @@ void conv_tc_plan(const fn2_conv_desc* d, int N, int W, int Ho, int Wo, int ci_s
     out8[4] = pl.p.split_first; out8[5] = pl.p.split_z;
 }
 
+int conv_tn_applicable(const fn2_conv_desc* d);  // fn2_conv_tn.cu
+
 int conv_tc_eligible(const fn2_conv_desc* d, const T4& in, const T4& out) {
     if (!tc_enabled()) return 0;
     if (in.sc != 1 || out.sc != 1) return 0;
@@ -732,6 +739,10 @@ int conv_tc_eligible(const fn2_conv_desc* d, const T4& in, const T4& out) {
     if (((uintptr_t)in.p & 15) || (in.sw & 3) || (in.sh & 3) || (in.sn & 3)) return 0;
     if (((uintptr_t)out.p & 15) || (out.sw & 3) || (out.sh & 3) || (out.sn & 3)) return 0;
     if (!tc_encode_fn()) return 0;
+    // the per-tap engine refuses a deconvolution whose kernel is shorter than its stride (parity classes without taps); the
+    // taps-on-N engine takes its own shapes whole
+    TcPlan pl;
+    if (!conv_tn_applicable(d) && !tc_plan(d, in.n, in.w, out.h, out.w, (int)in.sw, 0, &pl)) return 0;
     return 1;
 }
 
@@ -763,9 +774,11 @@ int conv_tc_forward(const fn2_conv_desc* d, const T4& in, const float* wp, const
     EncodeTiledFn enc = tc_encode_fn();
     if (!enc) { set_error("conv_tc: cuTensorMapEncodeTiled unavailable"); return FN2_ERR_CUDA; }
     TcPlan pl;
-    if (!tc_plan(d, in.n, in.w, out.h, out.w, (int)in.sw, ws ? ws_floats : 0, &pl)) {
+    const size_t avail = ws && ws_floats > TC_WS_SLACK ? ws_floats - TC_WS_SLACK : 0;
+    if (!tc_plan(d, in.n, in.w, out.h, out.w, (int)in.sw, avail, &pl)) {
         set_error("conv_tc: layer not supported (deconvolution parity class without taps)"); return FN2_ERR_INVALID;
     }
+    ws = reinterpret_cast<float*>(((uintptr_t)ws + 15) & ~(uintptr_t)15);
     TcParams& p = pl.p;
     const TcSmallCi& sm = pl.sm;
     const int NT = pl.NT, su = p.su, sv = p.sv;

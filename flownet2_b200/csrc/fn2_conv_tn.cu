@@ -529,12 +529,14 @@ int conv_tn_pack(const fn2_conv_desc* d, const float* w, float* wp, cudaStream_t
     return FN2_OK;
 }
 
-// plan8 (fn2_conv_plan): {NT = -(accumulator columns of the widest pass), units, K blocks, mode 3 = taps on N, passes, strips, segments, 0}
+// plan8 (fn2_conv_plan): {NT = -(accumulator columns of the widest pass), 0, K blocks, mode 3 = taps on N, passes, strips,
+// W stages (0 = all resident, else the ring depth RW), tiles between two flushes of the output ring F}
 int conv_tn_plan(const fn2_conv_desc* d, int N, int Ho, int Wo, int* out8) {
     TnParams p;
     if (!tn_layer_plan(d, &p)) return 0;
     const int nstrips = (Wo - (p.S * p.cshift + p.xa) + p.S * p.stepx - 1) / (p.S * p.stepx);
     out8[0] = -p.ngmax; out8[2] = p.cblocks; out8[3] = 3; out8[4] = p.npass; out8[5] = nstrips;
+    out8[6] = p.wres ? 0 : p.RW; out8[7] = p.F;
     return 1;
 }
 

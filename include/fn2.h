@@ -172,7 +172,10 @@ typedef struct fn2_conv_desc {
     float negative_slope;
     int32_t engine;            /* 0 default (tensor cores when eligible), 1 SIMT fp32, 2 tensor cores (wgmma 3xTF32) */
     int32_t input_guard_bytes; /* readable (never used) bytes the caller guarantees before AND after the bottom tensor's
-                                * storage; >= 512 lets small-Ci convolutions fetch whole kernel rows per TMA box. 0 = none */
+                                * storage; >= 512 lets small-Ci convolutions fetch whole kernel rows per TMA box. 0 = none.
+                                * Those rows include the padding channels of a bottom whose pixel stride is Ci rounded up
+                                * to 4: with a guard band they must hold finite values (they meet zero weights, and
+                                * 0 * NaN is NaN).  Without one they are never read. */
     int32_t out_pad_h, out_pad_w; /* deconvolution only: extra output rows / columns at the bottom / right (0 for every Caffe
                                 * layer; the adjoint of a strided convolution needs (H + 2 pad - k) mod stride of them to
                                 * reach the whole bottom, fn2_conv_backward_data_desc) */
@@ -185,15 +188,16 @@ FN2_API int fn2_conv_packed_floats(const fn2_conv_desc* d, int ci_stride, size_t
 FN2_API int fn2_conv_pack_weights(const fn2_conv_desc* d, int ci_stride,
                                   const float* caffe_weights_dev, float* packed_dev, void* stream);
 FN2_API int fn2_conv_out_shape(const fn2_conv_desc* d, int H, int W, int* Ho, int* Wo);
-/* Scratch the forward may use for this shape (split-K partials of small spatial maps); may be 0.
- * Passing a NULL / too small workspace is allowed: the kernel then runs unsplit. */
+/* Scratch the forward may use for this shape (split-K partials of small spatial maps); may be 0.  It may start at any 4-byte
+ * boundary.  Passing a NULL / too small workspace is allowed: the kernel then runs unsplit. */
 FN2_API int fn2_conv_workspace_bytes(const fn2_conv_desc* d, int N, int H, int W, size_t* bytes);
 /* Host-side plan of the tensor-core engine for a layer shape (introspection; needs no GPU): plan8 = {NT (output channels per
  * tile; 0 = a shape the engine does not take), tile units, K steps per tile, small-Ci mode (0 plain K blocks, 1 tap groups,
  * 2 kernel rows), first split tile, K ranges per split tile (1 = unsplit), 0, 0}.  The tiles from the first split tile on
  * have their K loops cut into that many ranges, which run on different SMs: all tiles of a layer whose tile list cannot fill
  * the GPU, else the tiles of the last, partial wave.  The taps-on-N engine (mode 3) reports {-accumulator columns of the
- * widest pass, 0, K blocks, 3, passes, strips, 0, 0}. */
+ * widest pass, 0, K blocks, 3, passes, strips, W stages (0: the whole packed weight matrix resident in shared memory, else
+ * the depth of the weight-stage ring), tiles between two flushes of the output-row ring}. */
 FN2_API int fn2_conv_plan(const fn2_conv_desc* d, int N, int H, int W, int ci_stride, int32_t* plan8);
 FN2_API int fn2_conv_forward(const fn2_conv_desc* d, const fn2_tensor* bottom,
                              const float* packed_weights_dev, const float* bias_dev,

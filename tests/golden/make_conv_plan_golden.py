@@ -105,11 +105,7 @@ def main():
         b = C.c_size_t()
         assert l.fn2_conv_workspace_bytes(C.byref(d), N, H, W, C.byref(b)) == 0
         p = list(o)
-        if p[0] > 0:
-            # this layout had {NT, tiles, steps, mode, uniform K splits, first tail tile, tail K ranges, 0}: a uniform split
-            # is the K split with first split tile 0
-            uniform[i] = p[4] > 1
-            p = p[:4] + ([0, p[4]] if uniform[i] else [p[5], p[6]]) + [0, 0]
+        uniform[i] = p[0] > 0 and p[4] == 0 and p[5] > 1
         desc[i] = [getattr(d, f) for f in INT_FIELDS]
         shape[i] = (N, H, W, cis)
         plan[i] = p

@@ -1,0 +1,660 @@
+"""Forward convolution and deconvolution on the tensor cores (fn2_conv_forward) against a float64 reference, plan by plan.
+
+Two engines run these layers.  The per-tap engine (fn2_conv_tc.cu, conv_tc_forward) takes every layer with whole 16-channel
+output tiles, at most 49 taps and a stride of at most 2; the taps-on-N engine (fn2_conv_tn.cu, conv_tn_forward) takes the
+layers with 16 or 32 output channels, 17-256 input channels and at most 4 x 4 taps (mode 3 of fn2_conv_plan).  The cases of
+PLAN_CASES are built so that, together, they reach every value of their plans: output channels per tile NT with several Co
+tiles, tile widths 8-128 and a map wider than 128, K steps of 1 and of counts that are not a multiple of the 4-step chunk, Ci
+tails, both K-split regimes (every tile, tail wave) at NT 128 and NT <= 64 up to 8 ranges, deconvolutions of stride 1 and of
+stride 2 with kernels 2-5 and odd sizes, anisotropic strides, kernels and pads, an out_pad from fn2_conv_backward_data_desc,
+tap-group (mode 1) and kernel-row (mode 2) packing of small Ci, and the taps-on-N passes, accumulator widths, strips,
+segments and weight regimes.  `test_conv_tc_plan_coverage` checks that they do on the card the suite runs on (the split
+depends on its SM count), `test_conv_tc_route_kernels` that each case runs the kernels of its plan.  DEPLOY_CASES are the
+layers of FlowNet2 at bench.py's workload (4 pairs of 1024 x 436, adapted to 448 rows), GRAD_CASES the data-gradient
+operators of the training graphs at 448 x 320, batch 8; both are drawn like the nets' (post-ReLU bottom), with weights of one
+sign, so that every product of a reduction has the same sign.
+
+Reference: per kernel tap one float64 BLAS product of the tap's weights with the gathered input pixels (`ref_at`; a
+deconvolution is its scatter transpose), evaluated on the device in float64 and pinned to oracle.conv_fwd / deconv_fwd.  On
+large maps it evaluates a sample of output pixels (`sample`): every pixel of the first and last tile row and column, every
+pixel of the K-split tiles and 2048 seeded random others.  Tolerance: 1e-6 of the largest |output| (at least 1).
+"""
+import ctypes as C
+import math
+import zlib
+from collections import namedtuple
+
+import numpy as np
+import pytest
+
+from oracle import oracle as O
+from tests.util import deploy_convs, kernels_per_case, train_convs
+
+pytestmark = pytest.mark.gpu
+torch = pytest.importorskip("torch")
+
+TOL = 1e-6
+SLOPE = 0.1
+SENTINEL = 7.0
+GUARD = 256                 # floats of NaN before and after every bottom's storage (Blob::kGuardFloats)
+FULL = 1 << 16              # output pixels up to which the reference evaluates every pixel
+SAMPLE = 2048
+
+
+@pytest.fixture(scope="module")
+def ops(fn2):
+    from flownet2_b200 import ops as _ops
+    return _ops
+
+
+def _lib():
+    from flownet2_b200 import lib
+    return lib()
+
+
+def _check(rc):
+    from flownet2_b200 import check
+    check(rc)
+
+
+# ---- cases ----------------------------------------------------------------------------------------------------------------
+# fwd: None, or the layer whose data gradient the case is: (Ci, Co, k, s, p, deconv, H, W, needs_flip, real output channels)
+Case = namedtuple("Case", "name N Ci H W Co k s p deconv op bias layout engine fwd")
+
+
+def _pair(v):
+    return (v, v) if isinstance(v, int) else tuple(v)
+
+
+def case(name, N, Ci, H, W, Co, k, s=1, p=0, deconv=False, bias=True, layout="nhwc", engine=2):
+    return Case(name, N, Ci, H, W, Co, _pair(k), _pair(s), _pair(p), deconv, (0, 0), bias, layout, engine, None)
+
+
+def cstride(c):
+    """Blob::compute_cstride: the nets' pixel stride (channels rounded up to 4 below 32, else to 32)."""
+    return (c + 3) // 4 * 4 if c < 32 else (c + 31) // 32 * 32
+
+
+def padded_co(co):
+    """The output channels BaseConvolutionLayer::BackwardData gives a convolution adjoint (layers.cpp, BackwardData: a
+    multiple of 128 when that costs at most 1/8 more channels, else of 64; of 16 up to 64 channels)."""
+    if co <= 16 or co % 16 == 0:
+        return co
+    c128, c64 = (co + 127) // 128 * 128, (co + 63) // 64 * 64
+    return (co + 15) // 16 * 16 if co <= 64 else (c128 if (c128 - co) * 8 <= co else c64)
+
+
+def adjoint(name, N, Ci, H, W, Co, k, s=1, p=0, deconv=False, layout="pad", engine=2):
+    """The forward operator that computes the data gradient of a layer (fn2_conv_backward_data_desc) on its top diff, with
+    BackwardData's padded output channels."""
+    from flownet2_b200 import fn2_conv_desc
+    (kh, kw), (sh, sw), (ph, pw) = _pair(k), _pair(s), _pair(p)
+    d = fn2_conv_desc(Ci, Co, kh, kw, sh, sw, ph, pw, int(deconv), 1, 0, 0.0, 0, 0)
+    bd, flip, ho, wo = fn2_conv_desc(), C.c_int(), C.c_int(), C.c_int()
+    _check(_lib().fn2_conv_backward_data_desc(C.byref(d), H, W, C.byref(bd), C.byref(flip)))
+    _check(_lib().fn2_conv_out_shape(C.byref(d), H, W, C.byref(ho), C.byref(wo)))
+    co = padded_co(bd.co) if not bd.deconv else bd.co
+    return Case(name, N, bd.ci, ho.value, wo.value, co, (bd.kh, bd.kw), (bd.stride_h, bd.stride_w), (bd.pad_h, bd.pad_w),
+                bool(bd.deconv), (bd.out_pad_h, bd.out_pad_w), False, layout, engine,
+                (Ci, Co, (kh, kw), (sh, sw), (ph, pw), deconv, H, W, bool(flip.value), bd.co))
+
+
+PLAN_CASES = [
+    # per-tap engine, plain K blocks (mode 0); comments: NT x Co tiles, tile width, K steps, split
+    case("nt16_split_all", 1, 40, 20, 24, 16, 5, 1, 2),                   # NT 16, tw 32, 50 steps: every tile split
+    case("nt16_co48_split", 1, 300, 9, 13, 48, 3, 1, 1, bias=False),      # NT 16 x 3, Ci tail 300, 90 steps (not 4k)
+    case("nt32_co96_s2", 1, 64, 30, 40, 96, 3, 2, 1),                     # NT 32 x 3, 18 steps: split of 12 tiles
+    case("nt64_co192_split", 2, 128, 14, 20, 192, 3, 1, 1),               # NT 64 x 3, every tile split
+    case("nt128_co256_split", 1, 256, 12, 20, 256, 3, 1, 1),              # NT 128 x 2, every tile split
+    case("z8_tw16", 1, 512, 7, 16, 128, 3, 1, 1),                         # one tile of 16 x 8, 144 steps in 8 ranges
+    case("nt128_tail_ci473", 1, 473, 150, 128, 128, 3, 1, 1, bias=False),  # 150 tiles: the last wave's 18 split
+    case("nt16_tail", 1, 300, 140, 128, 16, 3, 1, 1),                     # 140 tiles of NT 16: tail wave split
+    case("d_k3_odd_split", 1, 1024, 4, 6, 128, 3, 2, 1, True),            # classes of 4 / 2 / 2 / 1 taps, 7 x 11, tw 8
+    case("d_s1", 1, 64, 20, 30, 64, 3, 1, 1, True),                       # one class
+    case("d_k2", 2, 64, 15, 17, 128, 2, 2, 0, True),                      # one tap per class
+    case("d_k4", 1, 256, 13, 19, 64, 4, 2, 1, True),
+    case("d_k5_odd", 1, 96, 11, 14, 64, 5, 2, 2, True),                   # 9 / 6 / 6 / 4 taps, 21 x 25
+    case("s12_k3x5", 1, 48, 17, 40, 64, (3, 5), (1, 2), (1, 2)),
+    case("s21_k5x3", 1, 40, 30, 19, 32, (5, 3), (2, 1), (2, 0)),
+    case("tw64_ci33", 1, 33, 12, 50, 64, 3, 1, 1),                        # Ci tail of 1
+    case("wide150", 1, 96, 6, 150, 128, 3, 1, 1),                         # two tile columns of 128
+    case("k1_steps1", 1, 32, 12, 20, 64, 1, 1, 0),                        # one K step
+    case("k1_ci20", 2, 20, 9, 14, 32, 1, 1, 0),                           # one K step with a Ci tail
+    adjoint("adj_outpad_10", 1, 32, 20, 21, 64, 3, 2, 1),                 # deconvolution with out_pad (1, 0)
+    # tap groups (mode 1): cs 4 / 8 / 12 / 16, each with a partial last group
+    case("grp_cs4", 2, 3, 20, 28, 64, 7, 2, 3),
+    case("grp_cs8_nt128", 1, 7, 15, 22, 128, 5, 1, 2),
+    case("grp_cs12", 1, 10, 13, 17, 32, 3, 1, 1),
+    case("grp_cs16_nt16", 1, 16, 12, 18, 16, (3, 5), 2, (1, 2)),
+    # kernel rows (mode 2): the nets' padded pixel stride and guard band
+    case("row_ci12_s2", 2, 12, 20, 28, 64, 7, 2, 3, layout="pad"),         # three K blocks per kernel row
+    case("row_wide_s1", 2, 3, 10, 300, 64, 7, 1, 3, layout="pad"),         # rows of 300 outputs: three tiles wide
+    case("row_ci6", 1, 6, 18, 22, 64, 3, 1, 1, layout="pad"),
+    # taps on N (mode 3): passes x accumulator columns
+    case("tn16_k2_ci17", 1, 17, 20, 40, 16, 2, 1, 0),                     # 1 x 64, Ci tail 17
+    case("tn16_k3_strips", 2, 82, 37, 70, 16, 3, 1, 1),                   # 2 x 80, three strips
+    case("tn32_k3_ci256", 1, 256, 20, 40, 32, 3, 1, 1),                   # 3 x 96, weight ring
+    case("tn32_d4", 2, 128, 13, 37, 32, 4, 2, 1, True),                   # 6 x 96
+    case("tn16_d4_tall", 1, 162, 70, 33, 16, 4, 2, 1, True),              # 3 x 96, vertical segments
+    case("tn16_d1x4", 1, 64, 12, 40, 16, (1, 4), 2, (0, 1), True),        # 1 x 64: no tap reaches the odd rows
+    case("tn32_k2x3", 1, 48, 20, 40, 32, (2, 3), 1, 1),                   # 2 x 96
+    case("tn16_tall", 1, 64, 150, 40, 16, 3, 1, 1, bias=False),           # vertical segments
+    case("tn32_d2", 1, 40, 20, 30, 32, 2, 2, 0, True),                    # 2 x 64
+]
+PLAN_IDS = [c.name for c in PLAN_CASES]
+BY_NAME = {c.name: c for c in PLAN_CASES}
+
+# deconvolutions with a parity class that no tap reaches: the per-tap engine does not take them, engine 0 runs them on SIMT
+NO_TAP_CASES = [
+    case("d1x1_s2", 1, 64, 9, 13, 64, 1, 2, 0, True, engine=0),
+    case("d1x4_s2", 1, 48, 8, 12, 64, (1, 4), 2, (0, 1), True, engine=0),
+    adjoint("adj_k1_s2", 1, 64, 17, 18, 128, 1, 2, 0, engine=0),         # data gradient of a 1 x 1 stride-2 convolution
+]
+
+
+# ---- device data ------------------------------------------------------------------------------------------------------------
+def seed_of(c):
+    return zlib.crc32(repr(c[:10]).encode())
+
+
+def weight_shape(c):
+    """Caffe layout of the weights the reference uses: those of the case, or of the layer it is the data gradient of."""
+    if c.fwd:
+        Ci, Co, (kh, kw), _, _, deconv, _, _, _, _ = c.fwd
+        return (Ci, Co, kh, kw) if deconv else (Co, Ci, kh, kw)
+    return (c.Ci, c.Co) + c.k if c.deconv else (c.Co, c.Ci) + c.k
+
+
+def draw(c, seed, same_sign=False):
+    """bottom (NCHW, dense), weights (Caffe layout) and bias on the device.  same_sign: a post-ReLU bottom and weights of one
+    sign (|N(0,1)| sqrt(2 / K)), else N(0,1) and N(0,1) sqrt(2 / K)."""
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    x = torch.randn((c.N, c.Ci, c.H, c.W), generator=g, device="cuda")
+    ws = weight_shape(c)
+    w = torch.randn(ws, generator=g, device="cuda") * math.sqrt(2.0 / (ws[1] * ws[2] * ws[3]))
+    b = torch.randn(c.Co, generator=g, device="cuda") if c.bias else None
+    if same_sign:
+        x, w = x.clamp_min(0.0), w.abs()
+    return x, w, b
+
+
+# layout -> (first channel, pixel stride, padding channels, guard promise)
+LAYOUTS = {
+    "nhwc": (0, lambda c: (c + 3) // 4 * 4, "nan", False),      # channels_last, 16-byte pixels
+    "pad": (0, cstride, "zero", True),                          # the nets' blobs
+    "padjunk": (0, cstride, "junk", True),                      # ... with finite garbage in the padding channels
+    "padnan": (0, cstride, "nan", False),                       # ... with NaN there, and no guard promise
+    "slice": (4, lambda c: (c + 3) // 4 * 4 + 8, "nan", False),  # a zero-copy concat child
+    "misaligned": (1, lambda c: c + 4, "nan", False),           # first channel not on a 16-byte boundary
+}
+
+
+def bottom(x, layout):
+    """A view of x in one of LAYOUTS.  The storage has GUARD floats of NaN before and after it; the channels outside the view
+    hold NaN, zero or finite garbage (1e30)."""
+    n, c, h, w = x.shape
+    off, cs, fill, _ = LAYOUTS[layout]
+    cs = cs(c)
+    flat = torch.full((2 * GUARD + n * h * w * cs,), float("nan"), device="cuda")
+    body = flat[GUARD:GUARD + n * h * w * cs].view(n, h, w, cs)
+    if fill != "nan":
+        body.fill_(0.0 if fill == "zero" else 1e30)
+    body[..., off:off + c] = x.permute(0, 2, 3, 1)
+    return body.permute(0, 3, 1, 2)[:, off:off + c]
+
+
+def guard_bytes(layout):
+    return 4 * GUARD if LAYOUTS[layout][3] else 0
+
+
+def desc(c, engine=None, layout=None):
+    from flownet2_b200 import fn2_conv_desc
+    (kh, kw), (sh, sw), (ph, pw) = c.k, c.s, c.p
+    d = fn2_conv_desc(c.Ci, c.Co, kh, kw, sh, sw, ph, pw, int(c.deconv), int(c.bias), int(c.bias), SLOPE,
+                      c.engine if engine is None else engine, guard_bytes(layout or c.layout))
+    d.out_pad_h, d.out_pad_w = c.op
+    return d
+
+
+def out_hw(c):
+    ho, wo = C.c_int(), C.c_int()
+    _check(_lib().fn2_conv_out_shape(C.byref(desc(c)), c.H, c.W, C.byref(ho), C.byref(wo)))
+    return ho.value, wo.value
+
+
+def plan_of(c, layout=None):
+    layout = layout or c.layout
+    cis = LAYOUTS[layout][1](c.Ci)
+    out = (C.c_int32 * 8)()
+    _check(_lib().fn2_conv_plan(C.byref(desc(c, layout=layout)), c.N, c.H, c.W, cis, out))
+    return list(out)
+
+
+def split_bytes(pl):
+    """Workspace of the per-tap engine's K split: the partial tiles plus 4 floats to align them (conv_tc_workspace_floats)."""
+    return ((pl[1] - pl[4]) * pl[5] * 128 * pl[0] + 4) * 4 if pl[0] > 0 and pl[5] > 1 else 0
+
+
+def ws_bytes(c):
+    nb = C.c_size_t()
+    _check(_lib().fn2_conv_workspace_bytes(C.byref(desc(c)), c.N, c.H, c.W, C.byref(nb)))
+    return nb.value
+
+
+def op_weights(c, w):
+    """The Caffe-layout weights of the operator: the case's own, or for a data gradient the layer's, flipped and transposed
+    when fn2_conv_backward_data_desc asks for it, with BackwardData's zero rows for padded output channels."""
+    if not c.fwd:
+        return w
+    Ci, Co, k, s, p, deconv, H, W, flip, co_real = c.fwd
+    if flip:
+        from flownet2_b200 import fn2_conv_desc
+        d = fn2_conv_desc(Ci, Co, k[0], k[1], s[0], s[1], p[0], p[1], int(deconv), 1, 0, 0.0, 0, 0)
+        w2 = torch.empty((Ci, Co) + tuple(k), device="cuda")
+        _check(_lib().fn2_conv_flip_transpose_weights(C.byref(d), w.data_ptr(), w2.data_ptr(), torch.cuda.current_stream().cuda_stream))
+        w = w2
+    if c.Co > co_real:
+        w = torch.cat([w, torch.zeros((c.Co - co_real,) + tuple(w.shape[1:]), device="cuda")])
+    return w.contiguous()
+
+
+Run = namedtuple("Run", "go wide out ws_buf")
+
+
+def prepare(c, x, w, b, layout=None, engine=None, ws="exact"):
+    """Pack the weights and allocate the top (channels [16, 16 + Co) of a channels_last buffer of Co + 32 filled with
+    SENTINEL).  -> Run whose go() enqueues fn2_conv_forward.  ws: "exact" the reported bytes 4 bytes past a 256-byte boundary,
+    followed by 0xA5 bytes; "short" one float fewer than the K split takes (the report covers the SIMT route's needs too);
+    "null" no workspace."""
+    from flownet2_b200 import ops as _ops
+    layout = layout or c.layout
+    l, d, xv = _lib(), desc(c, engine, layout), bottom(x, layout)
+    cis = xv.stride(3) if xv.stride(1) == 1 else c.Ci
+    nf = C.c_size_t()
+    _check(l.fn2_conv_packed_floats(C.byref(d), cis, C.byref(nf)))
+    packed = torch.empty(max(nf.value, 1), device="cuda")
+    _check(l.fn2_conv_pack_weights(C.byref(d), cis, op_weights(c, w).data_ptr(), packed.data_ptr(),
+                                   torch.cuda.current_stream().cuda_stream))
+    ho, wo = out_hw(c)
+    wide = torch.full((c.N, c.Co + 32, ho, wo), SENTINEL, device="cuda").contiguous(memory_format=torch.channels_last)
+    out = wide[:, 16:16 + c.Co]
+    nb = ws_bytes(c)
+    buf, wsp, wsn = None, None, 0
+    if ws != "null":
+        buf = torch.full((nb + 512 + 4096,), 0xA5, dtype=torch.uint8, device="cuda")
+        off = (-buf.data_ptr()) % 256 + 4
+        wsp, wsn = buf.data_ptr() + off, (min(nb, split_bytes(plan_of(c, layout))) - 4 if ws == "short" else nb)
+        buf = (buf, off + wsn)
+    dx, dout = _ops.desc(xv), _ops.desc(out)
+
+    def go():
+        _check(l.fn2_conv_forward(C.byref(d), C.byref(dx), packed.data_ptr(), b.data_ptr() if b is not None else None,
+                                  C.byref(dout), wsp, wsn, torch.cuda.current_stream().cuda_stream))
+    go.keep = (xv, packed, b)
+    return Run(go, wide, out, buf)
+
+
+# ---- reference ----------------------------------------------------------------------------------------------------------------
+def ref_at(x, w, deconv, s, p, n, oy, ox):
+    """float64 (P, Co) outputs at the pixels (n, oy, ox) without bias: per kernel tap one BLAS product of the tap's weights with
+    the input pixels it reads there.  x (N, Ci, H, W); w in Caffe layout; a deconvolution's tap (ky, kx) reads input pixel
+    ((oy + ph - ky) / sh, (ox + pw - kx) / sw) where both divide exactly."""
+    (sh, sw), (ph, pw) = s, p
+    x, w = x.double(), w.double()
+    N, Ci, H, W = x.shape
+    kh, kw = w.shape[2:]
+    out = torch.zeros((len(n), w.shape[1] if deconv else w.shape[0]), dtype=torch.float64, device=x.device)
+
+    def coord(o, st, pd, kk, size):
+        if deconv:
+            t = o + pd - kk
+            i = torch.div(t, st, rounding_mode="floor")
+            ok = (i * st == t)
+        else:
+            i = o * st + kk - pd
+            ok = torch.ones_like(i, dtype=torch.bool)
+        return i, ok & (i >= 0) & (i < size)
+
+    for ky in range(kh):
+        iy, oky = coord(oy, sh, ph, ky, H)
+        for kx in range(kw):
+            ix, okx = coord(ox, sw, pw, kx, W)
+            sel = (oky & okx).nonzero().squeeze(1)
+            if len(sel):
+                wt = w[:, :, ky, kx] if deconv else w[:, :, ky, kx].T             # (Ci, Co)
+                out.index_add_(0, sel, x[n[sel], :, iy[sel], ix[sel]] @ wt)
+    return out
+
+
+def reference(c, x, w, b, n, oy, ox):
+    """The case's outputs at (n, oy, ox) in float64, in chunks that keep the gathered inputs small; a data-gradient operator
+    is computed as the transpose of its layer, from the layer's weights."""
+    if c.fwd:
+        _, _, _, s, p, deconv, _, _, _, _ = c.fwd
+        deconv = not deconv
+    else:
+        s, p, deconv = c.s, c.p, c.deconv
+    step = max(256, (1 << 25) // c.Ci)
+    out = torch.cat([ref_at(x, w, deconv, s, p, n[i:i + step], oy[i:i + step], ox[i:i + step]) for i in range(0, len(n), step)])
+    if b is not None:
+        out = out + b.double()
+        out = torch.where(out > 0, out, out * SLOPE)
+    return out
+
+
+def tile_width(c, Wo):
+    """The per-tap engine's tile width: the smallest power of two >= the widest parity class, clamped to [8, 128]."""
+    wmax = -(-Wo // c.s[1]) if c.deconv else Wo
+    tw = 8
+    while tw < wmax and tw < 128:
+        tw *= 2
+    return tw
+
+
+def classes(c, Ho, Wo):
+    sh, sw = c.s if c.deconv else (1, 1)
+    return [(py, px) for py in range(min(sh, Ho)) for px in range(min(sw, Wo))]
+
+
+def sample(c, pl, Ho, Wo, seed):
+    """Output pixels the reference evaluates: all of a small map; else every pixel of the first and last tile row and column
+    (of every parity class), of every K-split tile (tile ((cls * cotiles + cot) * ntiles + pix), tc_whole_tile) and SAMPLE
+    seeded random others.  The taps-on-N engine's tiles are 32 columns by 4 input rows."""
+    if c.N * Ho * Wo <= FULL:
+        m = torch.ones((c.N, Ho, Wo), dtype=torch.bool, device="cuda")
+        return [t.contiguous() for t in m.nonzero().unbind(1)]
+    ou, ov = c.s if c.deconv else (1, 1)
+    tw = 32 if pl[3] == 3 else tile_width(c, Wo)
+    th = 4 if pl[3] == 3 else 128 // tw
+    hmax, wmax = -(-Ho // ou), -(-Wo // ov)
+    tiles_y, tiles_x = -(-hmax // th), -(-wmax // tw)
+    m = torch.zeros((c.N, Ho, Wo), dtype=torch.bool, device="cuda")
+    u, v = torch.arange(Ho, device="cuda") // ou, torch.arange(Wo, device="cuda") // ov
+    m[:, (u < th) | (u >= (tiles_y - 1) * th), :] = True
+    m[:, :, (v < tw) | (v >= (tiles_x - 1) * tw)] = True
+    if pl[3] != 3 and pl[5] > 1:
+        cls, ntiles = classes(c, Ho, Wo), c.N * tiles_x * tiles_y
+        for t in range(pl[4], pl[1]):
+            pix, r = t % ntiles, t // ntiles
+            py, px = cls[r // (c.Co // pl[0])]
+            tx, q = pix % tiles_x, pix // tiles_x
+            ty, nn = q % tiles_y, q // tiles_y
+            m[nn, ty * th * ou + py:(ty + 1) * th * ou:ou, tx * tw * ov + px:(tx + 1) * tw * ov:ov] = True
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    m.view(-1)[torch.randint(0, m.numel(), (SAMPLE,), generator=g, device="cuda")] = True
+    return [t.contiguous() for t in m.nonzero().unbind(1)]
+
+
+def shrink(got, want):
+    """mean signed error relative to mean |want|: < 0 when the engine's sums come out systematically too small in magnitude"""
+    return float(((got - want) * torch.sign(want)).mean() / want.abs().mean())
+
+
+def check(c, seed=None, same_sign=False, layout=None, engine=None, ws="exact", twice=False):
+    """Run the case and compare the sampled outputs with the reference.  -> (max error / max(1, max |want|), shrink)"""
+    seed = seed_of(c) if seed is None else seed
+    x, w, b = draw(c, seed, same_sign)
+    r = prepare(c, x, w, b, layout, engine, ws)
+    r.go()
+    if twice:
+        first = r.wide.contiguous()
+        r.go()
+        assert torch.equal(first.view(torch.int32), r.wide.contiguous().view(torch.int32)), "two calls differ"
+    assert bool((r.wide[:, :16] == SENTINEL).all()) and bool((r.wide[:, 16 + c.Co:] == SENTINEL).all()), "write outside the top"
+    if r.ws_buf is not None:
+        buf, end = r.ws_buf
+        assert bool((buf[end:] == 0xA5).all()), "write past the end of the workspace"
+    ho, wo = out_hw(c)
+    n, oy, ox = sample(c, plan_of(c, layout), ho, wo, seed)
+    want = reference(c, x, w, b, n, oy, ox)
+    got = r.out[n, :, oy, ox].double()
+    real = c.fwd[9] if c.fwd else c.Co
+    assert bool((got[:, real:] == 0).all()), "padded output channels are not 0"
+    got = got[:, :real]
+    assert bool(torch.isfinite(got).all()), "non-finite output"
+    err = float((got - want).abs().max()) / max(1.0, float(want.abs().max()))
+    assert err <= TOL, (c.name, err)
+    return err, shrink(got, want)
+
+
+# ---- the reference itself ----------------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("c", [case("c", 2, 5, 9, 11, 7, 3, 1, 1), case("c_s2", 1, 6, 10, 13, 4, 5, 2, 2),
+                               case("c_k3x5", 1, 3, 8, 12, 5, (3, 5), (2, 1), (0, 2)),
+                               case("d_s2", 2, 4, 4, 5, 3, 4, 2, 1, True), case("d_k3x5_s1", 1, 3, 5, 6, 4, (3, 5), 1, (1, 2), True)],
+                         ids=lambda c: c.name)
+def test_reference_matches_oracle(c):
+    """ref_at against oracle.conv_fwd / deconv_fwd (float64 accumulation, result rounded to float32) on small cases: every entry
+    is the oracle's to within the float32 rounding of the oracle's result."""
+    r = np.random.default_rng(3)
+    x = r.standard_normal((c.N, c.Ci, c.H, c.W)).astype(np.float32)
+    w = r.standard_normal(weight_shape(c)).astype(np.float32)
+    want = (O.deconv_fwd if c.deconv else O.conv_fwd)(x, w, None, c.s, c.p, f64acc=True)
+    m = torch.ones(want.shape[0:1] + want.shape[2:], dtype=torch.bool)
+    n, oy, ox = m.nonzero().unbind(1)
+    got = ref_at(torch.from_numpy(x), torch.from_numpy(w), c.deconv, c.s, c.p, n, oy, ox).numpy()
+    want = want.transpose(0, 2, 3, 1).reshape(-1, want.shape[1])
+    assert (np.abs(got - want) <= 2 ** -24 * np.abs(got) + 1e-12 * np.abs(got).max()).all()
+
+
+# ---- plan coverage and routes -------------------------------------------------------------------------------------------------
+def test_conv_tc_plan_coverage(ops):
+    """The table reaches every plan value listed in the module docstring on this card."""
+    tc, tn = [], []
+    for c in PLAN_CASES:
+        pl = plan_of(c)
+        assert pl[0] != 0, (c.name, pl)
+        ho, wo = out_hw(c)
+        (tn if pl[3] == 3 else tc).append((c, pl, ho, wo))
+    m0 = [(c, pl, ho, wo) for c, pl, ho, wo in tc if pl[3] == 0]
+    split = [(c, pl) for c, pl, _, _ in m0 if pl[5] > 1]
+    for nt in (16, 32, 64, 128):
+        assert any(pl[0] == nt and c.Co > nt for c, pl, _, _ in m0), nt
+    assert {tile_width(c, wo) for c, pl, ho, wo in m0} >= {8, 16, 32, 64, 128}
+    assert any(wo > 128 for c, pl, ho, wo in m0)
+    assert any(pl[2] == 1 for _, pl, _, _ in m0) and any(pl[2] % 4 for _, pl, _, _ in m0 if pl[2] > 4)
+    assert any(c.Ci % 32 and c.Ci > 32 for c, pl, _, _ in m0) and any(c.Ci < 32 and pl[2] == 1 for c, pl, _, _ in m0)
+    assert {c.s for c, _, _, _ in m0 if not c.deconv} >= {(1, 1), (2, 2), (1, 2), (2, 1)}
+    assert any(c.k[0] != c.k[1] for c, _, _, _ in m0) and any(c.p[0] != c.p[1] for c, _, _, _ in m0)
+    # K split: both regimes at NT 128 and NT <= 64 (NT 16 included), z up to 8, with and without bias
+    for nts in ({128}, {16, 32, 64}, {16}):
+        assert any(pl[0] in nts and pl[4] == 0 for _, pl in split), nts
+        assert any(pl[0] in nts and pl[4] > 0 for _, pl in split), nts
+    assert max(pl[5] for _, pl in split) == 8
+    assert any(c.bias for c, _ in split) and any(not c.bias for c, _ in split)
+    assert any(c.deconv and (ho % 2 or wo % 2) for c, pl, ho, wo in m0 if pl[5] > 1)
+    # deconvolution: stride 1, stride 2 with k 2-5, odd sizes, an out_pad with out_pad_h != out_pad_w
+    dec = [(c, ho, wo) for c, pl, ho, wo in m0 if c.deconv]
+    assert any(c.s == (1, 1) for c, _, _ in dec)
+    assert {c.k[0] for c, _, _ in dec if c.s == (2, 2)} >= {2, 3, 4, 5}
+    assert any(ho % 2 and wo % 2 for c, ho, wo in dec if c.s == (2, 2))
+    assert any(c.op[0] != c.op[1] for c, _, _ in dec)
+    # tap groups: cs 4, 8, 12, 16 with a partial last group, NT 128
+    m1 = [(c, pl) for c, pl, _, _ in tc if pl[3] == 1]
+    cs = lambda c: (c.Ci + 3) // 4 * 4
+    assert {cs(c) for c, pl in m1 if (c.k[0] * c.k[1]) % (32 // cs(c))} == {4, 8, 12, 16}
+    assert any(pl[0] == 128 for _, pl in m1)
+    # kernel rows: several K blocks per row, stride 1 and 2, a row wider than a tile, N > 1
+    m2 = [(c, pl, wo) for c, pl, _, wo in tc if pl[3] == 2]
+    assert any(pl[2] > c.k[0] for c, pl, _ in m2)
+    assert {c.s for c, _, _ in m2} == {(1, 1), (2, 2)} and any(wo > 128 for _, _, wo in m2) and any(c.N > 1 for c, _, _ in m2)
+    # taps on N: Co 16 and 32 at stride 1 and as stride-2 deconvolutions; passes, widths, kh != kw, Ci tail and 256, several
+    # strips and segments, weights resident and in a ring
+    assert {(c.Co, c.deconv) for c, _, _, _ in tn} == {(16, False), (16, True), (32, False), (32, True)}
+    assert {pl[4] for _, pl, _, _ in tn} >= {1, 2, 3, 6} and {-pl[0] for _, pl, _, _ in tn} == {64, 80, 96}
+    assert any(c.k == (1, 4) and c.deconv for c, _, _, _ in tn) and any(c.k[0] != c.k[1] and not c.deconv for c, _, _, _ in tn)
+    assert {17, 256} <= {c.Ci for c, _, _, _ in tn}
+    assert any(pl[5] > 1 for _, pl, _, _ in tn) and any(ho >= 100 for _, _, ho, _ in tn)
+    assert {min(pl[6], 1) for _, pl, _, _ in tn} == {0, 1}
+
+
+def expected_kernels(c, pl):
+    """Name fragments of the kernels the case must launch, and of those it must not."""
+    if pl[3] == 3:
+        return ["conv_tn_kernel<%d, %d>" % (c.Co, 2 if c.deconv else 1)], ["conv_tc_kernel<", "tc_split_reduce_kernel<"]
+    want = ["conv_tc_kernel<%d, %d>" % (pl[0], pl[3])]
+    reduce = "tc_split_reduce_kernel<%d>" % pl[0]
+    return (want + [reduce], []) if pl[5] > 1 else (want, [reduce])
+
+
+@pytest.mark.parametrize("c", PLAN_CASES + NO_TAP_CASES, ids=PLAN_IDS + [c.name for c in NO_TAP_CASES])
+def test_conv_tc_route_kernels(ops, c):
+    """The case runs the kernels of its plan and nothing else: conv_tc_kernel<NT, mode> with the planned NT, and
+    tc_split_reduce_kernel<NT> exactly when the plan splits K; conv_tn_kernel<Co, S> for mode 3.  A deconvolution with a parity
+    class that no tap reaches runs on the SIMT engine."""
+    x, w, b = draw(c, 1)
+    r = prepare(c, x, w, b)
+    got, = kernels_per_case([r.go])
+    pl = plan_of(c)
+    if c in NO_TAP_CASES:
+        assert pl[0] == 0 and got and not any("conv_tc_kernel" in k or "conv_tn_kernel" in k for k in got), sorted(got)
+        return
+    want, not_want = expected_kernels(c, pl)
+    assert all(any(k in n for n in got) for k in want), (want, sorted(got))
+    assert len(got) == len(want) and not any(k in n for k in not_want for n in got), (want, sorted(got))
+
+
+@pytest.mark.parametrize("c", PLAN_CASES, ids=PLAN_IDS)
+def test_conv_tc_plan_case(ops, c):
+    """Within 1e-6 of the reference, nothing written outside the top's channel slice or past the workspace, and two calls
+    bit-identical."""
+    check(c, twice=True)
+
+
+@pytest.mark.parametrize("c", NO_TAP_CASES, ids=[c.name for c in NO_TAP_CASES])
+def test_deconv_with_untapped_class(ops, fn2, c):
+    """A deconvolution whose kernel is shorter than its stride (1 x 1 or 1 x 4 at stride 2, and the data gradient of a 1 x 1
+    stride-2 convolution) leaves output rows or columns that no tap reaches: they hold bias plus ReLU.  The default engine runs
+    it on SIMT; the tensor-core engine refuses it."""
+    check(c)
+    x, w, b = draw(c, 2)
+    with pytest.raises(fn2.Fn2Error, match="fn2 error -1"):
+        prepare(c, x, w, b, engine=2).go()
+
+
+# ---- layouts, workspace ----------------------------------------------------------------------------------------------------
+LAYOUT_CASES = [BY_NAME[n] for n in ("nt64_co192_split", "d_k5_odd", "grp_cs4", "row_ci12_s2", "row_ci6", "tn16_k3_strips",
+                                     "tn32_d4")]
+
+
+@pytest.mark.parametrize("layout", ["nhwc", "pad", "padjunk", "padnan", "slice"])
+@pytest.mark.parametrize("c", LAYOUT_CASES, ids=[c.name for c in LAYOUT_CASES])
+def test_conv_tc_bottom_layouts(ops, c, layout):
+    """Bottom as channels_last with 16-byte pixels, with the nets' padded pixel stride and guard band, and as a channel slice of
+    a wider parent whose other channels hold NaN.  The padding channels: zero; finite garbage under the guard promise (the
+    kernel-row packing reads them against zero weights: fn2.h, input_guard_bytes); NaN without it (never read)."""
+    if c.name.startswith("row_"):
+        assert plan_of(c, layout)[3] == (2 if guard_bytes(layout) else 1), layout
+    check(c, layout=layout)
+
+
+@pytest.mark.parametrize("c", [BY_NAME["nt32_co96_s2"], BY_NAME["d_k4"], BY_NAME["tn16_k3_strips"]], ids=lambda c: c.name)
+def test_conv_tc_misaligned_bottom(ops, fn2, c):
+    """A bottom whose first channel is not on a 16-byte boundary is no tensor-core operand: the default engine falls back to
+    SIMT, the tensor-core engine refuses it."""
+    check(c, layout="misaligned", engine=0)
+    x, w, b = draw(c, 2)
+    with pytest.raises(fn2.Fn2Error, match="fn2 error -1"):
+        prepare(c, x, w, b, layout="misaligned", engine=2).go()
+
+
+WS_CASES = [BY_NAME[n] for n in ("nt16_split_all", "nt128_co256_split", "z8_tw16", "nt128_tail_ci473", "d_k3_odd_split")]
+
+
+@pytest.mark.parametrize("c", WS_CASES, ids=lambda c: c.name)
+def test_conv_tc_workspace_contract(ops, c):
+    """Exactly the reported bytes, 4 bytes past a 256-byte boundary, suffice for the K split and nothing after them is written;
+    one float fewer than the split takes, or no workspace at all, runs the layer unsplit (no reduction kernel) to the same
+    tolerance."""
+    pl = plan_of(c)
+    assert pl[5] > 1 and ws_bytes(c) >= split_bytes(pl)
+    check(c, ws="exact")
+    x, w, b = draw(c, 4)
+    for ws in ("short", "null"):
+        check(c, ws=ws)
+        got, = kernels_per_case([prepare(c, x, w, b, ws=ws).go])
+        assert any("conv_tc_kernel<" in n for n in got) and not any("tc_split_reduce_kernel" in n for n in got), (ws, sorted(got))
+
+
+# ---- shapes the nets run ------------------------------------------------------------------------------------------------------
+def plan_key(c):
+    pl = plan_of(c)
+    ho, wo = out_hw(c)
+    return (pl[0], pl[3], pl[5] > 1, pl[4] == 0, len(classes(c, ho, wo)), tile_width(c, wo), pl[4] if pl[3] == 3 else 0)
+
+
+def _deploy_cases():
+    cases, keys = [], set()
+    for name, ci, h, w, co, k, s, p, deconv, _ in deploy_convs("FlowNet2", 1024, 436):
+        c = case("deploy-" + name, 4, ci, h, w, co, k, s, p, deconv, bias=False, layout="pad")
+        if plan_of(c)[0] == 0 or plan_key(c) in keys:
+            continue
+        keys.add(plan_key(c))
+        cases.append(c)
+    return cases
+
+
+def _grad_cases():
+    cases, seen, keys = [], set(), set()
+    for model in ("FlowNet2-C", "FlowNet2-SD", "FlowNet2"):
+        for name, ci, h, w, co, k, s, p, deconv, _ in train_convs(model):
+            if ci <= 16:
+                continue                  # the layers on the input images: no data gradient
+            c = adjoint("%s-%s" % (model[9:] or "fusion", name), 8, ci, h, w, co, k, s, p, deconv)
+            if plan_of(c)[0] == 0 or c[1:] in seen:
+                continue
+            if model != "FlowNet2-C" and plan_key(c) in keys:
+                continue                  # the SD and fusion stages add the operators whose plan the C graph does not reach
+            seen.add(c[1:])
+            keys.add(plan_key(c))
+            cases.append(c)
+    return cases
+
+
+DEPLOY_CASES = _deploy_cases()
+GRAD_CASES = _grad_cases()
+
+# Bound on |shrink| per case.  The tensor-core chains truncate, and with same-sign products every chunk loses magnitude; the
+# engines add back TRUNC_LOSS_PER_MMA per chained MMA (the per-tap engine per chunk, the taps-on-N engine per pass, p->comp).
+# Measured on an H100 80GB HBM3 (700 W power limit) over 4 seeds, with that library and with one built with the constant set
+# to 0: the compensation takes back about 65 % of the loss at NT = 128 (-9.7e-8 -> -3.3e-8), about 50 % at NT <= 64 (4-step
+# chunks: -4.1e-7 -> -2.1e-7), 60-80 % on the taps-on-N engine (fuse_deconv0: -1.12e-6 -> -3.0e-7), and over-corrects the
+# tap-group adjoints of the 2-channel predictors (-7.3e-8 -> +2.7e-8).  Each bound lies between max |shrink| + 3 x spread of
+# the compensating library and half the smallest |shrink| without it (by a factor >= 1.1), so it fails when the compensation
+# is lost.  The cases not listed keep only the 1e-6 bound: there the two libraries' shrinks are not that far apart (the NT 64
+# and NT 32 layers, where the compensated residual is about half the uncompensated loss, and the over-corrected predictors).
+SHRINK_BOUND = {
+    'deploy-net1_conv1': 1.3e-07, 'deploy-net1_conv2': 4e-08, 'deploy-net1_conv3': 4.1e-08, 'deploy-net1_conv4': 4e-08,
+    'deploy-net1_conv4_1': 4.1e-08, 'deploy-net1_conv5': 4.1e-08, 'deploy-net1_conv6': 4.1e-08, 'deploy-net1_deconv5': 4e-08,
+    'deploy-net1_deconv4': 4.1e-08, 'deploy-net1_deconv3': 4e-08, 'deploy-fuse_conv0': 1e-07, 'deploy-fuse_deconv1': 2.9e-07,
+    'deploy-fuse_interconv1': 4.1e-07, 'deploy-fuse_deconv0': 4.3e-07, 'deploy-fuse_interconv0': 1.5e-07, 'C-conv3': 4.1e-08,
+    'C-conv_redir': 4.3e-08, 'C-conv3_1': 4.1e-08, 'C-conv4': 4e-08, 'C-conv4_1': 4.1e-08, 'C-conv5': 4.1e-08,
+    'C-conv5_1': 4.2e-08, 'C-conv6': 4.1e-08, 'C-conv6_1': 4.1e-08, 'C-deconv5': 4e-08, 'C-predict_flow5': 2.9e-08,
+    'C-deconv4': 4.1e-08, 'C-predict_flow4': 3.3e-08, 'C-predict_flow2': 2.5e-08, 'SD-conv2': 4.1e-08, 'SD-conv2_1': 4.1e-08,
+    'SD-conv3_1': 4e-08, 'SD-predict_flow4': 2.4e-08, 'SD-predict_flow3': 2.2e-08,
+}
+
+
+def test_shrink_bounds_name_cases():
+    assert set(SHRINK_BOUND) <= {c.name for c in DEPLOY_CASES + GRAD_CASES}
+
+
+@pytest.mark.parametrize("c", DEPLOY_CASES, ids=[c.name for c in DEPLOY_CASES])
+def test_conv_tc_deploy_shapes(ops, c):
+    """FlowNet2's convolutions and deconvolutions at 4 pairs of 1024 x 448, one per plan key: post-ReLU bottom with the nets'
+    pixel stride, weights of one sign; within 1e-6 and, where listed, without the systematic shrink of uncompensated
+    truncating chains (SHRINK_BOUND)."""
+    err, sh = check(c, same_sign=True)
+    print("%s plan %s maxerr %.3g shrink %.3g" % (c.name, plan_of(c), err, sh))
+    if c.name in SHRINK_BOUND:
+        assert abs(sh) <= SHRINK_BOUND[c.name], (c.name, sh)
+
+
+@pytest.mark.parametrize("c", GRAD_CASES, ids=[c.name for c in GRAD_CASES])
+def test_conv_tc_data_gradient_operators(ops, c):
+    """The data-gradient operators of the training graphs at 448 x 320, batch 8, built like BaseConvolutionLayer::BackwardData
+    (fn2_conv_backward_data_desc, flipped weights, padded output channels that must come out exactly 0), on a post-ReLU top
+    diff; compared with the transpose of the layer itself."""
+    err, sh = check(c, same_sign=True)
+    print("%s plan %s maxerr %.3g shrink %.3g" % (c.name, plan_of(c), err, sh))
+    if c.name in SHRINK_BOUND:
+        assert abs(sh) <= SHRINK_BOUND[c.name], (c.name, sh)

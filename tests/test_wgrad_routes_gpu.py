@@ -18,9 +18,8 @@ import zlib
 import numpy as np
 import pytest
 
-from oracle import net as onet
 from oracle import oracle as O
-from tests.util import kernels_per_case, maxabs, rng
+from tests.util import kernels_per_case, maxabs, rng, train_convs
 
 pytestmark = pytest.mark.gpu
 torch = pytest.importorskip("torch")
@@ -348,66 +347,6 @@ def test_wgrad_argument_errors(ops, fn2):
 
 
 # ---- training shapes ------------------------------------------------------------------------------------------------------------
-def train_convs(model, width=448, height=320):
-    """The Convolution / Deconvolution layers of models/<model>_train.prototxt.template at a width x height crop: (name, Ci, H, W,
-    Co, (kh, kw), s, (ph, pw), deconv, trainable), from the oracle's prototxt parser and a walk over the blob shapes."""
-    from flownet2_b200 import fill_train_template, ops as _ops, train_template
-    get, getall = onet.get, onet.getall
-    text = fill_train_template(train_template(model), width, height, width + 64, height + 64, 1)
-    shp, out = {}, []
-    for l in getall(onet.parse_prototxt(text), "layer"):
-        ty, bots, tops = get(l, "type"), getall(l, "bottom"), getall(l, "top")
-        b = [shp.get(n) for n in bots]
-        if ty == "Input":
-            for t, s in zip(tops, getall(get(l, "input_param"), "shape")):
-                shp[t] = tuple(int(d) for d in getall(s, "dim"))[1:]
-        elif ty in ("Convolution", "Deconvolution"):
-            cp = get(l, "convolution_param")
-            kh, kw = onet._hw(cp, "kernel_size", "kernel_h", "kernel_w", 0)
-            sh, sw = onet._hw(cp, "stride", "stride_h", "stride_w", 1)
-            ph, pw = onet._hw(cp, "pad", "pad_h", "pad_w", 0)
-            assert sh == sw
-            ci, h, w = b[0]
-            co = int(get(cp, "num_output"))
-            if ty == "Deconvolution":
-                ho, wo = sh * (h - 1) + kh - 2 * ph, sw * (w - 1) + kw - 2 * pw
-            else:
-                ho, wo = (h + 2 * ph - kh) // sh + 1, (w + 2 * pw - kw) // sw + 1
-            for t in tops:
-                shp[t] = (co, ho, wo)
-            lr = [float(get(pp, "lr_mult", 1)) for pp in getall(l, "param")]
-            out.append((get(l, "name"), ci, h, w, co, (kh, kw), sh, (ph, pw), ty == "Deconvolution", any(lr) or not lr))
-        elif ty == "DataAugmentation":
-            ap = get(l, "augmentation_param")
-            shp[tops[0]] = (b[0][0], int(get(ap, "crop_height")), int(get(ap, "crop_width")))
-            for t in tops[1:]:
-                shp[t] = (1, 1, 1)
-        elif ty == "GenerateAugmentationParameters":
-            shp[tops[0]] = (1, 1, 1)
-        elif ty == "FlowAugmentation":
-            ap = get(l, "augmentation_param")
-            shp[tops[0]] = (b[0][0], int(get(ap, "crop_height")), int(get(ap, "crop_width")))
-        elif ty == "Correlation":
-            cp = get(l, "correlation_param")
-            shp[tops[0]] = _ops.correlation_shape(b[0][1], b[0][2], int(get(cp, "pad", 0)), int(get(cp, "kernel_size")),
-                                                  int(get(cp, "max_displacement")), int(get(cp, "stride_1", 1)),
-                                                  int(get(cp, "stride_2", 1)))
-        elif ty == "Concat":
-            shp[tops[0]] = (sum(x[0] for x in b),) + b[0][1:]
-        elif ty in ("Downsample", "Resample"):
-            rp = get(l, "resample_param", [])
-            hw = b[1][1:] if len(b) > 1 else (int(get(rp, "height", get(get(l, "downsample_param", []), "top_height"))),
-                                               int(get(rp, "width", get(get(l, "downsample_param", []), "top_width"))))
-            shp[tops[0]] = (b[0][0],) + tuple(hw)
-        elif ty == "ChannelNorm":
-            shp[tops[0]] = (1,) + b[0][1:]
-        elif ty in ("ReLU", "Eltwise", "FlowWarp"):
-            shp[tops[0]] = b[0]
-        else:
-            assert ty in ("L1Loss", "Silence"), ty
-    return out
-
-
 def _train_cases():
     from flownet2_b200 import ops as _ops
     cases, seen, keys = [], set(), set()

@@ -32,6 +32,83 @@ def maxabs(a, b):
     return float(d.max()) if d.size else 0.0
 
 
+def net_convs(text):
+    """The Convolution / Deconvolution layers of a filled prototxt: (name, Ci, H, W, Co, (kh, kw), s, (ph, pw), deconv,
+    trainable), from the oracle's prototxt parser and a walk over the blob shapes.  A layer with two bottoms (the deploy nets'
+    conv1 on both images) is listed once; its bottoms have the same shape."""
+    from flownet2_b200 import ops as _ops
+    from oracle import net as onet
+    get, getall = onet.get, onet.getall
+    net = onet.parse_prototxt(text)
+    shp, out = {}, []
+    for t, s in zip(getall(net, "input"), getall(net, "input_shape")):            # legacy deploy inputs
+        shp[t] = tuple(int(d) for d in getall(s, "dim"))[1:]
+    for l in getall(net, "layer"):
+        ty, bots, tops = get(l, "type"), getall(l, "bottom"), getall(l, "top")
+        b = [shp.get(n) for n in bots]
+        if ty == "Input":
+            for t, s in zip(tops, getall(get(l, "input_param"), "shape")):
+                shp[t] = tuple(int(d) for d in getall(s, "dim"))[1:]
+        elif ty in ("Convolution", "Deconvolution"):
+            cp = get(l, "convolution_param")
+            kh, kw = onet._hw(cp, "kernel_size", "kernel_h", "kernel_w", 0)
+            sh, sw = onet._hw(cp, "stride", "stride_h", "stride_w", 1)
+            ph, pw = onet._hw(cp, "pad", "pad_h", "pad_w", 0)
+            assert sh == sw and all(x == b[0] for x in b)
+            ci, h, w = b[0]
+            co = int(get(cp, "num_output"))
+            if ty == "Deconvolution":
+                ho, wo = sh * (h - 1) + kh - 2 * ph, sw * (w - 1) + kw - 2 * pw
+            else:
+                ho, wo = (h + 2 * ph - kh) // sh + 1, (w + 2 * pw - kw) // sw + 1
+            for t in tops:
+                shp[t] = (co, ho, wo)
+            lr = [float(get(pp, "lr_mult", 1)) for pp in getall(l, "param")]
+            out.append((get(l, "name"), ci, h, w, co, (kh, kw), sh, (ph, pw), ty == "Deconvolution", any(lr) or not lr))
+        elif ty == "DataAugmentation":
+            ap = get(l, "augmentation_param")
+            shp[tops[0]] = (b[0][0], int(get(ap, "crop_height")), int(get(ap, "crop_width")))
+            for t in tops[1:]:
+                shp[t] = (1, 1, 1)
+        elif ty == "GenerateAugmentationParameters":
+            shp[tops[0]] = (1, 1, 1)
+        elif ty == "FlowAugmentation":
+            ap = get(l, "augmentation_param")
+            shp[tops[0]] = (b[0][0], int(get(ap, "crop_height")), int(get(ap, "crop_width")))
+        elif ty == "Correlation":
+            cp = get(l, "correlation_param")
+            shp[tops[0]] = _ops.correlation_shape(b[0][1], b[0][2], int(get(cp, "pad", 0)), int(get(cp, "kernel_size")),
+                                                  int(get(cp, "max_displacement")), int(get(cp, "stride_1", 1)),
+                                                  int(get(cp, "stride_2", 1)))
+        elif ty == "Concat":
+            shp[tops[0]] = (sum(x[0] for x in b),) + b[0][1:]
+        elif ty in ("Downsample", "Resample"):
+            # the size of the second bottom, else the layer's own (the deploy nets' 436 -> 448 adaptation)
+            rp = get(l, "resample_param", [])
+            hw = b[1][1:] if len(b) > 1 else (int(get(rp, "height", get(get(l, "downsample_param", []), "top_height"))),
+                                               int(get(rp, "width", get(get(l, "downsample_param", []), "top_width"))))
+            shp[tops[0]] = (b[0][0],) + tuple(hw)
+        elif ty == "ChannelNorm":
+            shp[tops[0]] = (1,) + b[0][1:]
+        elif ty in ("ReLU", "Eltwise", "FlowWarp"):
+            shp[tops[0]] = b[0]
+        else:
+            assert ty in ("L1Loss", "Silence"), ty
+    return out
+
+
+def train_convs(model, width=448, height=320):
+    """net_convs of models/<model>_train.prototxt.template at a width x height crop."""
+    from flownet2_b200 import fill_train_template, train_template
+    return net_convs(fill_train_template(train_template(model), width, height, width + 64, height + 64, 1))
+
+
+def deploy_convs(model, width=1024, height=436):
+    """net_convs of models/<model>_deploy.prototxt.template for width x height frames (adapted to multiples of 64 inside)."""
+    from flownet2_b200 import fill_template, model_template
+    return net_convs(fill_template(model_template(model), width, height))
+
+
 def kernels_per_case(runs):
     """Names of the kernels each of runs launches, from one profiler session.  Every run sits in a window of its own between
     synchronisations, 2 ms from the next.  A kernel belongs to the window of its launch call (the profiler gives both the
