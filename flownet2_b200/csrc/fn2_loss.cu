@@ -235,12 +235,15 @@ int fn2_l1loss_workspace_bytes(int N, int H, int W, size_t* bytes) {
 
 int fn2_l1loss_forward(const fn2_tensor* bottom0, const fn2_tensor* bottom1, const fn2_l1loss_desc* d, float* state_dev,
                        float* loss_dev, void* workspace, size_t workspace_bytes, void* stream) {
-    FN2_CHECK_ARG(valid(bottom0) && d && state_dev && workspace, "l1loss_forward: null argument");
+    FN2_CHECK_ARG(valid(bottom0) && d && state_dev, "l1loss_forward: null argument");
     T4 a = view(bottom0), b = a;
     if (bottom1) { FN2_CHECK_ARG(valid(bottom1), "l1loss_forward: bad second bottom"); b = view(bottom1); FN2_CHECK_ARG(same_dims(a, b), "l1loss_forward: bottoms differ in shape"); }
     const long long P = (long long)a.n * a.h * a.w;
     const int grid = loss_grid(P);
-    FN2_CHECK_ARG(workspace_bytes >= (size_t)grid * 2 * sizeof(float), "l1loss_forward: workspace too small");
+    if (!workspace || workspace_bytes < (size_t)grid * 2 * sizeof(float)) {
+        set_error("l1loss_forward: workspace too small (%zu < %zu)", workspace_bytes, (size_t)grid * 2 * sizeof(float));
+        return FN2_ERR_WORKSPACE;
+    }
     const L1P p = l1_params(d, a, bottom1);
     cudaStream_t st = (cudaStream_t)stream;
     if (p.l2_per_location) l1loss_fwd_kernel<true><<<grid, 256, 0, st>>>(a, b, p, (float*)workspace);

@@ -10,7 +10,7 @@ import ctypes as C
 
 import torch
 
-from . import check, fn2_conv_desc, fn2_tensor, lib
+from . import check, fn2_conv_desc, fn2_l1loss_desc, fn2_tensor, lib
 
 
 def desc(t):
@@ -116,8 +116,9 @@ def flow_warp(image, flow, fill_nan=False, out=None):
     return out
 
 
-def flow_warp_backward(image, flow, warped_diff):
-    gi, gf = torch.empty_like(image), torch.empty_like(flow)
+def flow_warp_backward(image, flow, warped_diff, out=None):
+    """-> (image_diff, flow_diff), into out = (image_diff, flow_diff) if given."""
+    gi, gf = out if out is not None else (torch.empty_like(image), torch.empty_like(flow))
     check(lib().fn2_flow_warp_backward(desc(image), desc(flow), desc(warped_diff), desc(gi), desc(gf), _stream()))
     return gi, gf
 
@@ -128,8 +129,9 @@ def resample(x, out_h, out_w, rtype=2, antialias=True):
     return out
 
 
-def spatial_augmentation(x, mats, out_h, out_w):
-    out = _empty((x.shape[0], x.shape[1], out_h, out_w), x)
+def spatial_augmentation(x, mats, out_h, out_w, out=None):
+    if out is None:
+        out = _empty((x.shape[0], x.shape[1], out_h, out_w), x)
     mats = mats.contiguous()
     check(lib().fn2_spatial_augmentation(desc(x), desc(out), _ptr(mats), _stream()))
     return out
@@ -323,6 +325,49 @@ def downsample(x, top_h, top_w, out=None):
     if out is None:
         out = _empty((x.shape[0], x.shape[1], top_h, top_w), x)
     check(lib().fn2_downsample_forward(desc(x), desc(out), _stream()))
+    return out
+
+
+def _l1_desc(l2_per_location, l2_prescale_by_channels, normalize_by_num_entries, epsilon, plateau):
+    return fn2_l1loss_desc(1 if l2_per_location else 0, 1 if l2_prescale_by_channels else 0, 1 if normalize_by_num_entries else 0,
+                           float(epsilon), float(plateau))
+
+
+def l1loss(b0, b1=None, *, l2_per_location=False, l2_prescale_by_channels=False, normalize_by_num_entries=False, epsilon=1e-2,
+           plateau=0.0, workspace=None):
+    """L1LossLayer::Forward_gpu through the C-ABI -> (loss, state): two device float tensors, the loss (1 float) and the state
+    {loss, normalize_coeff, masked sum, not-NaN count} the backward reads.  workspace: a uint8 CUDA tensor whose bytes are the
+    workspace (default: one of the reported size)."""
+    l = lib()
+    d = _l1_desc(l2_per_location, l2_prescale_by_channels, normalize_by_num_entries, epsilon, plateau)
+    if workspace is None:
+        workspace = _ws(_size(l.fn2_l1loss_workspace_bytes, b0.shape[0], b0.shape[2], b0.shape[3]), b0.device)
+    assert workspace.dtype == torch.uint8 and workspace.is_contiguous()
+    loss = torch.empty(1, dtype=torch.float32, device=b0.device)
+    state = torch.empty(4, dtype=torch.float32, device=b0.device)
+    check(l.fn2_l1loss_forward(desc(b0), desc(b1) if b1 is not None else None, d, _ptr(state), _ptr(loss), _ptr(workspace),
+                               workspace.numel(), _stream()))
+    return loss, state
+
+
+def l1loss_backward(b0, b1=None, *, l2_per_location=False, l2_prescale_by_channels=False, normalize_by_num_entries=False,
+                    epsilon=1e-2, plateau=0.0, state, top_diff, out0=None, out1=None, accumulate0=False, accumulate1=False):
+    """L1LossLayer::Backward_gpu: writes (accumulate: adds) the gradient of each bottom into out0 / out1; None: do not
+    propagate to that bottom.  state: from l1loss(); top_diff: the loss weight as a device float tensor.  -> (out0, out1)"""
+    d = _l1_desc(l2_per_location, l2_prescale_by_channels, normalize_by_num_entries, epsilon, plateau)
+    check(lib().fn2_l1loss_backward(desc(b0), desc(b1) if b1 is not None else None, d, _ptr(state), _ptr(top_diff),
+                                    desc(out0) if out0 is not None else None, desc(out1) if out1 is not None else None,
+                                    1 if accumulate0 else 0, 1 if accumulate1 else 0, _stream()))
+    return out0, out1
+
+
+def flow_augmentation(flow, mats1, mats2_inverse, out_h, out_w, out=None):
+    """FlowAugmentation: the flow (N, 2, H, W) of the pair augmented by mats1 / the inverse of mats2 (N x 6 floats each, NAME
+    order t0..t5, device tensors) -> out (N, 2, out_h, out_w), a new tensor if None."""
+    if out is None:
+        out = _empty((flow.shape[0], 2, out_h, out_w), flow)
+    mats1, mats2_inverse = mats1.contiguous(), mats2_inverse.contiguous()
+    check(lib().fn2_flow_augmentation(desc(flow), desc(out), _ptr(mats1), _ptr(mats2_inverse), _stream()))
     return out
 
 

@@ -231,7 +231,8 @@ FN2_API int fn2_conv_flip_transpose_weights(const fn2_conv_desc* d, const float*
  * L1Loss -- replaces L1LossLayer::Forward_gpu / Backward_gpu (l1loss_layer.cu:67-192; the CPU paths are NOT_IMPLEMENTED in the
  * reference, l1loss_layer.cpp:93-102).  bottom1 may be NULL (single-bottom form).  state_dev: 4 device floats the forward
  * writes and the backward reads: {loss, normalize_coeff, masked sum, not-NaN count}; loss_dev (may be NULL) also receives the
- * loss.  top_diff_dev: device scalar (the loss weight).  The backward recomputes the difference and the NaN / plateau masks from
+ * loss.  workspace: at least fn2_l1loss_workspace_bytes(N, H, W) bytes, 4-byte aligned; a NULL or smaller one returns
+ * FN2_ERR_WORKSPACE.  The forward reduces its per-block partials in a fixed order: equal inputs give bit-identical state.  top_diff_dev: device scalar (the loss weight).  The backward recomputes the difference and the NaN / plateau masks from
  * the bottoms; a NULL diff pointer means "do not propagate to this bottom"; accumulate != 0 adds to the diff. */
 typedef struct fn2_l1loss_desc {
     int32_t l2_per_location, l2_prescale_by_channels, normalize_by_num_entries;   /* L1LossParameter, caffe.proto:619-625 */

@@ -19,7 +19,7 @@ import numpy as np
 import pytest
 
 from oracle import oracle as O
-from tests.util import kernels_per_case, maxabs, rng, train_convs
+from tests.util import device_view, kernels_per_case, maxabs, rng, train_convs
 
 pytestmark = pytest.mark.gpu
 torch = pytest.importorskip("torch")
@@ -127,23 +127,7 @@ def seed_of(c):
     return zlib.crc32(repr(c).encode())
 
 
-def dev(a, layout="nhwc"):
-    """nchw / nhwc dense; "pad": the nets' pixel stride (Blob::compute_cstride: channels rounded up to 4 below 32, else to 32);
-    "slice": channels [5, 5 + C) of a wider channels_last parent (a zero-copy concat child).  Channels outside the view hold NaN."""
-    t = torch.from_numpy(np.ascontiguousarray(a, np.float32)).cuda()
-    if layout == "nchw":
-        return t
-    if layout == "nhwc":
-        return t.contiguous(memory_format=torch.channels_last)
-    n, c, h, w = t.shape
-    if layout == "pad":
-        align = 4 if c < 32 else 32
-        off, width = 0, (c + align - 1) // align * align
-    else:
-        off, width = 5, c + 8
-    parent = torch.full((n, width, h, w), float("nan"), device="cuda").contiguous(memory_format=torch.channels_last)
-    parent[:, off:off + c] = t
-    return parent[:, off:off + c]
+dev = device_view
 
 
 def weight_shape(c):

@@ -32,15 +32,46 @@ def maxabs(a, b):
     return float(d.max()) if d.size else 0.0
 
 
+def device_view(a, layout="nhwc"):
+    """a (N, C, H, W) on the device: "nchw" / "nhwc" dense; "pad": the nets' pixel stride (Blob::compute_cstride: channels
+    rounded up to 4 below 32, else to 32); "slice": channels [5, 5 + C) of a wider channels_last parent (a zero-copy concat
+    child).  Channels outside the view hold NaN, so a stray read shows in any sum and a stray write replaces a NaN."""
+    import torch
+    t = torch.from_numpy(np.ascontiguousarray(a, np.float32)).cuda()
+    if layout == "nchw":
+        return t
+    if layout == "nhwc":
+        return t.contiguous(memory_format=torch.channels_last)
+    n, c, h, w = t.shape
+    if layout == "pad":
+        align = 4 if c < 32 else 32
+        off, width = 0, (c + align - 1) // align * align
+    else:
+        off, width = 5, c + 8
+    parent = torch.full((n, width, h, w), float("nan"), device="cuda").contiguous(memory_format=torch.channels_last)
+    parent[:, off:off + c] = t
+    return parent[:, off:off + c]
+
+
 def net_convs(text):
     """The Convolution / Deconvolution layers of a filled prototxt: (name, Ci, H, W, Co, (kh, kw), s, (ph, pw), deconv,
     trainable), from the oracle's prototxt parser and a walk over the blob shapes.  A layer with two bottoms (the deploy nets'
     conv1 on both images) is listed once; its bottoms have the same shape."""
+    return net_walk(text)[0]
+
+
+def net_losses(text):
+    """The L1Loss layers of a filled prototxt: (name, (C, H, W) of its first bottom), by the walk of net_convs."""
+    return net_walk(text)[1]
+
+
+def net_walk(text):
+    """-> (net_convs, net_losses) of a filled prototxt."""
     from flownet2_b200 import ops as _ops
     from oracle import net as onet
     get, getall = onet.get, onet.getall
     net = onet.parse_prototxt(text)
-    shp, out = {}, []
+    shp, out, losses = {}, [], []
     for t, s in zip(getall(net, "input"), getall(net, "input_shape")):            # legacy deploy inputs
         shp[t] = tuple(int(d) for d in getall(s, "dim"))[1:]
     for l in getall(net, "layer"):
@@ -92,9 +123,11 @@ def net_convs(text):
             shp[tops[0]] = (1,) + b[0][1:]
         elif ty in ("ReLU", "Eltwise", "FlowWarp"):
             shp[tops[0]] = b[0]
+        elif ty == "L1Loss":
+            losses.append((get(l, "name"), b[0]))
         else:
-            assert ty in ("L1Loss", "Silence"), ty
-    return out
+            assert ty == "Silence", ty
+    return out, losses
 
 
 def train_convs(model, width=448, height=320):
