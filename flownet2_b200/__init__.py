@@ -1,6 +1,6 @@
 """flownet2_b200 -- Hopper-native FlowNet2 forward path.
 
-Python here is only a ctypes front end over the C-ABI in include/fn2.h (libfn2.so: hand-written
+Python here is only a ctypes front end over the C-ABI in include/fn2.h and include/fn2_solver.h (libfn2.so: hand-written
 sm_90a CUDA + the Caffe-surface C++ host).  It mirrors the slice of pycaffe that the reference's
 driver uses (scripts/run-flownet.py:64-98): ``Net(prototxt, weights, phase)``, ``net.inputs``,
 ``net.forward(img0=..., img1=...)``, ``net.blobs[name].data``.
@@ -20,8 +20,12 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB = None
 TRAIN, TEST = 0, 1
 
-with open(os.path.join(os.path.dirname(_HERE), "include", "fn2.h")) as _f:
-    _STRUCTS, _PROTOTYPES = read_header(_f.read())
+_STRUCTS, _PROTOTYPES = {}, {}
+for _name in ("fn2.h", "fn2_solver.h"):
+    with open(os.path.join(os.path.dirname(_HERE), "include", _name)) as _f:
+        _s, _p = read_header(_f.read())
+    _STRUCTS.update(_s)
+    _PROTOTYPES.update(_p)
 fn2_tensor, fn2_conv_desc, fn2_l1loss_desc = (_STRUCTS[n] for n in ("fn2_tensor", "fn2_conv_desc", "fn2_l1loss_desc"))
 
 
@@ -80,6 +84,14 @@ def device_allocations():
     live = C.c_uint64()
     n = lib().fn2_device_allocations(C.byref(live))
     return int(n), int(live.value)
+
+
+def _read_text(text_or_path):
+    """A prototxt given as text or as a path -> its text."""
+    if "\n" not in text_or_path and os.path.exists(text_or_path):
+        with open(text_or_path) as f:
+            return f.read()
+    return text_or_path
 
 
 # ------------------------------------------------------------------------------------------------
@@ -169,9 +181,7 @@ class Net(object):
 
     def __init__(self, prototxt, weights=None, phase=TEST, batch=0):
         l = lib()
-        if "\n" not in prototxt and os.path.exists(prototxt):
-            with open(prototxt) as f:
-                prototxt = f.read()
+        prototxt = _read_text(prototxt)
         h = C.c_void_p()
         check(l.fn2_net_create_batch(prototxt.encode(), int(phase), int(batch), C.byref(h)))
         self._h = h
@@ -326,6 +336,205 @@ class Net(object):
     @property
     def launches_per_forward(self):
         return int(lib().fn2_net_launches_per_forward(self._h))
+
+
+# ------------------------------------------------------------------------------------------------
+# Solver (pycaffe-like: python/caffe/_caffe.cpp:338-371; the loop of src/caffe/solver.cpp:194-481)
+# ------------------------------------------------------------------------------------------------
+def solver_params(solver):
+    """Resolved parameters of a solver prototxt (text or path): {field: value}, defaults filled in, solver_type upgraded to
+    type; stepvalue is a list."""
+    out = {"stepvalue": []}
+    text = sized_output(lib().fn2_solver_params, _read_text(solver).encode())[:-1].decode()
+    for line in text.splitlines():
+        k, v = line.split(": ", 1)
+        if v.startswith('"'):
+            v = v[1:-1]
+        elif v in ("true", "false"):
+            v = v == "true"
+        else:
+            v = float(v) if any(c in v for c in ".eEna") else int(v)
+        if k == "stepvalue":
+            out[k].append(v)
+        else:
+            out[k] = v
+    return out
+
+
+def learning_rate(solver, iteration, current_step=0):
+    """SGDSolver::GetLearningRate at `iteration` -> (rate, current_step after the call); multistep advances at most one step."""
+    cs, rate = C.c_int(int(current_step)), C.c_float()
+    check(lib().fn2_solver_learning_rate(_read_text(solver).encode(), int(iteration), C.byref(cs), C.byref(rate)))
+    return rate.value, cs.value
+
+
+def get_solver(solver, net):
+    """caffe.get_solver look-alike: solver prototxt (text or path) over a TRAIN Net."""
+    return Solver(solver, net)
+
+
+class Solver(object):
+    """Caffe's SGD / Adam solver over a TRAIN Net (src/caffe/solver.cpp:194-481, solvers/sgd_solver.cpp, adam_solver.cpp).
+
+    ``step(n, feed)`` runs n iterations: ClearParamDiffs, the on_start callbacks, iter_size x (feed, forward, backward), the
+    on_gradients_ready callbacks, the update on the device, iter += 1, and a snapshot when one is due.  ``feed()`` returns
+    {input name: ndarray or CUDA tensor} and is called before every forward.  Within an iteration the only host
+    synchronisation is the read of the loss outputs, after the update has been enqueued.  Data-parallel training all-reduces
+    the gradients in ``on_gradients_ready`` (parallel.allreduce_gradients(parallel.grad_arena_tensor(net,
+    trainable_only=True))); every rank then applies the same update.
+    """
+
+    def __init__(self, solver, net):
+        self._text = _read_text(solver)
+        self.net = net
+        self.param = solver_params(self._text)
+        h = C.c_void_p()
+        check(lib().fn2_solver_create(self._text.encode(), net._h, C.byref(h)))
+        self._h = h
+        self._callbacks = []
+        w = (C.c_float * len(net.outputs))()
+        check(lib().fn2_solver_output_loss_weights(h, w, len(net.outputs)))
+        self._loss_outputs = [(o, float(x)) for o, x in zip(net.outputs, w) if x != 0]
+        for o, _ in self._loss_outputs:
+            if int(np.prod(net.blobs[o].shape)) != 1:
+                raise Fn2Error("loss output %s is not a scalar: %s" % (o, net.blobs[o].shape))
+        self._loss_buf = None
+        self._losses = []
+        self.smoothed_loss = 0.0
+
+    def __del__(self):
+        try:
+            if getattr(self, "_h", None):
+                lib().fn2_solver_destroy(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+    def _status(self):
+        it, cs = C.c_int(), C.c_int()
+        check(lib().fn2_solver_iter(self._h, C.byref(it), C.byref(cs)))
+        return it.value, cs.value
+
+    @property
+    def iter(self):
+        return self._status()[0]
+
+    @property
+    def lr(self):
+        """The learning rate the next update uses."""
+        it, cs = self._status()
+        return learning_rate(self._text, it, cs)[0]
+
+    def add_callback(self, on_start, on_gradients_ready):
+        self._callbacks.append((on_start, on_gradients_ready))
+
+    def _feed(self, inputs):
+        import torch
+        for name, value in inputs.items():
+            if isinstance(value, torch.Tensor):
+                t = value.detach().to(torch.float32).contiguous()
+                if tuple(t.shape) != self.net.blobs[name].shape or not t.is_cuda:
+                    raise Fn2Error("input %s: a CUDA tensor of shape %s is expected" % (name, self.net.blobs[name].shape))
+                ready = torch.cuda.Event()
+                ready.record()
+                torch.cuda.ExternalStream(self.net.stream).wait_event(ready)       # the net reads it after torch wrote it
+                self._keep.append(t)
+                self.net.set_input_device(name, t.data_ptr())
+            else:
+                self.net.set_input(name, value)
+
+    def step(self, iters, feed=None):
+        import torch
+        it0 = self.iter
+        iter_size = int(self.param["iter_size"])
+        self._losses, self.smoothed_loss = [], 0.0
+        if self._loss_outputs and (self._loss_buf is None or self._loss_buf.shape[0] != iter_size):
+            self._loss_buf = torch.empty((iter_size, len(self._loss_outputs)), dtype=torch.float32, device="cuda")
+        weights = [wt for _, wt in self._loss_outputs]
+        net_stream = torch.cuda.ExternalStream(self.net.stream)
+        for _ in range(int(iters)):
+            self._keep = []
+            self.net.clear_param_diffs()
+            for on_start, _ in self._callbacks:
+                on_start()
+            for i in range(iter_size):
+                if feed is not None:
+                    self._feed(feed())
+                self.net.forward_async()
+                self.net.backward_async()
+                for j, (name, _) in enumerate(self._loss_outputs):
+                    self.net.get_blob_device(name, self._loss_buf[i, j].data_ptr())
+            if self._callbacks:
+                # the callbacks' work (an all-reduce of the gradient arena) runs on torch's current stream after the backward,
+                # and the update on the net's stream after the callbacks' work: ordered on the device, no host wait
+                done = torch.cuda.Event()
+                done.record(net_stream)
+                torch.cuda.current_stream().wait_event(done)
+                for _, on_gradients_ready in self._callbacks:
+                    on_gradients_ready()
+                reduced = torch.cuda.Event()
+                reduced.record()
+                net_stream.wait_event(reduced)
+            check(lib().fn2_solver_apply_update(self._h))
+            self.net.sync()
+            if self._loss_outputs:
+                per_pass = self._loss_buf.cpu().numpy().astype(np.float64) @ np.asarray(weights, np.float64)
+                self._update_smoothed_loss(float(per_pass.sum()) / iter_size, it0)
+            it = self.iter
+            if self.param["snapshot"] and it % self.param["snapshot"] == 0:
+                self.snapshot()
+        self._keep = []
+
+    def _update_smoothed_loss(self, loss, start_iter):
+        """Solver::UpdateSmoothedLoss (solver.cpp:484-495)."""
+        average = int(self.param["average_loss"])
+        if len(self._losses) < average:
+            self._losses.append(loss)
+            self.smoothed_loss = (self.smoothed_loss * (len(self._losses) - 1) + loss) / len(self._losses)
+        else:
+            idx = (self.iter - 1 - start_iter) % average
+            self.smoothed_loss += (loss - self._losses[idx]) / average
+            self._losses[idx] = loss
+
+    def solve(self, feed=None, resume=None):
+        """Solver::Solve (solver.cpp:277-330): optionally restore, step to max_iter, and snapshot at the end unless that
+        iteration was just snapshotted or snapshot_after_train is false."""
+        if resume is not None:
+            self.restore(resume)
+        self.step(int(self.param["max_iter"]) - self.iter, feed)
+        snap = self.param["snapshot"]
+        if self.param["snapshot_after_train"] and (not snap or self.iter % snap != 0):
+            self.snapshot()
+
+    def state(self, learned_net=""):
+        """The SolverState message as bytes (history in Net::learnable_params order; Adam: every m, then every v)."""
+        return sized_output(lib().fn2_solver_state, self._h, learned_net.encode())
+
+    def snapshot(self):
+        """Solver::Snapshot (solver.cpp:447-469): <prefix>_iter_<N>.caffemodel and <prefix>_iter_<N>.solverstate.
+        Returns (caffemodel path, solverstate path)."""
+        prefix = self.param["snapshot_prefix"]
+        if not prefix:
+            raise Fn2Error("snapshot: snapshot_prefix is not set")
+        base = "%s_iter_%d" % (prefix, self.iter)
+        model, state = base + ".caffemodel", base + ".solverstate"
+        with open(model, "wb") as f:
+            f.write(self.net.to_caffemodel())
+        with open(state, "wb") as f:
+            f.write(self.state(model))
+        return model, state
+
+    def restore(self, state):
+        """Solver::Restore (sgd_solver.cpp:305-322): a .solverstate path or its bytes.  Restores iter, current_step and the
+        history, and loads the weights of learned_net through Net.copy_from when the state names one."""
+        if isinstance(state, str):
+            with open(state, "rb") as f:
+                state = f.read()
+        buf = (C.c_char * len(state)).from_buffer_copy(state)
+        learned = sized_output(lib().fn2_solverstate_learned_net, buf, len(state))[:-1].decode()
+        check(lib().fn2_solver_restore(self._h, buf, len(state)))
+        if learned:
+            self.net.copy_from(learned)
 
 
 # ------------------------------------------------------------------------------------------------

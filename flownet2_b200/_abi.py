@@ -1,4 +1,5 @@
-"""ctypes structs and prototypes of libfn2.so, read from include/fn2.h: the header is the only statement of the ABI.
+"""ctypes structs and prototypes of libfn2.so, read from include/fn2.h and include/fn2_solver.h: the headers are the only
+statement of the ABI.
 
 Types map through one table; a type it does not know raises, so a new header entry cannot go undeclared."""
 import ctypes as C
@@ -6,8 +7,8 @@ import re
 
 SCALARS = {"int": C.c_int, "unsigned int": C.c_uint, "int32_t": C.c_int32, "int64_t": C.c_int64, "uint64_t": C.c_uint64,
            "unsigned long long": C.c_ulonglong, "size_t": C.c_size_t, "float": C.c_float, "double": C.c_double}
-# data pointers and the opaque net handle: c_void_p takes ints from data_ptr(), numpy / ctypes pointers, arrays and None
-OPAQUE = ("void", "float", "fn2_net")
+# data pointers and the opaque net and solver handles: c_void_p takes ints from data_ptr(), numpy / ctypes pointers, arrays and None
+OPAQUE = ("void", "float", "fn2_net", "fn2_solver")
 
 
 def ctype(t, known):

@@ -35,11 +35,13 @@ SOURCES = [
     ("fn2_conv_tn.cu", []),
     ("fn2_train.cu", []),
     ("fn2_loss.cu", []),
+    ("fn2_solver.cu", ["-fmad=false"]),     # bit-exact update, see file header
     ("caffe/proto.cpp", []),
     ("caffe/blob.cpp", []),
     ("caffe/layers.cpp", []),
     ("caffe/net.cpp", []),
     ("caffe/hdf5_min.cpp", []),
+    ("caffe/solver.cpp", []),
     ("caffe/capi.cpp", []),
 ]
 

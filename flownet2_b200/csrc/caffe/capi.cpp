@@ -1,9 +1,12 @@
-// extern "C" net-level entry points of include/fn2.h over caffe::Net<float>.
+// extern "C" net-level entry points of include/fn2.h over caffe::Net<float>, and the solver's of include/fn2_solver.h over
+// caffe::Solver.
 #include <cstring>
 #include <type_traits>
 
+#include "../../../include/fn2_solver.h"
 #include "net.hpp"
 #include "hdf5_min.hpp"
+#include "solver.hpp"
 
 namespace fn2 { void set_error(const char* fmt, ...); }
 
@@ -314,6 +317,76 @@ int fn2_caffemodel_summary(const void* caffemodel, size_t n, char* out, size_t* 
             s += "\n";
         }
         return emit("caffemodel_summary", s, true, out, bytes);
+    FN2_CATCH
+}
+
+// ---- solver (include/fn2_solver.h) ----
+struct fn2_solver {
+    fn2_net* net;
+    std::unique_ptr<caffe::Solver> solver;
+};
+
+int fn2_solver_create(const char* solver_text, fn2_net* net, fn2_solver** out) {
+    return net_call("solver_create", solver_text && net && out, [&] {
+        *out = nullptr;
+        std::unique_ptr<fn2_solver> h(new fn2_solver());
+        h->net = net;
+        h->solver.reset(new caffe::Solver(caffe::SolverParameter::FromText(solver_text), net->net.get()));
+        *out = h.release();
+    });
+}
+
+void fn2_solver_destroy(fn2_solver* solver) { delete solver; }
+
+int fn2_solver_apply_update(fn2_solver* solver) {
+    return net_call("solver_apply_update", solver, [&] { solver->solver->ApplyUpdate(); });
+}
+
+int fn2_solver_iter(fn2_solver* solver, int* iter, int* current_step) {
+    return net_call("solver_iter", solver && iter && current_step, [&] {
+        *iter = solver->solver->iter();
+        *current_step = solver->solver->current_step();
+    });
+}
+
+int fn2_solver_output_loss_weights(fn2_solver* solver, float* weights, int n) {
+    return net_call("solver_output_loss_weights", solver && weights, [&] {
+        const auto& outs = solver->net->net->output_blob_indices();
+        if (n != (int)outs.size()) { fn2::set_error("solver_output_loss_weights: the net has %d outputs", (int)outs.size()); return FN2_ERR_INVALID; }
+        for (int i = 0; i < n; i++) weights[i] = solver->net->net->blob_loss_weight(outs[i]);
+        return FN2_OK;
+    });
+}
+
+int fn2_solver_state(fn2_solver* solver, const char* learned_net, void* out, size_t* bytes) {
+    return net_call("solver_state", solver && learned_net && bytes, [&] {
+        return emit("solver_state", solver->solver->State(learned_net), false, out, bytes);
+    });
+}
+
+int fn2_solver_restore(fn2_solver* solver, const void* state, size_t bytes) {
+    return net_call("solver_restore", solver && state, [&] { solver->solver->Restore(state, bytes); });
+}
+
+int fn2_solverstate_learned_net(const void* state, size_t n, char* out, size_t* bytes) {
+    if (!state) { fn2::set_error("solverstate_learned_net: null state"); return FN2_ERR_INVALID; }
+    FN2_TRY
+        return emit("solverstate_learned_net", caffe::ParseSolverState(state, n).learned_net, true, out, bytes);
+    FN2_CATCH
+}
+
+int fn2_solver_learning_rate(const char* solver_text, int iter, int* current_step, float* rate) {
+    return net_call("solver_learning_rate", solver_text && current_step && rate, [&] {
+        const caffe::SolverParameter p = caffe::SolverParameter::FromText(solver_text);
+        caffe::Solver::Validate(p);
+        *rate = caffe::Solver::LearningRate(p, iter, current_step);
+    });
+}
+
+int fn2_solver_params(const char* solver_text, char* out, size_t* bytes) {
+    if (!solver_text) { fn2::set_error("solver_params: null text"); return FN2_ERR_INVALID; }
+    FN2_TRY
+        return emit("solver_params", caffe::SolverParameter::FromText(solver_text).Resolved(), true, out, bytes);
     FN2_CATCH
 }
 

@@ -1033,7 +1033,16 @@ class DataAugmentationLayer : public Layer<Dtype> {
         this->layer_param_.m->set("reshape_every_iter", "false");      // data_augmentation_layer.cpp:39
         if (this->blobs_.size() == 0) {
             this->blobs_.resize(aug.recompute_mean() ? 3 : 1);
-            for (auto& b : this->blobs_) b.reset(new Blob<Dtype>());
+            for (auto& b : this->blobs_) {
+                b.reset(new Blob<Dtype>());
+                // the iteration counter and the running means are state, not weights: one ParamSpec {lr_mult: 0 decay_mult: 0}
+                // per blob keeps a solver off them (data_augmentation_layer.cpp:48-65)
+                Field f;
+                f.name = "param"; f.is_msg = true; f.msg = std::make_shared<Message>();
+                f.msg->add("lr_mult", "0");
+                f.msg->add("decay_mult", "0");
+                this->layer_param_.m->fields.push_back(f);
+            }
             this->blobs_[0]->Reshape(1, 1, 1, 1);
         }
     }

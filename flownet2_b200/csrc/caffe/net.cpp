@@ -556,6 +556,45 @@ float Net<Dtype>::lr_mult(int layer, int param) const {
     return param < lp.m->count("param") ? lp.m->msg("param", param).f("lr_mult", 1.f) : 1.f;      // ParamSpec default 1
 }
 
+template <typename Dtype>
+float Net<Dtype>::decay_mult(int layer, int param) const {
+    const LayerParameter& lp = layers_[layer]->layer_param();
+    return param < lp.m->count("param") ? lp.m->msg("param", param).f("decay_mult", 1.f) : 1.f;   // ParamSpec default 1
+}
+
+template <typename Dtype>
+vector<typename Net<Dtype>::LearnableParam> Net<Dtype>::LearnableParams() {
+    vector<LearnableParam> out;
+    size_t off = 0;
+    for (size_t i = 0; i < layers_.size(); i++)
+        for (size_t pi = 0; pi < layers_[i]->blobs().size(); pi++) {
+            const Blob<Dtype>& b = *layers_[i]->blobs()[pi];
+            out.push_back({(int)i, (int)pi, off, b.count(), b.shape(), lr_mult((int)i, (int)pi), decay_mult((int)i, (int)pi)});
+            off += arena_slot(b);
+        }
+    return out;
+}
+
+template <typename Dtype>
+void Net<Dtype>::ParamsUpdated(const vector<int>& learnable_ids) {
+    vector<Blob<Dtype>*> all;
+    vector<int> layer_of;
+    for (size_t i = 0; i < layers_.size(); i++)
+        for (auto& b : layers_[i]->blobs()) { all.push_back(b.get()); layer_of.push_back((int)i); }
+    std::set<int> touched;
+    for (int id : learnable_ids) { all[id]->MarkDeviceNewer(); touched.insert(layer_of[id]); }
+    Caffe::stream() = stream_;
+    for (int i : touched) layers_[i]->ParamsChanged();
+}
+
+template <typename Dtype>
+Dtype Net<Dtype>::blob_loss_weight(int b) const {
+    for (size_t i = 0; i < layers_.size(); i++)
+        for (size_t t = 0; t < top_id_vecs_[i].size(); t++)
+            if (top_id_vecs_[i][t] == b && layers_[i]->loss_weight((int)t) != 0) return layers_[i]->loss_weight((int)t);
+    return 0;
+}
+
 // Which layers need backward and which blobs carry a gradient, from the graph alone (net.cpp:120-170, :223-262): a layer needs
 // backward if it has a parameter with lr_mult != 0 or a bottom that needs it (every input blob with force_backward), and it
 // allows backward.  propagate_down: false then cuts single bottoms in PlanBackward.  The warp-block fusion and the trainable

@@ -41,6 +41,18 @@ class Net {
     void ArenaWritten();                               // device arena overwritten externally (broadcast)
     void ParamArena(void** dev, size_t* bytes) { *dev = arena_.get(); *bytes = arena_floats_ * sizeof(Dtype); }
 
+    // Net::learnable_params (net.cpp:440-490): every layer's parameter blobs in layer order x parameter index, where each one
+    // lies in the parameter and gradient arenas, and its ParamSpec multipliers (lr_mult, decay_mult; default 1).
+    struct LearnableParam { int layer, index; size_t offset; int count; vector<int> shape; float lr_mult, decay_mult; };
+    vector<LearnableParam> LearnableParams();
+    float lr_mult(int layer, int param) const;
+    float decay_mult(int layer, int param) const;
+    // Net::Update (net.cpp:957-964) ran on the device for the given learnable parameters: their device copies are newer, and
+    // their layers re-derive what they keep from them (packed convolution weights) on the net's stream.  No host sync.
+    void ParamsUpdated(const vector<int>& learnable_ids);
+    // loss weight of blob b as a loss layer top (Net::blob_loss_weights, net.cpp:189-196), 0 for other blobs
+    Dtype blob_loss_weight(int b) const;
+
     const vector<string>& layer_names() const { return layer_names_; }
     const vector<shared_ptr<Layer<Dtype> > >& layers() const { return layers_; }
     const vector<string>& blob_names() const { return blob_names_; }
@@ -77,7 +89,6 @@ class Net {
     struct WarpBlock { int resample, warp, sub, norm, scale; float coeff; int fill_nan; };
     std::map<int, WarpBlock> warp_head_;        // by the Resample layer's index
     vector<char> absorbed_;
-    float lr_mult(int layer, int param) const;
     void NeedBackward(vector<char>* layer_need, vector<char>* blob_need) const;
     void PlanBackward();
     void BuildDiffArena();

@@ -539,6 +539,15 @@ void put_bytes(std::string& o, int fn, const std::string& s) {
     put_varint(o, s.size());
     o += s;
 }
+// BlobProto {data = 5 (packed), shape = 7 {dim = 1 (packed)}} as field fn of the enclosing message
+void put_blob(std::string& o, int fn, const BlobProtoData& b) {
+    std::string bb, dims, shape;
+    for (int d : b.shape) put_varint(dims, (uint64_t)d);
+    put_bytes(shape, 1, dims);
+    put_bytes(bb, 5, std::string((const char*)b.data.data(), b.data.size() * 4));
+    put_bytes(bb, 7, shape);
+    put_bytes(o, fn, bb);
+}
 }  // namespace
 
 std::vector<LayerBlobs> ParseCaffemodel(const void* bytes, size_t n) {
@@ -561,20 +570,85 @@ std::string SerializeCaffemodel(const std::string& net_name, const std::vector<L
         std::string lb;
         put_bytes(lb, 1, l.name);
         put_bytes(lb, 2, l.type);
-        for (const auto& b : l.blobs) {
-            std::string bb;
-            std::string dims;
-            for (int d : b.shape) put_varint(dims, (uint64_t)d);
-            std::string shape;
-            put_bytes(shape, 1, dims);
-            std::string data((const char*)b.data.data(), b.data.size() * 4);
-            put_bytes(bb, 5, data);
-            put_bytes(bb, 7, shape);
-            put_bytes(lb, 7, bb);
-        }
+        for (const auto& b : l.blobs) put_blob(lb, 7, b);
         put_bytes(o, 100, lb);
     }
     return o;
+}
+
+SolverStateData ParseSolverState(const void* bytes, size_t n) {
+    Reader r{(const uint8_t*)bytes, (const uint8_t*)bytes + n};
+    SolverStateData s;
+    while (r.ok()) {
+        uint64_t key = r.varint();
+        int fn = (int)(key >> 3), wt = (int)(key & 7);
+        if (fn == 1 && wt == 0) s.iter = (int)r.varint();
+        else if (fn == 2 && wt == 2) { Reader t = r.sub(); s.learned_net.assign((const char*)t.p, t.end - t.p); }
+        else if (fn == 3 && wt == 2) s.history.push_back(parse_blob(r.sub()));
+        else if (fn == 4 && wt == 0) s.current_step = (int)r.varint();
+        else r.skip(wt);
+    }
+    return s;
+}
+
+std::string SerializeSolverState(const SolverStateData& s) {
+    std::string o;
+    put_key(o, 1, 0); put_varint(o, (uint64_t)(int64_t)s.iter);
+    put_bytes(o, 2, s.learned_net);
+    for (const auto& b : s.history) put_blob(o, 3, b);
+    put_key(o, 4, 0); put_varint(o, (uint64_t)(int64_t)s.current_step);
+    return o;
+}
+
+// ------------------------------------------------------------------------------------------
+// SolverParameter
+// ------------------------------------------------------------------------------------------
+SolverParameter SolverParameter::FromText(const std::string& text) {
+    SolverParameter p;
+    p.m = std::make_shared<Message>(ParseTextFormat(text));
+    Message& m = *p.m;
+    if (!m.has("solver_type")) return p;
+    if (m.has("type"))
+        throw ParseError("Failed to upgrade solver: old solver_type field (enum) and new type field (string) cannot be both "
+                         "specified in solver proto text.");
+    static const char* const kEnum[][3] = {{"SGD", "0", "SGD"}, {"NESTEROV", "1", "Nesterov"}, {"ADAGRAD", "2", "AdaGrad"},
+                                           {"RMSPROP", "3", "RMSProp"}, {"ADADELTA", "4", "AdaDelta"}, {"ADAM", "5", "Adam"}};
+    const std::string old = m.str("solver_type");
+    std::string type;
+    for (const auto& e : kEnum) if (old == e[0] || old == e[1]) type = e[2];
+    if (type.empty()) throw ParseError("Unknown SolverParameter solver_type: " + old);
+    std::vector<Field> kept;
+    for (auto& f : m.fields) if (f.name != "solver_type") kept.push_back(f);
+    m.fields = kept;
+    m.set("type", type);
+    return p;
+}
+
+std::string SolverParameter::Resolved() const {
+    std::string s;
+    char buf[64];
+    auto num = [&](const char* name, double v, const char* fmt) { snprintf(buf, sizeof(buf), fmt, v); s += std::string(name) + ": " + buf + "\n"; };
+    auto str = [&](const char* name, const std::string& v) { s += std::string(name) + ": \"" + v + "\"\n"; };
+    str("type", type());
+    num("base_lr", base_lr(), "%.9g");
+    str("lr_policy", lr_policy());
+    num("gamma", gamma(), "%.9g");
+    num("power", power(), "%.9g");
+    num("stepsize", stepsize(), "%.0f");
+    for (int i = 0; i < stepvalue_size(); i++) num("stepvalue", stepvalue(i), "%.0f");
+    num("max_iter", max_iter(), "%.0f");
+    num("momentum", momentum(), "%.9g");
+    num("momentum2", momentum2(), "%.9g");
+    num("delta", delta(), "%.9g");
+    num("weight_decay", weight_decay(), "%.9g");
+    str("regularization_type", regularization_type());
+    num("clip_gradients", clip_gradients(), "%.9g");
+    num("iter_size", iter_size(), "%.0f");
+    num("average_loss", average_loss(), "%.0f");
+    num("snapshot", snapshot(), "%.0f");
+    str("snapshot_prefix", snapshot_prefix());
+    s += std::string("snapshot_after_train: ") + (snapshot_after_train() ? "true" : "false") + "\n";
+    return s;
 }
 
 }  // namespace caffe

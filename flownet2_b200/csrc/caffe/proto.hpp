@@ -184,6 +184,36 @@ struct NetParameter {
     static NetParameter FromText(const std::string& prototxt);
 };
 
+// SolverParameter, caffe.proto:104-244, read from a solver prototxt.  FromText applies UpgradeSolverType
+// (upgrade_proto.cpp:1002-1037: the deprecated solver_type enum becomes the type string) and nothing else; which values the
+// engine's solver accepts is Solver's business (solver.cpp Validate).
+struct SolverParameter {
+    std::shared_ptr<Message> m;
+    static SolverParameter FromText(const std::string& text);
+    std::string type() const { return m->str_or("type", "SGD"); }
+    float base_lr() const { return m->f("base_lr", 0); }
+    std::string lr_policy() const { return m->str_or("lr_policy", ""); }
+    float gamma() const { return m->f("gamma", 0); }
+    float power() const { return m->f("power", 0); }
+    int stepsize() const { return m->i("stepsize", 0); }
+    int stepvalue_size() const { return m->count("stepvalue"); }
+    int stepvalue(int i) const { return m->i("stepvalue", 0, i); }
+    int max_iter() const { return m->i("max_iter", 0); }
+    float momentum() const { return m->f("momentum", 0); }
+    float momentum2() const { return m->f("momentum2", 0.999f); }
+    float delta() const { return m->f("delta", 1e-8f); }
+    float weight_decay() const { return m->f("weight_decay", 0); }
+    std::string regularization_type() const { return m->str_or("regularization_type", "L2"); }
+    float clip_gradients() const { return m->f("clip_gradients", -1); }
+    int iter_size() const { return m->i("iter_size", 1); }
+    int average_loss() const { return m->i("average_loss", 1); }
+    int snapshot() const { return m->i("snapshot", 0); }
+    std::string snapshot_prefix() const { return m->str_or("snapshot_prefix", ""); }
+    bool snapshot_after_train() const { return m->b("snapshot_after_train", true); }
+    // every field above as `name: value` lines in this order (the resolved view tests compare with caffe_pb2)
+    std::string Resolved() const;
+};
+
 // ---- binary .caffemodel subset ------------------------------------------------------------
 struct BlobProtoData {
     std::vector<int> shape;                    // from shape{dim} or legacy num/channels/height/width
@@ -197,5 +227,15 @@ struct LayerBlobs {
 // BlobProto.{shape=7{dim=1}, data=5, double_data=8, num..width=1..4}   caffe.proto:10-22,94,313-331
 std::vector<LayerBlobs> ParseCaffemodel(const void* bytes, size_t n);
 std::string SerializeCaffemodel(const std::string& net_name, const std::vector<LayerBlobs>& layers);
+// SolverState, caffe.proto:247-252: iter = 1, learned_net = 2, history = 3 (BlobProto), current_step = 4.  To and from bytes
+// with the .caffemodel's BlobProto encoding (sgd_solver.cpp:260-322).
+struct SolverStateData {
+    int iter = 0;
+    int current_step = 0;
+    std::string learned_net;
+    std::vector<BlobProtoData> history;
+};
+SolverStateData ParseSolverState(const void* bytes, size_t n);
+std::string SerializeSolverState(const SolverStateData& s);
 
 }  // namespace caffe
