@@ -1,6 +1,6 @@
 """flownet2_b200 -- Hopper-native FlowNet2 forward path.
 
-Python here is only a ctypes front end over the C-ABI in include/fn2.h and include/fn2_solver.h (libfn2.so: hand-written
+Python here is only a ctypes front end over the C-ABI in include/fn2.h, fn2_solver.h and fn2_frames.h (libfn2.so: hand-written
 sm_90a CUDA + the Caffe-surface C++ host).  It mirrors the slice of pycaffe that the reference's
 driver uses (scripts/run-flownet.py:64-98): ``Net(prototxt, weights, phase)``, ``net.inputs``,
 ``net.forward(img0=..., img1=...)``, ``net.blobs[name].data``.
@@ -21,9 +21,9 @@ _LIB = None
 TRAIN, TEST = 0, 1
 
 _STRUCTS, _PROTOTYPES = {}, {}
-for _name in ("fn2.h", "fn2_solver.h"):
+for _name in ("fn2.h", "fn2_solver.h", "fn2_frames.h"):
     with open(os.path.join(os.path.dirname(_HERE), "include", _name)) as _f:
-        _s, _p = read_header(_f.read())
+        _s, _p = read_header(_f.read(), _STRUCTS)
     _STRUCTS.update(_s)
     _PROTOTYPES.update(_p)
 fn2_tensor, fn2_conv_desc, fn2_l1loss_desc = (_STRUCTS[n] for n in ("fn2_tensor", "fn2_conv_desc", "fn2_l1loss_desc"))
@@ -247,6 +247,36 @@ class Net(object):
 
     def get_blob_device(self, name, dev_ptr):
         check(lib().fn2_net_get_blob_device(self._h, name.encode(), C.c_void_p(dev_ptr)))
+
+    def set_input_image(self, name, frames):
+        """8-bit frames -> input blob (N, 3, H, W) as BGR floats, converted on the device (include/fn2_frames.h).  frames: uint8
+        (N, H, W, K) with K = 1 (gray), 3 (RGB) or 4 (RGBA, alpha ignored), or (H, W, K) / (H, W) for N = 1.  The blob equals
+        set_input of image_to_blob(frame) (a gray frame broadcast to the three channels)."""
+        a = np.asarray(frames)
+        if a.dtype != np.uint8:
+            raise Fn2Error("input %s: frames must be uint8, got %s" % (name, a.dtype))
+        a = a[np.newaxis, :, :, np.newaxis] if a.ndim == 2 else a[np.newaxis] if a.ndim == 3 else a
+        n, c, h, w = self.blobs[name].shape
+        if a.ndim != 4 or a.shape[:3] != (n, h, w):
+            raise Fn2Error("input %s: frames of shape %s, net expects (%d, %d, %d, K)" % (name, np.shape(frames), n, h, w))
+        a = np.ascontiguousarray(a)
+        self._keep = getattr(self, "_keep", {})
+        self._keep[name] = a       # must outlive the async H2D copy
+        check(lib().fn2_net_set_input_frames(self._h, name.encode(), a.ctypes.data_as(C.c_void_p), a.shape[3]))
+
+    def set_input_image_device(self, name, dev_ptr, channels):
+        """dev_ptr: device address of dense uint8 frames (N, H, W, channels) for the (N, 3, H, W) input blob `name`."""
+        check(lib().fn2_net_set_input_frames_device(self._h, name.encode(), C.c_void_p(dev_ptr), int(channels)))
+
+    def get_blob_nhwc(self, name):
+        """The blob as an (N, H, W, C) array; for the flow, (N, H, W, 2) is the payload of a .flo file per pair."""
+        n, c, h, w = self.blobs[name].shape
+        out = np.empty((n, h, w, c), np.float32)
+        check(lib().fn2_net_get_blob_nhwc(self._h, name.encode(), out.ctypes.data_as(C.c_void_p)))
+        return out
+
+    def get_blob_nhwc_device(self, name, dev_ptr):
+        check(lib().fn2_net_get_blob_nhwc_device(self._h, name.encode(), C.c_void_p(dev_ptr)))
 
     def forward_async(self):
         check(lib().fn2_net_forward(self._h))

@@ -1,4 +1,4 @@
-"""ctypes structs and prototypes of libfn2.so, read from include/fn2.h and include/fn2_solver.h: the headers are the only
+"""ctypes structs and prototypes of libfn2.so, read from include/fn2.h, fn2_solver.h and fn2_frames.h: the headers are the only
 statement of the ABI.
 
 Types map through one table; a type it does not know raises, so a new header entry cannot go undeclared."""
@@ -33,11 +33,12 @@ def _split(decl):
     return m.group(1) + (m.group(2) or "")
 
 
-def read_header(text):
-    """-> ({struct name: ctypes.Structure}, {function: (restype, argtypes)}) of every typedef'd struct and FN2_API declaration."""
+def read_header(text, included=None):
+    """-> ({struct name: ctypes.Structure}, {function: (restype, argtypes)}) of every typedef'd struct and FN2_API declaration.
+    included: the structs of headers this one includes (fn2.h's fn2_tensor for fn2_frames.h)."""
     text = re.sub(r"/\*.*?\*/", " ", text, flags=re.S)
     text = re.sub(r"^\s*#.*$", "", text, flags=re.M)
-    known, structs = dict(SCALARS), {}
+    known, structs = dict(SCALARS, **(included or {})), {}
     for name, body in re.findall(r"typedef struct (\w+) \{(.*?)\} \1;", text, re.S):
         fields = []
         for member in filter(None, (m.strip() for m in body.split(";"))):

@@ -1,8 +1,9 @@
-// extern "C" net-level entry points of include/fn2.h over caffe::Net<float>, and the solver's of include/fn2_solver.h over
-// caffe::Solver.
+// extern "C" net-level entry points of include/fn2.h and include/fn2_frames.h over caffe::Net<float>, and the solver's of
+// include/fn2_solver.h over caffe::Solver.
 #include <cstring>
 #include <type_traits>
 
+#include "../../../include/fn2_frames.h"
 #include "../../../include/fn2_solver.h"
 #include "net.hpp"
 #include "hdf5_min.hpp"
@@ -151,6 +152,21 @@ int fn2_net_get_blob(fn2_net* net, const char* blob, float* host_nchw) {
 }
 int fn2_net_get_blob_device(fn2_net* net, const char* blob, float* dev_nchw) {
     return net_call("get_blob_device", net && blob && dev_nchw, [&] { net->net->GetBlobDevice(blob, dev_nchw); });
+}
+
+// ---- 8-bit frames in, NHWC out (include/fn2_frames.h) ----
+int fn2_net_set_input_frames(fn2_net* net, const char* blob, const void* host_frames, int channels) {
+    return net_call("set_input_frames", net && blob && host_frames, [&] { net->net->SetInputFrames(blob, host_frames, channels); });
+}
+int fn2_net_set_input_frames_device(fn2_net* net, const char* blob, const void* dev_frames, int channels) {
+    return net_call("set_input_frames_device", net && blob && dev_frames,
+                    [&] { net->net->SetInputFramesDevice(blob, dev_frames, channels); });
+}
+int fn2_net_get_blob_nhwc(fn2_net* net, const char* blob, float* host) {
+    return net_call("get_blob_nhwc", net && blob && host, [&] { net->net->GetBlobNHWC(blob, host); });
+}
+int fn2_net_get_blob_nhwc_device(fn2_net* net, const char* blob, float* dev) {
+    return net_call("get_blob_nhwc_device", net && blob && dev, [&] { net->net->GetBlobNHWCDevice(blob, dev); });
 }
 
 int fn2_net_forward(fn2_net* net) { return net_call("forward", net, [&] { net->net->Forward(); }); }

@@ -93,4 +93,12 @@ inline fn2_tensor nchw_view(float* p, int n, int c, int h, int w) {
     return t;
 }
 
+// Dense NHWC view of n x c x h x w floats at p (channels fastest)
+inline fn2_tensor nhwc_view(float* p, int n, int c, int h, int w) {
+    fn2_tensor t;
+    t.data = p; t.n = n; t.c = c; t.h = h; t.w = w;
+    t.sc = 1; t.sw = c; t.sh = (int64_t)w * c; t.sn = (int64_t)h * w * c;
+    return t;
+}
+
 }  // namespace caffe

@@ -1,5 +1,6 @@
 #include "net.hpp"
 #include "hdf5_min.hpp"
+#include "../../../include/fn2_frames.h"
 
 #include <cstdlib>
 #include <cstring>
@@ -832,6 +833,53 @@ void Net<Dtype>::GetBlob(const string& blob, Dtype* host_nchw) {
     Dtype* st = staging(blob + "#out", (size_t)b->count());
     GetBlobDevice(blob, st);
     CUDA_CHECK(cudaMemcpyAsync(host_nchw, st, (size_t)b->count() * sizeof(Dtype), cudaMemcpyDeviceToHost, stream_));
+    CUDA_CHECK(cudaStreamSynchronize(stream_));
+}
+
+// The input blob frames go to: refuses a channel count other than 1, 3, 4 and a blob that is not (N, 3, H, W).
+template <typename Dtype>
+static shared_ptr<Blob<Dtype> > frames_blob(const Net<Dtype>& net, const string& blob, int channels) {
+    CHECK(channels == 1 || channels == 3 || channels == 4) << "set_input_frames: channels must be 1, 3 or 4 (gray, RGB, RGBA), got "
+                                                           << channels;
+    shared_ptr<Blob<Dtype> > b = net.blob_by_name(blob);
+    CHECK(b->num_axes() == 4 && b->channels() == 3) << "set_input_frames: blob " << blob << " must have shape (N, 3, H, W), has "
+                                                    << b->num_axes() << " axes and " << b->channels() << " channels";
+    return b;
+}
+
+template <typename Dtype>
+void Net<Dtype>::SetInputFramesDevice(const string& blob, const void* dev_frames, int channels) {
+    Caffe::stream() = stream_;
+    shared_ptr<Blob<Dtype> > b = frames_blob(*this, blob, channels);
+    fn2_tensor dst = b->mutable_tensor();
+    FN2_CALL(fn2_frames_to_tensor(dev_frames, channels, &dst, stream_));
+}
+
+template <typename Dtype>
+void Net<Dtype>::SetInputFrames(const string& blob, const void* host_frames, int channels) {
+    Caffe::stream() = stream_;
+    shared_ptr<Blob<Dtype> > b = frames_blob(*this, blob, channels);
+    const size_t bytes = (size_t)b->num() * b->height() * b->width() * channels;
+    Dtype* st = staging(blob, (bytes + sizeof(Dtype) - 1) / sizeof(Dtype));        // the buffer SetInput stages the blob in
+    CUDA_CHECK(cudaMemcpyAsync(st, host_frames, bytes, cudaMemcpyHostToDevice, stream_));
+    SetInputFramesDevice(blob, st, channels);
+}
+
+template <typename Dtype>
+void Net<Dtype>::GetBlobNHWCDevice(const string& blob, Dtype* dev_nhwc) {
+    Caffe::stream() = stream_;
+    shared_ptr<Blob<Dtype> > b = blob_by_name(blob);
+    fn2_tensor src = b->tensor();
+    fn2_tensor dst = nhwc_view(dev_nhwc, b->num(), b->channels(), b->height(), b->width());
+    FN2_CALL(fn2_copy(&src, &dst, stream_));
+}
+
+template <typename Dtype>
+void Net<Dtype>::GetBlobNHWC(const string& blob, Dtype* host_nhwc) {
+    shared_ptr<Blob<Dtype> > b = blob_by_name(blob);
+    Dtype* st = staging(blob + "#out", (size_t)b->count());
+    GetBlobNHWCDevice(blob, st);
+    CUDA_CHECK(cudaMemcpyAsync(host_nhwc, st, (size_t)b->count() * sizeof(Dtype), cudaMemcpyDeviceToHost, stream_));
     CUDA_CHECK(cudaStreamSynchronize(stream_));
 }
 

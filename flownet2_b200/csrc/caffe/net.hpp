@@ -67,6 +67,12 @@ class Net {
     void SetInputDevice(const string& blob, const Dtype* dev_nchw);
     void GetBlob(const string& blob, Dtype* host_nchw);
     void GetBlobDevice(const string& blob, Dtype* dev_nchw);
+    // 8-bit frames [N][H][W][channels] (1, 3 or 4) -> an (N, 3, H, W) input blob as BGR floats (fn2_frames_to_tensor), and a
+    // blob read back as dense NHWC (include/fn2_frames.h)
+    void SetInputFrames(const string& blob, const void* host_frames, int channels);
+    void SetInputFramesDevice(const string& blob, const void* dev_frames, int channels);
+    void GetBlobNHWC(const string& blob, Dtype* host_nhwc);
+    void GetBlobNHWCDevice(const string& blob, Dtype* dev_nhwc);
 
     void TimeLayers(float* ms);
     void LayerWork(int i, double* flops, double* bytes) const { layers_[i]->WorkEstimate(bottom_vecs_[i], top_vecs_[i], flops, bytes); }

@@ -1,6 +1,6 @@
 // Streaming (HBM-bound) layers: FlowWarp, Resample, DataAugmentation kernels, ChannelNorm, the warp block, and the
 // element-wise ops of the forward and backward passes (ReLU and its backward, Eltwise SUM, y = alpha*x + beta*y, strided
-// copy and fill).
+// copy and fill), and the conversion of 8-bit frames into an input blob.
 //
 // This translation unit is compiled with -fmad=false: every expression below is evaluated
 // with separately rounded multiplies and adds in the order written, which is also how the CPU
@@ -16,6 +16,7 @@
 #include <initializer_list>
 
 #include "fn2_common.cuh"
+#include "../../include/fn2_frames.h"
 
 namespace fn2 {
 
@@ -724,6 +725,28 @@ static float warp_fill(int fill_nan) {
 // The F4 route of FlowWarp, ChannelNorm and the warp block: every pixel of t (c <= 4) is one 16-byte float4 group.
 static bool px_one_group(const T4& t) { return t.c <= 4 && t.px_float4_groups(); }
 
+// ---------------------------------------------------------------------------------------------
+// 8-bit frames [N][H][W][K] -> (N, 3, H, W) BGR floats (scripts/run-flownet.py:30-35: HWC RGB to NCHW BGR; a gray frame is
+// broadcast to the three channels like pycaffe's blob assignment, RGBA drops alpha).  One thread per pixel; byte loads need no
+// alignment (W*K may be odd).  A byte converts to float exactly, so the blob equals one filled from image_to_blob's floats.
+// Channel-fast views store through px_store (never a lane beyond C), others channel by channel.
+// ---------------------------------------------------------------------------------------------
+template <int K>
+__global__ void frames_to_tensor_kernel(const uint8_t* __restrict__ frames, PxView dst) {
+    const T4& d = dst.t;
+    for_each_pixel(d.n, d.h, d.w, [&](int n, int y, int x) {
+        const uint8_t* p = frames + (((long long)n * d.h + y) * d.w + x) * K;
+        const float4 r = K == 1 ? make_float4(p[0], p[0], p[0], 0.f) : make_float4(p[2], p[1], p[0], 0.f);
+        if (d.sc == 1) {
+            px_store(dst, d.off(n, 0, y, x), 0, r);
+        } else {
+            d.p[d.off(n, 0, y, x)] = r.x;
+            d.p[d.off(n, 1, y, x)] = r.y;
+            d.p[d.off(n, 2, y, x)] = r.z;
+        }
+    });
+}
+
 }  // namespace fn2
 
 using namespace fn2;
@@ -942,6 +965,20 @@ int fn2_fill(const fn2_tensor* dst, float value, void* stream) {
     FN2_CHECK_ARG(valid(dst), "fill: null/empty tensor");
     T4 d = view(dst);
     return ew_run(FillOp{px_view(d), value}, d, {}, stream);
+}
+
+int fn2_frames_to_tensor(const void* frames_dev, int channels, const fn2_tensor* dst, void* stream) {
+    FN2_CHECK_ARG(frames_dev, "frames_to_tensor: frames is null");
+    FN2_CHECK_ARG(valid(dst), "frames_to_tensor: dst is null or empty");
+    FN2_CHECK_ARG(channels == 1 || channels == 3 || channels == 4,
+                  "frames_to_tensor: channels must be 1, 3 or 4 (gray, RGB, RGBA), got %d", channels);
+    T4 d = view(dst);
+    FN2_CHECK_ARG(d.c == 3, "frames_to_tensor: dst must have 3 channels (B, G, R), has %d", d.c);
+    const uint8_t* f = static_cast<const uint8_t*>(frames_dev);
+    const long long total = (long long)d.n * d.h * d.w;
+    if (channels == 1) return ew_launch(frames_to_tensor_kernel<1>, total, stream, f, px_view(d));
+    if (channels == 3) return ew_launch(frames_to_tensor_kernel<3>, total, stream, f, px_view(d));
+    return ew_launch(frames_to_tensor_kernel<4>, total, stream, f, px_view(d));
 }
 
 }  // extern "C"

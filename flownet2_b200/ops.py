@@ -379,3 +379,12 @@ def copy(src, dst):
 def fill(dst, value):
     check(lib().fn2_fill(desc(dst), value, _stream()))
     return dst
+
+
+def frames_to_tensor(frames, dst):
+    """uint8 CUDA frames (N, H, W, K), K = 1, 3 or 4, dense -> dst, a float32 (N, 3, H, W) view, as BGR 0..255."""
+    assert frames.is_cuda and frames.dtype == torch.uint8 and frames.dim() == 4 and frames.is_contiguous(), \
+        "need dense uint8 CUDA frames (N, H, W, K)"
+    assert tuple(frames.shape[:3]) == (dst.shape[0], dst.shape[2], dst.shape[3]), (tuple(frames.shape), tuple(dst.shape))
+    check(lib().fn2_frames_to_tensor(frames.data_ptr(), frames.shape[3], desc(dst), _stream()))
+    return dst
