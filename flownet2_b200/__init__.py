@@ -1,7 +1,7 @@
 """flownet2_b200 -- Hopper-native FlowNet2 forward path.
 
-Python here is only a ctypes front end over the C-ABI in include/fn2.h, fn2_solver.h and fn2_frames.h (libfn2.so: hand-written
-sm_90a CUDA + the Caffe-surface C++ host).  It mirrors the slice of pycaffe that the reference's
+Python here is only a ctypes front end over the C-ABI in include/fn2.h, fn2_solver.h, fn2_frames.h and fn2_flow.h (libfn2.so:
+hand-written sm_90a CUDA + the Caffe-surface C++ host).  It mirrors the slice of pycaffe that the reference's
 driver uses (scripts/run-flownet.py:64-98): ``Net(prototxt, weights, phase)``, ``net.inputs``,
 ``net.forward(img0=..., img1=...)``, ``net.blobs[name].data``.
 
@@ -14,19 +14,24 @@ import os
 
 import numpy as np
 
-from ._abi import read_header
+from ._abi import read_defines, read_header
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB = None
 TRAIN, TEST = 0, 1
 
-_STRUCTS, _PROTOTYPES = {}, {}
-for _name in ("fn2.h", "fn2_solver.h", "fn2_frames.h"):
+_STRUCTS, _PROTOTYPES, _DEFINES = {}, {}, {}
+for _name in ("fn2.h", "fn2_solver.h", "fn2_frames.h", "fn2_flow.h"):
     with open(os.path.join(os.path.dirname(_HERE), "include", _name)) as _f:
-        _s, _p = read_header(_f.read(), _STRUCTS)
+        _text = _f.read()
+    _s, _p = read_header(_text, _STRUCTS)
     _STRUCTS.update(_s)
     _PROTOTYPES.update(_p)
+    _DEFINES.update(read_defines(_text))
 fn2_tensor, fn2_conv_desc, fn2_l1loss_desc = (_STRUCTS[n] for n in ("fn2_tensor", "fn2_conv_desc", "fn2_l1loss_desc"))
+# flow payload formats and flags of fn2_flow_to_tensor (include/fn2_flow.h)
+FLOW_FLO, FLOW_PFM, FLOW_PFM_BE, FLOW_UINT16FLOW = (_DEFINES[n] for n in ("FN2_FLOW_FLO", "FN2_FLOW_PFM", "FN2_FLOW_PFM_BE",
+                                                                          "FN2_FLOW_UINT16FLOW"))
 
 
 class Fn2Error(RuntimeError):
@@ -267,6 +272,11 @@ class Net(object):
     def set_input_image_device(self, name, dev_ptr, channels):
         """dev_ptr: device address of dense uint8 frames (N, H, W, channels) for the (N, 3, H, W) input blob `name`."""
         check(lib().fn2_net_set_input_frames_device(self._h, name.encode(), C.c_void_p(dev_ptr), int(channels)))
+
+    def set_input_flow_device(self, name, dev_ptr, format, flags=0):
+        """dev_ptr: device address of the payloads of N flow files (FLOW_FLO, FLOW_PFM or FLOW_PFM_BE; 4-byte aligned) for the
+        (N, 2, H, W) input blob `name`; flags FLOW_UINT16FLOW quantises as the reference's training data (include/fn2_flow.h)."""
+        check(lib().fn2_net_set_input_flow_device(self._h, name.encode(), C.c_void_p(dev_ptr), int(format), int(flags)))
 
     def get_blob_nhwc(self, name):
         """The blob as an (N, H, W, C) array; for the flow, (N, H, W, 2) is the payload of a .flo file per pair."""

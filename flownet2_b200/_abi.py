@@ -1,5 +1,5 @@
-"""ctypes structs and prototypes of libfn2.so, read from include/fn2.h, fn2_solver.h and fn2_frames.h: the headers are the only
-statement of the ABI.
+"""ctypes structs, prototypes and integer constants of libfn2.so, read from include/fn2.h, fn2_solver.h, fn2_frames.h and
+fn2_flow.h: the headers are the only statement of the ABI.
 
 Types map through one table; a type it does not know raises, so a new header entry cannot go undeclared."""
 import ctypes as C
@@ -31,6 +31,11 @@ def _split(decl):
     """'const fn2_tensor* bottom0' -> 'const fn2_tensor*'; 'int shape[4]' -> 'int[4]'."""
     m = re.fullmatch(r"(.*?)\s*\b\w+\s*(\[\d*\])?", decl.strip(), re.S)
     return m.group(1) + (m.group(2) or "")
+
+
+def read_defines(text):
+    """-> {name: int} of the header's integer constants (#define FN2_... <integer>)."""
+    return {k: int(v, 0) for k, v in re.findall(r"^\s*#define\s+(FN2_\w+)\s+(-?(?:0x[0-9a-fA-F]+|\d+))\s*$", text, re.M)}
 
 
 def read_header(text, included=None):

@@ -1,8 +1,9 @@
-// extern "C" net-level entry points of include/fn2.h and include/fn2_frames.h over caffe::Net<float>, and the solver's of
+// extern "C" net-level entry points of include/fn2.h, fn2_frames.h and fn2_flow.h over caffe::Net<float>, and the solver's of
 // include/fn2_solver.h over caffe::Solver.
 #include <cstring>
 #include <type_traits>
 
+#include "../../../include/fn2_flow.h"
 #include "../../../include/fn2_frames.h"
 #include "../../../include/fn2_solver.h"
 #include "net.hpp"
@@ -161,6 +162,9 @@ int fn2_net_set_input_frames(fn2_net* net, const char* blob, const void* host_fr
 int fn2_net_set_input_frames_device(fn2_net* net, const char* blob, const void* dev_frames, int channels) {
     return net_call("set_input_frames_device", net && blob && dev_frames,
                     [&] { net->net->SetInputFramesDevice(blob, dev_frames, channels); });
+}
+int fn2_net_set_input_flow_device(fn2_net* net, const char* blob, const void* dev, int format, int flags) {
+    return net_call("set_input_flow_device", net && blob && dev, [&] { net->net->SetInputFlowDevice(blob, dev, format, flags); });
 }
 int fn2_net_get_blob_nhwc(fn2_net* net, const char* blob, float* host) {
     return net_call("get_blob_nhwc", net && blob && host, [&] { net->net->GetBlobNHWC(blob, host); });

@@ -1,5 +1,6 @@
 #include "net.hpp"
 #include "hdf5_min.hpp"
+#include "../../../include/fn2_flow.h"
 #include "../../../include/fn2_frames.h"
 
 #include <cstdlib>
@@ -863,6 +864,16 @@ void Net<Dtype>::SetInputFrames(const string& blob, const void* host_frames, int
     Dtype* st = staging(blob, (bytes + sizeof(Dtype) - 1) / sizeof(Dtype));        // the buffer SetInput stages the blob in
     CUDA_CHECK(cudaMemcpyAsync(st, host_frames, bytes, cudaMemcpyHostToDevice, stream_));
     SetInputFramesDevice(blob, st, channels);
+}
+
+template <typename Dtype>
+void Net<Dtype>::SetInputFlowDevice(const string& blob, const void* dev, int format, int flags) {
+    Caffe::stream() = stream_;
+    shared_ptr<Blob<Dtype> > b = blob_by_name(blob);
+    CHECK(b->num_axes() == 4 && b->channels() == 2) << "set_input_flow: blob " << blob << " must have shape (N, 2, H, W), has "
+                                                    << b->num_axes() << " axes and " << b->channels() << " channels";
+    fn2_tensor dst = b->mutable_tensor();
+    FN2_CALL(fn2_flow_to_tensor(dev, format, flags, &dst, stream_));
 }
 
 template <typename Dtype>

@@ -71,6 +71,8 @@ class Net {
     // blob read back as dense NHWC (include/fn2_frames.h)
     void SetInputFrames(const string& blob, const void* host_frames, int channels);
     void SetInputFramesDevice(const string& blob, const void* dev_frames, int channels);
+    // flow file payloads on the device -> an (N, 2, H, W) input blob (fn2_flow_to_tensor)
+    void SetInputFlowDevice(const string& blob, const void* dev, int format, int flags);
     void GetBlobNHWC(const string& blob, Dtype* host_nhwc);
     void GetBlobNHWCDevice(const string& blob, Dtype* dev_nhwc);
 

@@ -17,6 +17,7 @@
 
 #include "fn2_common.cuh"
 #include "../../include/fn2_frames.h"
+#include "../../include/fn2_flow.h"
 
 namespace fn2 {
 
@@ -747,6 +748,38 @@ __global__ void frames_to_tensor_kernel(const uint8_t* __restrict__ frames, PxVi
     });
 }
 
+// ---------------------------------------------------------------------------------------------
+// Flow payloads -> (N, 2, H, W) floats (include/fn2_flow.h).  .flo is [N][H][W][2]; PFM is [N][H][W][3] stored bottom-up,
+// read top-down keeping channels 0, 1 (CImg load_pfm + mirror('y')), byte-swapped when big-endian.  UINT16FLOW restates the
+// reference's short(32 v) / 32 round trip (convert_imageset_and_flow.cpp:168-179, custom_data_layer.cpp:88-107): 32 v is
+// exact, trunc(32 v) in [-32768, 32766] survives as t / 32 (the int conversion turns a -0 truncation into +0), everything
+// else -- NaN, 32767 and above, below -32768 -- is NaN.  Every step is exact.
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ float flow_value(uint32_t bits, bool swap, int quantise) {
+    const float v = __uint_as_float(swap ? __byte_perm(bits, 0, 0x0123) : bits);
+    if (!quantise) return v;
+    const float s = v * 32.f;
+    return s < 32767.f && s > -32769.f ? (float)__float2int_rz(s) * 0.03125f : __uint_as_float(0x7fc00000u);
+}
+
+template <int FMT>
+__global__ void flow_to_tensor_kernel(const uint32_t* __restrict__ src, PxView dst, int quantise) {
+    const T4& d = dst.t;
+    constexpr int K = FMT == FN2_FLOW_FLO ? 2 : 3;
+    constexpr bool swap = FMT == FN2_FLOW_PFM_BE;
+    for_each_pixel(d.n, d.h, d.w, [&](int n, int y, int x) {
+        const int row = FMT == FN2_FLOW_FLO ? y : d.h - 1 - y;
+        const uint32_t* p = src + (((long long)n * d.h + row) * d.w + x) * K;
+        const float4 r = make_float4(flow_value(p[0], swap, quantise), flow_value(p[1], swap, quantise), 0.f, 0.f);
+        if (d.sc == 1) {
+            px_store(dst, d.off(n, 0, y, x), 0, r);
+        } else {
+            d.p[d.off(n, 0, y, x)] = r.x;
+            d.p[d.off(n, 1, y, x)] = r.y;
+        }
+    });
+}
+
 }  // namespace fn2
 
 using namespace fn2;
@@ -979,6 +1012,23 @@ int fn2_frames_to_tensor(const void* frames_dev, int channels, const fn2_tensor*
     if (channels == 1) return ew_launch(frames_to_tensor_kernel<1>, total, stream, f, px_view(d));
     if (channels == 3) return ew_launch(frames_to_tensor_kernel<3>, total, stream, f, px_view(d));
     return ew_launch(frames_to_tensor_kernel<4>, total, stream, f, px_view(d));
+}
+
+int fn2_flow_to_tensor(const void* src_dev, int format, int flags, const fn2_tensor* dst, void* stream) {
+    FN2_CHECK_ARG(src_dev, "flow_to_tensor: src is null");
+    FN2_CHECK_ARG((reinterpret_cast<uintptr_t>(src_dev) & 3) == 0, "flow_to_tensor: src must be 4-byte aligned");
+    FN2_CHECK_ARG(valid(dst), "flow_to_tensor: dst is null or empty");
+    FN2_CHECK_ARG(format == FN2_FLOW_FLO || format == FN2_FLOW_PFM || format == FN2_FLOW_PFM_BE,
+                  "flow_to_tensor: format must be FN2_FLOW_FLO, FN2_FLOW_PFM or FN2_FLOW_PFM_BE, got %d", format);
+    FN2_CHECK_ARG((flags & ~FN2_FLOW_UINT16FLOW) == 0, "flow_to_tensor: unknown flags 0x%x", flags);
+    T4 d = view(dst);
+    FN2_CHECK_ARG(d.c == 2, "flow_to_tensor: dst must have 2 channels (u, v), has %d", d.c);
+    const uint32_t* s = static_cast<const uint32_t*>(src_dev);
+    const long long total = (long long)d.n * d.h * d.w;
+    const int q = flags & FN2_FLOW_UINT16FLOW;
+    if (format == FN2_FLOW_FLO) return ew_launch(flow_to_tensor_kernel<FN2_FLOW_FLO>, total, stream, s, px_view(d), q);
+    if (format == FN2_FLOW_PFM) return ew_launch(flow_to_tensor_kernel<FN2_FLOW_PFM>, total, stream, s, px_view(d), q);
+    return ew_launch(flow_to_tensor_kernel<FN2_FLOW_PFM_BE>, total, stream, s, px_view(d), q);
 }
 
 }  // extern "C"

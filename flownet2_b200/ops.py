@@ -388,3 +388,11 @@ def frames_to_tensor(frames, dst):
     assert tuple(frames.shape[:3]) == (dst.shape[0], dst.shape[2], dst.shape[3]), (tuple(frames.shape), tuple(dst.shape))
     check(lib().fn2_frames_to_tensor(frames.data_ptr(), frames.shape[3], desc(dst), _stream()))
     return dst
+
+
+def flow_to_tensor(payload, format, flags, dst):
+    """Dense CUDA flow-file payloads (any dtype; .flo [N][H][W][2] or PFM [N][H][W][3] floats, format FLOW_FLO, FLOW_PFM or
+    FLOW_PFM_BE) -> dst, a float32 (N, 2, H, W) view; flags FLOW_UINT16FLOW quantises as the reference's training data."""
+    assert payload.is_cuda and payload.is_contiguous(), "need a dense CUDA payload"
+    check(lib().fn2_flow_to_tensor(payload.data_ptr(), int(format), int(flags), desc(dst), _stream()))
+    return dst

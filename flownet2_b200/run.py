@@ -214,6 +214,14 @@ def batches(pairs, batch):
     return out
 
 
+def write_pnm(path, a):
+    """Binary PGM (H, W) or PPM (H, W, 3) frame, maxval 255 -> path."""
+    with open(path, "wb") as f:
+        f.write(b"%s\n%d %d\n255\n" % (b"P5" if a.ndim == 2 else b"P6", a.shape[1], a.shape[0]))
+        f.write(np.ascontiguousarray(a, np.uint8).tobytes())
+    return str(path)
+
+
 def write_flo(path, flow_hw2):
     """.flo file (src/caffe/util/output.cpp:16-64): 'PIEH', width, height (int32), then (H, W, 2) float32."""
     h, w = flow_hw2.shape[:2]
