@@ -1,7 +1,7 @@
 """flownet2_b200 -- Hopper-native FlowNet2 forward path.
 
-Python here is only a ctypes front end over the C-ABI in include/fn2.h, fn2_solver.h, fn2_frames.h and fn2_flow.h (libfn2.so:
-hand-written sm_90a CUDA + the Caffe-surface C++ host).  It mirrors the slice of pycaffe that the reference's
+Python here is only a ctypes front end over the C-ABI in include/fn2.h, fn2_solver.h, fn2_frames.h, fn2_flow.h and fn2_lpq.h
+(libfn2.so: hand-written sm_90a CUDA + the Caffe-surface C++ host).  It mirrors the slice of pycaffe that the reference's
 driver uses (scripts/run-flownet.py:64-98): ``Net(prototxt, weights, phase)``, ``net.inputs``,
 ``net.forward(img0=..., img1=...)``, ``net.blobs[name].data``.
 
@@ -21,14 +21,16 @@ _LIB = None
 TRAIN, TEST = 0, 1
 
 _STRUCTS, _PROTOTYPES, _DEFINES = {}, {}, {}
-for _name in ("fn2.h", "fn2_solver.h", "fn2_frames.h", "fn2_flow.h"):
+for _name in ("fn2.h", "fn2_solver.h", "fn2_frames.h", "fn2_flow.h", "fn2_lpq.h"):
     with open(os.path.join(os.path.dirname(_HERE), "include", _name)) as _f:
         _text = _f.read()
     _s, _p = read_header(_text, _STRUCTS)
     _STRUCTS.update(_s)
     _PROTOTYPES.update(_p)
     _DEFINES.update(read_defines(_text))
-fn2_tensor, fn2_conv_desc, fn2_l1loss_desc = (_STRUCTS[n] for n in ("fn2_tensor", "fn2_conv_desc", "fn2_l1loss_desc"))
+fn2_tensor, fn2_conv_desc, fn2_l1loss_desc, fn2_lpqloss_desc = (_STRUCTS[n] for n in ("fn2_tensor", "fn2_conv_desc", "fn2_l1loss_desc",
+                                                                                     "fn2_lpqloss_desc"))
+LPQLOSS_STATE_FLOATS = _DEFINES["FN2_LPQLOSS_STATE_FLOATS"]            # device floats of an LpqLoss state (include/fn2_lpq.h)
 # flow payload formats and flags of fn2_flow_to_tensor (include/fn2_flow.h)
 FLOW_FLO, FLOW_PFM, FLOW_PFM_BE, FLOW_UINT16FLOW = (_DEFINES[n] for n in ("FN2_FLOW_FLO", "FN2_FLOW_PFM", "FN2_FLOW_PFM_BE",
                                                                           "FN2_FLOW_UINT16FLOW"))
@@ -298,6 +300,17 @@ class Net(object):
     def clear_param_diffs(self):
         check(lib().fn2_net_clear_param_diffs(self._h))
 
+    @property
+    def iter(self):
+        """Net::iter: the iteration the layers see (LpqLoss picks its p/q schedule step by it); 0 until set."""
+        it = C.c_int()
+        check(lib().fn2_net_iter(self._h, C.byref(it)))
+        return it.value
+
+    def set_iter(self, iteration):
+        """Net::set_iter.  Solver.step sets it at the start of every iteration."""
+        check(lib().fn2_net_set_iter(self._h, int(iteration)))
+
     def set_diff(self, name, array):
         a = np.ascontiguousarray(array, dtype=np.float32)
         if tuple(a.shape) != self.blobs[name].shape:
@@ -416,7 +429,7 @@ def get_solver(solver, net):
 class Solver(object):
     """Caffe's SGD / Adam solver over a TRAIN Net (src/caffe/solver.cpp:194-481, solvers/sgd_solver.cpp, adam_solver.cpp).
 
-    ``step(n, feed)`` runs n iterations: ClearParamDiffs, the on_start callbacks, iter_size x (feed, forward, backward), the
+    ``step(n, feed)`` runs n iterations: Net.set_iter(iter), ClearParamDiffs, the on_start callbacks, iter_size x (feed, forward, backward), the
     on_gradients_ready callbacks, the update on the device, iter += 1, and a snapshot when one is due.  ``feed()`` returns
     {input name: ndarray or CUDA tensor} and is called before every forward.  Within an iteration the only host
     synchronisation is the read of the loss outputs, after the update has been enqueued.  Data-parallel training all-reduces
@@ -494,6 +507,7 @@ class Solver(object):
         net_stream = torch.cuda.ExternalStream(self.net.stream)
         for _ in range(int(iters)):
             self._keep = []
+            self.net.set_iter(self.iter)                                   # solver.cpp:202, before ClearParamDiffs
             self.net.clear_param_diffs()
             for on_start, _ in self._callbacks:
                 on_start()

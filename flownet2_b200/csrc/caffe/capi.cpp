@@ -1,10 +1,11 @@
-// extern "C" net-level entry points of include/fn2.h, fn2_frames.h and fn2_flow.h over caffe::Net<float>, and the solver's of
+// extern "C" net-level entry points of include/fn2.h, fn2_frames.h, fn2_flow.h and fn2_lpq.h over caffe::Net<float>, and the solver's of
 // include/fn2_solver.h over caffe::Solver.
 #include <cstring>
 #include <type_traits>
 
 #include "../../../include/fn2_flow.h"
 #include "../../../include/fn2_frames.h"
+#include "../../../include/fn2_lpq.h"
 #include "../../../include/fn2_solver.h"
 #include "net.hpp"
 #include "hdf5_min.hpp"
@@ -226,6 +227,10 @@ int fn2_net_layer_need_backward(fn2_net* net, int layer) {
     } catch (...) { return -1; }
 }
 
+int fn2_net_set_iter(fn2_net* net, int iter) {
+    return net_call("set_iter", net && iter >= 0, [&] { net->net->set_iter(iter); });
+}
+int fn2_net_iter(fn2_net* net, int* iter) { return net_call("iter", net && iter, [&] { *iter = net->net->iter(); }); }
 int fn2_net_sync(fn2_net* net) { return net_call("sync", net, [&] { net->net->Sync(); }); }
 void* fn2_net_stream(fn2_net* net) { return net ? (void*)net->net->stream() : nullptr; }
 

@@ -63,9 +63,9 @@ class Layer {
     virtual void CustomCopyBlobs(const vector<Blob<Dtype>*>& blobs) {}          // layer.hpp:136
 
     // ---- engine hooks (not in the reference) ------------------------------------------------
-    // Called once per Net::Forward on the host before any kernel is enqueued (e.g. the
-    // DataAugmentation iteration counter, data_augmentation_layer.cu:353-354).
-    virtual void HostTick() {}
+    // Called once per Net::Forward on the host, with the net's iteration (Net::iter), before any kernel is enqueued (e.g. the
+    // DataAugmentation iteration counter, data_augmentation_layer.cu:353-354; LpqLoss's p/q schedule step).
+    virtual void HostTick(int iter) {}
     // false while the layer's launch sequence depends on host state (no CUDA-graph replay).
     virtual bool GraphSafe() const { return true; }
     // Parameters were (re)loaded: derive packed device copies.

@@ -8,7 +8,9 @@
 #include <map>
 #include <random>
 #include <set>
+#include <sstream>
 
+#include "../../../include/fn2_lpq.h"
 #include "layer.hpp"
 
 namespace caffe {
@@ -1107,7 +1109,7 @@ class DataAugmentationLayer : public Layer<Dtype> {
         }
         sampler_ = AugSampler((uint32_t)(seed * 2654435761u) ^ seed_of(this->layer_param_.name()));
     }
-    void HostTick() override {
+    void HostTick(int) override {
         float& num_iter = *(this->blobs_[0]->mutable_cpu_data());
         num_iter = (float)((int)num_iter + 1);                         // data_augmentation_layer.cu:353-354
         num_iter_ = num_iter;
@@ -1315,6 +1317,97 @@ class L1LossLayer : public Layer<Dtype> {
     DeviceBuffer state_, ws_;
 };
 REGISTER_LAYER_CLASS(L1Loss);
+
+// LpqLoss (lpq_loss_layer.hpp, lpq_loss_layer.cpp:13-138, lpq_loss_layer.cu:96-245): the robust NaN-masked
+// sum_locations (sum_c w (|d_c| + p_epsilon)^p + q_epsilon)^q / norm, with p and q following a schedule over the net's iteration
+template <typename Dtype>
+class LpqLossLayer : public Layer<Dtype> {
+ public:
+    explicit LpqLossLayer(const LayerParameter& p) : Layer<Dtype>(p) {}
+    const char* type() const override { return "LpqLoss"; }
+    bool IsLossLayer() const override { return true; }
+    typename Blob<Dtype>::Layout TopLayout() const override { return Blob<Dtype>::PLAIN; }
+    void LayerSetUp(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) override {
+        const Message& lp = this->layer_param_.m->msg("lpq_loss_param");
+        const int ns = lp.count("pq_episode_starts_at_iter"), np = lp.count("p"), nq = lp.count("q");
+        starts_.clear(); p_.clear(); q_.clear();
+        // lpq_loss_layer.cpp:19-82: one p and one q without start iterations are constant values; otherwise the three lists
+        // have equal, non-zero sizes, strictly increasing start iterations, and the first one is 0
+        if (ns == 0 && np == 1 && nq == 1) {
+            starts_.push_back(0);
+        } else {
+            if (ns != np || np != nq) {
+                std::ostringstream os;
+                os << "Incompatible sizes: (pq_episode_starts_at_iter -> " << ns << ", p -> " << np << ", q -> " << nq << ")";
+                throw CaffeError(os.str());
+            }
+            if (ns < 1) throw CaffeError("Lpq schedule parameters must not be empty");
+            for (int i = 0; i < ns; i++) starts_.push_back((unsigned)lp.num("pq_episode_starts_at_iter", 0, i));
+            for (int i = 0; i + 1 < ns; i++)
+                if (starts_[i] >= starts_[i + 1]) {
+                    std::ostringstream os;
+                    os << "pq_episode_starts_at_frame is not ordered or contains duplicates:";
+                    for (unsigned v : starts_) os << " " << v;
+                    throw CaffeError(os.str());
+                }
+            if (starts_[0] != 0) throw CaffeError("First entry in pq_episode_starts_at_frame is not 0, this is probably a mistake.");
+        }
+        for (int i = 0; i < np; i++) { p_.push_back(lp.f("p", 0.f, i)); q_.push_back(lp.f("q", 0.f, i)); }
+        CHECK(bottom.size() == 1 || bottom.size() == 2) << "LpqLossLayer needs one or two input blobs.";
+        d_.p_epsilon = lp.f("p_epsilon", 0.f);
+        d_.q_epsilon = lp.f("q_epsilon", 1e-2f);
+        d_.l2_prescale_by_channels = lp.b("l2_prescale_by_channels", false) ? 1 : 0;
+        d_.normalize_by_num_entries = lp.b("normalize_by_num_entries", false) ? 1 : 0;
+        state_.reserve(FN2_LPQLOSS_STATE_FLOATS * sizeof(float), S());
+        step_ = -1;
+    }
+    // The schedule step of iteration `iter`: the last one whose start iteration is <= iter.  The reference pops a queue as the
+    // iteration grows (lpq_loss_layer.cu:100-135), which gives the same step whenever the iteration only grows; the lookup also
+    // stays right after a Solver restore to an earlier iteration.  A changed (p, q) goes to the device state with one copy on
+    // the net's stream: after the previous backward, which still reads the old pair, and before this forward or its graph
+    // replay.  The source is pageable, so the copy has taken the values by the time it returns.
+    void HostTick(int iter) override {
+        int k = 0;
+        while (k + 1 < (int)starts_.size() && starts_[k + 1] <= (unsigned)iter) k++;
+        if (k == step_) return;
+        step_ = k;
+        pq_[0] = p_[k]; pq_[1] = q_[k];
+        CUDA_CHECK(cudaMemcpyAsync(state_.as<float>() + 4, pq_, sizeof(pq_), cudaMemcpyHostToDevice, S()));
+    }
+    void Reshape(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) override {
+        if (bottom.size() > 1) CHECK(bottom[0]->shape() == bottom[1]->shape()) << "LpqLoss: bottoms must have the same shape";
+        top[0]->set_layout(Blob<Dtype>::PLAIN);
+        top[0]->Reshape(vector<int>());                               // loss layers output a scalar (lpq_loss_layer.cpp:144-146)
+        size_t need = 0;
+        FN2_CALL(fn2_lpqloss_workspace_bytes(bottom[0]->num(), bottom[0]->height(), bottom[0]->width(), &need));
+        ws_.reserve(need);
+    }
+    void Forward_gpu(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) override {
+        fn2_tensor b0 = bottom[0]->tensor(), b1 = b0;
+        if (bottom.size() > 1) b1 = bottom[1]->tensor();
+        FN2_CALL(fn2_lpqloss_forward(&b0, bottom.size() > 1 ? &b1 : nullptr, &d_, state_.as<float>(), top[0]->mutable_gpu_data(), ws_.get(),
+                                     ws_.bytes(), S()));
+    }
+    void Backward_gpu(const vector<Blob<Dtype>*>& top, const vector<bool>& propagate_down, const vector<Blob<Dtype>*>& bottom) override {
+        const bool p0 = propagate_down[0], p1 = bottom.size() > 1 && propagate_down[1];
+        if (!p0 && !p1) return;
+        fn2_tensor b0 = bottom[0]->tensor(), b1 = b0, d0 = b0, d1 = b0;
+        if (bottom.size() > 1) b1 = bottom[1]->tensor();
+        if (p0) d0 = bottom[0]->diff_tensor();
+        if (p1) d1 = bottom[1]->diff_tensor();
+        fn2_tensor td = top[0]->diff_tensor();
+        FN2_CALL(fn2_lpqloss_backward(&b0, bottom.size() > 1 ? &b1 : nullptr, &d_, state_.as<float>(), td.data, p0 ? &d0 : nullptr, p1 ? &d1 : nullptr,
+                                      this->bottom_accumulate_[0] ? 1 : 0, bottom.size() > 1 && this->bottom_accumulate_[1] ? 1 : 0, S()));
+    }
+ protected:
+    fn2_lpqloss_desc d_;
+    vector<unsigned> starts_;
+    vector<float> p_, q_;
+    float pq_[2] = {0.f, 0.f};
+    int step_ = -1;
+    DeviceBuffer state_, ws_;
+};
+REGISTER_LAYER_CLASS(LpqLoss);
 
 // Downsample (downsample_layer.cpp:20-58, downsample_layer.cu:15-80): ground-truth pyramid for the multi-scale losses
 template <typename Dtype>

@@ -504,7 +504,7 @@ void Net<Dtype>::Forward() {
     Caffe::stream() = stream_;
     if (!params_ready_) ParamsChanged();
     bool safe = !graph_disabled_;
-    for (auto& l : layers_) l->HostTick();
+    for (auto& l : layers_) l->HostTick(iter_);
     for (auto& l : layers_) if (!l->GraphSafe()) safe = false;
     if (safe && graph_exec_) {
         CUDA_CHECK(cudaGraphLaunch(graph_exec_, stream_));
@@ -900,7 +900,7 @@ template <typename Dtype>
 void Net<Dtype>::TimeLayers(float* ms) {
     Caffe::stream() = stream_;
     if (!params_ready_) ParamsChanged();
-    for (auto& l : layers_) l->HostTick();
+    for (auto& l : layers_) l->HostTick(iter_);
     vector<cudaEvent_t> ev(layers_.size() + 1);
     for (auto& e : ev) CUDA_CHECK(cudaEventCreate(&e));
     CUDA_CHECK(cudaEventRecord(ev[0], stream_));

@@ -29,6 +29,10 @@ class Net {
     int launches_per_backward() const { return launches_per_backward_; }
     const vector<char>& layer_need_backward() { PlanBackward(); return bw_run_; }
     void Sync();
+    // Net::set_iter / iter (net.hpp:230-231): the iteration the layers see in HostTick (LpqLoss's p/q schedule).  The Solver
+    // sets it at the start of every iteration (solver.cpp:202); a net no solver drives stays at 0.
+    void set_iter(int iter) { iter_ = iter; }
+    int iter() const { return iter_; }
     cudaStream_t stream() const { return stream_; }
 
     // net.cpp:752-802 (binary proto) / :823-870 (HDF5, by signature).  Source layer X fills target layer prefix + X (a stage's
@@ -112,6 +116,7 @@ class Net {
     int launches_per_backward_ = 0;
 
     Phase phase_;
+    int iter_ = 0;
     string name_;
     vector<shared_ptr<Layer<Dtype> > > layers_;
     vector<string> layer_names_;

@@ -10,11 +10,19 @@
 // see the same masks.
 // state (device, 4 floats): [0] loss, [1] normalize_coeff, [2] masked sum, [3] not-NaN count.
 //
+// LpqLoss (lpq_loss_layer.cpp:19-82, lpq_loss_layer.cu:96-245; include/fn2_lpq.h).  The reference chains an Eltwise
+// difference, four element-wise kernels (NaN mask, KillMasked, ComputeSign, abs by multiplying with the sign), Power(p), a 1x1
+// sum convolution, Power(q), a cuBLAS dot and a host read; the backward runs the chain in reverse.  Here it has L1Loss's shape:
+// one pass writes a (loss, not-NaN count) partial per block, l1loss_final_kernel reduces them in a fixed order, and the
+// backward recomputes difference, mask, sign, the location's channel sum and both power derivatives from the bottoms.  p and
+// q are read from the state (state[4], state[5]), which the layer writes when its schedule step changes.
+//
 // Downsample (downsample_layer.cu:15-80): weighted box average around the rounded source position, NaN aware; the narrow and
 // the wide kernel share the centre, the tap and the final value (ds_centre, ds_tap, ds_value).
 // This file is compiled with FMA contraction (unlike fn2_ops.cu): moving code between the two changes its rounding.
 // FlowAugmentation (flow_augmentation_layer.cu:24-66): flow field of the augmented pair from the two spatial transforms.
 #include "fn2_common.cuh"
+#include "../../include/fn2_lpq.h"
 
 namespace fn2 {
 
@@ -48,6 +56,22 @@ __device__ __forceinline__ float l2_location(const T4& a, const T4& b, const L1P
     return kill ? 0.f : s;
 }
 
+// The block's (loss, count) partial into part[2 * blockIdx.x], part[2 * blockIdx.x + 1]: warp butterflies, then the first warp
+// over the warps' sums (L1Loss and LpqLoss forwards)
+__device__ __forceinline__ void block_partial(float loss, float cnt, float* __restrict__ part) {
+    __shared__ float sl[32], sc[32];
+    for (int o = 16; o; o >>= 1) { loss += __shfl_xor_sync(0xffffffffu, loss, o); cnt += __shfl_xor_sync(0xffffffffu, cnt, o); }
+    if ((threadIdx.x & 31) == 0) { sl[threadIdx.x >> 5] = loss; sc[threadIdx.x >> 5] = cnt; }
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        const int nw = blockDim.x >> 5;
+        loss = threadIdx.x < nw ? sl[threadIdx.x] : 0.f;
+        cnt = threadIdx.x < nw ? sc[threadIdx.x] : 0.f;
+        for (int o = 16; o; o >>= 1) { loss += __shfl_xor_sync(0xffffffffu, loss, o); cnt += __shfl_xor_sync(0xffffffffu, cnt, o); }
+        if (threadIdx.x == 0) { part[2 * blockIdx.x] = loss; part[2 * blockIdx.x + 1] = cnt; }
+    }
+}
+
 template <bool L2>
 __global__ void l1loss_fwd_kernel(T4 a, T4 b, L1P p, float* __restrict__ part /* [grid][2] */) {
     float loss = 0.f, cnt = 0.f;
@@ -64,19 +88,10 @@ __global__ void l1loss_fwd_kernel(T4 a, T4 b, L1P p, float* __restrict__ part /*
             }
         }
     });
-    __shared__ float sl[32], sc[32];
-    for (int o = 16; o; o >>= 1) { loss += __shfl_xor_sync(0xffffffffu, loss, o); cnt += __shfl_xor_sync(0xffffffffu, cnt, o); }
-    if ((threadIdx.x & 31) == 0) { sl[threadIdx.x >> 5] = loss; sc[threadIdx.x >> 5] = cnt; }
-    __syncthreads();
-    if (threadIdx.x < 32) {
-        const int nw = blockDim.x >> 5;
-        loss = threadIdx.x < nw ? sl[threadIdx.x] : 0.f;
-        cnt = threadIdx.x < nw ? sc[threadIdx.x] : 0.f;
-        for (int o = 16; o; o >>= 1) { loss += __shfl_xor_sync(0xffffffffu, loss, o); cnt += __shfl_xor_sync(0xffffffffu, cnt, o); }
-        if (threadIdx.x == 0) { part[2 * blockIdx.x] = loss; part[2 * blockIdx.x + 1] = cnt; }
-    }
+    block_partial(loss, cnt, part);
 }
 
+// Also LpqLoss's final kernel: its normaliser is L1Loss's (lpq_loss_layer.cu:156-161), and it leaves p and q (state[4..5]) alone.
 __global__ void l1loss_final_kernel(const float* __restrict__ part, int blocks, int num, int channels, int by_entries,
                                     float* __restrict__ state, float* __restrict__ loss_out) {
     if (threadIdx.x || blockIdx.x) return;
@@ -118,6 +133,77 @@ __global__ void l1loss_bwd_kernel(T4 a, T4 b, L1P p, const float* __restrict__ s
             }
             if (prop_a) { float* o = da.p + da.off(n, c, y, x); *o = acc_a ? *o + g : g; }
             if (prop_b && p.two) { float* o = db.p + db.off(n, c, y, x); *o = acc_b ? *o - g : -g; }
+        }
+    });
+}
+
+// ---- LpqLoss ---------------------------------------------------------------------------------------------------------------
+struct LpqP {
+    int two;
+    float w, pe, qe;    // channel weight of the sum convolution, the p and q Power layers' shifts
+};
+
+// PowerLayer::Forward_gpu (power_layer.cu:8-30) with scale 1: power 0 gives 1 (diff_scale_ == 0); the shift is added when it is
+// not 0; powf (caffe_gpu_powx's pow(float, float)) runs only when power != 1.
+__device__ __forceinline__ float lpq_pow(float x, float shift, float power) {
+    if (power == 0.f) return 1.f;
+    const float t = shift != 0.f ? __fadd_rn(x, shift) : x;
+    return power != 1.f ? powf(t, power) : t;
+}
+// PowerLayer::Backward_gpu (power_layer.cu:32-84) before its product with the top diff, y = lpq_pow(x): power 0: 0; power 1:
+// 1; power 2: 2x + 2 shift; shift 0: power * y / x; otherwise power * y / (x + shift).  One deviation: with shift 0 the
+// reference divides 0 / 0 = NaN at x == 0 (an exactly-zero difference for p, a zero channel sum for q) and the NaN reaches the
+// weights; here the derivative is 0 there (the subgradient; for power > 1 the true derivative).
+__device__ __forceinline__ float lpq_dpow(float x, float y, float shift, float power) {
+    if (power == 0.f) return 0.f;
+    if (power == 1.f) return 1.f;
+    if (power == 2.f) { const float g = __fmul_rn(2.f, x); return shift != 0.f ? __fadd_rn(g, __fmul_rn(2.f, shift)) : g; }
+    if (shift == 0.f) return x == 0.f ? 0.f : __fmul_rn(__fdiv_rn(y, x), power);
+    return __fmul_rn(__fdiv_rn(y, __fadd_rn(x, shift)), power);
+}
+// |d| as the reference forms it: KillMasked zeroes a NaN d BEFORE the powers (lpq_loss_layer.cu:163-169), so a NaN entry
+// still adds w * P(0) = w * p_epsilon^p, and a location whose channels are all NaN still adds Q(...) >= q_epsilon^q; then
+// ComputeSign (0 -> -1) and the product with the sign (:172-185), i.e. |d|.
+__device__ __forceinline__ float lpq_abs(float d) { return d == d ? fabsf(d) : 0.f; }
+// The location's channel sum s = sum_c w * P(|d_c|) (the 1x1 convolution with constant weight w, lpq_loss_layer.cpp:118-135);
+// cnt counts the not-NaN d (FindNotNaNs).
+__device__ __forceinline__ float lpq_location(const T4& a, const T4& b, const LpqP& lp, float p, int n, int y, int x, float& cnt) {
+    float s = 0.f;
+    for (int c = 0; c < a.c; c++) {
+        const float d = a.p[a.off(n, c, y, x)] - (lp.two ? b.p[b.off(n, c, y, x)] : 0.f);
+        cnt += d == d ? 1.f : 0.f;
+        s += lp.w * lpq_pow(lpq_abs(d), lp.pe, p);
+    }
+    return s;
+}
+
+__global__ void lpqloss_fwd_kernel(T4 a, T4 b, LpqP lp, const float* __restrict__ state, float* __restrict__ part /* [grid][2] */) {
+    const float p = state[4], q = state[5];
+    float loss = 0.f, cnt = 0.f;
+    for_each_pixel(a.n, a.h, a.w, [&](int n, int y, int x) {
+        loss += lpq_pow(lpq_location(a, b, lp, p, n, y, x, cnt), lp.qe, q);
+    });
+    block_partial(loss, cnt, part);
+}
+
+__global__ void lpqloss_bwd_kernel(T4 a, T4 b, LpqP lp, const float* __restrict__ state, const float* __restrict__ top_diff,
+                                   T4 da, T4 db, int prop_a, int prop_b, int acc_a, int acc_b) {
+    const float alpha = top_diff[0] / state[1];                         // lpq_loss_layer.cu:214
+    const float p = state[4], q = state[5];
+    for_each_pixel(a.n, a.h, a.w, [&](int n, int y, int x) {
+        float cnt = 0.f;
+        const float s = lpq_location(a, b, lp, p, n, y, x, cnt);
+        // Power(q) backward, then the sum convolution's data gradient: w * alpha * Q'(s) for every channel
+        const float gs = __fmul_rn(lp.w, __fmul_rn(alpha, lpq_dpow(s, lpq_pow(s, lp.qe, q), lp.qe, q)));
+        for (int c = 0; c < a.c; c++) {
+            const float d = a.p[a.off(n, c, y, x)] - (lp.two ? b.p[b.off(n, c, y, x)] : 0.f);
+            const bool ok = d == d;
+            const float ad = lpq_abs(d);
+            float g = __fmul_rn(gs, lpq_dpow(ad, lpq_pow(ad, lp.pe, p), lp.pe, p));   // Power(p) backward
+            g = __fmul_rn(g, ok && d > 0.f ? 1.f : -1.f);               // times the sign of the zeroed d (:225-231)
+            if (!ok) g = 0.f;                                           // KillMasked (:233-238)
+            if (prop_a) { float* o = da.p + da.off(n, c, y, x); *o = acc_a ? *o + g : g; }
+            if (prop_b && lp.two) { float* o = db.p + db.off(n, c, y, x); *o = acc_b ? *o - g : -g; }   // Eltwise coeff -1
         }
     });
 }
@@ -220,6 +306,13 @@ L1P l1_params(const fn2_l1loss_desc* d, const T4& a, bool two) {
     return p;
 }
 
+LpqP lpq_params(const fn2_lpqloss_desc* d, const T4& a, bool two) {
+    LpqP p;
+    p.two = two ? 1 : 0; p.pe = d->p_epsilon; p.qe = d->q_epsilon;
+    p.w = d->l2_prescale_by_channels ? 1.f / (float)a.c : 1.f;        // lpq_loss_layer.cpp:123-131
+    return p;
+}
+
 }  // namespace
 }  // namespace fn2
 
@@ -270,6 +363,46 @@ int fn2_l1loss_backward(const fn2_tensor* bottom0, const fn2_tensor* bottom1, co
         l1loss_bwd_kernel<true><<<grid, 256, 0, st>>>(a, b, p, state_dev, top_diff_dev, da, db, bottom0_diff ? 1 : 0, bottom1_diff ? 1 : 0, accumulate0, accumulate1);
     else
         l1loss_bwd_kernel<false><<<grid, 256, 0, st>>>(a, b, p, state_dev, top_diff_dev, da, db, bottom0_diff ? 1 : 0, bottom1_diff ? 1 : 0, accumulate0, accumulate1);
+    FN2_LAUNCH_CHECK();
+    return FN2_OK;
+}
+
+int fn2_lpqloss_workspace_bytes(int N, int H, int W, size_t* bytes) {
+    FN2_CHECK_ARG(bytes && N > 0 && H > 0 && W > 0, "lpqloss_workspace_bytes: bad argument");
+    *bytes = (size_t)loss_grid((long long)N * H * W) * 2 * sizeof(float);
+    return FN2_OK;
+}
+
+int fn2_lpqloss_forward(const fn2_tensor* bottom0, const fn2_tensor* bottom1, const fn2_lpqloss_desc* d, float* state_dev,
+                        float* loss_dev, void* workspace, size_t workspace_bytes, void* stream) {
+    FN2_CHECK_ARG(valid(bottom0) && d && state_dev, "lpqloss_forward: null argument");
+    T4 a = view(bottom0), b = a;
+    if (bottom1) { FN2_CHECK_ARG(valid(bottom1), "lpqloss_forward: bad second bottom"); b = view(bottom1); FN2_CHECK_ARG(same_dims(a, b), "lpqloss_forward: bottoms differ in shape"); }
+    const int grid = loss_grid((long long)a.n * a.h * a.w);
+    if (!workspace || workspace_bytes < (size_t)grid * 2 * sizeof(float)) {
+        set_error("lpqloss_forward: workspace too small (%zu < %zu)", workspace_bytes, (size_t)grid * 2 * sizeof(float));
+        return FN2_ERR_WORKSPACE;
+    }
+    cudaStream_t st = (cudaStream_t)stream;
+    lpqloss_fwd_kernel<<<grid, 256, 0, st>>>(a, b, lpq_params(d, a, bottom1), state_dev, (float*)workspace);
+    FN2_LAUNCH_CHECK();
+    l1loss_final_kernel<<<1, 32, 0, st>>>((const float*)workspace, grid, a.n, a.c, d->normalize_by_num_entries, state_dev, loss_dev);
+    FN2_LAUNCH_CHECK();
+    return FN2_OK;
+}
+
+int fn2_lpqloss_backward(const fn2_tensor* bottom0, const fn2_tensor* bottom1, const fn2_lpqloss_desc* d, const float* state_dev,
+                         const float* top_diff_dev, const fn2_tensor* bottom0_diff, const fn2_tensor* bottom1_diff,
+                         int accumulate0, int accumulate1, void* stream) {
+    FN2_CHECK_ARG(valid(bottom0) && d && state_dev && top_diff_dev, "lpqloss_backward: null argument");
+    FN2_CHECK_ARG(bottom0_diff || bottom1_diff, "lpqloss_backward: no gradient requested");
+    T4 a = view(bottom0), b = a, da = a, db = a;
+    if (bottom1) { b = view(bottom1); FN2_CHECK_ARG(same_dims(a, b), "lpqloss_backward: bottoms differ in shape"); }
+    if (bottom0_diff) { da = view(bottom0_diff); FN2_CHECK_ARG(same_dims(a, da), "lpqloss_backward: bottom0 diff shape"); }
+    if (bottom1_diff) { FN2_CHECK_ARG(bottom1, "lpqloss_backward: diff for a missing bottom"); db = view(bottom1_diff); FN2_CHECK_ARG(same_dims(a, db), "lpqloss_backward: bottom1 diff shape"); }
+    const int grid = loss_grid((long long)a.n * a.h * a.w);
+    lpqloss_bwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(a, b, lpq_params(d, a, bottom1), state_dev, top_diff_dev, da, db,
+                                                                bottom0_diff ? 1 : 0, bottom1_diff ? 1 : 0, accumulate0, accumulate1);
     FN2_LAUNCH_CHECK();
     return FN2_OK;
 }

@@ -10,7 +10,7 @@ import ctypes as C
 
 import torch
 
-from . import check, fn2_conv_desc, fn2_l1loss_desc, fn2_tensor, lib
+from . import LPQLOSS_STATE_FLOATS, check, fn2_conv_desc, fn2_l1loss_desc, fn2_lpqloss_desc, fn2_tensor, lib
 
 
 def desc(t):
@@ -358,6 +358,44 @@ def l1loss_backward(b0, b1=None, *, l2_per_location=False, l2_prescale_by_channe
     check(lib().fn2_l1loss_backward(desc(b0), desc(b1) if b1 is not None else None, d, _ptr(state), _ptr(top_diff),
                                     desc(out0) if out0 is not None else None, desc(out1) if out1 is not None else None,
                                     1 if accumulate0 else 0, 1 if accumulate1 else 0, _stream()))
+    return out0, out1
+
+
+def _lpq_desc(p_epsilon, q_epsilon, l2_prescale_by_channels, normalize_by_num_entries):
+    return fn2_lpqloss_desc(float(p_epsilon), float(q_epsilon), 1 if l2_prescale_by_channels else 0, 1 if normalize_by_num_entries else 0)
+
+
+def lpqloss(b0, b1=None, *, p, q, p_epsilon=0.0, q_epsilon=1e-2, l2_prescale_by_channels=False, normalize_by_num_entries=False,
+            state=None, workspace=None):
+    """LpqLossLayer::Forward_gpu through the C-ABI (include/fn2_lpq.h) -> (loss, state): the loss (1 float) and the state
+    {loss, normalize_coeff, loss sum, not-NaN count, p, q} the backward reads, both device float tensors.  p and q are written
+    into the state on the current stream first; p = None / q = None keep the ones a given state holds."""
+    l = lib()
+    d = _lpq_desc(p_epsilon, q_epsilon, l2_prescale_by_channels, normalize_by_num_entries)
+    if workspace is None:
+        workspace = _ws(_size(l.fn2_lpqloss_workspace_bytes, b0.shape[0], b0.shape[2], b0.shape[3]), b0.device)
+    assert workspace.dtype == torch.uint8 and workspace.is_contiguous()
+    if state is None:
+        state = torch.zeros(LPQLOSS_STATE_FLOATS, dtype=torch.float32, device=b0.device)
+    if p is not None:
+        state[4] = float(p)
+    if q is not None:
+        state[5] = float(q)
+    loss = torch.empty(1, dtype=torch.float32, device=b0.device)
+    check(l.fn2_lpqloss_forward(desc(b0), desc(b1) if b1 is not None else None, d, _ptr(state), _ptr(loss), _ptr(workspace),
+                                workspace.numel(), _stream()))
+    return loss, state
+
+
+def lpqloss_backward(b0, b1=None, *, p_epsilon=0.0, q_epsilon=1e-2, l2_prescale_by_channels=False, normalize_by_num_entries=False,
+                     state, top_diff, out0=None, out1=None, accumulate0=False, accumulate1=False):
+    """LpqLossLayer::Backward_gpu: writes (accumulate: adds) the gradient of each bottom into out0 / out1; None: do not
+    propagate to that bottom.  state: from lpqloss() (it holds p and q); top_diff: the loss weight as a device float tensor.
+    -> (out0, out1)"""
+    d = _lpq_desc(p_epsilon, q_epsilon, l2_prescale_by_channels, normalize_by_num_entries)
+    check(lib().fn2_lpqloss_backward(desc(b0), desc(b1) if b1 is not None else None, d, _ptr(state), _ptr(top_diff),
+                                     desc(out0) if out0 is not None else None, desc(out1) if out1 is not None else None,
+                                     1 if accumulate0 else 0, 1 if accumulate1 else 0, _stream()))
     return out0, out1
 
 
