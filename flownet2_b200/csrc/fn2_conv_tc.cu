@@ -360,7 +360,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                 } else {
 #pragma unroll
                     for (int q = 0; q < 16; q++)
-                        split_store(raw_at(st, (q & 1) ? r1 : r0, 2 * (q >> 2) + ((q >> 1) & 1), t), ah[q], al[q]);
+                        split_store<MODE == TC_CORR>(raw_at(st, (q & 1) ? r1 : r0, 2 * (q >> 2) + ((q >> 1) & 1), t), ah[q], al[q]);
                 }
                 const uint32_t bh = su32(st + A_TILE_BYTES);
                 const uint64_t dbh0 = make_desc_sw128(bh), dbl0 = make_desc_sw128(bh + G::B_TILE_BYTES);
@@ -881,7 +881,7 @@ __global__ void corr_split_kernel(const float* __restrict__ b, long long sn, lon
         float h[4], l[4];
 #pragma unroll
         for (int e = 0; e < 4; e++) {
-            const uint32_t hb = to_tf32(f[e]);
+            const uint32_t hb = to_tf32_nan(f[e]);
             h[e] = __uint_as_float(hb);
             l[e] = __uint_as_float(to_tf32(f[e] - h[e]));
         }

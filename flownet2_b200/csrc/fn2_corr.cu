@@ -16,7 +16,7 @@
 //                fn2_correlation_workspace_bytes reports; a non-null workspace that is too small is an error.
 //   * generic -- every other shape, Correlation1D, and any call without workspace (this file): one CTA per output pixel like
 //                the reference's CorrelateData (:46-114), but the zero padded NHWC copies (:24-42, :447-458) are never
-//                materialised (taps outside the image contribute 0) and the per-displacement reduction is a warp shuffle
+//                materialised (a tap outside the image contributes a * 0) and the per-displacement reduction is a warp shuffle
 //                instead of the reference's serial lane-0 sum (:101-105, which races with the next iteration's
 //                `sum[ch_off] = 0` on post-Volta parts).
 // The backward of both layers is fn2_corr_bwd.cu.
@@ -108,7 +108,11 @@ __global__ void __launch_bounds__(128) corr_generic_kernel(T4 b0, T4 b1, T4 top,
                 const bool inb = (yy >= 0 && yy < H && xx >= 0 && xx < W);
                 const float* ap = patch + (j * g.k + i) * C;
                 if (type == 0) {
-                    if (!inb) continue;                 // a * 0
+                    if (!inb) {
+                        // a * 0, as the reference's zero-padded copy: nothing for a finite a, NaN for a non-finite one
+                        for (int ch = lane; ch < C; ch += 32) acc = fmaf(ap[ch], 0.f, acc);
+                        continue;
+                    }
                     const float* bp = b1.p + b1.off(n, 0, yy, xx);
                     for (int ch = lane; ch < C; ch += 32) acc = fmaf(ap[ch], __ldg(bp + ch * b1.sc), acc);
                 } else if (inb) {

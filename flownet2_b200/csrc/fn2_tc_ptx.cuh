@@ -64,9 +64,15 @@ __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_grou
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 // keeps the compiler from moving accesses of the accumulator registers across the asynchronous MMAs
 __device__ __forceinline__ void reg_fence(float& r) { asm volatile("" : "+f"(r)::"memory"); }
+// x rounded half away from zero to TF32 (11 significant bits), as cvt.rna.tf32.f32 rounds a finite x.  A NaN does not survive
+// it: the rounding add carries the payload of the device's own NaN (0x7fffffff) into the sign bit, giving -0, and turns a NaN
+// with a small payload (0x7f800001) into Inf.  The convolution engines split with it in their MMA inner loop, where the NaN
+// test of to_tf32_nan cost 1.5 % of the FlowNet2 deploy step (H100 80GB HBM3, 700 W).
 __device__ __forceinline__ uint32_t to_tf32(float x) { return (__float_as_uint(x) + 0x1000u) & 0xffffe000u; }
-// weight packing: wp[idx] = v rounded to TF32, wp[per + idx] = the remainder rounded to TF32 (cvt.rna, which unlike
-// to_tf32 keeps a NaN a NaN)
+// to_tf32 that keeps a NaN a NaN (the canonical one: the tensor cores read only the upper 19 bits).  The correlation splits
+// both maps with it, so that a NaN in either bottom reaches the products as in the reference's FP32 code.
+__device__ __forceinline__ uint32_t to_tf32_nan(float x) { return x != x ? 0x7fffffffu : to_tf32(x); }
+// weight packing: wp[idx] = v rounded to TF32, wp[per + idx] = the remainder rounded to TF32 (cvt.rna)
 __device__ __forceinline__ void store_tf32_split(float* wp, long long per, long long idx, float v) {
     uint32_t h, l;
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(h) : "f"(v));
@@ -89,8 +95,11 @@ __device__ __forceinline__ uint64_t make_desc_sw128(uint32_t smem_addr) {
 // A operand of one K step in wgmma register-fragment order: a[4*kk + q] = element (row rq = q&1 ? r1 : r0, column
 // 8*kk + t + 4*(q>>1)) of the K block, split into hi / lo.  Plain layout: the raw tile is K-major SWIZZLE_128B (16-byte
 // chunk c of row r at chunk position c ^ (r & 7)); the 32 lanes of a warp hit 32 different banks.
+// KEEP_NAN: the high part keeps a NaN (to_tf32_nan); the remainder of a non-finite f needs no test, the high part already
+// carries it into every product.
+template <bool KEEP_NAN = false>
 __device__ __forceinline__ void split_store(float f, uint32_t& hi, uint32_t& lo) {
-    const uint32_t h = to_tf32(f);
+    const uint32_t h = KEEP_NAN ? to_tf32_nan(f) : to_tf32(f);
     hi = h;
     lo = to_tf32(f - __uint_as_float(h));
 }
