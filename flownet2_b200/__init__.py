@@ -1,7 +1,7 @@
 """flownet2_b200 -- Hopper-native FlowNet2 forward path.
 
-Python here is only a ctypes front end over the C-ABI in include/fn2.h, fn2_solver.h, fn2_frames.h, fn2_flow.h and fn2_lpq.h
-(libfn2.so: hand-written sm_90a CUDA + the Caffe-surface C++ host).  It mirrors the slice of pycaffe that the reference's
+Python here is only a ctypes front end over the C-ABI in include/fn2.h, fn2_solver.h, fn2_frames.h, fn2_flow.h, fn2_lpq.h and
+fn2_eval.h (libfn2.so: hand-written sm_90a CUDA + the Caffe-surface C++ host).  It mirrors the slice of pycaffe that the reference's
 driver uses (scripts/run-flownet.py:64-98): ``Net(prototxt, weights, phase)``, ``net.inputs``,
 ``net.forward(img0=..., img1=...)``, ``net.blobs[name].data``.
 
@@ -21,7 +21,7 @@ _LIB = None
 TRAIN, TEST = 0, 1
 
 _STRUCTS, _PROTOTYPES, _DEFINES = {}, {}, {}
-for _name in ("fn2.h", "fn2_solver.h", "fn2_frames.h", "fn2_flow.h", "fn2_lpq.h"):
+for _name in ("fn2.h", "fn2_solver.h", "fn2_frames.h", "fn2_flow.h", "fn2_lpq.h", "fn2_eval.h"):
     with open(os.path.join(os.path.dirname(_HERE), "include", _name)) as _f:
         _text = _f.read()
     _s, _p = read_header(_text, _STRUCTS)
@@ -34,6 +34,11 @@ LPQLOSS_STATE_FLOATS = _DEFINES["FN2_LPQLOSS_STATE_FLOATS"]            # device 
 # flow payload formats and flags of fn2_flow_to_tensor (include/fn2_flow.h)
 FLOW_FLO, FLOW_PFM, FLOW_PFM_BE, FLOW_UINT16FLOW = (_DEFINES[n] for n in ("FN2_FLOW_FLO", "FN2_FLOW_PFM", "FN2_FLOW_PFM_BE",
                                                                           "FN2_FLOW_UINT16FLOW"))
+# the per-pair record of fn2_flow_error (include/fn2_eval.h): its field names, lower case, in record order
+FLOW_ERROR_FIELDS = tuple(sorted((k[len("FN2_FLOW_ERROR_"):].lower() for k in _DEFINES
+                                 if k.startswith("FN2_FLOW_ERROR_") and k != "FN2_FLOW_ERROR_FIELDS"),
+                                key=lambda f: _DEFINES["FN2_FLOW_ERROR_" + f.upper()]))
+assert len(FLOW_ERROR_FIELDS) == _DEFINES["FN2_FLOW_ERROR_FIELDS"]
 
 
 class Fn2Error(RuntimeError):

@@ -36,6 +36,7 @@ SOURCES = [
     ("fn2_train.cu", []),
     ("fn2_loss.cu", []),
     ("fn2_solver.cu", ["-fmad=false"]),     # bit-exact update, see file header
+    ("fn2_eval.cu", ["-fmad=false"]),       # per-pixel EPE restated exactly in float32, see file header
     ("caffe/proto.cpp", []),
     ("caffe/blob.cpp", []),
     ("caffe/layers.cpp", []),

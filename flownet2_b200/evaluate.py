@@ -1,0 +1,259 @@
+"""Score a net against ground-truth flow: end-point error, outlier rate and Sintel speed bands over an image-and-flow list.
+
+    python -m flownet2_b200.evaluate weights.caffemodel models/FlowNet2_deploy.prototxt.template val.txt [--batch B]
+                                     [--per-pair out.tsv] [--gpu G]
+
+The list is the train command's: one ``img0 img1 flow`` line per pair (data.read_list; an occlusion field is refused), flows as
+.flo or 'PF' PFM of either byte order.  Frame sizes may differ from line to line; a flow must have its frames' size.  The
+pairs run through flownet2_b200.run's pipeline (one net per frame size, the weights read once, decoding and copies overlapped
+with the forwards); only what happens to each batch's flow differs.  The reader pool reads each ground-truth payload into a
+pinned slot beside the frames, the copy stream moves it to the device, and on the net's stream it is converted
+(fn2_flow_to_tensor, the file's floats unquantised) and scored against the prediction by fn2_flow_error (include/fn2_eval.h).
+Only the per-pair records come back to the host; the padded pairs of a size's last batch are dropped.
+
+Metrics.  A ground-truth pixel is valid when both components are finite and at most 1e9 in absolute value.  EPE is the
+float32 sqrt(du^2 + dv^2) of the prediction minus the ground truth; a valid pixel whose prediction is not finite is counted in
+nonfinite_px and left out of every average.  Printed as one JSON line:
+  epe            pooled over every counted pixel of the list (the Sintel and Middlebury convention);
+  epe_pair_mean  the mean of the per-pair EPE over the pairs with a counted pixel (the per-image convention, e.g. KITTI's);
+  fl_percent     counted pixels with EPE > 3 px and EPE > 5 % of |gt| (KITTI's Fl), in percent;
+  s0-10, s10-40, s40+   pooled EPE over the pixels whose |gt| is in [0, 10), [10, 40), [40, inf) (null when a band is empty);
+and pairs, valid_px, invalid_px, nonfinite_px, batch, ranks and wall (s).  --per-pair writes a TSV row per list line: where,
+img0, img1, flow, valid pixels, EPE, Fl %.  A list with no valid pixel is refused (status 2).  When a prediction is not finite
+its pairs are named on stderr and the status is 1, as in run.
+
+Under torchrun (WORLD_SIZE, RANK, LOCAL_RANK) rank r scores the lines i with i % WORLD_SIZE == r; rank 0 gathers every rank's
+records, puts them back in list order (combine_shards) and prints the summary, so at --batch 1 it does not depend on the
+number of ranks.  At larger batches a pair's flow, and so its record, can differ in the last bits (see run).
+"""
+import argparse
+import json
+import os
+import sys
+import time
+
+import numpy as np
+
+from . import FLOW_ERROR_FIELDS
+from .data import flow_header, read_flow_payload, read_list
+from .run import RunError, check_inputs, probe_pairs, run_groups, shard
+
+FIELD = {name: i for i, name in enumerate(FLOW_ERROR_FIELDS)}
+BANDS = (("s0-10", "n_s0_10", "sum_s0_10"), ("s10-40", "n_s10_40", "sum_s10_40"), ("s40+", "n_s40", "sum_s40"))
+PAYLOAD_PX_BYTES = 12                      # the larger payload per pixel: PFM's three floats (.flo holds two)
+
+
+def probe_samples(samples):
+    """Sets each sample's frame size and channels (run.probe_pairs) and its flow header; refuses missing or unreadable
+    files, unknown flow suffixes and a flow whose size differs from its frames', naming the list line."""
+    probe_pairs(samples)
+    for s in samples:
+        try:
+            fh = flow_header(s.flow)
+        except RunError as e:
+            raise RunError("%s: %s" % (s.where, e))
+        if (fh.width, fh.height) != s.size:
+            raise RunError("%s: %s is %dx%d but its frames are %dx%d" % (s.where, s.flow, fh.width, fh.height, s.size[0], s.size[1]))
+        s.flow_header = fh
+
+
+class Scores(object):
+    """evaluate's per-batch sink for run._group_batches (the interface is described at run.FlowFiles): the ground-truth payloads
+    ride in the frames' slots, are converted on the net's stream before the forward, and each batch's flow is scored on the
+    net's stream; the records of the real pairs land in records[sample.index]."""
+
+    def __init__(self, n):
+        self.records = np.full((n, len(FLOW_ERROR_FIELDS)), np.nan)
+        self.stats = {"collect": 0.0}
+
+    def payload_bytes(self, batch, H, W):
+        return batch * H * W * PAYLOAD_PX_BYTES
+
+    def read_payload(self, p, out):
+        try:
+            read_flow_payload(p.flow, p.flow_header, out[:p.flow_header.nbytes])
+        except (OSError, RunError) as e:
+            raise RunError("%s: %s" % (p.where, e))
+
+    def bind(self, torch, batch, H, W, flow_dev):
+        from . import ops
+        self.ops = ops
+        fields = len(FLOW_ERROR_FIELDS)
+        self.pred = [f.permute(0, 3, 1, 2) for f in flow_dev]                       # (B, 2, H, W) views of the NHWC flow
+        self.gt = [torch.empty((batch, 2, H, W), device="cuda") for _ in range(2)]
+        self.dev = [torch.empty((batch, fields), dtype=torch.float64, device="cuda") for _ in range(2)]
+        self.host = [torch.empty((batch, fields), dtype=torch.float64).pin_memory() for _ in range(2)]
+        self.workspace = torch.empty(max(ops.flow_error_workspace_bytes(batch, H, W), 8), dtype=torch.uint8, device="cuda")
+
+    def stage(self, pairs, s, payload, stride):
+        """On the net's stream: pair i's payload, at payload[i * stride], into gt[s][i] (formats may differ per pair)."""
+        for i, p in enumerate(pairs):
+            fh = p.flow_header
+            self.ops.flow_to_tensor(payload[i * stride:i * stride + fh.nbytes], fh.format, 0, self.gt[s][i:i + 1])
+
+    def score(self, s):
+        self.ops.flow_error(self.pred[s], self.gt[s], out=self.dev[s], workspace=self.workspace)
+
+    def take(self, pairs, s, n_real):
+        t0 = time.perf_counter()
+        rec = self.host[s].numpy()
+        for i, p in enumerate(pairs[:n_real]):
+            self.records[p.index] = rec[i]
+        self.stats["collect"] += time.perf_counter() - t0
+
+
+def combine_shards(shards):
+    """Per-rank record arrays, rank r holding list lines r, r + world, ... in order (run.shard) -> one array in list order."""
+    world = len(shards)
+    out = np.empty((sum(len(s) for s in shards),) + tuple(np.shape(shards[0])[1:]), np.float64)
+    for r, s in enumerate(shards):
+        out[r::world] = s
+    return out
+
+
+def _ratio(num, den):
+    return float(num / den) if den > 0 else None
+
+
+def summarize(records, pixels, name):
+    """The summary of per-pair records in list order ((n, FIELDS) float64) and each pair's pixel count -> dict; refuses a
+    list with no valid pixel, naming it."""
+    records = np.asarray(records, np.float64)
+    col = lambda f: records[:, FIELD[f]]
+    valid, nonfinite = col("valid"), col("nonfinite")
+    if not len(records) or valid.sum() == 0:
+        raise RunError("%s: no ground-truth pixel is valid in any of its %d pairs" % (name, len(records)))
+    counted = valid - nonfinite
+    has = counted > 0
+    out = {"pairs": len(records), "valid_px": int(valid.sum()), "invalid_px": int(np.sum(pixels) - valid.sum()),
+           "nonfinite_px": int(nonfinite.sum()),
+           "epe": _ratio(col("epe_sum").sum(), counted.sum()),
+           "epe_pair_mean": float(np.mean(col("epe_sum")[has] / counted[has])) if has.any() else None,
+           "fl_percent": _ratio(100.0 * col("outliers").sum(), counted.sum())}
+    for key, n, s in BANDS:
+        out[key] = _ratio(col(s).sum(), col(n).sum())
+    return out
+
+
+def pair_rows(records):
+    """-> per pair (valid pixels, EPE, Fl %), NaN where no pixel counts."""
+    rows = []
+    for r in np.asarray(records, np.float64):
+        counted = r[FIELD["valid"]] - r[FIELD["nonfinite"]]
+        epe = r[FIELD["epe_sum"]] / counted if counted > 0 else float("nan")
+        fl = 100.0 * r[FIELD["outliers"]] / counted if counted > 0 else float("nan")
+        rows.append((int(r[FIELD["valid"]]), epe, fl))
+    return rows
+
+
+def write_per_pair(path, samples, records):
+    with open(path, "w") as f:
+        f.write("where\timg0\timg1\tflow\tvalid\tepe\tfl_percent\n")
+        for s, (valid, epe, fl) in zip(samples, pair_rows(records)):
+            f.write("%s\t%s\t%s\t%s\t%d\t%.9g\t%.9g\n" % (s.where, s.img0, s.img1, s.flow, valid, epe, fl))
+
+
+def not_finite(samples, records):
+    """The samples with a valid pixel whose prediction is not finite."""
+    return [s for s, r in zip(samples, records) if r[FIELD["nonfinite"]] > 0]
+
+
+def _list_name(samples):
+    return samples[0].where.rsplit(":", 1)[0] if samples else "the list"
+
+
+def _score(caffemodel, template, samples, batch, device, threads):
+    """-> (records in the samples' order, per-stage busy seconds, number of sizes)."""
+    t0 = time.perf_counter()
+    check_inputs(caffemodel, template, batch)
+    probe_samples(samples)
+    for i, s in enumerate(samples):
+        s.index = i
+    sink = Scores(len(samples))
+    stats, sizes = run_groups(caffemodel, template, samples, batch, device, threads, sink, t0)
+    return sink.records, stats, sizes
+
+
+def evaluate(caffemodel, template, samples, batch=1, device=0, threads=None):
+    """Scores the net on every data.Sample -> (summary dict, per-pair records): the summary of summarize() plus batch, sizes,
+    wall (s), per-stage busy seconds and the samples whose prediction is not finite; the records are an (n, FIELDS) float64
+    array in the samples' order (fields: flownet2_b200.FLOW_ERROR_FIELDS)."""
+    t0 = time.perf_counter()
+    records, stats, sizes = _score(caffemodel, template, samples, batch, device, threads)
+    summary = summarize(records, [s.size[0] * s.size[1] for s in samples], _list_name(samples))
+    summary.update({"batch": batch, "sizes": sizes, "wall": time.perf_counter() - t0, "busy": stats,
+                    "not_finite": [s.where for s in not_finite(samples, records)]})
+    return summary, records
+
+
+def gather_records(local, n_total, world, rank):
+    """Every rank's (n_r, cols) records -> the list-order array on rank 0 (None elsewhere): one gather of equal, zero-padded
+    float64 tensors on the process group's device, then combine_shards."""
+    import torch
+    import torch.distributed as dist
+    mx = (n_total + world - 1) // world
+    dev = "cuda" if dist.get_backend() == "nccl" else "cpu"
+    t = torch.zeros((mx, local.shape[1]), dtype=torch.float64, device=dev)
+    t[:len(local)] = torch.from_numpy(local)
+    got = [torch.empty_like(t) for _ in range(world)] if rank == 0 else None
+    dist.gather(t, got, dst=0)
+    if rank != 0:
+        return None
+    return combine_shards([g[:len(range(r, n_total, world))].cpu().numpy() for r, g in enumerate(got)])
+
+
+def parse_args(argv):
+    ap = argparse.ArgumentParser(prog="python -m flownet2_b200.evaluate", description=__doc__.split("\n\n")[0])
+    ap.add_argument("caffemodel", help="weights: .caffemodel or .caffemodel.h5")
+    ap.add_argument("deployproto", help="deploy prototxt template, e.g. models/FlowNet2_deploy.prototxt.template")
+    ap.add_argument("listfile", help="list of 'img0 img1 flow' lines, flows as .flo or .pfm")
+    ap.add_argument("--batch", type=int, default=1, help="pairs per forward (records reproduce single-pair runs only at 1)")
+    ap.add_argument("--per-pair", metavar="TSV", help="write one row per list line: where, img0, img1, flow, valid, EPE, Fl %%")
+    ap.add_argument("--gpu", type=int, default=0, help="device to use without torchrun")
+    return ap.parse_args(argv)
+
+
+def main(argv=None):
+    a = parse_args(sys.argv[1:] if argv is None else argv)
+    world, rank = int(os.environ.get("WORLD_SIZE", "1")), int(os.environ.get("RANK", "0"))
+    device = int(os.environ.get("LOCAL_RANK", a.gpu)) if "WORLD_SIZE" in os.environ else a.gpu
+    t0 = time.perf_counter()
+    dist = None
+    try:
+        check_inputs(a.caffemodel, a.deployproto, a.batch)
+        samples = read_list(a.listfile)
+        if not samples:
+            raise RunError("%s: the list holds no pairs" % a.listfile)
+        if world > 1:
+            import torch
+            import torch.distributed as dist
+            torch.cuda.set_device(device)
+            dist.init_process_group("nccl")
+        mine = shard(samples, world, rank)
+        local = np.empty((0, len(FLOW_ERROR_FIELDS) + 1))               # this rank's records, each pair's pixel count last
+        if mine:
+            records = _score(a.caffemodel, a.deployproto, mine, a.batch, device, None)[0]
+            local = np.concatenate([records, [[s.size[0] * s.size[1]] for s in mine]], axis=1)
+        full = gather_records(local, len(samples), world, rank) if world > 1 else local
+        if rank != 0:
+            return 1 if np.any(local[:, FIELD["nonfinite"]] > 0) else 0
+        records, pixels = full[:, :-1], full[:, -1]
+        summary = summarize(records, pixels, a.listfile)
+    except RunError as e:
+        sys.stderr.write("error: %s\n" % e)
+        return 2
+    finally:
+        if dist is not None and dist.is_initialized():
+            dist.destroy_process_group()
+    summary.update({"batch": a.batch, "ranks": world, "wall": time.perf_counter() - t0})
+    if a.per_pair:
+        write_per_pair(a.per_pair, samples, records)
+    bad = not_finite(samples, records)
+    for s in bad:
+        sys.stderr.write("%s: the flow of %s %s is not finite\n" % (s.where, s.img0, s.img1))
+    print(json.dumps(summary), flush=True)
+    return 1 if bad else 0
+
+
+if __name__ == "__main__":
+    sys.exit(main())

@@ -10,7 +10,7 @@ import ctypes as C
 
 import torch
 
-from . import LPQLOSS_STATE_FLOATS, check, fn2_conv_desc, fn2_l1loss_desc, fn2_lpqloss_desc, fn2_tensor, lib
+from . import FLOW_ERROR_FIELDS, LPQLOSS_STATE_FLOATS, check, fn2_conv_desc, fn2_l1loss_desc, fn2_lpqloss_desc, fn2_tensor, lib
 
 
 def desc(t):
@@ -434,3 +434,23 @@ def flow_to_tensor(payload, format, flags, dst):
     assert payload.is_cuda and payload.is_contiguous(), "need a dense CUDA payload"
     check(lib().fn2_flow_to_tensor(payload.data_ptr(), int(format), int(flags), desc(dst), _stream()))
     return dst
+
+
+def flow_error_workspace_bytes(N, H, W):
+    return _size(lib().fn2_flow_error_workspace_bytes, N, H, W)
+
+
+def flow_error(pred, gt, out=None, workspace=None):
+    """Per-pair scores of a predicted flow against ground truth (include/fn2_eval.h): pred and gt are float32 (N, 2, H, W) CUDA
+    views of any strides -> out, an (N, len(FLOW_ERROR_FIELDS)) float64 CUDA tensor (a new one if None) with the fields of
+    FLOW_ERROR_FIELDS.  workspace: a uint8 CUDA tensor whose bytes are the workspace (default: one of the reported size)."""
+    N, _, H, W = pred.shape
+    if workspace is None:
+        workspace = _ws(flow_error_workspace_bytes(N, H, W), pred.device)
+    assert workspace.dtype == torch.uint8 and workspace.is_contiguous()
+    if out is None:
+        out = torch.empty((N, len(FLOW_ERROR_FIELDS)), dtype=torch.float64, device=pred.device)
+    assert out.dtype == torch.float64 and out.is_contiguous() and out.numel() == N * len(FLOW_ERROR_FIELDS)
+    check(lib().fn2_flow_error(desc(pred), desc(gt), C.cast(out.data_ptr(), C.POINTER(C.c_double)), _ptr(workspace),
+                               workspace.numel(), _stream()))
+    return out

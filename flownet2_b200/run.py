@@ -234,25 +234,69 @@ def write_flo(path, flow_hw2):
 # ------------------------------------------------------------------------------------------------
 # The pipeline
 # ------------------------------------------------------------------------------------------------
-def _group_batches(torch, F, net, size, pairs, batch, pool, stats, bad):
-    """Runs one size's pairs through `net`, B per forward, with decode, copies, forward and writes overlapped."""
+def _align(n, a=16):
+    return (n + a - 1) // a * a
+
+
+class FlowFiles(object):
+    """run's per-batch sink: each pair's flow goes to the host and into its .flo file; a pair whose flow is not finite is named
+    on stderr and kept in `bad`.
+
+    The sink interface of _group_batches: payload_bytes(batch, H, W) pinned bytes per slot beyond the frames, read_payload(p,
+    out) the host read of one pair's part of them (on the pool), stage(...) the net stream's use of them before the forward;
+    bind(...) allocates dev[s] / host[s] for one frame size, score(s) runs on the net's stream after the flow is in
+    flow_dev[s] and fills dev[s], which then goes to host[s] on the copy-back stream, and take(pairs, s, n_real)
+    consumes host[s] on the writer thread."""
+
+    def __init__(self):
+        self.bad = []
+        self.stats = {"write": 0.0}
+
+    def payload_bytes(self, batch, H, W):
+        return 0
+
+    read_payload = stage = None
+
+    def bind(self, torch, batch, H, W, flow_dev):
+        self.dev = flow_dev
+        self.host = [torch.empty((batch, H, W, 2)).pin_memory() for _ in range(2)]
+
+    def score(self, s):
+        pass
+
+    def take(self, pairs, s, n_real):
+        t0 = time.perf_counter()
+        flows = self.host[s].numpy()
+        for i, p in enumerate(pairs[:n_real]):
+            if not np.isfinite(flows[i]).all():
+                self.bad.append(p)
+                sys.stderr.write("%s: the flow of %s %s is not finite\n" % (p.where, p.img0, p.img1))
+            write_flo(p.out, flows[i])
+        self.stats["write"] += time.perf_counter() - t0
+
+
+def _group_batches(torch, net, size, pairs, batch, pool, stats, sink):
+    """Runs one size's pairs through `net`, B per forward, with decode, copies, forward and the sink's work overlapped."""
     W, H = size
     in0, in1 = net.inputs[:2]
     todo = batches(pairs, batch)
     px = batch * H * W                                             # pixels of one input's frames; bytes: px * K, K <= 4
-    pin = [torch.empty(2 * px * 4, dtype=torch.uint8).pin_memory() for _ in range(2)]
-    dev = [torch.empty(2 * px * 4, dtype=torch.uint8, device="cuda") for _ in range(2)]
+    pay_off = _align(2 * px * 4)                                   # the sink's payload follows the frames
+    pay_bytes = sink.payload_bytes(batch, H, W)
+    pay_one = pay_bytes // batch
+    pin = [torch.empty(pay_off + pay_bytes, dtype=torch.uint8).pin_memory() for _ in range(2)]
+    dev = [torch.empty(pay_off + pay_bytes, dtype=torch.uint8, device="cuda") for _ in range(2)]
     flow_dev = [torch.empty((batch, H, W, 2), device="cuda") for _ in range(2)]
-    flow_host = [torch.empty((batch, H, W, 2)).pin_memory() for _ in range(2)]
+    sink.bind(torch, batch, H, W, flow_dev)
     net_stream = torch.cuda.ExternalStream(net.stream)
     h2d_stream, d2h_stream = torch.cuda.Stream(), torch.cuda.Stream()
     ev = lambda: torch.cuda.Event(enable_timing=True)
     ev_h2d = [torch.cuda.Event() for _ in range(2)]                # pin[s] copied to dev[s]
     ev_used = [torch.cuda.Event() for _ in range(2)]               # the net has converted dev[s]
-    ev_flow = [torch.cuda.Event() for _ in range(2)]               # flow_dev[s] holds the batch's flow
-    ev_d2h = [torch.cuda.Event() for _ in range(2)]                # flow_host[s] holds it
+    ev_flow = [torch.cuda.Event() for _ in range(2)]               # sink.dev[s] holds the batch's result
+    ev_d2h = [torch.cuda.Event() for _ in range(2)]                # sink.host[s] holds it
     timing = []                                                    # per batch: (h2d, forward, d2h) event pairs
-    writes = [None, None]
+    takes = [None, None]
     kinds = [None] * len(todo)
 
     def channels_of(b):
@@ -269,26 +313,28 @@ def _group_batches(torch, F, net, size, pairs, batch, pool, stats, bad):
         pin[s][o:o + H * W * k].numpy()[:] = a.reshape(-1)
         return time.perf_counter() - t0
 
+    def read_one(p, s, i):
+        t0 = time.perf_counter()
+        o = pay_off + i * pay_one
+        sink.read_payload(p, pin[s][o:o + pay_one].numpy())
+        return time.perf_counter() - t0
+
     def decode(k_batch):
         s = k_batch & 1
         b = todo[k_batch][0]
         kinds[k_batch] = channels_of(b)
         ev_h2d[s].synchronize()                                    # the copy out of pin[s] two batches ago is done
-        return [pool.submit(decode_one, p, j, s, i, kinds[k_batch]) for i, p in enumerate(b) for j in (0, 1)]
+        futs = [pool.submit(decode_one, p, j, s, i, kinds[k_batch]) for i, p in enumerate(b) for j in (0, 1)]
+        if pay_bytes:
+            futs += [pool.submit(read_one, p, s, i) for i, p in enumerate(b)]
+        return futs
 
-    def write(k_batch, s, n_real):
+    def take(k_batch, s, n_real):
         ev_d2h[s].synchronize()
-        t0 = time.perf_counter()
-        flows = flow_host[s].numpy()
-        for i, p in enumerate(todo[k_batch][0][:n_real]):
-            if not np.isfinite(flows[i]).all():
-                bad.append(p)
-                sys.stderr.write("%s: the flow of %s %s is not finite\n" % (p.where, p.img0, p.img1))
-            write_flo(p.out, flows[i])
-        stats["write"] += time.perf_counter() - t0
+        sink.take(todo[k_batch][0], s, n_real)
 
     decoding = decode(0)
-    with ThreadPoolExecutor(max_workers=1) as writer:
+    with ThreadPoolExecutor(max_workers=1) as taker:
         for kb, (b, n_real) in enumerate(todo):
             s, k = kb & 1, kinds[kb]
             stats["decode"] += sum(f.result() for f in decoding)
@@ -297,6 +343,8 @@ def _group_batches(torch, F, net, size, pairs, batch, pool, stats, bad):
                 h2d_stream.wait_event(ev_used[s])                  # dev[s] was converted two batches ago
                 t[0].record(h2d_stream)
                 dev[s][:2 * px * k].copy_(pin[s][:2 * px * k], non_blocking=True)
+                if pay_bytes:
+                    dev[s][pay_off:].copy_(pin[s][pay_off:], non_blocking=True)
                 t[1].record(h2d_stream)
                 ev_h2d[s].record(h2d_stream)
             if kb + 1 < len(todo):
@@ -306,23 +354,26 @@ def _group_batches(torch, F, net, size, pairs, batch, pool, stats, bad):
                 t[2].record(net_stream)
                 net.set_input_image_device(in0, dev[s].data_ptr(), k)
                 net.set_input_image_device(in1, dev[s].data_ptr() + px * k, k)
+                if pay_bytes:
+                    sink.stage(b, s, dev[s][pay_off:], pay_one)
                 ev_used[s].record(net_stream)
                 net.forward_async()
-                net_stream.wait_event(ev_d2h[s])                   # flow_dev[s] has left for the host two batches ago
+                net_stream.wait_event(ev_d2h[s])                   # sink.dev[s] has left for the host two batches ago
                 net.get_blob_nhwc_device("predict_flow_final", flow_dev[s].data_ptr())
+                sink.score(s)
                 t[3].record(net_stream)
                 ev_flow[s].record(net_stream)
-            if writes[s] is not None:
-                writes[s].result()                                 # flow_host[s] written out two batches ago
+            if takes[s] is not None:
+                takes[s].result()                                  # sink.host[s] taken two batches ago
             with torch.cuda.stream(d2h_stream):
                 d2h_stream.wait_event(ev_flow[s])
                 t[4].record(d2h_stream)
-                flow_host[s].copy_(flow_dev[s], non_blocking=True)
+                sink.host[s].copy_(sink.dev[s], non_blocking=True)
                 t[5].record(d2h_stream)
                 ev_d2h[s].record(d2h_stream)
             timing.append(t)
-            writes[s] = writer.submit(write, kb, s, n_real)
-        for w in writes:
+            takes[s] = taker.submit(take, kb, s, n_real)
+        for w in takes:
             if w is not None:
                 w.result()
     torch.cuda.synchronize()
@@ -332,40 +383,56 @@ def _group_batches(torch, F, net, size, pairs, batch, pool, stats, bad):
         stats["d2h"] += t[4].elapsed_time(t[5]) * 1e-3
 
 
-def run(caffemodel, template, pairs, batch=1, device=0, threads=None):
-    """Flow of every Pair into its .flo file -> summary dict: pairs, sizes, nets, wall (s), per-stage busy seconds (build:
-    checking the inputs, reading the weights and constructing the nets; decode: host, summed over the pool's threads;
-    h2d / forward / d2h: device; write: host) and the pairs whose flow is not finite."""
-    import torch
-    import flownet2_b200 as F
-    t0 = time.perf_counter()
+def check_inputs(caffemodel, template, batch):
+    """Refuses a batch below 1 and a missing caffemodel or template, before anything is read."""
     if batch < 1:
         raise RunError("--batch must be at least 1, got %d" % batch)
     for path, what in ((caffemodel, "caffemodel"), (template, "deploy prototxt template")):
         if not os.path.isfile(path):
             raise RunError("%s: no such %s" % (path, what))
-    probe_pairs(pairs)
+
+
+def run_groups(caffemodel, template, pairs, batch, device, threads, sink, t0):
+    """The pipeline of run and evaluate over probed pairs (probe_pairs): one net per frame size, the weights read once, each
+    size's batches through _group_batches into `sink` -> (per-stage busy seconds, number of sizes).  The build time counts
+    from t0, when the caller started checking its inputs."""
+    import torch
+    import flownet2_b200 as F
     torch.cuda.set_device(device)
-    stats = {k: 0.0 for k in ("build", "decode", "h2d", "forward", "d2h", "write")}
+    stats = {k: 0.0 for k in ("build", "decode", "h2d", "forward", "d2h")}
+    stats.update(sink.stats)
     with open(template) as f:
         text = f.read()
     with open(caffemodel, "rb") as f:
         weights = f.read()
     stats["build"] += time.perf_counter() - t0
-    bad, groups = [], group_by_size(pairs)
+    groups = group_by_size(pairs)
     with ThreadPoolExecutor(max_workers=threads or min(16, os.cpu_count() or 4)) as pool:
         for size, group in groups:
             tb = time.perf_counter()
             net = F.Net(F.fill_template(text, size[0], size[1]), weights, F.TEST, batch=batch)
             stats["build"] += time.perf_counter() - tb
             try:
-                _group_batches(torch, F, net, size, group, batch, pool, stats, bad)
+                _group_batches(torch, net, size, group, batch, pool, stats, sink)
             finally:
                 del net
                 gc.collect()                                       # the net's blob views refer back to it: free it now
                 torch.cuda.empty_cache()
-    return {"pairs": len(pairs), "sizes": len(groups), "nets": len(groups), "batch": batch, "wall": time.perf_counter() - t0,
-            "busy": stats, "not_finite": [p.where for p in bad]}
+    stats.update(sink.stats)
+    return stats, len(groups)
+
+
+def run(caffemodel, template, pairs, batch=1, device=0, threads=None):
+    """Flow of every Pair into its .flo file -> summary dict: pairs, sizes, nets, wall (s), per-stage busy seconds (build:
+    checking the inputs, reading the weights and constructing the nets; decode: host, summed over the pool's threads;
+    h2d / forward / d2h: device; write: host) and the pairs whose flow is not finite."""
+    t0 = time.perf_counter()
+    check_inputs(caffemodel, template, batch)
+    probe_pairs(pairs)
+    sink = FlowFiles()
+    stats, sizes = run_groups(caffemodel, template, pairs, batch, device, threads, sink, t0)
+    return {"pairs": len(pairs), "sizes": sizes, "nets": sizes, "batch": batch, "wall": time.perf_counter() - t0,
+            "busy": stats, "not_finite": [p.where for p in sink.bad]}
 
 
 def parse_args(argv):
