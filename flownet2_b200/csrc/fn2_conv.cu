@@ -297,7 +297,9 @@ __global__ void __launch_bounds__(256) conv_tiny_kernel(T4 in, const float* __re
 //   conv_pf3_warp_kernel:  3x3 / stride 1, larger Ci (the other predict_flow layers) -- one warp per 4 outputs of a row
 //   conv_pf_warp_kernel:   other shapes with larger Ci -- one warp per output pixel, lanes stride the channel vectors,
 //                          shuffle reduce
-// Channels [Ci, 4*C4) are blob padding: their weights are zero (the padding itself is finite, the arena is zero-filled).
+// Channels [Ci, 4*C4) of a pixel are blob padding or a neighbouring view's channels: their weights are zero.  Under the guard
+// promise (fn2_conv_desc.input_guard_bytes) they are finite, and the kernels read them against those zeros; without it
+// (MASK) the kernels select 0 for them, since 0 * NaN is NaN.
 __device__ __forceinline__ void pf_stage_weights(float2* wsm, const float* __restrict__ wp, int taps, int Ci, int C4) {
     const int cp = C4 * 4;
     for (int i = threadIdx.x; i < taps * cp; i += blockDim.x) {
@@ -306,13 +308,21 @@ __device__ __forceinline__ void pf_stage_weights(float2* wsm, const float* __res
     }
     __syncthreads();
 }
+// v with the lanes from `real` on set to 0: real = the channels of its float4 group that lie below Ci (>= 4 for every group
+// but the last when Ci % 4 != 0)
+__device__ __forceinline__ float4 pf_lanes(float4 v, int real) {
+    v.y = real > 1 ? v.y : 0.f;
+    v.z = real > 2 ? v.z : 0.f;
+    v.w = real > 3 ? v.w : 0.f;
+    return v;
+}
 __device__ __forceinline__ void pf_store(const T4& out, const ConvP& p, const float* __restrict__ bias, int n, int oy, int ox, float a0, float a1) {
     if (p.has_bias) { a0 += __ldg(bias); a1 += __ldg(bias + 1); }
     if (p.relu) { a0 = a0 > 0 ? a0 : a0 * p.slope; a1 = a1 > 0 ? a1 : a1 * p.slope; }
     out.p[out.off(n, 0, oy, ox)] = a0;
     out.p[out.off(n, 1, oy, ox)] = a1;
 }
-template <int C4>
+template <int C4, bool MASK>
 __global__ void __launch_bounds__(256) conv_pf_thread_kernel(T4 in, const float* __restrict__ wp, const float* __restrict__ bias, T4 out, ConvP p) {
     extern __shared__ float2 pf_wsm[];
     pf_stage_weights(pf_wsm, wp, p.kh * p.kw, p.Ci, C4);
@@ -332,7 +342,7 @@ __global__ void __launch_bounds__(256) conv_pf_thread_kernel(T4 in, const float*
                 const float4* w = reinterpret_cast<const float4*>(pf_wsm + (r * p.kw + s) * C4 * 4);
 #pragma unroll
                 for (int q = 0; q < C4; q++) {
-                    const float4 a = __ldg(ip + q);
+                    const float4 a = MASK && q == C4 - 1 ? pf_lanes(__ldg(ip + q), p.Ci - 4 * q) : __ldg(ip + q);
                     const float4 w01 = w[2 * q], w23 = w[2 * q + 1];       // (c0.o0, c0.o1, c1.o0, c1.o1), (c2.., c3..)
                     a0 = fmaf(a.x, w01.x, a0); a1 = fmaf(a.x, w01.y, a1);
                     a0 = fmaf(a.y, w01.z, a0); a1 = fmaf(a.y, w01.w, a1);
@@ -344,7 +354,8 @@ __global__ void __launch_bounds__(256) conv_pf_thread_kernel(T4 in, const float*
         pf_store(out, p, bias, n, oy, ox, a0, a1);
     }
 }
-__global__ void __launch_bounds__(256) conv_pf_warp_kernel(T4 in, const float* __restrict__ wp, const float* __restrict__ bias, T4 out, ConvP p, int C4) {
+template <bool MASK>
+__device__ __forceinline__ void pf_warp(const T4& in, const float* __restrict__ wp, const float* __restrict__ bias, const T4& out, const ConvP& p, int C4) {
     extern __shared__ float2 pf_wsm[];
     pf_stage_weights(pf_wsm, wp, p.kh * p.kw, p.Ci, C4);
     const long long M = (long long)p.N * p.Ho * p.Wo;
@@ -366,7 +377,7 @@ __global__ void __launch_bounds__(256) conv_pf_warp_kernel(T4 in, const float* _
                 const float4* w = reinterpret_cast<const float4*>(pf_wsm + (long long)(r * p.kw + s) * C4 * 4);
 #pragma unroll 2
                 for (int q = lane; q < C4; q += 32) {
-                    const float4 a = __ldg(ip + q);
+                    const float4 a = MASK ? pf_lanes(__ldg(ip + q), p.Ci - 4 * q) : __ldg(ip + q);
                     const float4 w01 = w[2 * q], w23 = w[2 * q + 1];
                     a0 = fmaf(a.x, w01.x, a0); a1 = fmaf(a.x, w01.y, a1);
                     a0 = fmaf(a.y, w01.z, a0); a1 = fmaf(a.y, w01.w, a1);
@@ -388,7 +399,7 @@ __global__ void __launch_bounds__(256) conv_pf_warp_kernel(T4 in, const float* _
 // input halo at (bx*32 - pw, by*8 - ph), fetched with fully coalesced 128-bit loads (a thread per output pixel would read
 // 64..128-byte pixels at a 64..128-byte lane stride: 16 L1 wavefronts per load instruction).  Halo pixels outside the input
 // are zero.
-template <int C4>
+template <int C4, bool MASK>
 __global__ void __launch_bounds__(256) conv_pf3_tile_kernel(T4 in, const float* __restrict__ wp, const float* __restrict__ bias, T4 out, ConvP p) {
     extern __shared__ float2 pf_wsm[];
     constexpr int TW = 32, TH = 8, HW = TW + 2, HH = TH + 2, PS = C4 + 1;         // PS: pixel stride in float4 (odd: no bank conflicts)
@@ -406,6 +417,7 @@ __global__ void __launch_bounds__(256) conv_pf3_tile_kernel(T4 in, const float* 
             const int ix = x0 + px_, iy = y0 + py_;
             float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
             if (ix >= 0 && ix < p.W && iy >= 0 && iy < p.H) v = __ldg(reinterpret_cast<const float4*>(in.p + in.off(n, 0, iy, ix)) + q);
+            if (MASK) v = pf_lanes(v, p.Ci - 4 * q);
             tile[(py_ * HW + px_) * PS + q] = v;
         }
         __syncthreads();
@@ -436,7 +448,8 @@ __global__ void __launch_bounds__(256) conv_pf3_tile_kernel(T4 in, const float* 
 
 // one warp per PX = 4 consecutive output pixels of a row: the 6 input columns and the weights of a kernel row are loaded
 // once for the four of them (shared memory bandwidth for the weights was the limit of the one-pixel version)
-__global__ void __launch_bounds__(256) conv_pf3_warp_kernel(T4 in, const float* __restrict__ wp, const float* __restrict__ bias, T4 out, ConvP p, int C4) {
+template <bool MASK>
+__device__ __forceinline__ void pf3_warp(const T4& in, const float* __restrict__ wp, const float* __restrict__ bias, const T4& out, const ConvP& p, int C4) {
     extern __shared__ float2 pf_wsm[];
     pf_stage_weights(pf_wsm, wp, 9, p.Ci, C4);
     constexpr int PX = 4;
@@ -473,6 +486,10 @@ __global__ void __launch_bounds__(256) conv_pf3_warp_kernel(T4 in, const float* 
 #pragma unroll
                 for (int c = 0; c < PX + 2; c++)
                     a[c] = colok[c] ? __ldg(rowp[r] + col0 + c * px4 + q) : make_float4(0.f, 0.f, 0.f, 0.f);
+                if (MASK) {
+#pragma unroll
+                    for (int c = 0; c < PX + 2; c++) a[c] = pf_lanes(a[c], p.Ci - 4 * q);
+                }
 #pragma unroll
                 for (int s = 0; s < 3; s++) {
                     const float4* w = reinterpret_cast<const float4*>(pf_wsm + (long long)(r * 3 + s) * C4 * 4);
@@ -503,6 +520,23 @@ __global__ void __launch_bounds__(256) conv_pf3_warp_kernel(T4 in, const float* 
         }
     }
 }
+
+// The warp kernels' MASK instances are overloads that take a MaskLanes argument, so both instances keep the kernel's name.
+struct MaskLanes {};
+__global__ void __launch_bounds__(256) conv_pf_warp_kernel(T4 in, const float* __restrict__ wp, const float* __restrict__ bias, T4 out, ConvP p, int C4) {
+    pf_warp<false>(in, wp, bias, out, p, C4);
+}
+__global__ void __launch_bounds__(256) conv_pf_warp_kernel(T4 in, const float* __restrict__ wp, const float* __restrict__ bias, T4 out, ConvP p, int C4, MaskLanes) {
+    pf_warp<true>(in, wp, bias, out, p, C4);
+}
+__global__ void __launch_bounds__(256) conv_pf3_warp_kernel(T4 in, const float* __restrict__ wp, const float* __restrict__ bias, T4 out, ConvP p, int C4) {
+    pf3_warp<false>(in, wp, bias, out, p, C4);
+}
+__global__ void __launch_bounds__(256) conv_pf3_warp_kernel(T4 in, const float* __restrict__ wp, const float* __restrict__ bias, T4 out, ConvP p, int C4, MaskLanes) {
+    pf3_warp<true>(in, wp, bias, out, p, C4);
+}
+using PfWarpKernel = void (*)(T4, const float*, const float*, T4, ConvP, int);
+using PfWarpMaskedKernel = void (*)(T4, const float*, const float*, T4, ConvP, int, MaskLanes);
 
 // Caffe weights -> packed [k][co].  conv: w[co][ci][r][s]; deconv: w[ci][co][r][s].
 __global__ void pack_weights_kernel(const float* __restrict__ w, float* __restrict__ wp, int Ci, int Co,
@@ -580,8 +614,9 @@ static int make_params(const fn2_conv_desc* d, const T4& in, const T4& out, Conv
 // The SIMT kernels, in the order simt_route tries them.
 enum class SimtRoute { fewci, nhwc, pf3_tile, pf_thread, pf3_warp, pf_warp, tiny, smallco, igemm };
 
-// smem: dynamic shared memory bytes; C4: float4 groups per input pixel of the flow predictors; nhwc plans its own launches
-struct SimtLaunch { SimtRoute route; dim3 grid; size_t smem; int C4; };
+// smem: dynamic shared memory bytes; C4: float4 groups per input pixel of the flow predictors, mask: whether they must select 0
+// for the lanes beyond Ci (Ci % 4 != 0 without the guard promise); nhwc plans its own launches
+struct SimtLaunch { SimtRoute route; dim3 grid; size_t smem; int C4; bool mask = false; };
 
 // Which SIMT kernel runs a layer the tensor-core engines do not take, and its launch geometry.
 static SimtLaunch simt_route(const fn2_conv_desc* d, const T4& in, const T4& out) {
@@ -593,27 +628,29 @@ static SimtLaunch simt_route(const fn2_conv_desc* d, const T4& in, const T4& out
     const size_t pf_smem = (size_t)taps * C4 * 4 * sizeof(float2);
     if (!d->deconv && d->co == 2 && in.px_float4_groups() && pf_smem <= 200 * 1024) {
         const bool k3 = d->kh == 3 && d->kw == 3 && d->stride_h == 1 && d->stride_w == 1;
+        const bool mask = d->ci % 4 && !d->input_guard_bytes;
         if (C4 <= 8 && k3) {
             const long long tiles = (long long)out.n * ((out.w + 31) / 32) * ((out.h + 7) / 8);
             return {SimtRoute::pf3_tile, dim3((unsigned)min((long long)num_sms() * 4, tiles)),
-                    pf_smem + (size_t)10 * 34 * (C4 + 1) * sizeof(float4), C4};
+                    pf_smem + (size_t)10 * 34 * (C4 + 1) * sizeof(float4), C4, mask};
         }
-        if (C4 <= 8) return {SimtRoute::pf_thread, dim3((unsigned)min((long long)num_sms() * 8, (M + 255) / 256)), pf_smem, C4};
+        if (C4 <= 8) return {SimtRoute::pf_thread, dim3((unsigned)min((long long)num_sms() * 8, (M + 255) / 256)), pf_smem, C4, mask};
         const long long per_sm = max((size_t)1, min((size_t)8, (size_t)(220 * 1024) / (pf_smem + 1024)));
         const long long warps = k3 ? (long long)out.n * out.h * ((out.w + 3) / 4) : M;       // pf3_warp: 4 outputs of a row
-        return {k3 ? SimtRoute::pf3_warp : SimtRoute::pf_warp, dim3((unsigned)min(num_sms() * per_sm, (warps + 7) / 8)), pf_smem, C4};
+        return {k3 ? SimtRoute::pf3_warp : SimtRoute::pf_warp, dim3((unsigned)min(num_sms() * per_sm, (warps + 7) / 8)), pf_smem, C4,
+                mask};
     }
     if (d->co <= 4 && d->ci <= 32) return {SimtRoute::tiny, dim3(ew_grid(M, 256)), (size_t)taps * d->ci * d->co * sizeof(float), 0};
     if (d->co <= 4) return {SimtRoute::smallco, dim3(ew_grid(M * 32, 256)), 0, 0};
     return {SimtRoute::igemm, dim3((unsigned)((M + BM - 1) / BM), (unsigned)((d->co + BN - 1) / BN)), 0, 0};
 }
 
-// conv_pf3_tile_kernel<C4> or conv_pf_thread_kernel<C4>, for C4 in 1..8
-template <int C = 1>
-static auto pf_thread_kernel(bool tile, int C4) -> decltype(&conv_pf_thread_kernel<1>) {
+// conv_pf3_tile_kernel<C4, MASK> or conv_pf_thread_kernel<C4, MASK>, for C4 in 1..8
+template <bool MASK, int C = 1>
+static auto pf_thread_kernel(bool tile, int C4) -> decltype(&conv_pf_thread_kernel<1, MASK>) {
     if constexpr (C < 8)
-        if (C4 > C) return pf_thread_kernel<C + 1>(tile, C4);
-    return tile ? conv_pf3_tile_kernel<C> : conv_pf_thread_kernel<C>;
+        if (C4 > C) return pf_thread_kernel<MASK, C + 1>(tile, C4);
+    return tile ? conv_pf3_tile_kernel<C, MASK> : conv_pf_thread_kernel<C, MASK>;
 }
 
 static inline int floordiv(int a, int b) { return (a >= 0) ? a / b : -((-a + b - 1) / b); }
@@ -730,10 +767,12 @@ int fn2_conv_forward(const fn2_conv_desc* d, const fn2_tensor* bottom, const flo
     case SimtRoute::fewci: return launch(conv_fewci_kernel);
     case SimtRoute::nhwc:
         return conv_nhwc_forward(d, in, packed_weights_dev, bias_dev, out, (float*)workspace, workspace_bytes / sizeof(float), st);
-    case SimtRoute::pf3_tile: return launch(pf_thread_kernel(true, L.C4));
-    case SimtRoute::pf_thread: return launch(pf_thread_kernel(false, L.C4));
-    case SimtRoute::pf3_warp: return launch(conv_pf3_warp_kernel, L.C4);
-    case SimtRoute::pf_warp: return launch(conv_pf_warp_kernel, L.C4);
+    case SimtRoute::pf3_tile: return launch(L.mask ? pf_thread_kernel<true>(true, L.C4) : pf_thread_kernel<false>(true, L.C4));
+    case SimtRoute::pf_thread: return launch(L.mask ? pf_thread_kernel<true>(false, L.C4) : pf_thread_kernel<false>(false, L.C4));
+    case SimtRoute::pf3_warp:
+        return L.mask ? launch(PfWarpMaskedKernel(conv_pf3_warp_kernel), L.C4, MaskLanes{}) : launch(PfWarpKernel(conv_pf3_warp_kernel), L.C4);
+    case SimtRoute::pf_warp:
+        return L.mask ? launch(PfWarpMaskedKernel(conv_pf_warp_kernel), L.C4, MaskLanes{}) : launch(PfWarpKernel(conv_pf_warp_kernel), L.C4);
     case SimtRoute::tiny: return launch(d->deconv ? conv_tiny_kernel<true> : conv_tiny_kernel<false>);
     case SimtRoute::smallco: return launch(d->deconv ? conv_smallco_kernel<true, 4> : conv_smallco_kernel<false, 4>);
     case SimtRoute::igemm: return launch(d->deconv ? conv_igemm_kernel<true> : conv_igemm_kernel<false>);

@@ -175,7 +175,10 @@ typedef struct fn2_conv_desc {
                                 * storage; >= 512 lets small-Ci convolutions fetch whole kernel rows per TMA box. 0 = none.
                                 * Those rows include the padding channels of a bottom whose pixel stride is Ci rounded up
                                 * to 4: with a guard band they must hold finite values (they meet zero weights, and
-                                * 0 * NaN is NaN).  Without one they are never read. */
+                                * 0 * NaN is NaN).  The SIMT flow-predictor kernels (Co = 2) read each pixel as whole
+                                * float4 groups, so with a guard band the channels of a pixel's last group beyond Ci
+                                * (padding, or a neighbouring view's channels) must be finite too.  Without one none of
+                                * these channels is used. */
     int32_t out_pad_h, out_pad_w; /* deconvolution only: extra output rows / columns at the bottom / right (0 for every Caffe
                                 * layer; the adjoint of a strided convolution needs (H + 2 pad - k) mod stride of them to
                                 * reach the whole bottom, fn2_conv_backward_data_desc) */

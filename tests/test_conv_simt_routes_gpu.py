@@ -10,6 +10,7 @@ import numpy as np
 import pytest
 
 from oracle import oracle as O
+from tests.conv_ref import ROUTE_KERNEL
 from tests.util import kernels_per_case, maxabs, rng
 
 pytestmark = pytest.mark.gpu
@@ -33,14 +34,6 @@ def dev(a, layout="nchw"):
     padded[:, :c] = t
     return padded[:, :c]
 
-
-# the kernel each route launches, as the profiler names it
-ROUTE_KERNEL = {
-    "pf3_tile": "conv_pf3_tile_kernel<", "pf_thread": "conv_pf_thread_kernel<", "pf3_warp": "conv_pf3_warp_kernel(",
-    "pf_warp": "conv_pf_warp_kernel(", "tiny_deconv": "conv_tiny_kernel<true>", "tiny_conv": "conv_tiny_kernel<false>",
-    "smallco_deconv": "conv_smallco_kernel<true", "smallco_conv": "conv_smallco_kernel<false", "fewci": "conv_fewci_kernel(",
-    "nhwc": "conv_nhwc_kernel<", "igemm_deconv": "conv_igemm_kernel<true>", "igemm_conv": "conv_igemm_kernel<false>",
-}
 
 ROUTE_CASES = [
     # route, (N, Ci, H, W, Co, k, stride, pad, deconv), layouts

@@ -28,6 +28,8 @@ import numpy as np
 import pytest
 
 from oracle import oracle as O
+from tests.conv_ref import (LAYOUTS, _check, _lib, adjoint, bottom, case, guard_bytes, op_weights, ref_at, reference,
+                            weight_shape)
 from tests.util import deploy_convs, kernels_per_case, train_convs
 
 pytestmark = pytest.mark.gpu
@@ -36,7 +38,6 @@ torch = pytest.importorskip("torch")
 TOL = 1e-6
 SLOPE = 0.1
 SENTINEL = 7.0
-GUARD = 256                 # floats of NaN before and after every bottom's storage (Blob::kGuardFloats)
 FULL = 1 << 16              # output pixels up to which the reference evaluates every pixel
 SAMPLE = 2048
 
@@ -47,58 +48,7 @@ def ops(fn2):
     return _ops
 
 
-def _lib():
-    from flownet2_b200 import lib
-    return lib()
-
-
-def _check(rc):
-    from flownet2_b200 import check
-    check(rc)
-
-
 # ---- cases ----------------------------------------------------------------------------------------------------------------
-# fwd: None, or the layer whose data gradient the case is: (Ci, Co, k, s, p, deconv, H, W, needs_flip, real output channels)
-Case = namedtuple("Case", "name N Ci H W Co k s p deconv op bias layout engine fwd")
-
-
-def _pair(v):
-    return (v, v) if isinstance(v, int) else tuple(v)
-
-
-def case(name, N, Ci, H, W, Co, k, s=1, p=0, deconv=False, bias=True, layout="nhwc", engine=2):
-    return Case(name, N, Ci, H, W, Co, _pair(k), _pair(s), _pair(p), deconv, (0, 0), bias, layout, engine, None)
-
-
-def cstride(c):
-    """Blob::compute_cstride: the nets' pixel stride (channels rounded up to 4 below 32, else to 32)."""
-    return (c + 3) // 4 * 4 if c < 32 else (c + 31) // 32 * 32
-
-
-def padded_co(co):
-    """The output channels BaseConvolutionLayer::BackwardData gives a convolution adjoint (layers.cpp, BackwardData: a
-    multiple of 128 when that costs at most 1/8 more channels, else of 64; of 16 up to 64 channels)."""
-    if co <= 16 or co % 16 == 0:
-        return co
-    c128, c64 = (co + 127) // 128 * 128, (co + 63) // 64 * 64
-    return (co + 15) // 16 * 16 if co <= 64 else (c128 if (c128 - co) * 8 <= co else c64)
-
-
-def adjoint(name, N, Ci, H, W, Co, k, s=1, p=0, deconv=False, layout="pad", engine=2):
-    """The forward operator that computes the data gradient of a layer (fn2_conv_backward_data_desc) on its top diff, with
-    BackwardData's padded output channels."""
-    from flownet2_b200 import fn2_conv_desc
-    (kh, kw), (sh, sw), (ph, pw) = _pair(k), _pair(s), _pair(p)
-    d = fn2_conv_desc(Ci, Co, kh, kw, sh, sw, ph, pw, int(deconv), 1, 0, 0.0, 0, 0)
-    bd, flip, ho, wo = fn2_conv_desc(), C.c_int(), C.c_int(), C.c_int()
-    _check(_lib().fn2_conv_backward_data_desc(C.byref(d), H, W, C.byref(bd), C.byref(flip)))
-    _check(_lib().fn2_conv_out_shape(C.byref(d), H, W, C.byref(ho), C.byref(wo)))
-    co = padded_co(bd.co) if not bd.deconv else bd.co
-    return Case(name, N, bd.ci, ho.value, wo.value, co, (bd.kh, bd.kw), (bd.stride_h, bd.stride_w), (bd.pad_h, bd.pad_w),
-                bool(bd.deconv), (bd.out_pad_h, bd.out_pad_w), False, layout, engine,
-                (Ci, Co, (kh, kw), (sh, sw), (ph, pw), deconv, H, W, bool(flip.value), bd.co))
-
-
 PLAN_CASES = [
     # per-tap engine, plain K blocks (mode 0); comments: NT x Co tiles, tile width, K steps, split
     case("nt16_split_all", 1, 40, 20, 24, 16, 5, 1, 2),                   # NT 16, tw 32, 50 steps: every tile split
@@ -157,14 +107,6 @@ def seed_of(c):
     return zlib.crc32(repr(c[:10]).encode())
 
 
-def weight_shape(c):
-    """Caffe layout of the weights the reference uses: those of the case, or of the layer it is the data gradient of."""
-    if c.fwd:
-        Ci, Co, (kh, kw), _, _, deconv, _, _, _, _ = c.fwd
-        return (Ci, Co, kh, kw) if deconv else (Co, Ci, kh, kw)
-    return (c.Ci, c.Co) + c.k if c.deconv else (c.Co, c.Ci) + c.k
-
-
 def draw(c, seed, same_sign=False):
     """bottom (NCHW, dense), weights (Caffe layout) and bias on the device.  same_sign: a post-ReLU bottom and weights of one
     sign (|N(0,1)| sqrt(2 / K)), else N(0,1) and N(0,1) sqrt(2 / K)."""
@@ -176,35 +118,6 @@ def draw(c, seed, same_sign=False):
     if same_sign:
         x, w = x.clamp_min(0.0), w.abs()
     return x, w, b
-
-
-# layout -> (first channel, pixel stride, padding channels, guard promise)
-LAYOUTS = {
-    "nhwc": (0, lambda c: (c + 3) // 4 * 4, "nan", False),      # channels_last, 16-byte pixels
-    "pad": (0, cstride, "zero", True),                          # the nets' blobs
-    "padjunk": (0, cstride, "junk", True),                      # ... with finite garbage in the padding channels
-    "padnan": (0, cstride, "nan", False),                       # ... with NaN there, and no guard promise
-    "slice": (4, lambda c: (c + 3) // 4 * 4 + 8, "nan", False),  # a zero-copy concat child
-    "misaligned": (1, lambda c: c + 4, "nan", False),           # first channel not on a 16-byte boundary
-}
-
-
-def bottom(x, layout):
-    """A view of x in one of LAYOUTS.  The storage has GUARD floats of NaN before and after it; the channels outside the view
-    hold NaN, zero or finite garbage (1e30)."""
-    n, c, h, w = x.shape
-    off, cs, fill, _ = LAYOUTS[layout]
-    cs = cs(c)
-    flat = torch.full((2 * GUARD + n * h * w * cs,), float("nan"), device="cuda")
-    body = flat[GUARD:GUARD + n * h * w * cs].view(n, h, w, cs)
-    if fill != "nan":
-        body.fill_(0.0 if fill == "zero" else 1e30)
-    body[..., off:off + c] = x.permute(0, 2, 3, 1)
-    return body.permute(0, 3, 1, 2)[:, off:off + c]
-
-
-def guard_bytes(layout):
-    return 4 * GUARD if LAYOUTS[layout][3] else 0
 
 
 def desc(c, engine=None, layout=None):
@@ -239,23 +152,6 @@ def ws_bytes(c):
     nb = C.c_size_t()
     _check(_lib().fn2_conv_workspace_bytes(C.byref(desc(c)), c.N, c.H, c.W, C.byref(nb)))
     return nb.value
-
-
-def op_weights(c, w):
-    """The Caffe-layout weights of the operator: the case's own, or for a data gradient the layer's, flipped and transposed
-    when fn2_conv_backward_data_desc asks for it, with BackwardData's zero rows for padded output channels."""
-    if not c.fwd:
-        return w
-    Ci, Co, k, s, p, deconv, H, W, flip, co_real = c.fwd
-    if flip:
-        from flownet2_b200 import fn2_conv_desc
-        d = fn2_conv_desc(Ci, Co, k[0], k[1], s[0], s[1], p[0], p[1], int(deconv), 1, 0, 0.0, 0, 0)
-        w2 = torch.empty((Ci, Co) + tuple(k), device="cuda")
-        _check(_lib().fn2_conv_flip_transpose_weights(C.byref(d), w.data_ptr(), w2.data_ptr(), torch.cuda.current_stream().cuda_stream))
-        w = w2
-    if c.Co > co_real:
-        w = torch.cat([w, torch.zeros((c.Co - co_real,) + tuple(w.shape[1:]), device="cuda")])
-    return w.contiguous()
 
 
 Run = namedtuple("Run", "go wide out ws_buf")
@@ -295,53 +191,6 @@ def prepare(c, x, w, b, layout=None, engine=None, ws="exact"):
 
 
 # ---- reference ----------------------------------------------------------------------------------------------------------------
-def ref_at(x, w, deconv, s, p, n, oy, ox):
-    """float64 (P, Co) outputs at the pixels (n, oy, ox) without bias: per kernel tap one BLAS product of the tap's weights with
-    the input pixels it reads there.  x (N, Ci, H, W); w in Caffe layout; a deconvolution's tap (ky, kx) reads input pixel
-    ((oy + ph - ky) / sh, (ox + pw - kx) / sw) where both divide exactly."""
-    (sh, sw), (ph, pw) = s, p
-    x, w = x.double(), w.double()
-    N, Ci, H, W = x.shape
-    kh, kw = w.shape[2:]
-    out = torch.zeros((len(n), w.shape[1] if deconv else w.shape[0]), dtype=torch.float64, device=x.device)
-
-    def coord(o, st, pd, kk, size):
-        if deconv:
-            t = o + pd - kk
-            i = torch.div(t, st, rounding_mode="floor")
-            ok = (i * st == t)
-        else:
-            i = o * st + kk - pd
-            ok = torch.ones_like(i, dtype=torch.bool)
-        return i, ok & (i >= 0) & (i < size)
-
-    for ky in range(kh):
-        iy, oky = coord(oy, sh, ph, ky, H)
-        for kx in range(kw):
-            ix, okx = coord(ox, sw, pw, kx, W)
-            sel = (oky & okx).nonzero().squeeze(1)
-            if len(sel):
-                wt = w[:, :, ky, kx] if deconv else w[:, :, ky, kx].T             # (Ci, Co)
-                out.index_add_(0, sel, x[n[sel], :, iy[sel], ix[sel]] @ wt)
-    return out
-
-
-def reference(c, x, w, b, n, oy, ox):
-    """The case's outputs at (n, oy, ox) in float64, in chunks that keep the gathered inputs small; a data-gradient operator
-    is computed as the transpose of its layer, from the layer's weights."""
-    if c.fwd:
-        _, _, _, s, p, deconv, _, _, _, _ = c.fwd
-        deconv = not deconv
-    else:
-        s, p, deconv = c.s, c.p, c.deconv
-    step = max(256, (1 << 25) // c.Ci)
-    out = torch.cat([ref_at(x, w, deconv, s, p, n[i:i + step], oy[i:i + step], ox[i:i + step]) for i in range(0, len(n), step)])
-    if b is not None:
-        out = out + b.double()
-        out = torch.where(out > 0, out, out * SLOPE)
-    return out
-
-
 def tile_width(c, Wo):
     """The per-tap engine's tile width: the smallest power of two >= the widest parity class, clamped to [8, 128]."""
     wmax = -(-Wo // c.s[1]) if c.deconv else Wo

@@ -66,17 +66,19 @@ def net_losses(text):
 
 
 def net_walk(text):
-    """-> (net_convs, net_losses) of a filled prototxt."""
+    """-> (net_convs, net_losses, concats, io) of a filled prototxt.  concats: {bottom blob of a Concat of two or more bottoms:
+    (the concat's top, the bottom's first channel in it, the top's channels)}; io: {layer name: (bottom blobs, top blobs)}."""
     from flownet2_b200 import ops as _ops
     from oracle import net as onet
     get, getall = onet.get, onet.getall
     net = onet.parse_prototxt(text)
-    shp, out, losses = {}, [], []
+    shp, out, losses, concats, io = {}, [], [], {}, {}
     for t, s in zip(getall(net, "input"), getall(net, "input_shape")):            # legacy deploy inputs
         shp[t] = tuple(int(d) for d in getall(s, "dim"))[1:]
     for l in getall(net, "layer"):
         ty, bots, tops = get(l, "type"), getall(l, "bottom"), getall(l, "top")
         b = [shp.get(n) for n in bots]
+        io[get(l, "name")] = (bots, tops)
         if ty == "Input":
             for t, s in zip(tops, getall(get(l, "input_param"), "shape")):
                 shp[t] = tuple(int(d) for d in getall(s, "dim"))[1:]
@@ -113,6 +115,11 @@ def net_walk(text):
                                                   int(get(cp, "stride_2", 1)))
         elif ty == "Concat":
             shp[tops[0]] = (sum(x[0] for x in b),) + b[0][1:]
+            c0 = 0
+            for n_, x in zip(bots, b):
+                if len(bots) > 1:
+                    concats.setdefault(n_, (tops[0], c0, shp[tops[0]][0]))
+                c0 += x[0]
         elif ty in ("Downsample", "Resample"):
             # the size of the second bottom, else the layer's own (the deploy nets' 436 -> 448 adaptation)
             rp = get(l, "resample_param", [])
@@ -127,7 +134,7 @@ def net_walk(text):
             losses.append((get(l, "name"), b[0]))
         else:
             assert ty == "Silence", ty
-    return out, losses
+    return out, losses, concats, io
 
 
 def train_convs(model, width=448, height=320):
