@@ -285,6 +285,11 @@ class Net(object):
         (N, 2, H, W) input blob `name`; flags FLOW_UINT16FLOW quantises as the reference's training data (include/fn2_flow.h)."""
         check(lib().fn2_net_set_input_flow_device(self._h, name.encode(), C.c_void_p(dev_ptr), int(format), int(flags)))
 
+    def set_input_kitti_flow_device(self, name, dev_ptr, flags=0):
+        """dev_ptr: device address of the payloads of N KITTI flow PNGs ([N][H][W][3] big-endian uint16, 2-byte aligned;
+        flownet2_b200.kitti) for the (N, 2, H, W) input blob `name`; flags FLOW_UINT16FLOW as in set_input_flow_device."""
+        check(lib().fn2_net_set_input_kitti_flow_device(self._h, name.encode(), C.c_void_p(dev_ptr), int(flags)))
+
     def get_blob_nhwc(self, name):
         """The blob as an (N, H, W, C) array; for the flow, (N, H, W, 2) is the payload of a .flo file per pair."""
         n, c, h, w = self.blobs[name].shape

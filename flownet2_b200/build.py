@@ -42,6 +42,7 @@ SOURCES = [
     ("caffe/layers.cpp", []),
     ("caffe/net.cpp", []),
     ("caffe/hdf5_min.cpp", []),
+    ("caffe/png_unfilter.cpp", []),
     ("caffe/solver.cpp", []),
     ("caffe/capi.cpp", []),
 ]

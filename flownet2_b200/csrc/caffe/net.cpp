@@ -866,14 +866,27 @@ void Net<Dtype>::SetInputFrames(const string& blob, const void* host_frames, int
     SetInputFramesDevice(blob, st, channels);
 }
 
+// The input blob a flow goes to: refuses a blob that is not (N, 2, H, W).
+template <typename Dtype>
+static shared_ptr<Blob<Dtype> > flow_blob(const Net<Dtype>& net, const string& blob) {
+    shared_ptr<Blob<Dtype> > b = net.blob_by_name(blob);
+    CHECK(b->num_axes() == 4 && b->channels() == 2) << "set_input_flow: blob " << blob << " must have shape (N, 2, H, W), has "
+                                                    << b->num_axes() << " axes and " << b->channels() << " channels";
+    return b;
+}
+
 template <typename Dtype>
 void Net<Dtype>::SetInputFlowDevice(const string& blob, const void* dev, int format, int flags) {
     Caffe::stream() = stream_;
-    shared_ptr<Blob<Dtype> > b = blob_by_name(blob);
-    CHECK(b->num_axes() == 4 && b->channels() == 2) << "set_input_flow: blob " << blob << " must have shape (N, 2, H, W), has "
-                                                    << b->num_axes() << " axes and " << b->channels() << " channels";
-    fn2_tensor dst = b->mutable_tensor();
+    fn2_tensor dst = flow_blob(*this, blob)->mutable_tensor();
     FN2_CALL(fn2_flow_to_tensor(dev, format, flags, &dst, stream_));
+}
+
+template <typename Dtype>
+void Net<Dtype>::SetInputKittiFlowDevice(const string& blob, const void* dev, int flags) {
+    Caffe::stream() = stream_;
+    fn2_tensor dst = flow_blob(*this, blob)->mutable_tensor();
+    FN2_CALL(fn2_kitti_flow_to_tensor(dev, flags, &dst, stream_));
 }
 
 template <typename Dtype>

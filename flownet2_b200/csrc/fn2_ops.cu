@@ -780,6 +780,65 @@ __global__ void flow_to_tensor_kernel(const uint32_t* __restrict__ src, PxView d
     });
 }
 
+// ---------------------------------------------------------------------------------------------
+// KITTI flow PNGs (include/fn2_flow.h).  Decode: the unfiltered payload [N][H][W][3] big-endian uint16 -> (N, 2, H, W) floats,
+// one thread per pixel; (R - 32768) / 64 is exact, an invalid pixel (B = 0) is NaN in both channels, and UINT16FLOW goes
+// through flow_value's quantisation.  Encode: each thread encodes its own pixel and its left, up and up-left neighbours from
+// the flow and Paeth-filters its 6 bytes against them, so no thread reads another's output; the thread of x = 0 also writes
+// the row's filter byte.
+// ---------------------------------------------------------------------------------------------
+__global__ void kitti_flow_to_tensor_kernel(const uint16_t* __restrict__ src, PxView dst, int quantise) {
+    const T4& d = dst.t;
+    for_each_pixel(d.n, d.h, d.w, [&](int n, int y, int x) {
+        const uint16_t* p = src + (((long long)n * d.h + y) * d.w + x) * 3;
+        const uint32_t r = __byte_perm(p[0], 0, 0x4401), g = __byte_perm(p[1], 0, 0x4401), b = p[2];
+        const float nan = __uint_as_float(0x7fc00000u);
+        const float u = b ? flow_value(__float_as_uint((float)((int)r - 32768) * 0.015625f), false, quantise) : nan;
+        const float v = b ? flow_value(__float_as_uint((float)((int)g - 32768) * 0.015625f), false, quantise) : nan;
+        if (d.sc == 1) {
+            px_store(dst, d.off(n, 0, y, x), 0, make_float4(u, v, 0.f, 0.f));
+        } else {
+            d.p[d.off(n, 0, y, x)] = u;
+            d.p[d.off(n, 1, y, x)] = v;
+        }
+    });
+}
+
+// The stored samples (R, G, B) of flow pixel (n, y, x); (0, 0, 0) outside the image, PNG's value left of and above it.
+struct KittiPx { uint32_t s[3]; };
+__device__ __forceinline__ KittiPx kitti_encode(const T4& f, int n, int y, int x) {
+    KittiPx r = {{0u, 0u, 0u}};
+    if (x < 0 || y < 0) return r;
+    const float u = f.p[f.off(n, 0, y, x)], v = f.p[f.off(n, 1, y, x)];
+    if (!isfinite(u) || !isfinite(v)) return r;
+    r.s[0] = __float2uint_rz(fmaxf(fminf(u * 64.f + 32768.f, 65535.f), 0.f));
+    r.s[1] = __float2uint_rz(fmaxf(fminf(v * 64.f + 32768.f, 65535.f), 0.f));
+    r.s[2] = 1u;
+    return r;
+}
+__device__ __forceinline__ uint32_t paeth_predict(int a, int b, int c) {
+    const int p = a + b - c, pa = abs(p - a), pb = abs(p - b), pc = abs(p - c);
+    return (uint32_t)(pa <= pb && pa <= pc ? a : pb <= pc ? b : c);
+}
+
+__global__ void flow_to_kitti_png_rows_kernel(T4 f, uint8_t* __restrict__ rows) {
+    const long long row_bytes = 1 + 6LL * f.w;
+    for_each_pixel(f.n, f.h, f.w, [&](int n, int y, int x) {
+        const KittiPx self = kitti_encode(f, n, y, x), left = kitti_encode(f, n, y, x - 1), up = kitti_encode(f, n, y - 1, x),
+                      upleft = kitti_encode(f, n, y - 1, x - 1);
+        uint8_t* row = rows + ((long long)n * f.h + y) * row_bytes;
+        if (x == 0) row[0] = 4;
+        uint8_t* o = row + 1 + 6LL * x;
+        #pragma unroll
+        for (int i = 0; i < 6; i++) {
+            const int sh = i & 1 ? 0 : 8;                                          // big-endian: the high byte first
+            const int j = i >> 1;
+            const uint32_t raw = (self.s[j] >> sh) & 0xff;
+            o[i] = (uint8_t)(raw - paeth_predict((left.s[j] >> sh) & 0xff, (up.s[j] >> sh) & 0xff, (upleft.s[j] >> sh) & 0xff));
+        }
+    });
+}
+
 }  // namespace fn2
 
 using namespace fn2;
@@ -1029,6 +1088,26 @@ int fn2_flow_to_tensor(const void* src_dev, int format, int flags, const fn2_ten
     if (format == FN2_FLOW_FLO) return ew_launch(flow_to_tensor_kernel<FN2_FLOW_FLO>, total, stream, s, px_view(d), q);
     if (format == FN2_FLOW_PFM) return ew_launch(flow_to_tensor_kernel<FN2_FLOW_PFM>, total, stream, s, px_view(d), q);
     return ew_launch(flow_to_tensor_kernel<FN2_FLOW_PFM_BE>, total, stream, s, px_view(d), q);
+}
+
+int fn2_kitti_flow_to_tensor(const void* src_dev, int flags, const fn2_tensor* dst, void* stream) {
+    FN2_CHECK_ARG(src_dev, "kitti_flow_to_tensor: src is null");
+    FN2_CHECK_ARG((reinterpret_cast<uintptr_t>(src_dev) & 1) == 0, "kitti_flow_to_tensor: src must be 2-byte aligned");
+    FN2_CHECK_ARG(valid(dst), "kitti_flow_to_tensor: dst is null or empty");
+    FN2_CHECK_ARG((flags & ~FN2_FLOW_UINT16FLOW) == 0, "kitti_flow_to_tensor: unknown flags 0x%x", flags);
+    T4 d = view(dst);
+    FN2_CHECK_ARG(d.c == 2, "kitti_flow_to_tensor: dst must have 2 channels (u, v), has %d", d.c);
+    return ew_launch(kitti_flow_to_tensor_kernel, (long long)d.n * d.h * d.w, stream, static_cast<const uint16_t*>(src_dev),
+                     px_view(d), flags & FN2_FLOW_UINT16FLOW);
+}
+
+int fn2_flow_to_kitti_png_rows(const fn2_tensor* src, void* dst_dev, void* stream) {
+    FN2_CHECK_ARG(valid(src), "flow_to_kitti_png_rows: src is null or empty");
+    FN2_CHECK_ARG(dst_dev, "flow_to_kitti_png_rows: dst is null");
+    FN2_CHECK_ARG((reinterpret_cast<uintptr_t>(src->data) & 3) == 0, "flow_to_kitti_png_rows: src must be 4-byte aligned");
+    T4 f = view(src);
+    FN2_CHECK_ARG(f.c == 2, "flow_to_kitti_png_rows: src must have 2 channels (u, v), has %d", f.c);
+    return ew_launch(flow_to_kitti_png_rows_kernel, (long long)f.n * f.h * f.w, stream, f, static_cast<uint8_t*>(dst_dev));
 }
 
 }  // extern "C"

@@ -7,7 +7,8 @@
 
 The list file holds one ``img0 img1 flow`` line per sample (the converter's format); blank lines are skipped and an occlusion
 field is refused.  Frames are whatever flownet2_b200.run reads (PPM / PGM here, anything else through Pillow); flows are .flo
-or PFM ('PF' only), one format per list, and every file has one size, as one LMDB has one Datum shape.
+or PFM ('PF' only), one format per list, and every file has one size, as one LMDB has one Datum shape.  With kitti=True every
+flow is a KITTI 16-bit PNG (flownet2_b200.kitti): invalid pixels become NaN, which L1Loss, Downsample and LpqLoss leave out.
 
 Order.  CustomData's (custom_data_layer.cpp:28-41, 394-470): the list line i is key i; the keys are optionally permuted with
 libstdc++'s std::random_shuffle after std::srand(rand_permute_seed) -- glibc's rand(), restated in Python -- per block of
@@ -19,13 +20,15 @@ sequence.  seek(b) moves to batch b of this rank; after Solver.restore the train
 resumed run sees what an uninterrupted one would have seen (the reference restarts its sequence at 0 on resume).
 
 Ground truth.  With flow_encoding "uint16" (the default) the flow blob holds what the reference's LMDB hands its net:
-trunc(32 v) / 32, NaN for NaN and out-of-range values (include/fn2_flow.h).  "float" passes the file's floats through.
+trunc(32 v) / 32, NaN for NaN and out-of-range values (include/fn2_flow.h).  "float" passes the file's floats through (for a
+KITTI PNG: its exact (R - 32768) / 64).
 
 Pipeline.  Frames and flows are not converted on the host: a thread pool reads the PPM rasters and the flow payloads of the
 batches ahead straight into slices of a pinned slot (other image formats decode through Pillow into the slice), the slot goes
 to the device on a copy stream, and the net's stream waits for that copy, converts the three inputs on the device
 (fn2_net_set_input_frames_device twice, fn2_net_set_input_flow_device once) and records that the slot is free again.  The
-step's path never synchronises with the device.  busy() reports the per-stage times.
+step's path never synchronises with the device.  busy() reports the per-stage times.  A KITTI PNG is inflated and unfiltered
+by the reader thread into the slot (its raw big-endian samples) and converted by fn2_net_set_input_kitti_flow_device.
 """
 import os
 import struct
@@ -35,7 +38,7 @@ from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 
-from . import FLOW_FLO, FLOW_PFM, FLOW_PFM_BE, FLOW_UINT16FLOW, image_to_blob
+from . import FLOW_FLO, FLOW_PFM, FLOW_PFM_BE, FLOW_UINT16FLOW, image_to_blob, kitti as kitti_png
 from .run import RunError, _pnm_header, frame_as, probe_image, read_image
 
 FLO_TAG = 202021.25                        # 'PIEH' read as a little-endian float
@@ -235,9 +238,10 @@ def read_list(path):
     return out
 
 
-def probe_samples(samples):
+def probe_samples(samples, kitti=False):
     """Probes every frame and flow without decoding pixels -> (width, height, flow format); refuses missing or truncated files,
-    bad flow files, mixed flow formats and any file whose size differs from the first sample's."""
+    bad flow files, mixed flow formats and any file whose size differs from the first sample's.  kitti: every flow is a KITTI
+    PNG (kitti.probe)."""
     size = fmt = None
     for s in samples:
         try:
@@ -251,7 +255,7 @@ def probe_samples(samples):
                     raise RunError("%s: truncated raster (%d of %d bytes)" % (p, os.path.getsize(p) - hdr[4], w * h * k))
                 dims.append((p, w, h))
                 chans.append(k)
-            fh = flow_header(s.flow)
+            fh = kitti_png.probe(s.flow) if kitti else flow_header(s.flow)
             dims.append((s.flow, fh.width, fh.height))
         except RunError as e:
             raise RunError("%s: %s" % (s.where, e))
@@ -268,7 +272,16 @@ def probe_samples(samples):
 
 
 def _fmt_name(fmt):
-    return {FLOW_FLO: ".flo", FLOW_PFM: "little-endian .pfm", FLOW_PFM_BE: "big-endian .pfm"}[fmt]
+    return {FLOW_FLO: ".flo", FLOW_PFM: "little-endian .pfm", FLOW_PFM_BE: "big-endian .pfm",
+            kitti_png.KITTI: "KITTI .png"}[fmt]
+
+
+def read_flow_into(path, hdr, out):
+    """The payload of a flow file (flow_header or kitti.probe) into `out`: as stored, or a KITTI PNG's unfiltered samples."""
+    if hdr.format == kitti_png.KITTI:
+        kitti_png.read_payload(path, hdr, out)
+    else:
+        read_flow_payload(path, hdr, out)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -285,10 +298,11 @@ class FlowDataset(object):
     range_end, rand_permute_order: CustomData's data_param fields (the defaults are the train command's: permuted, seed 77).
     flow_encoding: "uint16" (the reference's LMDB values) or "float".  world, rank: data-parallel shard (default: the
     initialised torch.distributed group, else 1, 0).  slots: batches in flight (2 or 3).  threads: reader pool size.
+    kitti: the flows are KITTI 16-bit PNGs.
     """
 
     def __init__(self, list_file, batch, rand_permute=True, rand_permute_seed=77, block_size=0, range_start=0, range_end=-1,
-                 rand_permute_order=ORDERS[0], flow_encoding="uint16", world=None, rank=None, slots=3, threads=None):
+                 rand_permute_order=ORDERS[0], flow_encoding="uint16", world=None, rank=None, slots=3, threads=None, kitti=False):
         if batch < 1:
             raise RunError("batch must be at least 1, got %d" % batch)
         if flow_encoding not in ENCODINGS:
@@ -298,7 +312,7 @@ class FlowDataset(object):
         if world is None:
             world, rank = _dist_world()
         self.samples = read_list(list_file)
-        w, h, self.flow_format = probe_samples(self.samples)
+        w, h, self.flow_format = probe_samples(self.samples, kitti)
         self.size = (w, h)
         self.batch, self.world, self.rank = int(batch), int(world), int(rank)
         self.flow_encoding, self.slots, self.threads = flow_encoding, slots, threads
@@ -324,7 +338,8 @@ class FlowDataset(object):
         """Batch k restated on the host -> (img0, img1, flow) float32 NCHW arrays, the blobs the device path fills."""
         img = [np.stack([image_to_blob(frame_as(read_image(getattr(self.samples[i], n)), 3))[0] for i in self.keys(k)])
                for n in ("img0", "img1")]
-        flow = np.stack([read_flow(self.samples[i].flow).transpose(2, 0, 1) for i in self.keys(k)])
+        read = kitti_png.read_kitti_flow if self.flow_format == kitti_png.KITTI else read_flow
+        flow = np.stack([read(self.samples[i].flow).transpose(2, 0, 1) for i in self.keys(k)])
         if self.flow_encoding == "uint16":
             flow = uint16flow(flow)
         return img[0], img[1], flow
@@ -344,9 +359,8 @@ class FlowDataset(object):
         self.close()
         self.net, self.inputs = net, names
         px = B * H * W
-        fpp = 2 if self.flow_format == FLOW_FLO else 3
         self._flow_off = _align(2 * px * 4)                            # frames of img0, then of img1 ([B][H][W][K] each, K <= 4)
-        self._bytes = self._flow_off + px * fpp * 4
+        self._bytes = self._flow_off + px * self._flow_px_bytes()
         S = self.slots
         self._pin = [torch.empty(self._bytes, dtype=torch.uint8).pin_memory() for _ in range(S)]
         self._host = [p.numpy() for p in self._pin]
@@ -393,7 +407,7 @@ class FlowDataset(object):
             fh = smp.flow_header
             o = self._flow_off + i * fh.nbytes
             try:
-                read_flow_payload(smp.flow, fh, out[o:o + fh.nbytes])
+                read_flow_into(smp.flow, fh, out[o:o + fh.nbytes])
             except (OSError, RunError) as e:
                 raise RunError("%s: %s" % (smp.where, e))
             return time.perf_counter() - t0
@@ -431,7 +445,7 @@ class FlowDataset(object):
         self._busy["host_wait"] += time.perf_counter() - t0
         W, H = self.size
         px = B * H * W
-        fb = px * (2 if self.flow_format == FLOW_FLO else 3) * 4
+        fb = px * self._flow_px_bytes()
         ev = [torch.cuda.Event(enable_timing=True) for _ in range(5)]
         with torch.cuda.stream(self._copy_stream):
             self._copy_stream.wait_event(self._ev_free[s])               # dev[s] was converted `slots` batches ago
@@ -448,8 +462,11 @@ class FlowDataset(object):
         base = self._dev[s].data_ptr()
         self.net.set_input_image_device(self.inputs[0], base, K)
         self.net.set_input_image_device(self.inputs[1], base + px * K, K)
-        self.net.set_input_flow_device(self.inputs[2], base + self._flow_off, self.flow_format,
-                                       FLOW_UINT16FLOW if self.flow_encoding == "uint16" else 0)
+        flags = FLOW_UINT16FLOW if self.flow_encoding == "uint16" else 0
+        if self.flow_format == kitti_png.KITTI:
+            self.net.set_input_kitti_flow_device(self.inputs[2], base + self._flow_off, flags)
+        else:
+            self.net.set_input_flow_device(self.inputs[2], base + self._flow_off, self.flow_format, flags)
         ev[4].record(ns)
         self._ev_free[s].record(ns)
         self._timing.append(ev)
@@ -458,6 +475,9 @@ class FlowDataset(object):
         self._calls += 1
         self._submit(k + self.slots)                                     # reads into pin[s] once its copy is done
         return {}
+
+    def _flow_px_bytes(self):
+        return {FLOW_FLO: 8, kitti_png.KITTI: kitti_png.PAYLOAD_PX_BYTES}.get(self.flow_format, 12)
 
     def _harvest(self, block):
         while self._timing and (block or self._timing[0][4].query()):

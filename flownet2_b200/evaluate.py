@@ -1,7 +1,7 @@
 """Score a net against ground-truth flow: end-point error, outlier rate and Sintel speed bands over an image-and-flow list.
 
     python -m flownet2_b200.evaluate weights.caffemodel models/FlowNet2_deploy.prototxt.template val.txt [--batch B]
-                                     [--per-pair out.tsv] [--gpu G]
+                                     [--per-pair out.tsv] [--gpu G] [--kitti]
 
 The list is the train command's: one ``img0 img1 flow`` line per pair (data.read_list; an occlusion field is refused), flows as
 .flo or 'PF' PFM of either byte order.  Frame sizes may differ from line to line; a flow must have its frames' size.  The
@@ -10,6 +10,10 @@ with the forwards); only what happens to each batch's flow differs.  The reader 
 pinned slot beside the frames, the copy stream moves it to the device, and on the net's stream it is converted
 (fn2_flow_to_tensor, the file's floats unquantised) and scored against the prediction by fn2_flow_error (include/fn2_eval.h).
 Only the per-pair records come back to the host; the padded pairs of a size's last batch are dropped.
+
+--kitti: every flow of the list is a KITTI 16-bit PNG (flownet2_b200.kitti), the ground truth of KITTI 2012 and 2015; sizes
+may differ by line.  The reader pool inflates and unfilters each file into the slot, and fn2_kitti_flow_to_tensor turns the
+samples into the flow on the net's stream, unquantised, with NaN at the pixels the file marks invalid.
 
 Metrics.  A ground-truth pixel is valid when both components are finite and at most 1e9 in absolute value.  EPE is the
 float32 sqrt(du^2 + dv^2) of the prediction minus the ground truth; a valid pixel whose prediction is not finite is counted in
@@ -35,21 +39,23 @@ import time
 import numpy as np
 
 from . import FLOW_ERROR_FIELDS
-from .data import flow_header, read_flow_payload, read_list
+from . import kitti as K
+from .data import flow_header, read_flow_into, read_list
 from .run import RunError, check_inputs, probe_pairs, run_groups, shard
 
 FIELD = {name: i for i, name in enumerate(FLOW_ERROR_FIELDS)}
 BANDS = (("s0-10", "n_s0_10", "sum_s0_10"), ("s10-40", "n_s10_40", "sum_s10_40"), ("s40+", "n_s40", "sum_s40"))
-PAYLOAD_PX_BYTES = 12                      # the larger payload per pixel: PFM's three floats (.flo holds two)
+PAYLOAD_PX_BYTES = 12                      # the larger payload per pixel: PFM's three floats (.flo two, a KITTI PNG 6 bytes)
 
 
-def probe_samples(samples):
+def probe_samples(samples, kitti=False):
     """Sets each sample's frame size and channels (run.probe_pairs) and its flow header; refuses missing or unreadable
-    files, unknown flow suffixes and a flow whose size differs from its frames', naming the list line."""
+    files, unknown flow suffixes and a flow whose size differs from its frames', naming the list line.  kitti: every flow is a
+    KITTI PNG (kitti.probe)."""
     probe_pairs(samples)
     for s in samples:
         try:
-            fh = flow_header(s.flow)
+            fh = K.probe(s.flow) if kitti else flow_header(s.flow)
         except RunError as e:
             raise RunError("%s: %s" % (s.where, e))
         if (fh.width, fh.height) != s.size:
@@ -71,7 +77,7 @@ class Scores(object):
 
     def read_payload(self, p, out):
         try:
-            read_flow_payload(p.flow, p.flow_header, out[:p.flow_header.nbytes])
+            read_flow_into(p.flow, p.flow_header, out[:p.flow_header.nbytes])
         except (OSError, RunError) as e:
             raise RunError("%s: %s" % (p.where, e))
 
@@ -89,7 +95,11 @@ class Scores(object):
         """On the net's stream: pair i's payload, at payload[i * stride], into gt[s][i] (formats may differ per pair)."""
         for i, p in enumerate(pairs):
             fh = p.flow_header
-            self.ops.flow_to_tensor(payload[i * stride:i * stride + fh.nbytes], fh.format, 0, self.gt[s][i:i + 1])
+            src = payload[i * stride:i * stride + fh.nbytes]
+            if fh.format == K.KITTI:
+                self.ops.kitti_flow_to_tensor(src, 0, self.gt[s][i:i + 1])
+            else:
+                self.ops.flow_to_tensor(src, fh.format, 0, self.gt[s][i:i + 1])
 
     def score(self, s):
         self.ops.flow_error(self.pred[s], self.gt[s], out=self.dev[s], workspace=self.workspace)
@@ -162,11 +172,11 @@ def _list_name(samples):
     return samples[0].where.rsplit(":", 1)[0] if samples else "the list"
 
 
-def _score(caffemodel, template, samples, batch, device, threads):
+def _score(caffemodel, template, samples, batch, device, threads, kitti=False):
     """-> (records in the samples' order, per-stage busy seconds, number of sizes)."""
     t0 = time.perf_counter()
     check_inputs(caffemodel, template, batch)
-    probe_samples(samples)
+    probe_samples(samples, kitti)
     for i, s in enumerate(samples):
         s.index = i
     sink = Scores(len(samples))
@@ -174,12 +184,12 @@ def _score(caffemodel, template, samples, batch, device, threads):
     return sink.records, stats, sizes
 
 
-def evaluate(caffemodel, template, samples, batch=1, device=0, threads=None):
+def evaluate(caffemodel, template, samples, batch=1, device=0, threads=None, kitti=False):
     """Scores the net on every data.Sample -> (summary dict, per-pair records): the summary of summarize() plus batch, sizes,
     wall (s), per-stage busy seconds and the samples whose prediction is not finite; the records are an (n, FIELDS) float64
-    array in the samples' order (fields: flownet2_b200.FLOW_ERROR_FIELDS)."""
+    array in the samples' order (fields: flownet2_b200.FLOW_ERROR_FIELDS).  kitti: the flows are KITTI PNGs."""
     t0 = time.perf_counter()
-    records, stats, sizes = _score(caffemodel, template, samples, batch, device, threads)
+    records, stats, sizes = _score(caffemodel, template, samples, batch, device, threads, kitti)
     summary = summarize(records, [s.size[0] * s.size[1] for s in samples], _list_name(samples))
     summary.update({"batch": batch, "sizes": sizes, "wall": time.perf_counter() - t0, "busy": stats,
                     "not_finite": [s.where for s in not_finite(samples, records)]})
@@ -206,10 +216,11 @@ def parse_args(argv):
     ap = argparse.ArgumentParser(prog="python -m flownet2_b200.evaluate", description=__doc__.split("\n\n")[0])
     ap.add_argument("caffemodel", help="weights: .caffemodel or .caffemodel.h5")
     ap.add_argument("deployproto", help="deploy prototxt template, e.g. models/FlowNet2_deploy.prototxt.template")
-    ap.add_argument("listfile", help="list of 'img0 img1 flow' lines, flows as .flo or .pfm")
+    ap.add_argument("listfile", help="list of 'img0 img1 flow' lines, flows as .flo or .pfm (KITTI .png with --kitti)")
     ap.add_argument("--batch", type=int, default=1, help="pairs per forward (records reproduce single-pair runs only at 1)")
     ap.add_argument("--per-pair", metavar="TSV", help="write one row per list line: where, img0, img1, flow, valid, EPE, Fl %%")
     ap.add_argument("--gpu", type=int, default=0, help="device to use without torchrun")
+    ap.add_argument("--kitti", action="store_true", help="the flows are KITTI 16-bit PNGs (KITTI 2012 / 2015 ground truth)")
     return ap.parse_args(argv)
 
 
@@ -232,7 +243,7 @@ def main(argv=None):
         mine = shard(samples, world, rank)
         local = np.empty((0, len(FLOW_ERROR_FIELDS) + 1))               # this rank's records, each pair's pixel count last
         if mine:
-            records = _score(a.caffemodel, a.deployproto, mine, a.batch, device, None)[0]
+            records = _score(a.caffemodel, a.deployproto, mine, a.batch, device, None, a.kitti)[0]
             local = np.concatenate([records, [[s.size[0] * s.size[1]] for s in mine]], axis=1)
         full = gather_records(local, len(samples), world, rank) if world > 1 else local
         if rank != 0:

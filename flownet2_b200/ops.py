@@ -436,6 +436,25 @@ def flow_to_tensor(payload, format, flags, dst):
     return dst
 
 
+def kitti_flow_to_tensor(payload, flags, dst):
+    """Dense CUDA KITTI flow payloads (any dtype; [N][H][W][3] big-endian uint16, the unfiltered PNG samples) -> dst, a float32
+    (N, 2, H, W) view, NaN at invalid pixels; flags FLOW_UINT16FLOW quantises as the reference's training data."""
+    assert payload.is_cuda and payload.is_contiguous(), "need a dense CUDA payload"
+    check(lib().fn2_kitti_flow_to_tensor(payload.data_ptr(), int(flags), desc(dst), _stream()))
+    return dst
+
+
+def flow_to_kitti_png_rows(flow, out=None):
+    """A float32 (N, 2, H, W) CUDA view of any strides -> out, N*H Paeth-filtered KITTI PNG scanlines of 1 + 6 W bytes (a dense
+    uint8 CUDA tensor of at least N*H*(1 + 6 W) bytes; a new (N, H, 1 + 6 W) one if None)."""
+    N, _, H, W = flow.shape
+    if out is None:
+        out = torch.empty((N, H, 1 + 6 * W), dtype=torch.uint8, device=flow.device)
+    assert out.is_cuda and out.dtype == torch.uint8 and out.is_contiguous() and out.numel() >= N * H * (1 + 6 * W)
+    check(lib().fn2_flow_to_kitti_png_rows(desc(flow), out.data_ptr(), _stream()))
+    return out
+
+
 def flow_error_workspace_bytes(N, H, W):
     return _size(lib().fn2_flow_error_workspace_bytes, N, H, W)
 

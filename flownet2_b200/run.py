@@ -1,7 +1,7 @@
 """Optical flow of image files: the command line of the reference's scripts/run-flownet.py and run-flownet-many.py.
 
     python -m flownet2_b200.run weights.caffemodel models/FlowNet2_deploy.prototxt.template img0.png img1.png out.flo
-    python -m flownet2_b200.run weights.caffemodel models/FlowNet2_deploy.prototxt.template pairs.txt [--batch 4]
+    python -m flownet2_b200.run weights.caffemodel models/FlowNet2_deploy.prototxt.template pairs.txt [--batch 4] [--kitti]
 
 The list file holds one ``img0 img1 out.flo`` line per pair; blank lines are skipped.  The weights (.caffemodel or
 .caffemodel.h5) are read once.  Pairs are grouped by frame size in order of first appearance, and each size gets one
@@ -13,6 +13,10 @@ them to the reference (palette to RGB or RGBA, LA to L).  The 8-bit frames are c
 converted there (fn2_net_set_input_frames_device), and the flow comes back as (H, W, 2), the payload order of .flo
 (fn2_net_get_blob_nhwc_device).  While batch k runs, batch k+1 is decoded on a thread pool into one of two pinned buffers and
 copied to the device on a copy stream, and batch k-1's flow is copied back on another and written by a writer thread.
+
+--kitti writes every output as a KITTI flow PNG (flownet2_b200.kitti, the format the KITTI benchmark takes) instead of a
+.flo: the flow becomes Paeth-filtered PNG scanlines on the net's stream (fn2_flow_to_kitti_png_rows, 6 bytes a pixel instead
+of 8), and the writer thread deflates them.  A pixel whose flow is not finite is stored as invalid.
 
 There is no NaN-retry loop (the reference retries for a race in its Caffe build that this engine does not have): a pair whose
 flow is not finite is named on stderr and the exit status is 1.  Under torchrun (WORLD_SIZE, RANK, LOCAL_RANK), rank r takes
@@ -275,6 +279,42 @@ class FlowFiles(object):
         self.stats["write"] += time.perf_counter() - t0
 
 
+class KittiFiles(FlowFiles):
+    """run --kitti's sink: on the net's stream each batch's flow becomes KITTI PNG scanlines (fn2_flow_to_kitti_png_rows) and
+    fn2_flow_error against a zero flow counts each pair's non-finite pixels; both come back in one copy, and the writer
+    thread deflates each pair's rows into its file.  A pair with a non-finite pixel is named on stderr and kept in `bad`."""
+
+    def bind(self, torch, batch, H, W, flow_dev):
+        from . import FLOW_ERROR_FIELDS, kitti, ops
+        self.ops, self.kitti, self.size = ops, kitti, (W, H)
+        self.nonfinite, fields = FLOW_ERROR_FIELDS.index("nonfinite"), len(FLOW_ERROR_FIELDS)
+        self.row_bytes = H * (1 + kitti.BPP * W)                          # one pair's scanlines
+        self.rec_off = _align(batch * self.row_bytes, 8)                  # then the pairs' float64 records
+        nb = self.rec_off + batch * fields * 8
+        self.pred = [f.permute(0, 3, 1, 2) for f in flow_dev]             # (B, 2, H, W) views of the NHWC flow
+        self.dev = [torch.empty(nb, dtype=torch.uint8, device="cuda") for _ in range(2)]
+        self.host = [torch.empty(nb, dtype=torch.uint8).pin_memory() for _ in range(2)]
+        self.records = [d[self.rec_off:].view(torch.float64).view(batch, fields) for d in self.dev]
+        self.zero = torch.zeros((batch, 2, H, W), device="cuda")
+        self.workspace = torch.empty(max(ops.flow_error_workspace_bytes(batch, H, W), 8), dtype=torch.uint8, device="cuda")
+
+    def score(self, s):
+        self.ops.flow_to_kitti_png_rows(self.pred[s], self.dev[s])
+        self.ops.flow_error(self.pred[s], self.zero, out=self.records[s], workspace=self.workspace)
+
+    def take(self, pairs, s, n_real):
+        t0 = time.perf_counter()
+        buf = self.host[s].numpy()
+        rec = buf[self.rec_off:].view(np.float64).reshape(len(pairs), -1)
+        n = self.row_bytes
+        for i, p in enumerate(pairs[:n_real]):
+            if rec[i, self.nonfinite] > 0:
+                self.bad.append(p)
+                sys.stderr.write("%s: the flow of %s %s is not finite\n" % (p.where, p.img0, p.img1))
+            self.kitti.write_png_rows(p.out, buf[i * n:(i + 1) * n], *self.size)
+        self.stats["write"] += time.perf_counter() - t0
+
+
 def _group_batches(torch, net, size, pairs, batch, pool, stats, sink):
     """Runs one size's pairs through `net`, B per forward, with decode, copies, forward and the sink's work overlapped."""
     W, H = size
@@ -422,14 +462,14 @@ def run_groups(caffemodel, template, pairs, batch, device, threads, sink, t0):
     return stats, len(groups)
 
 
-def run(caffemodel, template, pairs, batch=1, device=0, threads=None):
-    """Flow of every Pair into its .flo file -> summary dict: pairs, sizes, nets, wall (s), per-stage busy seconds (build:
-    checking the inputs, reading the weights and constructing the nets; decode: host, summed over the pool's threads;
-    h2d / forward / d2h: device; write: host) and the pairs whose flow is not finite."""
+def run(caffemodel, template, pairs, batch=1, device=0, threads=None, kitti=False):
+    """Flow of every Pair into its .flo file (kitti: its KITTI flow PNG) -> summary dict: pairs, sizes, nets, wall (s),
+    per-stage busy seconds (build: checking the inputs, reading the weights and constructing the nets; decode: host, summed
+    over the pool's threads; h2d / forward / d2h: device; write: host) and the pairs whose flow is not finite."""
     t0 = time.perf_counter()
     check_inputs(caffemodel, template, batch)
     probe_pairs(pairs)
-    sink = FlowFiles()
+    sink = KittiFiles() if kitti else FlowFiles()
     stats, sizes = run_groups(caffemodel, template, pairs, batch, device, threads, sink, t0)
     return {"pairs": len(pairs), "sizes": sizes, "nets": sizes, "batch": batch, "wall": time.perf_counter() - t0,
             "busy": stats, "not_finite": [p.where for p in sink.bad]}
@@ -444,6 +484,7 @@ def parse_args(argv):
     ap.add_argument("--gpu", type=int, default=0, help="device to use without torchrun")
     ap.add_argument("--verbose", action="store_true", help="accepted for compatibility; the engine does not log")
     ap.add_argument("--batch", type=int, default=1, help="pairs per forward (outputs bit-identical to single pairs only at 1)")
+    ap.add_argument("--kitti", action="store_true", help="write each output as a KITTI 16-bit flow PNG instead of a .flo")
     a = ap.parse_args(argv)
     if len(a.files) not in (1, 3):
         ap.error("expected img0 img1 out, or one list file; got %d paths" % len(a.files))
@@ -456,7 +497,7 @@ def main(argv=None):
     device = int(os.environ.get("LOCAL_RANK", a.gpu)) if "WORLD_SIZE" in os.environ else a.gpu
     try:
         pairs = read_list(a.files[0]) if len(a.files) == 1 else [Pair("command line", *a.files)]
-        s = run(a.caffemodel, a.deployproto, shard(pairs, world, rank), batch=a.batch, device=device)
+        s = run(a.caffemodel, a.deployproto, shard(pairs, world, rank), batch=a.batch, device=device, kitti=a.kitti)
     except RunError as e:
         sys.stderr.write("error: %s\n" % e)
         return 2

@@ -14,9 +14,10 @@ computed.  The solver's max_iter, snapshot and snapshot_prefix govern the run, a
 smoothed loss over the iterations since the last line.
 
 The data flags mirror CustomData's data_param: permuted with seed 77 unless told otherwise; --flow-encoding float turns off
-the reference's 16-bit quantisation of the ground truth.  Under torchrun (WORLD_SIZE, RANK, LOCAL_RANK) every rank builds the
-net, rank 0's parameters are broadcast, each rank takes its own batches and the gradients are all-reduced before every
-update; only rank 0 writes snapshots.  Refused inputs exit with status 2 and a one-line message.
+the reference's 16-bit quantisation of the ground truth.  --kitti reads every flow of the list as a KITTI 16-bit PNG (sparse
+ground truth: its invalid pixels are NaN, which the NaN-aware losses leave out).  Under torchrun (WORLD_SIZE, RANK,
+LOCAL_RANK) every rank builds the net, rank 0's parameters are broadcast, each rank takes its own batches and the gradients
+are all-reduced before every update; only rank 0 writes snapshots.  Refused inputs exit with status 2 and a one-line message.
 """
 import argparse
 import os
@@ -88,7 +89,8 @@ def train(a, world=1, rank=0, device=0, out=None):
         solver_text = f.read()
     ds = D.FlowDataset(a.data, a.batch, rand_permute=a.rand_permute, rand_permute_seed=a.rand_permute_seed,
                        block_size=a.block_size, range_start=a.range_start, range_end=a.range_end,
-                       rand_permute_order=a.rand_permute_order, flow_encoding=a.flow_encoding, world=world, rank=rank)
+                       rand_permute_order=a.rand_permute_order, flow_encoding=a.flow_encoding, world=world, rank=rank,
+                       kitti=a.kitti)
     torch.cuda.set_device(device)
     net = F.Net(model_text(a.model, crop, ds.size, a.batch), None, F.TRAIN)
     if not weights and not a.snapshot:
@@ -153,6 +155,7 @@ def parse_args(argv):
     ap.add_argument("--range-end", type=int, default=-1, help="last sample used, inclusive (-1: the last)")
     ap.add_argument("--flow-encoding", default="uint16", choices=("uint16", "float"),
                     help="ground truth as the reference's LMDB holds it (uint16, default) or the files' floats")
+    ap.add_argument("--kitti", action="store_true", help="the flows are KITTI 16-bit PNGs (KITTI 2012 / 2015 ground truth)")
     return ap.parse_args(argv)
 
 

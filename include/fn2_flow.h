@@ -15,6 +15,15 @@
  * NaN -> 32767) and CustomData's DecodeData (32767 -> NaN, else short / 32): t = trunc(32 v); NaN when v is NaN or t is
  * outside [-32768, 32766], else t / 32 (a t of zero gives +0).  Below -32768 the reference is undefined; here it is NaN, a
  * value the NaN-aware L1Loss and Downsample ignore.  Without the flag the floats pass through unchanged.
+ *
+ * KITTI flow PNGs (the KITTI 2012 / 2015 devkit's convention, readme.txt / io_flow.h): colour type 2 (RGB), bit depth 16,
+ * not interlaced; R = u, G = v, B = valid as stored.  The host only undoes the PNG container: inflate, then the per-row
+ * filters (fn2_png_unfilter), giving the payload [N][H][W][3] big-endian uint16, H*W*6 bytes per file.  Decode: a pixel is
+ * valid when B > 0, then u = (R - 32768) / 64 and v = (G - 32768) / 64 in float32 (exact); an invalid pixel is NaN in both
+ * channels, the project's marker for missing flow.  FN2_FLOW_UINT16FLOW applies the same trunc(32 v) / 32 as above.
+ * Encode (the devkit's writeFlowField): a pixel is valid when both components are finite; a valid pixel stores
+ * (uint16) max(min(64 v + 32768, 65535), 0) for u and v (float32, truncating) and B = 1, any other pixel (0, 0, 0).  Every
+ * encoded row is filtered with Paeth (type 4): the scanline is the filter byte 4, then the 6 W filtered bytes.
  */
 #ifndef FN2_FLOW_H_
 #define FN2_FLOW_H_
@@ -36,6 +45,21 @@ extern "C" {
 FN2_API int fn2_flow_to_tensor(const void* src_dev, int format, int flags, const fn2_tensor* dst, void* stream);
 /* Input blob `blob` of shape (N, 2, H, W) from device flow payloads, ordered on the net's stream. */
 FN2_API int fn2_net_set_input_flow_device(fn2_net* net, const char* blob, const void* dev, int format, int flags);
+
+/* src_dev (device KITTI payloads of dst.n files, back to back, [N][H][W][3] big-endian uint16, 2-byte aligned) -> dst, any
+ * float view of shape (N, 2, H, W), on stream.  Writes only dst's two channels.  FN2_ERR_INVALID for an unknown flag, an odd
+ * src_dev or dst.c != 2. */
+FN2_API int fn2_kitti_flow_to_tensor(const void* src_dev, int flags, const fn2_tensor* dst, void* stream);
+/* Input blob `blob` of shape (N, 2, H, W) from device KITTI payloads, ordered on the net's stream. */
+FN2_API int fn2_net_set_input_kitti_flow_device(fn2_net* net, const char* blob, const void* dev, int flags);
+/* src, any float view of shape (N, 2, H, W), 4-byte aligned -> dst_dev: N*H PNG scanlines of 1 + 6 W bytes, Paeth-filtered
+ * (image n's row y at (n H + y)(1 + 6 W); the first row of every image is filtered against zeros), on stream.
+ * FN2_ERR_INVALID for src.c != 2 or a misaligned src. */
+FN2_API int fn2_flow_to_kitti_png_rows(const fn2_tensor* src, void* dst_dev, void* stream);
+/* Host: undoes PNG's per-row filters (types 0-4) of `rows` scanlines of 1 + row_bytes bytes at src into rows * row_bytes
+ * bytes at dst; bpp: bytes per complete pixel (1..8), the filters' left distance.  The first row is filtered against zeros.
+ * FN2_ERR_INVALID for a filter type above 4, naming the row.  No device work. */
+FN2_API int fn2_png_unfilter(const void* src, int rows, size_t row_bytes, int bpp, void* dst);
 
 #ifdef __cplusplus
 }
