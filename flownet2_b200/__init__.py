@@ -32,8 +32,8 @@ fn2_tensor, fn2_conv_desc, fn2_l1loss_desc, fn2_lpqloss_desc = (_STRUCTS[n] for 
                                                                                      "fn2_lpqloss_desc"))
 LPQLOSS_STATE_FLOATS = _DEFINES["FN2_LPQLOSS_STATE_FLOATS"]            # device floats of an LpqLoss state (include/fn2_lpq.h)
 # flow payload formats and flags of fn2_flow_to_tensor (include/fn2_flow.h)
-FLOW_FLO, FLOW_PFM, FLOW_PFM_BE, FLOW_UINT16FLOW = (_DEFINES[n] for n in ("FN2_FLOW_FLO", "FN2_FLOW_PFM", "FN2_FLOW_PFM_BE",
-                                                                          "FN2_FLOW_UINT16FLOW"))
+FLOW_FLO, FLOW_PFM, FLOW_PFM_BE, FLOW_KITTI, FLOW_UINT16FLOW = (_DEFINES[n] for n in (
+    "FN2_FLOW_FLO", "FN2_FLOW_PFM", "FN2_FLOW_PFM_BE", "FN2_FLOW_KITTI", "FN2_FLOW_UINT16FLOW"))
 # the per-pair record of fn2_flow_error (include/fn2_eval.h): its field names, lower case, in record order
 FLOW_ERROR_FIELDS = tuple(sorted((k[len("FN2_FLOW_ERROR_"):].lower() for k in _DEFINES
                                  if k.startswith("FN2_FLOW_ERROR_") and k != "FN2_FLOW_ERROR_FIELDS"),
@@ -281,14 +281,10 @@ class Net(object):
         check(lib().fn2_net_set_input_frames_device(self._h, name.encode(), C.c_void_p(dev_ptr), int(channels)))
 
     def set_input_flow_device(self, name, dev_ptr, format, flags=0):
-        """dev_ptr: device address of the payloads of N flow files (FLOW_FLO, FLOW_PFM or FLOW_PFM_BE; 4-byte aligned) for the
-        (N, 2, H, W) input blob `name`; flags FLOW_UINT16FLOW quantises as the reference's training data (include/fn2_flow.h)."""
+        """dev_ptr: device address of the payloads of N flow files (FLOW_FLO, FLOW_PFM or FLOW_PFM_BE, 4-byte aligned; FLOW_KITTI,
+        2-byte aligned) for the (N, 2, H, W) input blob `name`; flags FLOW_UINT16FLOW quantises as the reference's training data
+        (include/fn2_flow.h)."""
         check(lib().fn2_net_set_input_flow_device(self._h, name.encode(), C.c_void_p(dev_ptr), int(format), int(flags)))
-
-    def set_input_kitti_flow_device(self, name, dev_ptr, flags=0):
-        """dev_ptr: device address of the payloads of N KITTI flow PNGs ([N][H][W][3] big-endian uint16, 2-byte aligned;
-        flownet2_b200.kitti) for the (N, 2, H, W) input blob `name`; flags FLOW_UINT16FLOW as in set_input_flow_device."""
-        check(lib().fn2_net_set_input_kitti_flow_device(self._h, name.encode(), C.c_void_p(dev_ptr), int(flags)))
 
     def get_blob_nhwc(self, name):
         """The blob as an (N, H, W, C) array; for the flow, (N, H, W, 2) is the payload of a .flo file per pair."""

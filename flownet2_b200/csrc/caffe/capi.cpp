@@ -167,9 +167,6 @@ int fn2_net_set_input_frames_device(fn2_net* net, const char* blob, const void* 
 int fn2_net_set_input_flow_device(fn2_net* net, const char* blob, const void* dev, int format, int flags) {
     return net_call("set_input_flow_device", net && blob && dev, [&] { net->net->SetInputFlowDevice(blob, dev, format, flags); });
 }
-int fn2_net_set_input_kitti_flow_device(fn2_net* net, const char* blob, const void* dev, int flags) {
-    return net_call("set_input_kitti_flow_device", net && blob && dev, [&] { net->net->SetInputKittiFlowDevice(blob, dev, flags); });
-}
 int fn2_net_get_blob_nhwc(fn2_net* net, const char* blob, float* host) {
     return net_call("get_blob_nhwc", net && blob && host, [&] { net->net->GetBlobNHWC(blob, host); });
 }

@@ -883,13 +883,6 @@ void Net<Dtype>::SetInputFlowDevice(const string& blob, const void* dev, int for
 }
 
 template <typename Dtype>
-void Net<Dtype>::SetInputKittiFlowDevice(const string& blob, const void* dev, int flags) {
-    Caffe::stream() = stream_;
-    fn2_tensor dst = flow_blob(*this, blob)->mutable_tensor();
-    FN2_CALL(fn2_kitti_flow_to_tensor(dev, flags, &dst, stream_));
-}
-
-template <typename Dtype>
 void Net<Dtype>::GetBlobNHWCDevice(const string& blob, Dtype* dev_nhwc) {
     Caffe::stream() = stream_;
     shared_ptr<Blob<Dtype> > b = blob_by_name(blob);

@@ -77,8 +77,6 @@ class Net {
     void SetInputFramesDevice(const string& blob, const void* dev_frames, int channels);
     // flow file payloads on the device -> an (N, 2, H, W) input blob (fn2_flow_to_tensor)
     void SetInputFlowDevice(const string& blob, const void* dev, int format, int flags);
-    // KITTI flow PNG payloads on the device -> an (N, 2, H, W) input blob (fn2_kitti_flow_to_tensor)
-    void SetInputKittiFlowDevice(const string& blob, const void* dev, int flags);
     void GetBlobNHWC(const string& blob, Dtype* host_nhwc);
     void GetBlobNHWCDevice(const string& blob, Dtype* dev_nhwc);
 

@@ -787,7 +787,7 @@ __global__ void flow_to_tensor_kernel(const uint32_t* __restrict__ src, PxView d
 // the flow and Paeth-filters its 6 bytes against them, so no thread reads another's output; the thread of x = 0 also writes
 // the row's filter byte.
 // ---------------------------------------------------------------------------------------------
-__global__ void kitti_flow_to_tensor_kernel(const uint16_t* __restrict__ src, PxView dst, int quantise) {
+__global__ void kitti_samples_to_tensor_kernel(const uint16_t* __restrict__ src, PxView dst, int quantise) {
     const T4& d = dst.t;
     for_each_pixel(d.n, d.h, d.w, [&](int n, int y, int x) {
         const uint16_t* p = src + (((long long)n * d.h + y) * d.w + x) * 3;
@@ -1075,10 +1075,11 @@ int fn2_frames_to_tensor(const void* frames_dev, int channels, const fn2_tensor*
 
 int fn2_flow_to_tensor(const void* src_dev, int format, int flags, const fn2_tensor* dst, void* stream) {
     FN2_CHECK_ARG(src_dev, "flow_to_tensor: src is null");
-    FN2_CHECK_ARG((reinterpret_cast<uintptr_t>(src_dev) & 3) == 0, "flow_to_tensor: src must be 4-byte aligned");
+    FN2_CHECK_ARG(format == FN2_FLOW_FLO || format == FN2_FLOW_PFM || format == FN2_FLOW_PFM_BE || format == FN2_FLOW_KITTI,
+                  "flow_to_tensor: format must be FN2_FLOW_FLO, FN2_FLOW_PFM, FN2_FLOW_PFM_BE or FN2_FLOW_KITTI, got %d", format);
+    const int align = format == FN2_FLOW_KITTI ? 2 : 4;
+    FN2_CHECK_ARG((reinterpret_cast<uintptr_t>(src_dev) & (align - 1)) == 0, "flow_to_tensor: src must be %d-byte aligned", align);
     FN2_CHECK_ARG(valid(dst), "flow_to_tensor: dst is null or empty");
-    FN2_CHECK_ARG(format == FN2_FLOW_FLO || format == FN2_FLOW_PFM || format == FN2_FLOW_PFM_BE,
-                  "flow_to_tensor: format must be FN2_FLOW_FLO, FN2_FLOW_PFM or FN2_FLOW_PFM_BE, got %d", format);
     FN2_CHECK_ARG((flags & ~FN2_FLOW_UINT16FLOW) == 0, "flow_to_tensor: unknown flags 0x%x", flags);
     T4 d = view(dst);
     FN2_CHECK_ARG(d.c == 2, "flow_to_tensor: dst must have 2 channels (u, v), has %d", d.c);
@@ -1087,18 +1088,8 @@ int fn2_flow_to_tensor(const void* src_dev, int format, int flags, const fn2_ten
     const int q = flags & FN2_FLOW_UINT16FLOW;
     if (format == FN2_FLOW_FLO) return ew_launch(flow_to_tensor_kernel<FN2_FLOW_FLO>, total, stream, s, px_view(d), q);
     if (format == FN2_FLOW_PFM) return ew_launch(flow_to_tensor_kernel<FN2_FLOW_PFM>, total, stream, s, px_view(d), q);
-    return ew_launch(flow_to_tensor_kernel<FN2_FLOW_PFM_BE>, total, stream, s, px_view(d), q);
-}
-
-int fn2_kitti_flow_to_tensor(const void* src_dev, int flags, const fn2_tensor* dst, void* stream) {
-    FN2_CHECK_ARG(src_dev, "kitti_flow_to_tensor: src is null");
-    FN2_CHECK_ARG((reinterpret_cast<uintptr_t>(src_dev) & 1) == 0, "kitti_flow_to_tensor: src must be 2-byte aligned");
-    FN2_CHECK_ARG(valid(dst), "kitti_flow_to_tensor: dst is null or empty");
-    FN2_CHECK_ARG((flags & ~FN2_FLOW_UINT16FLOW) == 0, "kitti_flow_to_tensor: unknown flags 0x%x", flags);
-    T4 d = view(dst);
-    FN2_CHECK_ARG(d.c == 2, "kitti_flow_to_tensor: dst must have 2 channels (u, v), has %d", d.c);
-    return ew_launch(kitti_flow_to_tensor_kernel, (long long)d.n * d.h * d.w, stream, static_cast<const uint16_t*>(src_dev),
-                     px_view(d), flags & FN2_FLOW_UINT16FLOW);
+    if (format == FN2_FLOW_PFM_BE) return ew_launch(flow_to_tensor_kernel<FN2_FLOW_PFM_BE>, total, stream, s, px_view(d), q);
+    return ew_launch(kitti_samples_to_tensor_kernel, total, stream, static_cast<const uint16_t*>(src_dev), px_view(d), q);
 }
 
 int fn2_flow_to_kitti_png_rows(const fn2_tensor* src, void* dst_dev, void* stream) {

@@ -3,17 +3,18 @@
     python -m flownet2_b200.evaluate weights.caffemodel models/FlowNet2_deploy.prototxt.template val.txt [--batch B]
                                      [--per-pair out.tsv] [--gpu G] [--kitti]
 
-The list is the train command's: one ``img0 img1 flow`` line per pair (data.read_list; an occlusion field is refused), flows as
-.flo or 'PF' PFM of either byte order.  Frame sizes may differ from line to line; a flow must have its frames' size.  The
-pairs run through flownet2_b200.run's pipeline (one net per frame size, the weights read once, decoding and copies overlapped
-with the forwards); only what happens to each batch's flow differs.  The reader pool reads each ground-truth payload into a
-pinned slot beside the frames, the copy stream moves it to the device, and on the net's stream it is converted
-(fn2_flow_to_tensor, the file's floats unquantised) and scored against the prediction by fn2_flow_error (include/fn2_eval.h).
-Only the per-pair records come back to the host; the padded pairs of a size's last batch are dropped.
+The list is the train command's: one ``img0 img1 flow`` line per pair (files.read_list; an occlusion field is refused), flows
+as .flo or 'PF' PFM of either byte order.  Frame sizes may differ from line to line; a flow must have its frames' size
+(files.probe checks every line before a net is built).  The pairs run through flownet2_b200.run's pipeline (one net per frame
+size, the weights read once, reads and copies overlapped with the forwards); only what happens to each batch's flow differs.
+The feeder's reader pool reads each ground-truth payload into a pinned slot beside the frames, the copy stream moves it to
+the device, and on the net's stream it is converted (fn2_flow_to_tensor, the file's floats unquantised) and scored against
+the prediction by fn2_flow_error (include/fn2_eval.h).  Only the per-pair records come back to the host; the padded pairs of
+a size's last batch are dropped.
 
 --kitti: every flow of the list is a KITTI 16-bit PNG (flownet2_b200.kitti), the ground truth of KITTI 2012 and 2015; sizes
-may differ by line.  The reader pool inflates and unfilters each file into the slot, and fn2_kitti_flow_to_tensor turns the
-samples into the flow on the net's stream, unquantised, with NaN at the pixels the file marks invalid.
+may differ by line.  The reader pool inflates and unfilters each file into the slot, and fn2_flow_to_tensor (FLOW_KITTI)
+turns the samples into the flow on the net's stream, unquantised, with NaN at the pixels the file marks invalid.
 
 Metrics.  A ground-truth pixel is valid when both components are finite and at most 1e9 in absolute value.  EPE is the
 float32 sqrt(du^2 + dv^2) of the prediction minus the ground truth; a valid pixel whose prediction is not finite is counted in
@@ -39,47 +40,25 @@ import time
 import numpy as np
 
 from . import FLOW_ERROR_FIELDS
-from . import kitti as K
-from .data import flow_header, read_flow_into, read_list
-from .run import RunError, check_inputs, probe_pairs, run_groups, shard
+from .files import FLOW_PX_BYTES, RunError, probe, read_list
+from .run import check_inputs, run_groups, shard
 
 FIELD = {name: i for i, name in enumerate(FLOW_ERROR_FIELDS)}
 BANDS = (("s0-10", "n_s0_10", "sum_s0_10"), ("s10-40", "n_s10_40", "sum_s10_40"), ("s40+", "n_s40", "sum_s40"))
-PAYLOAD_PX_BYTES = 12                      # the larger payload per pixel: PFM's three floats (.flo two, a KITTI PNG 6 bytes)
-
-
-def probe_samples(samples, kitti=False):
-    """Sets each sample's frame size and channels (run.probe_pairs) and its flow header; refuses missing or unreadable
-    files, unknown flow suffixes and a flow whose size differs from its frames', naming the list line.  kitti: every flow is a
-    KITTI PNG (kitti.probe)."""
-    probe_pairs(samples)
-    for s in samples:
-        try:
-            fh = K.probe(s.flow) if kitti else flow_header(s.flow)
-        except RunError as e:
-            raise RunError("%s: %s" % (s.where, e))
-        if (fh.width, fh.height) != s.size:
-            raise RunError("%s: %s is %dx%d but its frames are %dx%d" % (s.where, s.flow, fh.width, fh.height, s.size[0], s.size[1]))
-        s.flow_header = fh
 
 
 class Scores(object):
-    """evaluate's per-batch sink for run._group_batches (the interface is described at run.FlowFiles): the ground-truth payloads
-    ride in the frames' slots, are converted on the net's stream before the forward, and each batch's flow is scored on the
-    net's stream; the records of the real pairs land in records[sample.index]."""
+    """evaluate's per-batch sink for run._run_size (the interface is described at run.FlowFiles): the ground-truth payloads
+    ride in the frames' slots, each pair's at a stride that holds any format's, are converted on the net's stream before the
+    forward, and each batch's flow is scored on the net's stream; the records of the real pairs land in
+    records[sample.index]."""
 
     def __init__(self, n):
         self.records = np.full((n, len(FLOW_ERROR_FIELDS)), np.nan)
         self.stats = {"collect": 0.0}
 
-    def payload_bytes(self, batch, H, W):
-        return batch * H * W * PAYLOAD_PX_BYTES
-
-    def read_payload(self, p, out):
-        try:
-            read_flow_into(p.flow, p.flow_header, out[:p.flow_header.nbytes])
-        except (OSError, RunError) as e:
-            raise RunError("%s: %s" % (p.where, e))
+    def item_bytes(self, H, W):
+        return H * W * max(FLOW_PX_BYTES.values())
 
     def bind(self, torch, batch, H, W, flow_dev):
         from . import ops
@@ -95,11 +74,7 @@ class Scores(object):
         """On the net's stream: pair i's payload, at payload[i * stride], into gt[s][i] (formats may differ per pair)."""
         for i, p in enumerate(pairs):
             fh = p.flow_header
-            src = payload[i * stride:i * stride + fh.nbytes]
-            if fh.format == K.KITTI:
-                self.ops.kitti_flow_to_tensor(src, 0, self.gt[s][i:i + 1])
-            else:
-                self.ops.flow_to_tensor(src, fh.format, 0, self.gt[s][i:i + 1])
+            self.ops.flow_to_tensor(payload[i * stride:i * stride + fh.nbytes], fh.format, 0, self.gt[s][i:i + 1])
 
     def score(self, s):
         self.ops.flow_error(self.pred[s], self.gt[s], out=self.dev[s], workspace=self.workspace)
@@ -176,7 +151,7 @@ def _score(caffemodel, template, samples, batch, device, threads, kitti=False):
     """-> (records in the samples' order, per-stage busy seconds, number of sizes)."""
     t0 = time.perf_counter()
     check_inputs(caffemodel, template, batch)
-    probe_samples(samples, kitti)
+    probe(samples, ground_truth=True, kitti=kitti)
     for i, s in enumerate(samples):
         s.index = i
     sink = Scores(len(samples))
@@ -185,7 +160,7 @@ def _score(caffemodel, template, samples, batch, device, threads, kitti=False):
 
 
 def evaluate(caffemodel, template, samples, batch=1, device=0, threads=None, kitti=False):
-    """Scores the net on every data.Sample -> (summary dict, per-pair records): the summary of summarize() plus batch, sizes,
+    """Scores the net on every files.Pair -> (summary dict, per-pair records): the summary of summarize() plus batch, sizes,
     wall (s), per-stage busy seconds and the samples whose prediction is not finite; the records are an (n, FIELDS) float64
     array in the samples' order (fields: flownet2_b200.FLOW_ERROR_FIELDS).  kitti: the flows are KITTI PNGs."""
     t0 = time.perf_counter()

@@ -1,14 +1,14 @@
 """KITTI flow files: the 16-bit RGB PNGs of the KITTI 2012 / 2015 flow benchmarks, read as ground truth and written as
 predictions.  This module is the only place that knows the container; the value convention is stated in include/fn2_flow.h.
 
-    info = probe(path)                      # IHDR only: width, height, nbytes of the payload
+    info = probe(path)                      # IHDR only: a FlowHeader with width, height, nbytes of the payload
     read_payload(path, info, out)           # inflate + unfilter into `out`: [H][W][3] big-endian uint16, the file's own bytes
     write_png_rows(path, rows, w, h)        # scanlines already filtered (fn2_flow_to_kitti_png_rows) -> a PNG file
     read_kitti_flow(path) / write_kitti_flow(path, flow_hw2)     # host helpers in numpy, float32 (H, W, 2) with NaN = invalid
 
 The host only undoes (or makes) the PNG container: the chunks, zlib's deflate and the per-row filters.  The conversion
-between the raw samples and the flow runs on the device (fn2_kitti_flow_to_tensor, fn2_flow_to_kitti_png_rows) in the
-pipelines of data, evaluate and run; the numpy helpers here restate it for users converting files and for the tests.
+between the raw samples and the flow runs on the device (fn2_flow_to_tensor with FLOW_KITTI, fn2_flow_to_kitti_png_rows) in
+the pipelines of data, evaluate and run; the numpy helpers here restate it for users converting files and for the tests.
 
 Accepted: colour type 2 (RGB), bit depth 16, compression, filter and interlace methods 0, any number of IDAT chunks;
 ancillary chunks (and a suggested palette, PLTE) are skipped.  Refused, naming the file: another colour type or depth, an
@@ -21,22 +21,13 @@ import zlib
 
 import numpy as np
 
-from .run import RunError
+from . import FLOW_KITTI
+from .files import FlowHeader, RunError, read_flow
 
-KITTI = "kitti"                             # the flow format of a KITTI PNG (data.FlowHeader.format of .flo / PFM's kind)
 SIGNATURE = b"\x89PNG\r\n\x1a\n"
 BPP = 6                                     # bytes per pixel: three 16-bit samples
-PAYLOAD_PX_BYTES = 6
 LEVEL = 6                                   # zlib's default level, libpng's default
 KNOWN_CRITICAL = (b"IHDR", b"PLTE", b"IDAT", b"IEND")
-
-
-class KittiHeader(object):
-    """A KITTI PNG's size and payload bytes (H * W * 6), shaped like data.FlowHeader."""
-
-    def __init__(self, w, h):
-        self.format, self.width, self.height, self.offset = KITTI, w, h, 0
-        self.nbytes = w * h * PAYLOAD_PX_BYTES
 
 
 def _ihdr(path, head):
@@ -59,11 +50,11 @@ def _ihdr(path, head):
         raise RunError("%s: PNG compression method %d / filter method %d, expected 0 / 0" % (path, comp, filt))
     if w < 1 or h < 1 or w >= 1 << 31 or h >= 1 << 31:
         raise RunError("%s: PNG size %dx%d" % (path, w, h))
-    return KittiHeader(w, h)
+    return FlowHeader(FLOW_KITTI, w, h, 0)
 
 
 def probe(path):
-    """-> KittiHeader from the signature and IHDR alone; refuses what _ihdr refuses, naming the file."""
+    """-> FlowHeader (format FLOW_KITTI) from the signature and IHDR alone; refuses what _ihdr refuses, naming the file."""
     if not os.path.isfile(path):
         raise RunError("%s: no such file" % path)
     with open(path, "rb") as f:
@@ -180,10 +171,7 @@ def paeth_rows(samples):
 
 def read_kitti_flow(path):
     """Host reading of a KITTI flow PNG -> float32 (H, W, 2), NaN in both channels at invalid pixels (unquantised)."""
-    info = probe(path)
-    buf = np.empty(info.nbytes, np.uint8)
-    read_payload(path, info, buf)
-    return decode(buf.view(">u2").reshape(info.height, info.width, 3))
+    return read_flow(path, probe(path))
 
 
 def write_kitti_flow(path, flow_hw2):

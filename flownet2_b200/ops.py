@@ -430,17 +430,10 @@ def frames_to_tensor(frames, dst):
 
 def flow_to_tensor(payload, format, flags, dst):
     """Dense CUDA flow-file payloads (any dtype; .flo [N][H][W][2] or PFM [N][H][W][3] floats, format FLOW_FLO, FLOW_PFM or
-    FLOW_PFM_BE) -> dst, a float32 (N, 2, H, W) view; flags FLOW_UINT16FLOW quantises as the reference's training data."""
+    FLOW_PFM_BE; a KITTI PNG's unfiltered [N][H][W][3] big-endian uint16 samples, FLOW_KITTI, NaN at invalid pixels) -> dst, a
+    float32 (N, 2, H, W) view; flags FLOW_UINT16FLOW quantises as the reference's training data."""
     assert payload.is_cuda and payload.is_contiguous(), "need a dense CUDA payload"
     check(lib().fn2_flow_to_tensor(payload.data_ptr(), int(format), int(flags), desc(dst), _stream()))
-    return dst
-
-
-def kitti_flow_to_tensor(payload, flags, dst):
-    """Dense CUDA KITTI flow payloads (any dtype; [N][H][W][3] big-endian uint16, the unfiltered PNG samples) -> dst, a float32
-    (N, 2, H, W) view, NaN at invalid pixels; flags FLOW_UINT16FLOW quantises as the reference's training data."""
-    assert payload.is_cuda and payload.is_contiguous(), "need a dense CUDA payload"
-    check(lib().fn2_kitti_flow_to_tensor(payload.data_ptr(), int(flags), desc(dst), _stream()))
     return dst
 
 

@@ -25,7 +25,7 @@ import re
 import sys
 import time
 
-from .run import RunError
+from .files import RunError
 
 
 def parse_size(text):

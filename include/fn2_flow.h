@@ -1,15 +1,17 @@
 /*
- * fn2_flow.h -- C-ABI of libfn2.so for ground-truth flow files: the payloads of .flo and PFM files, copied to the device as
- * the bytes they hold after their header, converted there to a network input (the input side of the reference's
- * convert_imageset_and_flow + CustomData training path, without the host-side conversions).  The sibling of fn2_frames.h;
- * fn2.h, fn2_frames.h and this header together state the ABI, with fn2.h's conventions: status 0 or negative with the message
- * in fn2_last_error().
+ * fn2_flow.h -- C-ABI of libfn2.so for ground-truth flow files: the payloads of .flo, PFM and KITTI PNG files, copied to the
+ * device as the bytes they hold after their header (a PNG: once the host has undone its container), converted there to a
+ * network input (the input side of the reference's convert_imageset_and_flow + CustomData training path, without the
+ * host-side conversions).  The sibling of fn2_frames.h; fn2.h, fn2_frames.h and this header together state the ABI, with
+ * fn2.h's conventions: status 0 or negative with the message in fn2_last_error().
  *
  * Formats:
  *   FN2_FLOW_FLO      .flo: little-endian float [N][H][W][2], the payload after the 12-byte 'PIEH' header;
  *   FN2_FLOW_PFM      'PF' PFM with a negative scale (little-endian): float [N][H][W][3], rows stored bottom-to-top;
- *   FN2_FLOW_PFM_BE   the same with a positive scale (big-endian).
- * A PFM is read top-down and keeps channels 0 and 1, as the reference's CImg load_pfm + mirror('y') hands it over.
+ *   FN2_FLOW_PFM_BE   the same with a positive scale (big-endian);
+ *   FN2_FLOW_KITTI    a KITTI flow PNG's unfiltered samples: big-endian uint16 [N][H][W][3] (below).
+ * A payload is 4-byte aligned in the float formats and 2-byte aligned in FN2_FLOW_KITTI.  A PFM is read top-down and keeps
+ * channels 0 and 1, as the reference's CImg load_pfm + mirror('y') hands it over.
  *
  * Flag FN2_FLOW_UINT16FLOW gives the values the reference's training data holds after convert_imageset_and_flow (short(32 v),
  * NaN -> 32767) and CustomData's DecodeData (32767 -> NaN, else short / 32): t = trunc(32 v); NaN when v is NaN or t is
@@ -33,25 +35,20 @@
 #define FN2_FLOW_FLO 0
 #define FN2_FLOW_PFM 1
 #define FN2_FLOW_PFM_BE 2
+#define FN2_FLOW_KITTI 3
 #define FN2_FLOW_UINT16FLOW 1
 
 #ifdef __cplusplus
 extern "C" {
 #endif
 
-/* src_dev (device payloads of dst.n files, back to back, 4-byte aligned) -> dst, any float view of shape (N, 2, H, W), on
- * stream.  Writes only dst's two channels.  FN2_ERR_INVALID for an unknown format or flag, a misaligned src_dev or
- * dst.c != 2. */
+/* src_dev (device payloads of dst.n files of one format, back to back, aligned as the format needs) -> dst, any float view of
+ * shape (N, 2, H, W), on stream.  Writes only dst's two channels.  FN2_ERR_INVALID for an unknown format or flag, a
+ * misaligned src_dev or dst.c != 2. */
 FN2_API int fn2_flow_to_tensor(const void* src_dev, int format, int flags, const fn2_tensor* dst, void* stream);
 /* Input blob `blob` of shape (N, 2, H, W) from device flow payloads, ordered on the net's stream. */
 FN2_API int fn2_net_set_input_flow_device(fn2_net* net, const char* blob, const void* dev, int format, int flags);
 
-/* src_dev (device KITTI payloads of dst.n files, back to back, [N][H][W][3] big-endian uint16, 2-byte aligned) -> dst, any
- * float view of shape (N, 2, H, W), on stream.  Writes only dst's two channels.  FN2_ERR_INVALID for an unknown flag, an odd
- * src_dev or dst.c != 2. */
-FN2_API int fn2_kitti_flow_to_tensor(const void* src_dev, int flags, const fn2_tensor* dst, void* stream);
-/* Input blob `blob` of shape (N, 2, H, W) from device KITTI payloads, ordered on the net's stream. */
-FN2_API int fn2_net_set_input_kitti_flow_device(fn2_net* net, const char* blob, const void* dev, int flags);
 /* src, any float view of shape (N, 2, H, W), 4-byte aligned -> dst_dev: N*H PNG scanlines of 1 + 6 W bytes, Paeth-filtered
  * (image n's row y at (n H + y)(1 + 6 W); the first row of every image is filtered against zeros), on stream.
  * FN2_ERR_INVALID for src.c != 2 or a misaligned src. */

@@ -7,9 +7,9 @@ import numpy as np
 import pytest
 
 from flownet2_b200 import FLOW_ERROR_FIELDS
-from flownet2_b200 import evaluate as E
-from flownet2_b200.data import write_pfm
-from flownet2_b200.run import RunError, shard, write_flo
+from flownet2_b200 import evaluate as E, files as FI
+from flownet2_b200.files import RunError, write_flo, write_pfm
+from flownet2_b200.run import shard
 from tests.test_run_flownet_cpu import write_pnm
 
 FIELD = {f: i for i, f in enumerate(FLOW_ERROR_FIELDS)}
@@ -67,8 +67,8 @@ def test_refusals_name_the_list_line(files, capsys):
     refused(files, capsys, [], r"val\.txt: the list holds no pairs")
     lst = files["dir"] / "ok.txt"
     lst.write_text(good + "\n" + "%s %s %s\n" % (a, b, files["pfm"]))
-    samples = E.read_list(str(lst))
-    E.probe_samples(samples)                                            # a .flo and a PFM in one list are fine
+    samples = FI.read_list(str(lst))
+    FI.probe(samples, ground_truth=True)                                            # a .flo and a PFM in one list are fine
     assert [s.size for s in samples] == [(9, 7)] * 2 and [s.flow_header.nbytes for s in samples] == [9 * 7 * 8, 9 * 7 * 12]
     assert E.main([str(files["dir"] / "none.caffemodel"), str(files["proto"]), str(lst)]) == 2
     assert "none.caffemodel: no such caffemodel" in capsys.readouterr().err

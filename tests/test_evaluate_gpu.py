@@ -11,7 +11,7 @@ import pytest
 from flownet2_b200 import FLOW_ERROR_FIELDS
 from flownet2_b200 import evaluate as E
 from flownet2_b200 import run as R
-from flownet2_b200.data import read_flow, read_list, write_pfm
+from flownet2_b200.files import read_flow, read_list, write_flo, write_pfm
 from tests.flow_error_ref import assert_records_match, flow_error_ref
 from tests.test_run_flownet_cpu import write_pnm
 from tests.test_run_flownet_gpu import chairs_frames
@@ -46,7 +46,7 @@ def scene(tmp_path_factory):
         gt = ground_truth(size, 400 + i)
         if kind == "flo":
             g = str(d / ("g%d.flo" % i))
-            R.write_flo(g, gt)
+            write_flo(g, gt)
         else:
             g = write_pfm(str(d / ("g%d.pfm" % i)), np.concatenate([gt, np.zeros_like(gt[:, :, :1])], axis=2),
                           big_endian=kind == "pfm_be")

@@ -1,5 +1,5 @@
-"""GPU: KITTI flow PNGs on the device.  fn2_kitti_flow_to_tensor bit-exact against kitti.decode (and the uint16 quantisation),
-fn2_flow_to_kitti_png_rows byte-exact against kitti.paeth_rows(kitti.encode(...)), their refusals, and the three commands:
+"""GPU: KITTI flow PNGs on the device.  fn2_flow_to_tensor (FLOW_KITTI) bit-exact against kitti.decode (and the uint16
+quantisation), fn2_flow_to_kitti_png_rows byte-exact against kitti.paeth_rows(kitti.encode(...)), their refusals, and the three commands:
 evaluate on a KITTI list equal to evaluate on the .flo twin list, the dataset's blobs equal to the .flo twin's, and run --kitti
 writing the PNGs of the flows run writes as .flo."""
 import os
@@ -7,7 +7,7 @@ import os
 import numpy as np
 import pytest
 
-from flownet2_b200 import data as D, evaluate as E, kitti as K, run as R, train as T
+from flownet2_b200 import data as D, evaluate as E, files as FI, kitti as K, run as R, train as T
 from tests.test_run_flownet_cpu import write_pnm
 from tests.test_run_flownet_gpu import chairs_frames
 from tests.test_train_data_gpu import TINY_NET, train_net
@@ -33,7 +33,7 @@ def raw_samples(r, n, h, w):
 
 @pytest.mark.parametrize("quant", [0, 1])
 @pytest.mark.parametrize("layout", ["nchw", "pad", "slice"])
-def test_kitti_flow_to_tensor_bit_exact(fn2, quant, layout):
+def test_flow_to_tensor_kitti_bit_exact(fn2, quant, layout):
     import torch
     from flownet2_b200 import ops
     n, h, w = 3, 5, 37                                        # H*W odd: the second payload starts 2 bytes past a 4-byte boundary
@@ -50,7 +50,7 @@ def test_kitti_flow_to_tensor_bit_exact(fn2, quant, layout):
             memory_format=torch.channels_last), 0 if layout == "pad" else 2
     flags = fn2.FLOW_UINT16FLOW if quant else 0
     src = torch.from_numpy(payload.copy()).cuda()
-    ops.kitti_flow_to_tensor(src, flags, parent[:, lo:lo + 2])
+    ops.flow_to_tensor(src, fn2.FLOW_KITTI, flags, parent[:, lo:lo + 2])
     torch.cuda.synchronize()
     got = parent.cpu().numpy()
     assert np.array_equal(bits(got[:, lo:lo + 2]), bits(want))
@@ -58,7 +58,7 @@ def test_kitti_flow_to_tensor_bit_exact(fn2, quant, layout):
     assert np.isnan(want).any() and (np.isnan(want[:, 0]) == np.isnan(want[:, 1])).all()
     # pairs 1 and 2 alone, from a source that is only 2-byte aligned
     one = torch.full((2, 2, h, w), fill, device="cuda")
-    ops.kitti_flow_to_tensor(src[h * w * 6:], flags, one)
+    ops.flow_to_tensor(src[h * w * 6:], fn2.FLOW_KITTI, flags, one)
     assert (src[h * w * 6:].data_ptr() & 3) == 2
     assert np.array_equal(bits(one.cpu().numpy()), bits(want[1:]))
 
@@ -108,12 +108,12 @@ def test_refusals(fn2):
     from flownet2_b200 import ops
     src = torch.zeros(2 * 3 * 4 * 6 + 2, dtype=torch.uint8, device="cuda")
     dst = torch.zeros((2, 2, 3, 4), device="cuda")
-    with pytest.raises(fn2.Fn2Error, match="kitti_flow_to_tensor: unknown flags 0x2"):
-        ops.kitti_flow_to_tensor(src, 2, dst)
-    with pytest.raises(fn2.Fn2Error, match="kitti_flow_to_tensor: dst must have 2 channels"):
-        ops.kitti_flow_to_tensor(src, 0, torch.zeros((2, 3, 3, 4), device="cuda"))
-    with pytest.raises(fn2.Fn2Error, match="kitti_flow_to_tensor: src must be 2-byte aligned"):
-        ops.kitti_flow_to_tensor(src[1:], 0, dst)
+    with pytest.raises(fn2.Fn2Error, match="flow_to_tensor: unknown flags 0x2"):
+        ops.flow_to_tensor(src, fn2.FLOW_KITTI, 2, dst)
+    with pytest.raises(fn2.Fn2Error, match="flow_to_tensor: dst must have 2 channels"):
+        ops.flow_to_tensor(src, fn2.FLOW_KITTI, 0, torch.zeros((2, 3, 3, 4), device="cuda"))
+    with pytest.raises(fn2.Fn2Error, match="flow_to_tensor: src must be 2-byte aligned"):
+        ops.flow_to_tensor(src[1:], fn2.FLOW_KITTI, 0, dst)
     rows = torch.zeros(2 * 3 * (1 + 6 * 4), dtype=torch.uint8, device="cuda")
     with pytest.raises(fn2.Fn2Error, match="flow_to_kitti_png_rows: src must have 2 channels"):
         ops.flow_to_kitti_png_rows(torch.zeros((2, 3, 3, 4), device="cuda"), rows)
@@ -123,7 +123,7 @@ def test_refusals(fn2):
     assert fn2.lib().fn2_last_error().decode() == "flow_to_kitti_png_rows: src must be 4-byte aligned"
     net = fn2.Net(fn2.fill_train_template(fn2.train_template("FlowNet2-C"), 64, 64, 64, 64, 1), None, fn2.TRAIN)
     with pytest.raises(fn2.Fn2Error, match=r"blob img0 must have shape \(N, 2, H, W\)"):
-        net.set_input_kitti_flow_device("img0", src.data_ptr(), 0)
+        net.set_input_flow_device("img0", src.data_ptr(), fn2.FLOW_KITTI)
 
 
 # ---- the commands ----
@@ -145,7 +145,7 @@ def kitti_scene(d, spec, seed):
         a, b = write_pnm(d / ("p%d_0.ppm" % i), f0), write_pnm(d / ("p%d_1.ppm" % i), f1)
         png = K.write_kitti_flow(str(d / ("g%d.png" % i)), sparse_flow(r, *size))
         flo = str(d / ("g%d.flo" % i))
-        R.write_flo(flo, K.read_kitti_flow(png))
+        FI.write_flo(flo, K.read_kitti_flow(png))
         for k, g in (("kitti", png), ("flo", flo), ("run_flo", d / ("o%d.flo" % i)), ("run_png", d / ("o%d.png" % i))):
             lines[k].append("%s %s %s\n" % (a, b, g))
     for k, v in lines.items():
@@ -168,8 +168,8 @@ def test_evaluate_kitti_equals_flo_twin(fn2, flownet2s, capsys):
     d, weights, template = flownet2s
     lists = kitti_scene(d, [(128, 96), (192, 64), (128, 96)], 500)
     for batch in (1, 2):
-        s_png, rec_png = E.evaluate(weights, template, D.read_list(lists["kitti"]), batch=batch, kitti=True)
-        s_flo, rec_flo = E.evaluate(weights, template, D.read_list(lists["flo"]), batch=batch)
+        s_png, rec_png = E.evaluate(weights, template, FI.read_list(lists["kitti"]), batch=batch, kitti=True)
+        s_flo, rec_flo = E.evaluate(weights, template, FI.read_list(lists["flo"]), batch=batch)
         assert np.array_equal(rec_png, rec_flo), batch
         assert s_png["invalid_px"] > 0 and s_png["valid_px"] > 0
         for k in ("pairs", "valid_px", "invalid_px", "nonfinite_px", "epe", "epe_pair_mean", "fl_percent", "s0-10", "s10-40", "s40+"):
@@ -206,7 +206,7 @@ def test_kitti_sink_names_non_finite_pairs(fn2, capsys):
     flow_dev[1][2, 0, 0, 1] = float("nan")
     sink.score(1)
     sink.host[1].copy_(sink.dev[1])
-    pairs = [R.Pair("l:%d" % i, "a", "b", os.devnull) for i in range(B)]
+    pairs = [FI.Pair("l:%d" % i, "a", "b", os.devnull) for i in range(B)]
     sink.take(pairs, 1, 2)                                        # the third pair is padding
     assert [p.where for p in sink.bad] == ["l:1"]
     assert "l:1: the flow of a b is not finite" in capsys.readouterr().err

@@ -8,8 +8,9 @@ import zlib
 import numpy as np
 import pytest
 
-from flownet2_b200 import data as D, evaluate as E, kitti as K, train as T
-from flownet2_b200.run import RunError, write_flo
+import flownet2_b200 as F
+from flownet2_b200 import data as D, evaluate as E, feed as FD, files as FI, kitti as K, train as T
+from flownet2_b200.files import RunError, write_flo
 from tests.test_run_flownet_cpu import write_pnm
 
 Image = pytest.importorskip("PIL.Image")
@@ -170,7 +171,7 @@ def test_accepts_multiple_idats_and_skips_ancillary_chunks(tmp_path):
     p.write_bytes(encode_png(s, [4, 1], idat_parts=5, extra=extra))
     assert np.array_equal(payload_of(p), s)
     info = K.probe(str(p))
-    assert (info.width, info.height, info.nbytes, info.format) == (13, 9, 13 * 9 * 6, K.KITTI)
+    assert (info.width, info.height, info.nbytes, info.format) == (13, 9, 13 * 9 * 6, F.FLOW_KITTI)
 
 
 def refusals():
@@ -246,29 +247,29 @@ def test_refusals_name_the_list_line(tmp_path):
     lst, _, _ = kitti_list(tmp_path, bad=str(bad))
     with pytest.raises(RunError, match=r"kitti\.txt:3: .*interlaced\.png: an interlaced PNG"):
         D.FlowDataset(lst, 2, kitti=True)
-    samples = E.read_list(lst)
+    samples = FI.read_list(lst)
     with pytest.raises(RunError, match=r"kitti\.txt:3: .*interlaced\.png: an interlaced PNG"):
-        E.probe_samples(samples, kitti=True)
+        FI.probe(samples, ground_truth=True, kitti=True)
     # a file whose header is fine and whose data is not: refused by the read, naming the line
     crc = tmp_path / "crc.png"
     good = bytearray(encode_png(samples_of(1), [4]))
     good[good.index(b"IEND") - 5] ^= 0xff
     crc.write_bytes(bytes(good))
     lst, _, _ = kitti_list(tmp_path, bad=str(crc))
-    samples = E.read_list(lst)
-    E.probe_samples(samples, kitti=True)
+    samples = FI.read_list(lst)
+    FI.probe(samples, ground_truth=True, kitti=True)
     with pytest.raises(RunError, match=r"kitti\.txt:3: .*crc\.png: CRC mismatch in chunk IDAT"):
-        E.Scores(3).read_payload(samples[2], np.empty(13 * 9 * 12, np.uint8))
+        FD.read_part(samples[2], 2, (13, 9), 3, np.empty(13 * 9 * 12, np.uint8))
 
 
 def test_evaluate_kitti_list(tmp_path, capsys):
     assert E.parse_args(["w", "t", "l"]).kitti is False and E.parse_args(["w", "t", "l", "--kitti"]).kitti is True
     lst, pngs, flos = kitti_list(tmp_path)
-    samples = E.read_list(lst)
-    E.probe_samples(samples, kitti=True)
+    samples = FI.read_list(lst)
+    FI.probe(samples, ground_truth=True, kitti=True)
     assert [s.flow_header.nbytes for s in samples] == [13 * 9 * 6] * 3
     out = np.empty(13 * 9 * 12, np.uint8)
-    E.Scores(3).read_payload(samples[0], out)
+    FD.read_part(samples[0], 2, (13, 9), 3, out)
     assert np.array_equal(out[:13 * 9 * 6], payload_of(pngs[0]).astype(">u2").view(np.uint8).reshape(-1))
     model, proto = tmp_path / "m.caffemodel", tmp_path / "t.template"
     model.write_bytes(b"")
@@ -288,7 +289,7 @@ def test_train_kitti_list(tmp_path):
     lst, pngs, flos = kitti_list(tmp_path, n=4)
     for enc in ("uint16", "float"):
         ds = D.FlowDataset(lst, 2, flow_encoding=enc, kitti=True)
-        assert ds.size == (13, 9) and ds.flow_format == K.KITTI and ds._flow_px_bytes() == 6
+        assert ds.size == (13, 9) and ds.flow_format == F.FLOW_KITTI and FI.FLOW_PX_BYTES[ds.flow_format] == 6
         twin = tmp_path / "twin.txt"
         twin.write_text("".join(l.replace(p, f) for l, p, f in zip(open(lst).readlines(), pngs, flos)))
         ref = D.FlowDataset(str(twin), 2, flow_encoding=enc)

@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 
 from flownet2_b200 import run as R
+from flownet2_b200.files import read_image
 from tests.test_run_flownet_cpu import write_pnm
 
 pytestmark = pytest.mark.gpu
@@ -186,7 +187,7 @@ def test_single_pair_equals_net_forward(fn2, scene, tmp_path):
         out = str(tmp_path / ("single%d.flo" % i))
         assert R.main([model, TEMPLATE, a, b, out]) == 0
         net = fn2.Net(fn2.fill_template(open(TEMPLATE).read(), w, h), model, fn2.TEST, batch=1)
-        want = net.forward(img0=blob_of([R.read_image(a)]), img1=blob_of([R.read_image(b)]))["predict_flow_final"][0]
+        want = net.forward(img0=blob_of([read_image(a)]), img1=blob_of([read_image(b)]))["predict_flow_final"][0]
         got = fn2.read_flo(out)
         assert got.shape == (2, h, w) and np.array_equal(got, want)
 
@@ -204,8 +205,8 @@ def test_many_pairs_against_oracle_and_single_pair(fn2, scene, tmp_path):
     for size in ((128, 96), (192, 64)):
         idx = [i for i, p in enumerate(pairs) if p[0] == size]
         proto = fn2.fill_template(open(TEMPLATE).read(), *size)
-        img0 = blob_of([R.read_image(pairs[i][1]) for i in idx])
-        img1 = blob_of([R.read_image(pairs[i][2]) for i in idx])
+        img0 = blob_of([read_image(pairs[i][1]) for i in idx])
+        img1 = blob_of([read_image(pairs[i][2]) for i in idx])
         want = OracleNet(proto, weights, batch=len(idx), f64acc=True).forward(img0=img0, img1=img1)["predict_flow_final"]
         for j, i in enumerate(idx):
             got = fn2.read_flo(outs[i])

@@ -7,8 +7,7 @@ import numpy as np
 import pytest
 
 from flownet2_b200 import data as D, train as T
-from flownet2_b200.data import write_pfm
-from flownet2_b200.run import write_flo, write_pnm
+from flownet2_b200.files import write_flo, write_pfm, write_pnm
 
 pytestmark = pytest.mark.gpu
 
@@ -67,8 +66,8 @@ def test_flow_to_tensor_refusals(fn2):
     from flownet2_b200 import ops
     src = torch.zeros(4 * 2 * 3 * 4 * 4, dtype=torch.uint8, device="cuda")
     dst = torch.zeros((1, 2, 3, 4), device="cuda")
-    with pytest.raises(fn2.Fn2Error, match="format must be FN2_FLOW_FLO, FN2_FLOW_PFM or FN2_FLOW_PFM_BE, got 3"):
-        ops.flow_to_tensor(src, 3, 0, dst)
+    with pytest.raises(fn2.Fn2Error, match="format must be FN2_FLOW_FLO, FN2_FLOW_PFM, FN2_FLOW_PFM_BE or FN2_FLOW_KITTI, got 4"):
+        ops.flow_to_tensor(src, 4, 0, dst)
     with pytest.raises(fn2.Fn2Error, match="unknown flags 0x2"):
         ops.flow_to_tensor(src, fn2.FLOW_FLO, 2, dst)
     with pytest.raises(fn2.Fn2Error, match="dst must have 2 channels"):

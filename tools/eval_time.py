@@ -39,7 +39,7 @@ def card(index):
 
 def make_list(d, pairs, seed):
     """--pairs frame pairs with .flo ground truth -> (evaluate's list, run's list)."""
-    from flownet2_b200.run import write_flo, write_pnm
+    from flownet2_b200.files import write_flo, write_pnm
     r = np.random.default_rng(seed)
     yy, xx = np.mgrid[0:H, 0:W]
     ev, rn = [], []
@@ -60,7 +60,8 @@ def make_list(d, pairs, seed):
 
 def pipelines(d, template, pairs, seed):
     import flownet2_b200 as F
-    from flownet2_b200 import data, evaluate, run
+    from flownet2_b200 import evaluate, run
+    from flownet2_b200.files import read_list
     net = F.Net(F.fill_template(F.model_template("FlowNet2"), 128, 128), None, F.TEST, batch=1)
     net.fill_params(1701)
     weights = os.path.join(d, "w.caffemodel")
@@ -70,10 +71,10 @@ def pipelines(d, template, pairs, seed):
     val, rl = make_list(d, pairs, seed)
     out = {}
     for batch in (1, 8):
-        evaluate.evaluate(weights, template, data.read_list(val)[:batch], batch=batch)       # warm-up
-        run.run(weights, template, run.read_list(rl)[:batch], batch=batch)
-        s, _ = evaluate.evaluate(weights, template, data.read_list(val), batch=batch)
-        r = run.run(weights, template, run.read_list(rl), batch=batch)
+        evaluate.evaluate(weights, template, read_list(val)[:batch], batch=batch)       # warm-up
+        run.run(weights, template, read_list(rl, ground_truth=False)[:batch], batch=batch)
+        s, _ = evaluate.evaluate(weights, template, read_list(val), batch=batch)
+        r = run.run(weights, template, read_list(rl, ground_truth=False), batch=batch)
         for name, wall, build in (("evaluate", s["wall"], s["busy"]["build"]), ("run", r["wall"], r["busy"]["build"])):
             out["%s_b%d" % (name, batch)] = {"pairs_per_s": pairs / (wall - build), "wall_s": wall, "build_s": build}
     return out

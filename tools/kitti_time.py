@@ -3,7 +3,7 @@
   * host: --pairs synthetic KITTI ground-truth PNGs of 1242x375 (a smooth flow with half its pixels invalid, written by
     kitti.write_kitti_flow); the median time of kitti.read_payload per file on one thread, and the pool's throughput (files/s)
     reading every file once with 1, 4, 8 and 16 threads;
-  * kernels: fn2_kitti_flow_to_tensor and fn2_flow_to_kitti_png_rows at 8 x 2 x 375 x 1242; --calls back-to-back calls are
+  * kernels: fn2_flow_to_tensor (FLOW_KITTI) and fn2_flow_to_kitti_png_rows at 8 x 2 x 375 x 1242; --calls back-to-back calls are
     captured into one CUDA graph and CUDA events bracket each of --reps replays; the median per call is reported with the bytes
     the kernel must move (decode: 6 B read + 8 B written per pixel; encode: 8 B read + 6 B written per pixel, plus the filter
     bytes) and that rate's share of 3.35 TB/s (H100 SXM HBM3 data sheet);
@@ -36,7 +36,7 @@ W, H = 1242, 375
 def make_lists(d, pairs, seed):
     """Frames and ground truth -> paths of {kitti, flo: evaluate's lists; run_flo, run_png: run's lists} and the PNGs."""
     from flownet2_b200 import kitti
-    from flownet2_b200.run import write_flo, write_pnm
+    from flownet2_b200.files import write_flo, write_pnm
     r = np.random.default_rng(seed)
     yy, xx = np.mgrid[0:H, 0:W].astype(np.float32)
     lines = {k: [] for k in ("kitti", "flo", "run_flo", "run_png")}
@@ -109,7 +109,7 @@ def timed(fn, calls, reps):
 
 def kernels(calls, reps):
     import torch
-    from flownet2_b200 import ops
+    from flownet2_b200 import FLOW_KITTI, ops
     N = 8
     r = torch.Generator(device="cuda").manual_seed(1)
     payload = torch.randint(0, 256, (N * H * W * 6,), dtype=torch.uint8, device="cuda", generator=r)
@@ -117,7 +117,7 @@ def kernels(calls, reps):
     rows = torch.empty((N, H, 1 + 6 * W), dtype=torch.uint8, device="cuda")
     out = {}
     for name, fn, nbytes in (
-            ("kitti_flow_to_tensor", lambda: ops.kitti_flow_to_tensor(payload, 0, flow), N * H * W * 14),
+            ("flow_to_tensor_kitti", lambda: ops.flow_to_tensor(payload, FLOW_KITTI, 0, flow), N * H * W * 14),
             ("flow_to_kitti_png_rows", lambda: ops.flow_to_kitti_png_rows(flow, rows), N * H * W * 8 + rows.numel())):
         t = timed(fn, calls, reps)
         out[name] = {"shape": [N, 2, H, W], "us": t * 1e6, "bytes": nbytes, "gb_per_s": nbytes / t / 1e9,
@@ -127,7 +127,8 @@ def kernels(calls, reps):
 
 def pipelines(d, template, lists, pairs):
     import flownet2_b200 as F
-    from flownet2_b200 import data, evaluate, run
+    from flownet2_b200 import evaluate, run
+    from flownet2_b200.files import read_list
     net = F.Net(F.fill_template(F.model_template("FlowNet2"), 128, 128), None, F.TEST, batch=1)
     net.fill_params(1701)
     weights = os.path.join(d, "w.caffemodel")
@@ -139,11 +140,12 @@ def pipelines(d, template, lists, pairs):
     out = {}
     for batch in (1, 4):
         for name, lst, kitti in (("run_flo", lists["run_flo"], False), ("run_kitti", lists["run_png"], True)):
-            run.run(weights, template, run.read_list(lst)[:batch], batch=batch, kitti=kitti)           # warm-up
-            out["%s_b%d" % (name, batch)] = rate(run.run(weights, template, run.read_list(lst), batch=batch, kitti=kitti))
+            run.run(weights, template, read_list(lst, ground_truth=False)[:batch], batch=batch, kitti=kitti)           # warm-up
+            out["%s_b%d" % (name, batch)] = rate(run.run(weights, template, read_list(lst, ground_truth=False), batch=batch,
+                                                                kitti=kitti))
     for name, lst, kitti in (("evaluate_flo", lists["flo"], False), ("evaluate_kitti", lists["kitti"], True)):
-        evaluate.evaluate(weights, template, data.read_list(lst)[:1], kitti=kitti)
-        s, _ = evaluate.evaluate(weights, template, data.read_list(lst), kitti=kitti)
+        evaluate.evaluate(weights, template, read_list(lst)[:1], kitti=kitti)
+        s, _ = evaluate.evaluate(weights, template, read_list(lst), kitti=kitti)
         out[name + "_b1"] = {"pairs_per_s": pairs / (s["wall"] - s["busy"]["build"]), "wall_s": s["wall"],
                              "epe": s["epe"], "decode_s": s["busy"]["decode"]}
     return out

@@ -40,7 +40,7 @@ def gpu_info():
 
 
 def write_pairs(d, n, w, h, seed=1701):
-    from flownet2_b200 import run as R
+    from flownet2_b200 import files as FI
     try:
         from PIL import Image
     except ImportError:
@@ -61,7 +61,7 @@ def write_pairs(d, n, w, h, seed=1701):
                     fh.write(b"P6\n%d %d\n255\n" % (w, h) + f.tobytes())
             paths.append(p)
         lines.append(paths)
-    assert all(R.probe_image(p)[:2] == (w, h) for l in lines for p in l)
+    assert all(FI.probe_image(p)[:2] == (w, h) for l in lines for p in l)
     return lines
 
 
@@ -74,7 +74,7 @@ def write_list(path, lines, outdir):
     return outs
 
 
-def public_path(F, R, model, template, lines, outs, w, h):
+def public_path(F, FI, model, template, lines, outs, w, h):
     """(a): what a user of the Python API writes today, one pair per forward."""
     import torch
     t0 = time.perf_counter()
@@ -82,7 +82,7 @@ def public_path(F, R, model, template, lines, outs, w, h):
     build = time.perf_counter() - t0
     t1 = time.perf_counter()
     for (a, b), o in zip(lines, outs):
-        flow = net.forward(img0=F.image_to_blob(R.read_image(a)), img1=F.image_to_blob(R.read_image(b)))["predict_flow_final"]
+        flow = net.forward(img0=F.image_to_blob(FI.read_image(a)), img1=F.image_to_blob(FI.read_image(b)))["predict_flow_final"]
         F.write_flo(o, flow[0])
     torch.cuda.synchronize()
     wall = time.perf_counter() - t1
@@ -101,7 +101,7 @@ def main():
     import gc
     import torch
     import flownet2_b200 as F
-    from flownet2_b200 import run as R
+    from flownet2_b200 import files as FI, run as R
     assert torch.cuda.is_available(), "run_many_time.py measures on a GPU; there is no CPU fallback"
     torch.cuda.set_device(0)
     d = args.out or tempfile.mkdtemp(prefix="run_many_time_")
@@ -120,12 +120,12 @@ def main():
         res = {"workload": "%s deploy, %d pairs of %dx%d frames (PPM and PNG), files in to .flo out" % (args.model, args.pairs, w, h)}
         res.update(gpu_info())
         outs_a = write_list(os.path.join(d, "a.txt"), lines, os.path.join(d, "a"))
-        res["a_public_path"] = public_path(F, R, model, template, lines, outs_a, w, h)
+        res["a_public_path"] = public_path(F, FI, model, template, lines, outs_a, w, h)
         gc.collect()
         for key, batch in (("b_driver_batch1", 1), ("c_driver_batch4", 4)):
             lst = os.path.join(d, "%s.txt" % key)
             outs = write_list(lst, lines, os.path.join(d, key))
-            s = R.run(model, template, R.read_list(lst), batch=batch)
+            s = R.run(model, template, FI.read_list(lst, ground_truth=False), batch=batch)
             torch.cuda.synchronize()
             run_s = s["wall"] - s["busy"]["build"]
             res[key] = {"pairs_per_s": args.pairs / run_s, "wall_s": run_s, "build_s": s["busy"]["build"],

@@ -29,8 +29,7 @@ def card():
 def write_dataset(d, n, kind, seed):
     """n samples of 512x384 frames and flows: kind 'ppm' (PPM + .flo) or 'png' (PNG + big-endian PFM) -> list path."""
     from PIL import Image
-    from flownet2_b200.data import write_pfm
-    from flownet2_b200.run import write_flo, write_pnm
+    from flownet2_b200.files import write_flo, write_pfm, write_pnm
     r = np.random.default_rng(seed)
     W, H = 512, 384
     base = r.integers(0, 256, (H + 8, W + 8, 3), dtype=np.uint8)
