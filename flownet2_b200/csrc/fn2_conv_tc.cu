@@ -8,6 +8,11 @@
 //   * 3xTF32: a = a_hi + a_lo, w = w_hi + w_lo (each rounded to TF32), D = a_hi*w_hi + a_hi*w_lo + a_lo*w_hi.
 //     The activation split is done by the MMA warpgroups themselves: each thread reads its elements of the raw tile
 //     straight into the wgmma A register fragment and splits them there (RS form: A from registers, W from shared memory).
+//   * FP16 route (NT == 128, plain K blocks: three quarters of FlowNet2's flops): FP16 has TF32's 11-bit significand at half
+//     the tensor-pipe cost, and a power-of-two scale covers its narrow exponent range exactly.  Per K step and pixel row,
+//     a 2^-e = hi + 2^-11 lo' (e from the row's largest |a|); per layer, w 2^-f = w_hi + 2^-11 w_lo' (f from the largest
+//     |w|), packed as W_A = 2^11 w_hi, W_B = w_lo', W_C = w_hi.  Per 16-channel half, lo' W_C + hi W_B + hi W_A =
+//     2^(11-e-f) a w (m64n128k16 f16 MMAs) into the chunk accumulator, scaled back exactly when it is folded.
 //   * Accumulation: the tensor core truncates its FP32 accumulator, which over K up to 9216 and ~60 layers would shrink
 //     the flow.  Therefore the MMAs only chain over short chunks (kd K steps) in a register accumulator that is then added
 //     into a second, FP32 register accumulator with round-to-nearest, applying the mean truncation loss of a chain of that
@@ -20,6 +25,7 @@
 // epilogue of tile rows 0-63 and 64-127.  Small-Ci inputs use kernel-row or tap-group packing of the K blocks
 // (tc_small_ci).  DESIGN.md section 3 has the reasoning behind each of these choices.
 #include <cuda.h>
+#include <cuda_fp16.h>
 #include <mutex>
 
 #include "fn2_common.cuh"
@@ -63,13 +69,15 @@ struct TcParams {
     // Maps with few channels (wg_G = 8 .. 64 rows per tap) put 128 / wg_G taps side by side in one 128-row tile (wg_TPT).
     int wg_S, wg_ST, wg_BT, wg_segs, wg_segs_x, wg_sx, wg_G, wg_TPT, wg_taps;
     short dy[49], dx[49], widx[49];
+    const uint32_t* wmax;                         // FP16 route: bits of the layer's largest |w|, behind the packed tiles
 };
 
-template <int NT> struct TcGeo {
-    static constexpr int B_TILE_BYTES = NT * 128;
-    static constexpr int STAGE_BYTES = A_TILE_BYTES + 2 * B_TILE_BYTES;
-    // ring of R shared-memory stages (raw A tile + W hi/lo tiles), then the epilogue's staging buffer [128 pixels][STG]
-    static constexpr int R = NT == 128 ? 3 : (NT == 64 ? 4 : 6);
+// FP16 route (NT == 128, plain K blocks): W stage = three FP16 tiles [NT][32 halves] (W_A, W_B, W_C, see tc_pack_f16_kernel)
+template <int NT, bool F16 = false> struct TcGeo {
+    static constexpr int B_TILE_BYTES = F16 ? NT * 64 : NT * 128;
+    static constexpr int STAGE_BYTES = A_TILE_BYTES + (F16 ? 3 : 2) * B_TILE_BYTES;
+    // ring of R shared-memory stages (raw A tile + W tiles), then the epilogue's staging buffer [128 pixels][STG]
+    static constexpr int R = F16 ? 4 : (NT == 128 ? 3 : (NT == 64 ? 4 : 6));
     static constexpr int STG = NT + 4;                                             // floats per staged pixel row
     static constexpr int STG_BYTES = 128 * STG * 4;
     static constexpr int SMEM = R * STAGE_BYTES + STG_BYTES + 1024;
@@ -77,7 +85,8 @@ template <int NT> struct TcGeo {
     //   a_hi*[w_hi|w_lo] into two column blocks and a second one (N = NT, an accumulator of its own: MMAs of different
     //   shapes are not ordered on shared accumulator registers) computes a_lo*w_hi.  NT == 128: all three products chain into one accumulator, cross terms first in every step.
     static constexpr bool WIDE = NT <= 64;
-    static constexpr int MMAS_PER_STEP = 4;                                        // a_hi*w_hi MMAs per step (the chain that truncates)
+    static constexpr int MMAS_PER_STEP = F16 ? 2 : 4;                             // a_hi*w_hi MMAs per step (the chain that truncates)
+    static constexpr float TRUNC_LOSS = F16 ? TRUNC_LOSS_PER_MMA_F16 : TRUNC_LOSS_PER_MMA;
     static_assert(SMEM <= 227 * 1024, "shared memory overflow");
 };
 
@@ -91,6 +100,24 @@ struct TcTile {
 // MODE (compile time, so that each instantiation's role loops stay small -- the all-in-one kernel had ~1900 SASS instructions in
 // the converter loop and stalled on instruction fetch): 0 plain K blocks, 1 tap groups, 2 kernel rows, 3 correlation
 enum { TC_PLAIN = 0, TC_GROUP = 1, TC_ROW = 2, TC_CORR = 3, TC_WGRAD = 4 };
+// the instantiations that take the FP16 route: the forward of the NT = 128 layers in plain K-block mode
+__host__ __device__ constexpr bool tc_f16(int NT, int MODE) { return NT == 128 && MODE == TC_PLAIN; }
+
+// FP16 route, weights: one exponent f per layer from its largest |w| (the float bits `maxbits` that tc_absmax_kernel leaves
+// behind the packed tiles) puts the largest scaled weight in [8, 16), so that W_A = 2^11 w_hi stays below 2^15.  0 for a
+// non-finite maximum; clamped to [-100, 100], the range in which the kernels' power-of-two factors stay normal floats.
+__host__ __device__ __forceinline__ int tc_f16_wexp(uint32_t maxbits) {
+    const int E = (int)(maxbits >> 23);
+    return E >= 255 ? 0 : min(max(E - 130, -100), 100);
+}
+__device__ __forceinline__ float tc_pow2(int k) { return __int_as_float((127 + k) << 23); }     // 2^k, -126 <= k <= 127
+// K slot s (0..31) of a 32-channel block <-> channel of the block: the FP16 A fragment of thread t (t = lane % 4) takes K slots
+// {2t, 2t+1, 2t+8, 2t+9} of each 16-slot half h, which this order maps to channels 8t + 4h + {0, 1, 2, 3} -- one 16-byte chunk
+// of the raw tile row per half, read with one conflict-free 128-bit load.  The weights are packed in the same order.
+__host__ __device__ __forceinline__ int tc_f16_channel(int s) {
+    const int h = s >> 4, j = s & 15;
+    return 8 * ((j & 7) >> 1) + 4 * h + 2 * (j >> 3) + (j & 1);
+}
 
 // whole tile `tile` of the plain, tap-group and kernel-row modes: sample, pixel origin, Co tile, parity class and its taps
 template <int NT>
@@ -184,7 +211,8 @@ template <int NT, int MODE>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapW, const float* __restrict__ bias,
                float* __restrict__ out, float* __restrict__ ws, const TcParams p) {
-    using G = TcGeo<NT>;
+    constexpr bool F16 = tc_f16(NT, MODE);
+    using G = TcGeo<NT, F16>;
     // MMA N: the correlation's halo block has cbw * cbh = 112 pixels (corr_tc_forward)
     constexpr int NM = MODE == TC_CORR ? 112 : NT;
     extern __shared__ __align__(1024) unsigned char smem[];
@@ -220,8 +248,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                 if (!T.valid) continue;
                 const int cx0 = T.v0 * p.su, cy0 = T.u0 * p.sv;
                 auto load_w = [&](unsigned char* st, uint64_t* bar, int c0, int blk) {
-                    tma_load_4d(st + A_TILE_BYTES, &mapW, bar, c0, T.co0, blk, 0);
-                    tma_load_4d(st + A_TILE_BYTES + G::B_TILE_BYTES, &mapW, bar, c0, T.co0, blk, 1);
+                    if constexpr (F16) {
+                        // one box {32 halves, NT, 3 tiles} of K block (tap blk, channel block c0 / 32)
+                        tma_load_4d(st + A_TILE_BYTES, &mapW, bar, 0, T.co0, 0, blk * cblocks + c0 / 32);
+                    } else {
+                        tma_load_4d(st + A_TILE_BYTES, &mapW, bar, c0, T.co0, blk, 0);
+                        tma_load_4d(st + A_TILE_BYTES + G::B_TILE_BYTES, &mapW, bar, c0, T.co0, blk, 1);
+                    }
                 };
                 if constexpr (MODE == TC_CORR) {
                     const int py = T.cls / p.cS, px = T.cls % p.cS;
@@ -317,6 +350,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
         const int m = ct & 127, hf = ct >> 7;      // epilogue: pixel row m, column half hf
         constexpr int NH = NT / 2;
         const int yy = m / p.tw, xx = m % p.tw;
+        // FP16 route: the layer's weight exponent f and the range of the row exponents e that keeps 2^-e, 2^(11-e) and
+        // 2^(e+f-11) normal floats
+        int fw = 0, elo = 0, ehi = 0;
+        if constexpr (F16) {
+            fw = tc_f16_wexp(*p.wmax);
+            elo = max(-116, -115 - fw); ehi = min(126, 138 - fw);
+        }
         int s = 0;
         uint32_t ph = 0;
         for (int tile = blockIdx.x; tile < p.total; tile += gridDim.x) {
@@ -333,7 +373,38 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                 mbar_wait(&full[s], ph);
                 const unsigned char* st = smem + (size_t)s * G::STAGE_BYTES;
                 uint32_t ah[16], al[16];
-                if constexpr (MODE == TC_GROUP) {
+                float rs[2];                       // FP16 route: 2^(e+f-11) of rows r0, r1
+                if constexpr (F16) {
+                    // per row: e from the largest |a| of the row's 32 channels (8 per quad lane), so that |a| 2^-e < 2^15;
+                    // a 2^-e = hi + 2^-11 lo', both FP16 (a_hi / a_lo' in the fragments of the two 16-slot halves)
+#pragma unroll
+                    for (int e = 0; e < 2; e++) {
+                        const int r = e ? r1 : r0;
+                        const float4 v0 = *reinterpret_cast<const float4*>(st + r * 128 + (((2 * t) ^ (r & 7)) << 4));
+                        const float4 v1 = *reinterpret_cast<const float4*>(st + r * 128 + (((2 * t + 1) ^ (r & 7)) << 4));
+                        float mx = fmaxf(fmaxf(fmaxf(fabsf(v0.x), fabsf(v0.y)), fmaxf(fabsf(v0.z), fabsf(v0.w))),
+                                         fmaxf(fmaxf(fabsf(v1.x), fabsf(v1.y)), fmaxf(fabsf(v1.z), fabsf(v1.w))));
+                        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+                        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+                        const int E = (int)(__float_as_uint(mx) >> 23);
+                        const int ex = E == 255 ? 0 : min(max(E - 141, elo), ehi);          // E = 255: no finite max
+                        const float up = tc_pow2(-ex), up11 = tc_pow2(11 - ex);
+                        rs[e] = tc_pow2(ex + fw - 11);
+                        const float4 vh[2] = {v0, v1};
+#pragma unroll
+                        for (int hh = 0; hh < 2; hh++) {
+                            const float x[4] = {vh[hh].x, vh[hh].y, vh[hh].z, vh[hh].w};
+#pragma unroll
+                            for (int q = 0; q < 2; q++) {
+                                const __half2 h = __floats2half2_rn(x[2 * q] * up, x[2 * q + 1] * up);
+                                const float2 hf = __half22float2(h);
+                                const __half2 l = __floats2half2_rn(fmaf(-2048.f, hf.x, x[2 * q] * up11), fmaf(-2048.f, hf.y, x[2 * q + 1] * up11));
+                                ah[4 * hh + 2 * q + e] = *reinterpret_cast<const uint32_t*>(&h);
+                                al[4 * hh + 2 * q + e] = *reinterpret_cast<const uint32_t*>(&l);
+                            }
+                        }
+                    }
+                } else if constexpr (MODE == TC_GROUP) {
                     const int nt = min(gsz, T.ntaps - i * gsz);
                     if (p.gcs == 4) gather_taps<4>(st, r0, r1, t, nt, ah, al);
                     else if (p.gcs == 8) gather_taps<8>(st, r0, r1, t, nt, ah, al);
@@ -370,7 +441,18 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
 #pragma unroll
                 for (int j = 0; j < (int)(sizeof(cx) / sizeof(float)); j++) reg_fence(cx[j]);
                 wgmma_fence();
-                {
+                if constexpr (F16) {
+                    // per 16-slot half: a_lo' * W_C and a_hi * W_B (2^-11 smaller) first, then a_hi * W_A
+                    const uint64_t dA = make_desc_sw64(bh), dB = make_desc_sw64(bh + G::B_TILE_BYTES), dC = make_desc_sw64(bh + 2 * G::B_TILE_BYTES);
+                    const int acc0 = in_chunk != 0;
+#pragma unroll
+                    for (int hh = 0; hh < 2; hh++) {
+                        WgmmaF16<NT>::mma(c, al + 4 * hh, dC + (uint64_t)(2 * hh), acc0 | hh);
+                        WgmmaF16<NT>::mma(c, ah + 4 * hh, dB + (uint64_t)(2 * hh), 1);
+                    }
+#pragma unroll
+                    for (int hh = 0; hh < 2; hh++) WgmmaF16<NT>::mma(c, ah + 4 * hh, dA + (uint64_t)(2 * hh), 1);
+                } else {
                     const int acc0 = in_chunk != 0;
 #pragma unroll
                     for (int kk = 0; kk < 4; kk++) {
@@ -399,8 +481,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                 if (lane == 0) mbar_arrive(&done[s]);
                 if (chunk_end) {
                     // mean truncation loss of the a_hi*w_hi chain of this chunk
-                    const float comp = TRUNC_LOSS_PER_MMA * (float)(G::MMAS_PER_STEP * (in_chunk + 1));
-                    if constexpr (G::WIDE) {
+                    const float comp = G::TRUNC_LOSS * (float)(G::MMAS_PER_STEP * (in_chunk + 1));
+                    if constexpr (F16) {
+                        // the chunk holds 2^(11-e-f) sum a w (one K step: kd == 1); scaling back is exact
+#pragma unroll
+                        for (int j = 0; j < NM / 2; j++) acc[j] = fmaf(fmaf(c[j], comp, c[j]), rs[(j >> 1) & 1], acc[j]);
+                    } else if constexpr (G::WIDE) {
 #pragma unroll
                         for (int j = 0; j < NH; j++) acc[j] += fmaf(c[j], comp, c[j]) + (c[NH + j] + cx[j]);
                     } else {
@@ -502,6 +588,41 @@ __global__ void tc_pack_kernel(const float* __restrict__ w, float* __restrict__ 
         float v = 0.f;
         if (ci < Ci) v = deconv ? w[(((long long)ci * Co + co) * kh + r) * kw + s] : w[(((long long)co * Ci + ci) * kh + r) * kw + s];
         store_tf32_split(wp, per, idx, v);
+    }
+}
+
+// FP16 route: bits of the layer's largest |w| into *out (zeroed before; the bits of non-negative floats order like their values,
+// and a NaN's lie above infinity's)
+__global__ void tc_absmax_kernel(const float* __restrict__ w, long long n, uint32_t* __restrict__ out) {
+    uint32_t m = 0;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+        m = max(m, __float_as_uint(w[i]) & 0x7fffffffu);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if ((threadIdx.x & 31) == 0) atomicMax(out, m);
+}
+
+// FP16 route: [tap][channel block][W_A | W_B | W_C][Co][32 K slots] halves (K slot order tc_f16_channel).  With f from the
+// layer's largest |w| (*wmax) and w_hi = fp16(w 2^-f): W_A = 2^11 w_hi, W_B = fp16(2^11 (w 2^-f - w_hi)), W_C = w_hi (all but
+// the rounding of W_B exact).
+__global__ void tc_pack_f16_kernel(const float* __restrict__ w, __half* __restrict__ wp, int Ci, int Co, int kh, int kw, int cblocks,
+                                   int deconv, const uint32_t* __restrict__ wmax) {
+    const long long per = (long long)kh * kw * cblocks * 3 * Co * 32;
+    const float down = tc_pow2(-tc_f16_wexp(*wmax));
+    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < per; idx += (long long)gridDim.x * blockDim.x) {
+        const int sl = (int)(idx % 32);
+        long long r_ = idx / 32;
+        const int co = (int)(r_ % Co);
+        r_ /= Co;
+        const int part = (int)(r_ % 3), blk = (int)(r_ / 3);
+        const int t = blk / cblocks, ci = (blk % cblocks) * 32 + tc_f16_channel(sl);
+        const int r = t / kw, s = t % kw;
+        float v = 0.f;
+        if (ci < Ci) v = deconv ? w[(((long long)ci * Co + co) * kh + r) * kw + s] : w[(((long long)co * Ci + ci) * kh + r) * kw + s];
+        const float x = v * down;
+        const __half hi = __float2half_rn(x);
+        const float hf = __half2float(hi);
+        wp[idx] = part == 0 ? __float2half_rn(2048.f * hf) : (part == 1 ? __float2half_rn((x - hf) * 2048.f) : hi);
     }
 }
 
@@ -643,6 +764,10 @@ static int tc_split_plan(long long tiles, int steps, int NT, int* first) {
     return bz;
 }
 
+// operand route of a layer: the NT = 128 layers in plain K-block mode run on FP16 operands (three FP16 products per K step with
+// a power-of-two scale per pixel row and per layer), every other layer on TF32 (3xTF32); the weight packing follows it
+static bool tc_f16_route(const fn2_conv_desc* d, const TcSmallCi& sm) { return tc_nt(d->co) == 128 && !sm.mode; }
+
 // layer shapes the engine takes: whole 16-channel output tiles, at most 49 taps, convolution stride <= 2, deconvolution
 // stride 1 or 2 (at most 4 parity classes)
 static bool tc_takes(const fn2_conv_desc* d) {
@@ -655,6 +780,7 @@ struct TcPlan {
     TcParams p;
     TcSmallCi sm;
     int NT, steps;                                // output channels per tile, K steps per tile (the fewest of any parity class)
+    bool f16;                                     // operand route: FP16 (tc_f16_route) or TF32
 };
 // W: input width (kernel-row packing), ci_stride: input pixel stride, ws_floats: workspace available for a K split (a K split
 // that does not fit runs unsplit).  Returns false for a layer the engine does not take, including a deconvolution with a
@@ -671,9 +797,11 @@ static bool tc_plan(const fn2_conv_desc* d, int N, int W, int Ho, int Wo, int ci
     p->Ho = Ho; p->Wo = Wo;
     p->relu = d->relu; p->has_bias = d->has_bias; p->slope = d->negative_slope;
     // the kernel adds back the mean truncation loss of each chunk: TRUNC_LOSS_PER_MMA per a_hi*w_hi MMA chained into the
-    // chunk accumulator (4 per step; with NT == 128 the 8 cross-term MMAs of a step precede them while it is still small)
+    // chunk accumulator (4 per step; with NT == 128 the 8 cross-term MMAs of a step precede them while it is still small; the
+    // FP16 route: TRUNC_LOSS_PER_MMA_F16 per a_hi*W_A MMA, 2 per step after 4 cross-term MMAs, and its row scale needs kd == 1)
     p->kd = tc_chunk_steps(NT);
     *sm = tc_small_ci(d, ci_stride);
+    pl->f16 = tc_f16_route(d, *sm);
     p->gcs = sm->mode == 1 ? sm->cs : 0;
     p->rowmode = sm->mode == 2; p->rcs = sm->cs; p->rblocks = sm->rblocks; p->rsteps = d->kh * sm->rblocks;
     p->rkw = d->kw; p->rpad = d->pad_w; p->rW = W;
@@ -746,10 +874,15 @@ int conv_tc_eligible(const fn2_conv_desc* d, const T4& in, const T4& out) {
     return 1;
 }
 
+// FP16 route: the three FP16 tiles of every K block (48 floats per output channel), then 4 floats holding the bits of the largest
+// |w| (tc_absmax_kernel)
+static size_t tc_f16_tile_floats(const fn2_conv_desc* d) { return (size_t)48 * d->kh * d->kw * d->co * ((d->ci + 31) / 32); }
+
 size_t conv_tc_packed_floats(const fn2_conv_desc* d, int ci_stride) {
     if (d->co % 16) return 0;
     const TcSmallCi sm = tc_small_ci(d, ci_stride);
     if (sm.mode) return (size_t)2 * (sm.mode == 2 ? d->kh * sm.rblocks : sm.ngroups) * d->co * 32;
+    if (tc_f16_route(d, sm)) return tc_f16_tile_floats(d) + 4;
     return (size_t)2 * d->kh * d->kw * d->co * ((d->ci + 31) / 32 * 32);
 }
 
@@ -761,6 +894,17 @@ int conv_tc_pack(const fn2_conv_desc* d, int ci_stride, const float* w, float* w
     if (sm.mode) {
         if (sm.mode == 2) tc_pack_row_kernel<<<ew_grid((long long)floats / 2, 256), 256, 0, st>>>(w, wp, d->ci, d->co, d->kh, d->kw, sm.cs, sm.rblocks);
         else tc_pack_group_kernel<<<ew_grid((long long)floats / 2, 256), 256, 0, st>>>(w, wp, d->ci, d->co, d->kh, d->kw, sm.cs, sm.ngroups);
+        FN2_LAUNCH_CHECK();
+        return FN2_OK;
+    }
+    if (tc_f16_route(d, sm)) {
+        uint32_t* wmax = reinterpret_cast<uint32_t*>(wp + tc_f16_tile_floats(d));
+        const long long n = (long long)d->kh * d->kw * d->ci * d->co;
+        FN2_CUDA(cudaMemsetAsync(wmax, 0, sizeof(uint32_t), st));
+        tc_absmax_kernel<<<ew_grid(n, 256), 256, 0, st>>>(w, n, wmax);
+        FN2_LAUNCH_CHECK();
+        tc_pack_f16_kernel<<<ew_grid((long long)tc_f16_tile_floats(d) * 2, 256), 256, 0, st>>>(
+            w, reinterpret_cast<__half*>(wp), d->ci, d->co, d->kh, d->kw, cip / 32, d->deconv, wmax);
         FN2_LAUNCH_CHECK();
         return FN2_OK;
     }
@@ -783,9 +927,19 @@ int conv_tc_forward(const fn2_conv_desc* d, const T4& in, const float* wp, const
     const TcSmallCi& sm = pl.sm;
     const int NT = pl.NT, su = p.su, sv = p.sv;
     p.out_sn = out.sn; p.out_sh = out.sh; p.out_sw = out.sw;
-    // weights: [2][taps][Co][cip]   (group mode: [2][groups][Co][32])
+    // weights: [2][taps][Co][cip]   (group mode: [2][groups][Co][32]; FP16 route: [taps * cblocks][3][Co][32] halves)
     CUtensorMap mapW;
-    {
+    if (pl.f16) {
+        const int nblk = d->kh * d->kw * p.cblocks;
+        cuuint64_t dims[4] = {32, (cuuint64_t)d->co, 3, (cuuint64_t)nblk};
+        cuuint64_t strides[3] = {64, (cuuint64_t)d->co * 64, (cuuint64_t)d->co * 192};
+        cuuint32_t box[4] = {32, (cuuint32_t)NT, 3, 1};
+        cuuint32_t es[4] = {1, 1, 1, 1};
+        CUresult r = enc(&mapW, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, (void*)wp, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                         CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+        if (r != CUDA_SUCCESS) { set_error("conv_tc: weight tensor map failed (%d)", (int)r); return FN2_ERR_CUDA; }
+        p.wmax = reinterpret_cast<const uint32_t*>(wp + tc_f16_tile_floats(d));
+    } else {
         const int cip = p.cblocks * 32;
         const int kin = sm.mode ? 32 : cip;
         const int nblk = sm.mode == 2 ? p.rsteps : (sm.mode == 1 ? sm.ngroups : d->kh * d->kw);
@@ -825,14 +979,15 @@ int conv_tc_forward(const fn2_conv_desc* d, const T4& in, const float* wp, const
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr; cfg.numAttrs = 1;
+#define TC_SMEM(NTV, MODEV) (TcGeo<NTV, tc_f16(NTV, MODEV)>::SMEM)
 #define FN2_TC_LAUNCH(NTV, MODEV)                                                                                       \
     {                                                                                                                   \
         static bool attr_set = false;                                                                                   \
         if (!attr_set) {                                                                                                \
-            FN2_CUDA(cudaFuncSetAttribute(conv_tc_kernel<NTV, MODEV>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcGeo<NTV>::SMEM)); \
+            FN2_CUDA(cudaFuncSetAttribute(conv_tc_kernel<NTV, MODEV>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM(NTV, MODEV))); \
             attr_set = true;                                                                                            \
         }                                                                                                               \
-        cfg.dynamicSmemBytes = TcGeo<NTV>::SMEM;                                                                        \
+        cfg.dynamicSmemBytes = TC_SMEM(NTV, MODEV);                                                                     \
         FN2_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<NTV, MODEV>, mapA, mapW, bias, out.p, ws, p));                      \
     }
 #define FN2_TC_LAUNCH_NT(MODEV)                                                                                         \
@@ -845,6 +1000,7 @@ int conv_tc_forward(const fn2_conv_desc* d, const T4& in, const float* wp, const
     else { FN2_TC_LAUNCH_NT(TC_PLAIN) }
 #undef FN2_TC_LAUNCH_NT
 #undef FN2_TC_LAUNCH
+#undef TC_SMEM
     FN2_LAUNCH_CHECK();
     if (p.split_z > 1) {
         const long long work = (long long)(p.ntotal - p.split_first) * 128 * (NT / 4);
