@@ -18,8 +18,9 @@
 //     into a second, FP32 register accumulator with round-to-nearest, applying the mean truncation loss of a chain of that
 //     length as a correction.  Within a step the two cross terms (2^-11 smaller) are issued before a_hi*w_hi, so they
 //     enter the chunk accumulator while it is still small.
-//   * Epilogue: the accumulator fragments go through shared memory to one row of 128-bit stores per pixel: + bias, leaky
-//     ReLU, strided NHWC output view (or raw partials into the workspace when the K loop is split over SMs).
+//   * Epilogue: the accumulator fragments go through shared memory to 128-bit stores, consecutive threads along a pixel's
+//     channels (each warp stores whole pixels): + bias, leaky ReLU, strided NHWC output view (or raw partials into the
+//     workspace when the K loop is split over SMs).
 // Persistent kernel, one CTA per SM walking the tile list (pixel tile x Co tile x deconv parity class x K split).
 // Warp roles (384 threads, setmaxnreg re-balances registers): warp 0 TMA producer, warpgroups 1 and 2 the MMAs and the
 // epilogue of tile rows 0-63 and 64-127.  Small-Ci inputs use kernel-row or tap-group packing of the K blocks
@@ -349,7 +350,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
         const int r0 = 64 * wg + 16 * wi + g, r1 = r0 + 8;      // tile rows of this thread's fragment elements
         const int m = ct & 127, hf = ct >> 7;      // epilogue: pixel row m, column half hf
         constexpr int NH = NT / 2;
-        const int yy = m / p.tw, xx = m % p.tw;
+        const int tws = __ffs(p.tw) - 1;           // epilogue: log2 of the tile width (a power of two)
         // FP16 route: the layer's weight exponent f and the range of the row exponents e that keeps 2^-e, 2^(11-e) and
         // 2^(e+f-11) normal floats
         int fw = 0, elo = 0, ehi = 0;
@@ -549,28 +550,36 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                 for (int j = 0; j < NH; j += 4) *reinterpret_cast<float4*>(o + j) = *reinterpret_cast<const float4*>(srow + j);
                 continue;
             }
-            const int u = T.u0 + yy, v = T.v0 + xx;
-            if (u < p.cls_Hu[T.cls] && v < p.cls_Wu[T.cls]) {
-                const int oy = u * p.ou + p.cls_oy0[T.cls], ox = v * p.ov + p.cls_ox0[T.cls];
+            // one float4 of the tile per thread and pass, consecutive threads along a pixel's NT channels: every warp stores
+            // whole pixels (full 32-byte sectors, where a thread per pixel left half of each sector of a store to the next
+            // one), and a thread keeps its 4 channels -- and their bias -- in every pass
+            constexpr int CG = NT / 4, PX = 256 / CG;                  // float4 groups per pixel, pixels per pass
+            const int cg = ct % CG;
+            float bv[4] = {0.f, 0.f, 0.f, 0.f};
+            if (T.slot < 0 && p.has_bias) {
+#pragma unroll
+                for (int e = 0; e < 4; e++) bv[e] = __ldg(bias + T.co0 + 4 * cg + e);
+            }
+#pragma unroll
+            for (int k = 0; k < 128 / PX; k++) {
+                const int px = k * PX + ct / CG;                       // tile pixel
+                const int u = T.u0 + (px >> tws), v = T.v0 + (px & (p.tw - 1));
+                if (u >= p.cls_Hu[T.cls] || v >= p.cls_Wu[T.cls]) continue;
+                const float4 a = *reinterpret_cast<const float4*>(stg + px * G::STG + 4 * cg);
                 if (T.slot >= 0) {
                     // K split: raw partial sums of this K range, [slot][128 pixels][NT]
-                    float* o = ws + ((long long)T.slot * 128 + m) * NT + hf * NH;
-#pragma unroll
-                    for (int j = 0; j < NH; j += 4) *reinterpret_cast<float4*>(o + j) = *reinterpret_cast<const float4*>(srow + j);
-                } else {
-                    float* o = out + T.n * p.out_sn + (long long)oy * p.out_sh + (long long)ox * p.out_sw + T.co0 + hf * NH;
-#pragma unroll
-                    for (int j = 0; j < NH; j += 4) {
-                        const float4 a = *reinterpret_cast<const float4*>(srow + j);
-                        float r[4] = {a.x, a.y, a.z, a.w};
-#pragma unroll
-                        for (int e = 0; e < 4; e++) {
-                            if (p.has_bias) r[e] += __ldg(bias + T.co0 + hf * NH + j + e);
-                            if (p.relu) r[e] = r[e] > 0 ? r[e] : r[e] * p.slope;
-                        }
-                        *reinterpret_cast<float4*>(o + j) = make_float4(r[0], r[1], r[2], r[3]);
-                    }
+                    *reinterpret_cast<float4*>(ws + ((long long)T.slot * 128 + px) * NT + 4 * cg) = a;
+                    continue;
                 }
+                const int oy = u * p.ou + p.cls_oy0[T.cls], ox = v * p.ov + p.cls_ox0[T.cls];
+                float r[4] = {a.x, a.y, a.z, a.w};
+#pragma unroll
+                for (int e = 0; e < 4; e++) {
+                    if (p.has_bias) r[e] += bv[e];
+                    if (p.relu) r[e] = r[e] > 0 ? r[e] : r[e] * p.slope;
+                }
+                *reinterpret_cast<float4*>(out + T.n * p.out_sn + (long long)oy * p.out_sh + (long long)ox * p.out_sw + T.co0 + 4 * cg) =
+                    make_float4(r[0], r[1], r[2], r[3]);
             }
         }
     }
