@@ -15,21 +15,14 @@
 
 namespace fn2 {
 
-// per-tap tensor-core engine (fn2_conv_tc.cu)
+// tensor-core engines (fn2_conv_tc.cu: the per-tap engine, and the taps-on-N engine of fn2_conv_tn.cu for the layers it takes)
 int conv_tc_eligible(const fn2_conv_desc* d, const T4& in, const T4& out);
-int conv_tc_forward(const fn2_conv_desc* d, const T4& in, const float* wp, const float* bias,
-                    const T4& out, float* ws, size_t ws_floats, cudaStream_t st);
-size_t conv_tc_workspace_floats(const fn2_conv_desc* d, int N, int W, int Ho, int Wo);
-void conv_tc_plan(const fn2_conv_desc* d, int N, int W, int Ho, int Wo, int ci_stride, int* out8);
 size_t conv_tc_packed_floats(const fn2_conv_desc* d, int ci_stride);
 int conv_tc_pack(const fn2_conv_desc* d, int ci_stride, const float* w, float* wp, cudaStream_t st);
-// taps-on-N tensor-core engine for few output channels at high resolution (fn2_conv_tn.cu); it takes precedence over the
-// per-tap engine for the layers it applies to
-int conv_tn_applicable(const fn2_conv_desc* d);
-size_t conv_tn_packed_floats(const fn2_conv_desc* d);
-int conv_tn_pack(const fn2_conv_desc* d, const float* w, float* wp, cudaStream_t st);
-int conv_tn_plan(const fn2_conv_desc* d, int N, int Ho, int Wo, int* out8);
-int conv_tn_forward(const fn2_conv_desc* d, const T4& in, const float* wp, const float* bias, const T4& out, cudaStream_t st);
+void conv_tc_plan(const fn2_conv_desc* d, int N, int W, int Ho, int Wo, int ci_stride, int* out8);
+size_t conv_tc_workspace_floats(const fn2_conv_desc* d, int N, int W, int Ho, int Wo);
+int conv_tc_forward(const fn2_conv_desc* d, const T4& in, const float* wp, const float* bias,
+                    const T4& out, float* ws, size_t ws_floats, cudaStream_t st);
 // FP32 SIMT engine for NHWC tensors (fn2_conv_nhwc.cu)
 int conv_nhwc_eligible(const fn2_conv_desc* d, const T4& in, const T4& out);
 size_t conv_nhwc_workspace_floats(const fn2_conv_desc* d, int N, int Ho, int Wo);
@@ -702,7 +695,7 @@ int fn2_conv_out_shape(const fn2_conv_desc* d, int H, int W, int* Ho, int* Wo) {
 int fn2_conv_packed_floats(const fn2_conv_desc* d, int ci_stride, size_t* floats) {
     FN2_CHECK_ARG(d && floats, "conv_packed_floats: null argument");
     const size_t simt = (size_t)d->kh * d->kw * d->ci * d->co;
-    *floats = simt + (conv_tn_applicable(d) ? conv_tn_packed_floats(d) : conv_tc_packed_floats(d, ci_stride));
+    *floats = simt + conv_tc_packed_floats(d, ci_stride);
     return FN2_OK;
 }
 
@@ -713,7 +706,6 @@ int fn2_conv_pack_weights(const fn2_conv_desc* d, int ci_stride, const float* ca
     pack_weights_kernel<<<ew_grid(total, 256), 256, 0, (cudaStream_t)stream>>>(
         caffe_weights_dev, packed_dev, d->ci, d->co, d->kh, d->kw, d->ci, d->deconv);
     FN2_LAUNCH_CHECK();
-    if (conv_tn_applicable(d)) return conv_tn_pack(d, caffe_weights_dev, packed_dev + total, (cudaStream_t)stream);
     return conv_tc_pack(d, ci_stride, caffe_weights_dev, packed_dev + total, (cudaStream_t)stream);
 }
 
@@ -723,8 +715,7 @@ int fn2_conv_plan(const fn2_conv_desc* d, int N, int H, int W, int ci_stride, in
     int rc = fn2_conv_out_shape(d, H, W, &Ho, &Wo);
     if (rc) return rc;
     for (int i = 0; i < 8; i++) plan8[i] = 0;
-    if (conv_tn_applicable(d)) conv_tn_plan(d, N, Ho, Wo, plan8);
-    else conv_tc_plan(d, N, W, Ho, Wo, ci_stride, plan8);
+    conv_tc_plan(d, N, W, Ho, Wo, ci_stride, plan8);
     return FN2_OK;
 }
 
@@ -733,8 +724,7 @@ int fn2_conv_workspace_bytes(const fn2_conv_desc* d, int N, int H, int W, size_t
     int Ho, Wo;
     int rc = fn2_conv_out_shape(d, H, W, &Ho, &Wo);
     if (rc) return rc;
-    const size_t tc = conv_tn_applicable(d) ? 0 : conv_tc_workspace_floats(d, N, W, Ho, Wo);
-    *bytes = max(conv_nhwc_workspace_floats(d, N, Ho, Wo), tc) * sizeof(float);
+    *bytes = max(conv_nhwc_workspace_floats(d, N, Ho, Wo), conv_tc_workspace_floats(d, N, W, Ho, Wo)) * sizeof(float);
     return FN2_OK;
 }
 
@@ -749,11 +739,8 @@ int fn2_conv_forward(const fn2_conv_desc* d, const fn2_tensor* bottom, const flo
     if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     const long long simt_floats = (long long)d->kh * d->kw * d->ci * d->co;
-    if (d->engine != 1 && conv_tc_eligible(d, in, out)) {
-        const float* tcw = packed_weights_dev + simt_floats;
-        if (conv_tn_applicable(d)) return conv_tn_forward(d, in, tcw, bias_dev, out, st);
-        return conv_tc_forward(d, in, tcw, bias_dev, out, (float*)workspace, workspace_bytes / sizeof(float), st);
-    }
+    if (d->engine != 1 && conv_tc_eligible(d, in, out))
+        return conv_tc_forward(d, in, packed_weights_dev + simt_floats, bias_dev, out, (float*)workspace, workspace_bytes / sizeof(float), st);
     FN2_CHECK_ARG(d->engine != 2, "conv: tensor-core engine requested but the shape/layout is not eligible");
     const SimtLaunch L = simt_route(d, in, out);
     // Dynamic shared memory above the default 48 KB needs the kernel's limit raised (per device) to what the launch uses.

@@ -24,10 +24,11 @@
 // Persistent kernel, one CTA per SM walking the tile list (pixel tile x Co tile x deconv parity class x K split).
 // Warp roles (384 threads, setmaxnreg re-balances registers): warp 0 TMA producer, warpgroups 1 and 2 the MMAs and the
 // epilogue of tile rows 0-63 and 64-127.  Small-Ci inputs use kernel-row or tap-group packing of the K blocks
-// (tc_small_ci).  DESIGN.md section 3 has the reasoning behind each of these choices.
+// (tc_weights).  DESIGN.md section 3 has the reasoning behind each of these choices.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <mutex>
+#include <type_traits>
 
 #include "fn2_common.cuh"
 #include "fn2_tc_ptx.cuh"
@@ -698,17 +699,10 @@ __global__ void tc_split_reduce_kernel(const float* __restrict__ ws, const float
     }
 }
 
-int tc_enabled() {
-    static int v = -1;
-    if (v < 0) {
-        const char* e = getenv("FN2_TC");
-        v = (e && e[0] == '0') ? 0 : 1;
-    }
-    return v;
-}
-
-}  // namespace
-
+// The driver's cuTensorMapEncodeTiled, looked up once; nullptr if the driver does not provide it.
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 EncodeTiledFn tc_encode_fn() {
     static EncodeTiledFn fn = nullptr;
     static std::once_flag once;
@@ -721,25 +715,83 @@ EncodeTiledFn tc_encode_fn() {
     return fn;
 }
 
+// f(std::integral_constant<int, NT>()) for the tile width nt (128, 64, 32, else 16)
+template <class F>
+int tc_with_nt(int nt, const F& f) {
+    if (nt == 128) return f(std::integral_constant<int, 128>());
+    if (nt == 64) return f(std::integral_constant<int, 64>());
+    if (nt == 32) return f(std::integral_constant<int, 32>());
+    return f(std::integral_constant<int, 16>());
+}
+
+// conv_tc_kernel<nt, MODE> over p.total tile units; the forward modes with programmatic stream serialization, the weight gradient
+// without
+template <int MODE>
+int tc_run(int nt, cudaStream_t st, const CUtensorMap& mapA, const CUtensorMap& mapW, const float* bias, float* out, float* ws,
+           const TcParams& p) {
+    return tc_with_nt(nt, [&](auto c) {
+        constexpr int NT = decltype(c)::value;
+        return tc_launch<conv_tc_kernel<NT, MODE>>(p.total, TC_THREADS, TcGeo<NT, tc_f16(NT, MODE)>::SMEM, MODE != TC_WGRAD, st,
+                                                   mapA, mapW, bias, out, ws, p);
+    });
+}
+
+}  // namespace
+
+int tc_tensor_map(CUtensorMap* map, const char* what, CUtensorMapDataType dtype, const void* base, const cuuint64_t* dims,
+                  const cuuint64_t* strides, const cuuint32_t* box, const cuuint32_t* es, CUtensorMapSwizzle swizzle,
+                  CUtensorMapL2promotion l2) {
+    EncodeTiledFn enc = tc_encode_fn();
+    if (!enc) { set_error("%s tensor map: cuTensorMapEncodeTiled unavailable", what); return FN2_ERR_CUDA; }
+    const CUresult r = enc(map, dtype, 4, const_cast<void*>(base), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, l2,
+                           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) { set_error("%s tensor map failed (%d)", what, (int)r); return FN2_ERR_CUDA; }
+    return FN2_OK;
+}
+
 // output channels per tile (MMA N) of a layer with `co` output channels
 static int tc_nt(int co) { return (co % 128 == 0) ? 128 : (co % 64 == 0 ? 64 : (co % 32 == 0 ? 32 : 16)); }
 // K steps per accumulation chunk: NT == 128 chains the cross terms into the chunk accumulator too, so its chunks are one step
 static int tc_chunk_steps(int NT) { return NT == 128 ? 1 : 4; }
 
-// Small-Ci packing (plain convolutions with at most 16 input channels): mode 1 = tap groups (several taps share a 32-wide
-// K block, one small TMA box per tap), mode 2 = kernel rows (needs a dense input whose pixel stride equals the padded
-// channel count, and a guard band around the tensor because the row runs of the edge pixels reach a little outside it).
-struct TcSmallCi { int mode, cs, gs, ngroups, rblocks; };
-static TcSmallCi tc_small_ci(const fn2_conv_desc* d, int ci_stride) {
-    TcSmallCi m = {0, 0, 0, 0, 0};
-    if (d->deconv || d->ci > 16 || d->kh * d->kw < 2) return m;
-    m.cs = (d->ci + 3) / 4 * 4;
-    m.gs = 32 / m.cs;
-    m.ngroups = (d->kh * d->kw + m.gs - 1) / m.gs;
-    m.rblocks = (d->kw * m.cs + 31) / 32;
-    m.mode = 1;
-    if (d->input_guard_bytes >= 512 && ci_stride == m.cs && d->kh * m.rblocks <= m.ngroups) m.mode = 2;
-    return m;
+// The per-tap engine's packed weights of a layer read through an input of pixel stride ci_stride: its route and layout.
+//   TF32, plain K blocks:  [hi|lo][tap][Co][cip]                   blocks = taps, width = cip = 32 * cblocks floats
+//   TF32, tap groups:      [hi|lo][group][Co][32]                  K index j*cs + ci for tap group*(32/cs) + j
+//   TF32, kernel rows:     [hi|lo][r*rblocks + kb][Co][32]         K index kb*32 + k = s*cs + ci of kernel row r
+//   FP16:                  [tap*cblocks + cb][W_A|W_B|W_C][Co][32 halves] (tc_pack_f16_kernel), then 4 floats holding the bits
+//                          of the largest |w| (tc_absmax_kernel)
+// Small-Ci packing (plain convolutions with at most 16 input channels): tap groups (several taps share a 32-wide K block, one small
+// TMA box per tap), or kernel rows where they take no more K blocks (needs a dense input whose pixel stride equals the padded
+// channel count, and a guard band around the tensor because the row runs of the edge pixels reach a little outside it).  The
+// NT = 128 layers in plain K-block mode run on FP16 operands (three FP16 products per K step with a power-of-two scale per pixel
+// row and per layer), every other layer on TF32 (3xTF32).
+struct TcWeights {
+    int mode;                 // TC_PLAIN, TC_GROUP or TC_ROW
+    bool f16;                 // FP16 operands (three tiles per K block), else TF32 hi and lo tiles
+    int cs, rblocks;          // small-Ci packing: channels per tap padded to a multiple of 4, K blocks per kernel row
+    int blocks, width, tiles; // K blocks, elements per output channel of a block, tiles per block
+    size_t tile_floats;       // floats of the tiles
+    size_t floats;            // all floats; 0 for a layer without whole 16-channel output tiles
+};
+static TcWeights tc_weights(const fn2_conv_desc* d, int ci_stride) {
+    TcWeights w = {};
+    if (d->co % 16) return w;
+    const int taps = d->kh * d->kw, cblocks = (d->ci + 31) / 32;
+    w.width = 32; w.tiles = 2;
+    if (!d->deconv && d->ci <= 16 && taps >= 2) {
+        w.cs = (d->ci + 3) / 4 * 4;
+        const int gs = 32 / w.cs, ngroups = (taps + gs - 1) / gs;
+        w.rblocks = (d->kw * w.cs + 31) / 32;
+        w.mode = d->input_guard_bytes >= 512 && ci_stride == w.cs && d->kh * w.rblocks <= ngroups ? TC_ROW : TC_GROUP;
+        w.blocks = w.mode == TC_ROW ? d->kh * w.rblocks : ngroups;
+    } else if (tc_nt(d->co) == 128) {
+        w.f16 = true; w.blocks = taps * cblocks; w.tiles = 3;
+    } else {
+        w.blocks = taps; w.width = 32 * cblocks;
+    }
+    w.tile_floats = (size_t)w.blocks * d->co * w.width * w.tiles / (w.f16 ? 2 : 1);
+    w.floats = w.tile_floats + (w.f16 ? 4 : 0);
+    return w;
 }
 
 // K split of a layer with `tiles` tile units of `steps` K steps each (the fewest of any parity class): returns z (1 = unsplit)
@@ -773,10 +825,6 @@ static int tc_split_plan(long long tiles, int steps, int NT, int* first) {
     return bz;
 }
 
-// operand route of a layer: the NT = 128 layers in plain K-block mode run on FP16 operands (three FP16 products per K step with
-// a power-of-two scale per pixel row and per layer), every other layer on TF32 (3xTF32); the weight packing follows it
-static bool tc_f16_route(const fn2_conv_desc* d, const TcSmallCi& sm) { return tc_nt(d->co) == 128 && !sm.mode; }
-
 // layer shapes the engine takes: whole 16-channel output tiles, at most 49 taps, convolution stride <= 2, deconvolution
 // stride 1 or 2 (at most 4 parity classes)
 static bool tc_takes(const fn2_conv_desc* d) {
@@ -784,12 +832,11 @@ static bool tc_takes(const fn2_conv_desc* d) {
     return !d->deconv || d->stride_h == d->stride_w;
 }
 
-// The engine's plan of one layer: every TcParams field of a forward launch except the output view, and the small-Ci packing.
+// The engine's plan of one layer: every TcParams field of a forward launch except the output view, and the packed weights.
 struct TcPlan {
     TcParams p;
-    TcSmallCi sm;
+    TcWeights w;
     int NT, steps;                                // output channels per tile, K steps per tile (the fewest of any parity class)
-    bool f16;                                     // operand route: FP16 (tc_f16_route) or TF32
 };
 // W: input width (kernel-row packing), ci_stride: input pixel stride, ws_floats: workspace available for a K split (a K split
 // that does not fit runs unsplit).  Returns false for a layer the engine does not take, including a deconvolution with a
@@ -799,7 +846,7 @@ static bool tc_plan(const fn2_conv_desc* d, int N, int W, int Ho, int Wo, int ci
     ConvTaps tp;
     conv_taps(d, Ho, Wo, &tp);
     TcParams* p = &pl->p;
-    TcSmallCi* sm = &pl->sm;
+    const TcWeights& w = pl->w = tc_weights(d, ci_stride);
     memset(p, 0, sizeof(*p));
     const int NT = pl->NT = tc_nt(d->co);
     p->N = N; p->cblocks = (d->ci + 31) / 32;
@@ -809,10 +856,8 @@ static bool tc_plan(const fn2_conv_desc* d, int N, int W, int Ho, int Wo, int ci
     // chunk accumulator (4 per step; with NT == 128 the 8 cross-term MMAs of a step precede them while it is still small; the
     // FP16 route: TRUNC_LOSS_PER_MMA_F16 per a_hi*W_A MMA, 2 per step after 4 cross-term MMAs, and its row scale needs kd == 1)
     p->kd = tc_chunk_steps(NT);
-    *sm = tc_small_ci(d, ci_stride);
-    pl->f16 = tc_f16_route(d, *sm);
-    p->gcs = sm->mode == 1 ? sm->cs : 0;
-    p->rowmode = sm->mode == 2; p->rcs = sm->cs; p->rblocks = sm->rblocks; p->rsteps = d->kh * sm->rblocks;
+    p->gcs = w.mode == TC_GROUP ? w.cs : 0;
+    p->rowmode = w.mode == TC_ROW; p->rcs = w.cs; p->rblocks = w.rblocks; p->rsteps = d->kh * w.rblocks;
     p->rkw = d->kw; p->rpad = d->pad_w; p->rW = W;
     // A box element strides: the convolution stride (x, y); a deconvolution's classes are stride-1 convolutions
     p->su = d->deconv ? 1 : d->stride_w; p->sv = d->deconv ? 1 : d->stride_h;
@@ -826,8 +871,7 @@ static bool tc_plan(const fn2_conv_desc* d, int N, int W, int Ho, int Wo, int ci
         Wmax = max(Wmax, tp.Wu[c]); Hmax = max(Hmax, tp.Hu[c]);
     }
     memcpy(p->dy, tp.dy, sizeof(p->dy)); memcpy(p->dx, tp.dx, sizeof(p->dx)); memcpy(p->widx, tp.widx, sizeof(p->widx));
-    if (sm->mode == 1) steps = sm->ngroups;
-    if (sm->mode == 2) steps = p->rsteps;
+    if (w.mode) steps = w.blocks;                 // small-Ci packing: one K step per tap group or kernel-row block
     pl->steps = steps;
     // tile shape: widest power of two covering the (largest) row, 128 pixels per tile
     int tw = 8;
@@ -838,7 +882,7 @@ static bool tc_plan(const fn2_conv_desc* d, int N, int W, int Ho, int Wo, int ci
     p->cotiles = d->co / NT;
     p->ntotal = p->ntiles * p->cotiles * p->ncls;
     int first = p->ntotal, z = 1;
-    if (!sm->mode) z = tc_split_plan(p->ntotal, steps, NT, &first);           // small-Ci packing modes do not split
+    if (!w.mode) z = tc_split_plan(p->ntotal, steps, NT, &first);             // small-Ci packing modes do not split
     if (z > 1 && ws_floats < (size_t)(p->ntotal - first) * z * 128 * NT) { z = 1; first = p->ntotal; }
     p->split_first = first; p->split_z = z;
     p->total = first + (p->ntotal - first) * z;
@@ -851,26 +895,37 @@ static bool tc_plan(const fn2_conv_desc* d, int N, int W, int Ho, int Wo, int ci
 // of slack on top of the partials are the room to move it to a 16-byte boundary.
 constexpr size_t TC_WS_SLACK = 4;
 
+// ---------------------------------------------------------------------------------------------------------------------
+// The tensor-core convolution engines behind fn2_conv.cu: eligibility, packed weights, plan, workspace and forward of a layer.
+// The taps-on-N engine (fn2_conv_tn.cu) owns the layers it takes, the per-tap engine every other layer.
+// ---------------------------------------------------------------------------------------------------------------------
+int conv_tn_applicable(const fn2_conv_desc* d);
+size_t conv_tn_packed_floats(const fn2_conv_desc* d);
+int conv_tn_pack(const fn2_conv_desc* d, const float* w, float* wp, cudaStream_t st);
+int conv_tn_plan(const fn2_conv_desc* d, int N, int Ho, int Wo, int* out8);
+int conv_tn_forward(const fn2_conv_desc* d, const T4& in, const float* wp, const float* bias, const T4& out, cudaStream_t st);
+
+// Which engine owns a layer: taps-on-N (few output channels at high resolution) wherever it applies.
+static bool tc_taps_on_n(const fn2_conv_desc* d) { return conv_tn_applicable(d); }
+
 // workspace of the layer's K split; the pixel stride does not matter: only the small-Ci modes depend on it, and they never split
 size_t conv_tc_workspace_floats(const fn2_conv_desc* d, int N, int W, int Ho, int Wo) {
     TcPlan pl;
-    if (!tc_plan(d, N, W, Ho, Wo, d->ci, SIZE_MAX, &pl) || pl.p.split_z == 1) return 0;
+    if (tc_taps_on_n(d) || !tc_plan(d, N, W, Ho, Wo, d->ci, SIZE_MAX, &pl) || pl.p.split_z == 1) return 0;
     return (size_t)(pl.p.ntotal - pl.p.split_first) * pl.p.split_z * 128 * pl.NT + TC_WS_SLACK;
 }
 
-// plan8 (fn2_conv_plan): {NT, tile units, K steps per tile, small-Ci mode (0 plain, 1 tap groups, 2 kernel rows), first split
-// tile, K ranges per split tile, 0, 0}; left 0 for a layer the engine does not take
+// plan8 (fn2_conv_plan), per-tap engine: {NT, tile units, K steps per tile, small-Ci mode (0 plain, 1 tap groups, 2 kernel rows),
+// first split tile, K ranges per split tile, 0, 0}; taps-on-N: conv_tn_plan; left 0 for a layer neither engine takes
 void conv_tc_plan(const fn2_conv_desc* d, int N, int W, int Ho, int Wo, int ci_stride, int* out8) {
+    if (tc_taps_on_n(d)) { conv_tn_plan(d, N, Ho, Wo, out8); return; }
     TcPlan pl;
     if (!tc_plan(d, N, W, Ho, Wo, ci_stride, SIZE_MAX, &pl)) return;
-    out8[0] = pl.NT; out8[1] = pl.p.ntotal; out8[2] = pl.steps; out8[3] = pl.sm.mode;
+    out8[0] = pl.NT; out8[1] = pl.p.ntotal; out8[2] = pl.steps; out8[3] = pl.w.mode;
     out8[4] = pl.p.split_first; out8[5] = pl.p.split_z;
 }
 
-int conv_tn_applicable(const fn2_conv_desc* d);  // fn2_conv_tn.cu
-
 int conv_tc_eligible(const fn2_conv_desc* d, const T4& in, const T4& out) {
-    if (!tc_enabled()) return 0;
     if (in.sc != 1 || out.sc != 1) return 0;
     if (!tc_takes(d)) return 0;
     if (((uintptr_t)in.p & 15) || (in.sw & 3) || (in.sh & 3) || (in.sn & 3)) return 0;
@@ -879,53 +934,35 @@ int conv_tc_eligible(const fn2_conv_desc* d, const T4& in, const T4& out) {
     // the per-tap engine refuses a deconvolution whose kernel is shorter than its stride (parity classes without taps); the
     // taps-on-N engine takes its own shapes whole
     TcPlan pl;
-    if (!conv_tn_applicable(d) && !tc_plan(d, in.n, in.w, out.h, out.w, (int)in.sw, 0, &pl)) return 0;
-    return 1;
+    return tc_taps_on_n(d) || tc_plan(d, in.n, in.w, out.h, out.w, (int)in.sw, 0, &pl) ? 1 : 0;
 }
 
-// FP16 route: the three FP16 tiles of every K block (48 floats per output channel), then 4 floats holding the bits of the largest
-// |w| (tc_absmax_kernel)
-static size_t tc_f16_tile_floats(const fn2_conv_desc* d) { return (size_t)48 * d->kh * d->kw * d->co * ((d->ci + 31) / 32); }
-
 size_t conv_tc_packed_floats(const fn2_conv_desc* d, int ci_stride) {
-    if (d->co % 16) return 0;
-    const TcSmallCi sm = tc_small_ci(d, ci_stride);
-    if (sm.mode) return (size_t)2 * (sm.mode == 2 ? d->kh * sm.rblocks : sm.ngroups) * d->co * 32;
-    if (tc_f16_route(d, sm)) return tc_f16_tile_floats(d) + 4;
-    return (size_t)2 * d->kh * d->kw * d->co * ((d->ci + 31) / 32 * 32);
+    return tc_taps_on_n(d) ? conv_tn_packed_floats(d) : tc_weights(d, ci_stride).floats;
 }
 
 int conv_tc_pack(const fn2_conv_desc* d, int ci_stride, const float* w, float* wp, cudaStream_t st) {
-    const size_t floats = conv_tc_packed_floats(d, ci_stride);
-    if (!floats) return FN2_OK;
-    const int cip = (d->ci + 31) / 32 * 32;
-    const TcSmallCi sm = tc_small_ci(d, ci_stride);
-    if (sm.mode) {
-        if (sm.mode == 2) tc_pack_row_kernel<<<ew_grid((long long)floats / 2, 256), 256, 0, st>>>(w, wp, d->ci, d->co, d->kh, d->kw, sm.cs, sm.rblocks);
-        else tc_pack_group_kernel<<<ew_grid((long long)floats / 2, 256), 256, 0, st>>>(w, wp, d->ci, d->co, d->kh, d->kw, sm.cs, sm.ngroups);
-        FN2_LAUNCH_CHECK();
-        return FN2_OK;
-    }
-    if (tc_f16_route(d, sm)) {
-        uint32_t* wmax = reinterpret_cast<uint32_t*>(wp + tc_f16_tile_floats(d));
+    if (tc_taps_on_n(d)) return conv_tn_pack(d, w, wp, st);
+    const TcWeights L = tc_weights(d, ci_stride);
+    if (!L.floats) return FN2_OK;
+    if (L.f16) {
+        uint32_t* wmax = reinterpret_cast<uint32_t*>(wp + L.tile_floats);
         const long long n = (long long)d->kh * d->kw * d->ci * d->co;
         FN2_CUDA(cudaMemsetAsync(wmax, 0, sizeof(uint32_t), st));
-        tc_absmax_kernel<<<ew_grid(n, 256), 256, 0, st>>>(w, n, wmax);
-        FN2_LAUNCH_CHECK();
-        tc_pack_f16_kernel<<<ew_grid((long long)tc_f16_tile_floats(d) * 2, 256), 256, 0, st>>>(
-            w, reinterpret_cast<__half*>(wp), d->ci, d->co, d->kh, d->kw, cip / 32, d->deconv, wmax);
-        FN2_LAUNCH_CHECK();
-        return FN2_OK;
+        const int rc = ew_launch(tc_absmax_kernel, n, st, w, n, wmax);
+        if (rc) return rc;
+        return ew_launch(tc_pack_f16_kernel, (long long)L.tile_floats * 2, st, w, reinterpret_cast<__half*>(wp), d->ci, d->co, d->kh,
+                         d->kw, (d->ci + 31) / 32, d->deconv, wmax);
     }
-    tc_pack_kernel<<<ew_grid((long long)floats / 2, 256), 256, 0, st>>>(w, wp, d->ci, d->co, d->kh, d->kw, cip, d->deconv);
-    FN2_LAUNCH_CHECK();
-    return FN2_OK;
+    const long long per = (long long)L.tile_floats / 2;
+    if (L.mode == TC_ROW) return ew_launch(tc_pack_row_kernel, per, st, w, wp, d->ci, d->co, d->kh, d->kw, L.cs, L.rblocks);
+    if (L.mode == TC_GROUP) return ew_launch(tc_pack_group_kernel, per, st, w, wp, d->ci, d->co, d->kh, d->kw, L.cs, L.blocks);
+    return ew_launch(tc_pack_kernel, per, st, w, wp, d->ci, d->co, d->kh, d->kw, L.width, d->deconv);
 }
 
 int conv_tc_forward(const fn2_conv_desc* d, const T4& in, const float* wp, const float* bias, const T4& out, float* ws, size_t ws_floats,
                     cudaStream_t st) {
-    EncodeTiledFn enc = tc_encode_fn();
-    if (!enc) { set_error("conv_tc: cuTensorMapEncodeTiled unavailable"); return FN2_ERR_CUDA; }
+    if (tc_taps_on_n(d)) return conv_tn_forward(d, in, wp, bias, out, st);
     TcPlan pl;
     const size_t avail = ws && ws_floats > TC_WS_SLACK ? ws_floats - TC_WS_SLACK : 0;
     if (!tc_plan(d, in.n, in.w, out.h, out.w, (int)in.sw, avail, &pl)) {
@@ -933,32 +970,24 @@ int conv_tc_forward(const fn2_conv_desc* d, const T4& in, const float* wp, const
     }
     ws = reinterpret_cast<float*>(((uintptr_t)ws + 15) & ~(uintptr_t)15);
     TcParams& p = pl.p;
-    const TcSmallCi& sm = pl.sm;
+    const TcWeights& L = pl.w;
     const int NT = pl.NT, su = p.su, sv = p.sv;
     p.out_sn = out.sn; p.out_sh = out.sh; p.out_sw = out.sw;
-    // weights: [2][taps][Co][cip]   (group mode: [2][groups][Co][32]; FP16 route: [taps * cblocks][3][Co][32] halves)
+    // weights (tc_weights): TF32 {width, Co, blocks, hi|lo} read as boxes {32, NT}, one tile at a time; FP16 {32 halves, Co,
+    // W_A|W_B|W_C, blocks} read as one box {32, NT, 3} per K block
     CUtensorMap mapW;
-    if (pl.f16) {
-        const int nblk = d->kh * d->kw * p.cblocks;
-        cuuint64_t dims[4] = {32, (cuuint64_t)d->co, 3, (cuuint64_t)nblk};
-        cuuint64_t strides[3] = {64, (cuuint64_t)d->co * 64, (cuuint64_t)d->co * 192};
-        cuuint32_t box[4] = {32, (cuuint32_t)NT, 3, 1};
-        cuuint32_t es[4] = {1, 1, 1, 1};
-        CUresult r = enc(&mapW, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, (void*)wp, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                         CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) { set_error("conv_tc: weight tensor map failed (%d)", (int)r); return FN2_ERR_CUDA; }
-        p.wmax = reinterpret_cast<const uint32_t*>(wp + tc_f16_tile_floats(d));
-    } else {
-        const int cip = p.cblocks * 32;
-        const int kin = sm.mode ? 32 : cip;
-        const int nblk = sm.mode == 2 ? p.rsteps : (sm.mode == 1 ? sm.ngroups : d->kh * d->kw);
-        cuuint64_t dims[4] = {(cuuint64_t)kin, (cuuint64_t)d->co, (cuuint64_t)nblk, 2};
-        cuuint64_t strides[3] = {(cuuint64_t)kin * 4, (cuuint64_t)kin * d->co * 4, (cuuint64_t)kin * d->co * nblk * 4};
-        cuuint32_t box[4] = {32, (cuuint32_t)NT, 1, 1};
-        cuuint32_t es[4] = {1, 1, 1, 1};
-        CUresult r = enc(&mapW, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void*)wp, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) { set_error("conv_tc: weight tensor map failed (%d)", (int)r); return FN2_ERR_CUDA; }
+    {
+        const cuuint64_t row = (cuuint64_t)L.width * (L.f16 ? 2 : 4), tile = row * d->co;
+        const int inner = L.f16 ? L.tiles : L.blocks, outer = L.f16 ? L.blocks : L.tiles;
+        const cuuint64_t dims[4] = {(cuuint64_t)L.width, (cuuint64_t)d->co, (cuuint64_t)inner, (cuuint64_t)outer};
+        const cuuint64_t strides[3] = {row, tile, tile * inner};
+        const cuuint32_t box[4] = {32, (cuuint32_t)NT, L.f16 ? 3u : 1u, 1};
+        const cuuint32_t es[4] = {1, 1, 1, 1};
+        const int rc = tc_tensor_map(&mapW, "conv_tc: weight", L.f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32,
+                                     wp, dims, strides, box, es, L.f16 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
+                                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+        if (rc) return rc;
+        if (L.f16) p.wmax = reinterpret_cast<const uint32_t*>(wp + L.tile_floats);
     }
     CUtensorMap mapA;
     {
@@ -975,51 +1004,16 @@ int conv_tc_forward(const fn2_conv_desc* d, const T4& in, const float* wp, const
             box[1] = (cuuint32_t)p.tw; es[1] = 1;
             baseA = in.p - (long long)p.rpad * p.rcs;
         }
-        CUresult r = enc(&mapA, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void*)baseA, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                         p.gcs ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) { set_error("conv_tc: activation tensor map failed (%d)", (int)r); return FN2_ERR_CUDA; }
+        const int rc = tc_tensor_map(&mapA, "conv_tc: activation", CU_TENSOR_MAP_DATA_TYPE_FLOAT32, baseA, dims, strides, box, es,
+                                     p.gcs ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+        if (rc) return rc;
     }
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)min(p.total, num_sms()), 1, 1);
-    cfg.blockDim = dim3(TC_THREADS);
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-#define TC_SMEM(NTV, MODEV) (TcGeo<NTV, tc_f16(NTV, MODEV)>::SMEM)
-#define FN2_TC_LAUNCH(NTV, MODEV)                                                                                       \
-    {                                                                                                                   \
-        static bool attr_set = false;                                                                                   \
-        if (!attr_set) {                                                                                                \
-            FN2_CUDA(cudaFuncSetAttribute(conv_tc_kernel<NTV, MODEV>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM(NTV, MODEV))); \
-            attr_set = true;                                                                                            \
-        }                                                                                                               \
-        cfg.dynamicSmemBytes = TC_SMEM(NTV, MODEV);                                                                     \
-        FN2_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<NTV, MODEV>, mapA, mapW, bias, out.p, ws, p));                      \
-    }
-#define FN2_TC_LAUNCH_NT(MODEV)                                                                                         \
-    if (NT == 128) FN2_TC_LAUNCH(128, MODEV)                                                                            \
-    else if (NT == 64) FN2_TC_LAUNCH(64, MODEV)                                                                         \
-    else if (NT == 32) FN2_TC_LAUNCH(32, MODEV)                                                                         \
-    else FN2_TC_LAUNCH(16, MODEV)
-    if (sm.mode == 2) { FN2_TC_LAUNCH_NT(TC_ROW) }
-    else if (sm.mode == 1) { FN2_TC_LAUNCH_NT(TC_GROUP) }
-    else { FN2_TC_LAUNCH_NT(TC_PLAIN) }
-#undef FN2_TC_LAUNCH_NT
-#undef FN2_TC_LAUNCH
-#undef TC_SMEM
-    FN2_LAUNCH_CHECK();
-    if (p.split_z > 1) {
-        const long long work = (long long)(p.ntotal - p.split_first) * 128 * (NT / 4);
-        if (NT == 128) tc_split_reduce_kernel<128><<<ew_grid(work, 256), 256, 0, st>>>(ws, bias, out.p, p);
-        else if (NT == 64) tc_split_reduce_kernel<64><<<ew_grid(work, 256), 256, 0, st>>>(ws, bias, out.p, p);
-        else if (NT == 32) tc_split_reduce_kernel<32><<<ew_grid(work, 256), 256, 0, st>>>(ws, bias, out.p, p);
-        else tc_split_reduce_kernel<16><<<ew_grid(work, 256), 256, 0, st>>>(ws, bias, out.p, p);
-        FN2_LAUNCH_CHECK();
-    }
-    return FN2_OK;
+    const int rc = L.mode == TC_ROW     ? tc_run<TC_ROW>(NT, st, mapA, mapW, bias, out.p, ws, p)
+                   : L.mode == TC_GROUP ? tc_run<TC_GROUP>(NT, st, mapA, mapW, bias, out.p, ws, p)
+                                        : tc_run<TC_PLAIN>(NT, st, mapA, mapW, bias, out.p, ws, p);
+    if (rc || p.split_z == 1) return rc;
+    const long long work = (long long)(p.ntotal - p.split_first) * 128 * (NT / 4);
+    return tc_with_nt(NT, [&](auto c) { return ew_launch(tc_split_reduce_kernel<decltype(c)::value>, work, st, ws, bias, out.p, p); });
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -1195,7 +1189,7 @@ int conv_tc_wgrad_takes(const fn2_conv_desc* d) {
     return d->engine != 1 && d->kh * d->kw <= 49 && d->stride_w <= 8 && d->stride_h <= 8;
 }
 int conv_tc_wgrad_eligible(const fn2_conv_desc* d) {
-    return tc_enabled() && conv_tc_wgrad_takes(d) && tc_encode_fn() ? 1 : 0;
+    return conv_tc_wgrad_takes(d) && tc_encode_fn() ? 1 : 0;
 }
 size_t conv_tc_wgrad_workspace_floats(const fn2_conv_desc* d, int N, int H, int W) {
     const WgPlan g = wg_plan(d, N, H, W);
@@ -1210,8 +1204,6 @@ void conv_tc_wgrad_plan(const fn2_conv_desc* d, int N, int H, int W, int32_t* ou
 
 int conv_tc_wgrad(const fn2_conv_desc* d, const T4& bottom, const T4& top_diff, float* dw, float* db, int accumulate, float* ws,
                   size_t ws_floats, cudaStream_t st) {
-    EncodeTiledFn enc = tc_encode_fn();
-    if (!enc) { set_error("conv_tc_wgrad: cuTensorMapEncodeTiled unavailable"); return FN2_ERR_CUDA; }
     const WgPlan g = wg_plan(d, bottom.n, bottom.h, bottom.w);
     if (!ws || ws_floats < conv_tc_wgrad_workspace_floats(d, bottom.n, bottom.h, bottom.w)) { set_error("conv_tc_wgrad: workspace too small"); return FN2_ERR_WORKSPACE; }
     const T4& big = d->deconv ? top_diff : bottom;
@@ -1265,51 +1257,32 @@ int conv_tc_wgrad(const fn2_conv_desc* d, const T4& bottom, const T4& top_diff, 
         cuuint64_t strides[3] = {(cuuint64_t)g.Wq_p * 4, (cuuint64_t)g.Hb * g.sx * g.Wq_p * 4, (cuuint64_t)g.Cb * g.Hb * g.sx * g.Wq_p * 4};
         cuuint32_t box[4] = {32, 1, (cuuint32_t)g.G, 1};
         cuuint32_t es[4] = {1, 1, 1, 1};
-        CUresult r = enc(&mapA, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void*)bigT, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) { set_error("conv_tc_wgrad: big-map tensor map failed (%d)", (int)r); return FN2_ERR_CUDA; }
+        const int rc = tc_tensor_map(&mapA, "conv_tc_wgrad: big-map", CU_TENSOR_MAP_DATA_TYPE_FLOAT32, bigT, dims, strides, box, es,
+                                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+        if (rc) return rc;
     }
     {
         cuuint64_t dims[4] = {(cuuint64_t)g.Ws, (cuuint64_t)g.Hs, (cuuint64_t)g.Cs, (cuuint64_t)2 * g.N};
         cuuint64_t strides[3] = {(cuuint64_t)g.Ws_p * 4, (cuuint64_t)g.Hs * g.Ws_p * 4, (cuuint64_t)g.Cs * g.Hs * g.Ws_p * 4};
         cuuint32_t box[4] = {32, 1, (cuuint32_t)g.NT, 1};
         cuuint32_t es[4] = {1, 1, 1, 1};
-        CUresult r = enc(&mapB, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void*)smallT, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) { set_error("conv_tc_wgrad: small-map tensor map failed (%d)", (int)r); return FN2_ERR_CUDA; }
+        const int rc = tc_tensor_map(&mapB, "conv_tc_wgrad: small-map", CU_TENSOR_MAP_DATA_TYPE_FLOAT32, smallT, dims, strides, box, es,
+                                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+        if (rc) return rc;
     }
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)min(p.total, num_sms()), 1, 1);
-    cfg.blockDim = dim3(TC_THREADS);
-    cfg.stream = st;
-#define FN2_WG_LAUNCH(NTV)                                                                                              \
-    {                                                                                                                   \
-        static bool attr_set = false;                                                                                   \
-        if (!attr_set) {                                                                                                \
-            FN2_CUDA(cudaFuncSetAttribute(conv_tc_kernel<NTV, TC_WGRAD>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcGeo<NTV>::SMEM)); \
-            attr_set = true;                                                                                            \
-        }                                                                                                               \
-        cfg.dynamicSmemBytes = TcGeo<NTV>::SMEM;                                                                        \
-        FN2_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<NTV, TC_WGRAD>, mapA, mapB, (const float*)nullptr, (float*)nullptr, part, p)); \
-    }
-    if (g.NT == 128) FN2_WG_LAUNCH(128)
-    else if (g.NT == 64) FN2_WG_LAUNCH(64)
-    else if (g.NT == 32) FN2_WG_LAUNCH(32)
-    else FN2_WG_LAUNCH(16)
-#undef FN2_WG_LAUNCH
-    FN2_LAUNCH_CHECK();
+    const int rc = tc_run<TC_WGRAD>(g.NT, st, mapA, mapB, nullptr, nullptr, part, p);
+    if (rc) return rc;
     wg_reduce_kernel<<<ew_grid((long long)g.Cs * g.Cb * g.taps, 256), 256, 0, st>>>(part, dw, g, accumulate);
     FN2_LAUNCH_CHECK();
     return FN2_OK;
 }
 
 // The correlation route itself is chosen in fn2_corr.cu (corr_fwd_route); this says whether the tensor cores may take it.
-bool corr_tc_available() { return tc_enabled() && tc_encode_fn(); }
+bool corr_tc_available() { return tc_encode_fn() != nullptr; }
 size_t corr_tc_workspace_floats(int N, int C, int H, int W) { return (size_t)2 * N * H * W * C; }
 
 // R = 10, s2 <= 2, C % 32 == 0, channel-fast maps with 16-byte aligned pixels; ws holds corr_tc_workspace_floats
 int corr_tc_forward(const T4& b0, const T4& b1, const T4& top, int R, int s2, float* ws, cudaStream_t st) {
-    EncodeTiledFn enc = tc_encode_fn();
     const int N = b0.n, C = b0.c, H = b0.h, W = b0.w, S = s2;
     float* hi = ws; float* lo = ws + (size_t)N * H * W * C;
     corr_split_kernel<<<ew_grid((long long)N * H * W * (C / 4), 256), 256, 0, st>>>(b1.p, b1.sn, b1.sh, b1.sw, N, H, W, C, hi, lo);
@@ -1337,29 +1310,21 @@ int corr_tc_forward(const T4& b0, const T4& b1, const T4& top, int R, int s2, fl
         cuuint64_t strides[3] = {(cuuint64_t)b0.sw * 4, (cuuint64_t)b0.sh * 4, (cuuint64_t)b0.sn * 4};
         cuuint32_t box[4] = {32, (cuuint32_t)(p.tw * S), (cuuint32_t)(p.th * S), 1};
         cuuint32_t es[4] = {1, (cuuint32_t)S, (cuuint32_t)S, 1};
-        CUresult r = enc(&mapA, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void*)b0.p, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) { set_error("corr_tc: map-0 tensor map failed (%d)", (int)r); return FN2_ERR_CUDA; }
+        const int rc = tc_tensor_map(&mapA, "corr_tc: map-0", CU_TENSOR_MAP_DATA_TYPE_FLOAT32, b0.p, dims, strides, box, es,
+                                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+        if (rc) return rc;
     }
     {
         cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)2 * N};
         cuuint64_t strides[3] = {(cuuint64_t)C * 4, (cuuint64_t)W * C * 4, (cuuint64_t)H * W * C * 4};
         cuuint32_t box[4] = {32, (cuuint32_t)(p.cbw * S), (cuuint32_t)(p.cbh * S), 1};
         cuuint32_t es[4] = {1, (cuuint32_t)S, (cuuint32_t)S, 1};
-        CUresult r = enc(&mapB, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void*)hi, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) { set_error("corr_tc: map-1 tensor map failed (%d)", (int)r); return FN2_ERR_CUDA; }
+        const int rc = tc_tensor_map(&mapB, "corr_tc: map-1", CU_TENSOR_MAP_DATA_TYPE_FLOAT32, hi, dims, strides, box, es,
+                                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+        if (rc) return rc;
     }
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)min(p.total, num_sms()), 1, 1);
-    cfg.blockDim = dim3(TC_THREADS);
-    cfg.stream = st;
-    const int smem_bytes = TcGeo<NT>::SMEM;
-    FN2_CUDA(cudaFuncSetAttribute(conv_tc_kernel<NT, TC_CORR>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
-    cfg.dynamicSmemBytes = smem_bytes;
-    FN2_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<NT, TC_CORR>, mapA, mapB, (const float*)nullptr, top.p, (float*)nullptr, p));
-    FN2_LAUNCH_CHECK();
-    return FN2_OK;
+    return tc_launch<conv_tc_kernel<NT, TC_CORR>>(p.total, TC_THREADS, TcGeo<NT>::SMEM, false, st, mapA, mapB, (const float*)nullptr,
+                                                 top.p, (float*)nullptr, p);
 }
 
 }  // namespace fn2

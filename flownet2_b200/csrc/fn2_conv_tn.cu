@@ -276,37 +276,37 @@ conv_tn_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                             if (nrow > 1) ld8(tsrc + CO, v1);
                             if (nrow > 2) ld8(tsrc + 2 * CO, v2);
                             if (nrow > 3) ld8(tsrc + 3 * CO, v3);
-#define FN2_TN_COMP(x) fmaf(__uint_as_float(x), p.comp, __uint_as_float(x))
+#define TN_COMP(x) fmaf(__uint_as_float(x), p.comp, __uint_as_float(x))
 #pragma unroll
-                            for (int c = 0; c < 8; c++) a0[c] = FN2_TN_COMP(v0[c]);
+                            for (int c = 0; c < 8; c++) a0[c] = TN_COMP(v0[c]);
                             if constexpr (S == 1) {
                                 if (nrow > 1) {
 #pragma unroll
-                                    for (int c = 0; c < 8; c++) a0[c] += __shfl_down_sync(0xffffffffu, FN2_TN_COMP(v1[c]), 1);
+                                    for (int c = 0; c < 8; c++) a0[c] += __shfl_down_sync(0xffffffffu, TN_COMP(v1[c]), 1);
                                 }
                                 if (nrow > 2) {
 #pragma unroll
-                                    for (int c = 0; c < 8; c++) a0[c] += __shfl_down_sync(0xffffffffu, FN2_TN_COMP(v2[c]), 2);
+                                    for (int c = 0; c < 8; c++) a0[c] += __shfl_down_sync(0xffffffffu, TN_COMP(v2[c]), 2);
                                 }
                                 if (nrow > 3) {
 #pragma unroll
-                                    for (int c = 0; c < 8; c++) a0[c] += __shfl_down_sync(0xffffffffu, FN2_TN_COMP(v3[c]), 3);
+                                    for (int c = 0; c < 8; c++) a0[c] += __shfl_down_sync(0xffffffffu, TN_COMP(v3[c]), 3);
                                 }
                             } else {
                                 if (nrow > 1) {
 #pragma unroll
-                                    for (int c = 0; c < 8; c++) a1[c] = FN2_TN_COMP(v1[c]);
+                                    for (int c = 0; c < 8; c++) a1[c] = TN_COMP(v1[c]);
                                 }
                                 if (nrow > 2) {
 #pragma unroll
-                                    for (int c = 0; c < 8; c++) a0[c] += __shfl_up_sync(0xffffffffu, FN2_TN_COMP(v2[c]), 1);
+                                    for (int c = 0; c < 8; c++) a0[c] += __shfl_up_sync(0xffffffffu, TN_COMP(v2[c]), 1);
                                 }
                                 if (nrow > 3) {
 #pragma unroll
-                                    for (int c = 0; c < 8; c++) a1[c] += __shfl_up_sync(0xffffffffu, FN2_TN_COMP(v3[c]), 1);
+                                    for (int c = 0; c < 8; c++) a1[c] += __shfl_up_sync(0xffffffffu, TN_COMP(v3[c]), 1);
                                 }
                             }
-#undef FN2_TN_COMP
+#undef TN_COMP
                             // read-modify-write of 8 different channel planes: all loads first (the compiler must otherwise assume that
                             // the store of plane c aliases the load of plane c+1 and serialises 8 shared-memory round trips)
                             float* o = rowp + c0 * p.CW + ox0;
@@ -404,16 +404,9 @@ __global__ void tn_pack_kernel(const float* __restrict__ w, float* __restrict__ 
     }
 }
 
-int tn_enabled() {
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("FN2_TN"); v = (e && e[0] == '0') ? 0 : 1; }
-    return v;
-}
-
 // Everything that depends on the layer alone (not on the image size): taps, passes, tile shape, strip geometry, ring.
 static bool tn_layer_plan(const fn2_conv_desc* d, TnParams* p) {
     if (d->out_pad_h || d->out_pad_w) return false;               // gradient operators of strided convolutions: general engine
-    if (!tn_enabled()) return false;
     if (d->co != 16 && d->co != 32) return false;
     if (d->ci <= 16 || d->ci > 256) return false;
     if (d->kh > 4 || d->kw > 4 || d->kh * d->kw < 4) return false;
@@ -541,8 +534,6 @@ int conv_tn_plan(const fn2_conv_desc* d, int N, int Ho, int Wo, int* out8) {
 }
 
 int conv_tn_forward(const fn2_conv_desc* d, const T4& in, const float* wp, const float* bias, const T4& out, cudaStream_t st) {
-    EncodeTiledFn enc = tc_encode_fn();
-    if (!enc) { set_error("conv_tn: cuTensorMapEncodeTiled unavailable"); return FN2_ERR_CUDA; }
     TnParams p;
     if (!tn_layer_plan(d, &p)) { set_error("conv_tn: layer not eligible"); return FN2_ERR_INVALID; }
     p.N = in.n; p.Hin = in.h; p.Win = in.w; p.Ho = out.h; p.Wo = out.w;
@@ -572,9 +563,9 @@ int conv_tn_forward(const fn2_conv_desc* d, const T4& in, const float* wp, const
         cuuint64_t strides[3] = {(cuuint64_t)in.sw * 4, (cuuint64_t)in.sh * 4, (cuuint64_t)in.sn * 4};
         cuuint32_t box[4] = {32, (cuuint32_t)p.tw, (cuuint32_t)p.th, 1};
         cuuint32_t es[4] = {1, 1, 1, 1};
-        CUresult r = enc(&mapA, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void*)in.p, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) { set_error("conv_tn: activation tensor map failed (%d)", (int)r); return FN2_ERR_CUDA; }
+        const int rc = tc_tensor_map(&mapA, "conv_tn: activation", CU_TENSOR_MAP_DATA_TYPE_FLOAT32, in.p, dims, strides, box, es,
+                                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+        if (rc) return rc;
     }
     {
         const int nblk = p.npass * p.cblocks;
@@ -582,33 +573,15 @@ int conv_tn_forward(const fn2_conv_desc* d, const T4& in, const float* wp, const
         cuuint64_t strides[3] = {32 * 4, (cuuint64_t)32 * p.ngmax * 4, (cuuint64_t)32 * p.ngmax * nblk * 4};
         cuuint32_t box[4] = {32, (cuuint32_t)p.ngmax, 1, 1};
         cuuint32_t es[4] = {1, 1, 1, 1};
-        CUresult r = enc(&mapW, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void*)wp, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) { set_error("conv_tn: weight tensor map failed (%d)", (int)r); return FN2_ERR_CUDA; }
+        const int rc = tc_tensor_map(&mapW, "conv_tn: weight", CU_TENSOR_MAP_DATA_TYPE_FLOAT32, wp, dims, strides, box, es,
+                                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+        if (rc) return rc;
     }
-    const int smem_bytes = tn_smem_bytes(p);
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)min(p.total, nsm), 1, 1);
-    cfg.blockDim = dim3(TN_THREADS);
-    cfg.stream = st;
-    cfg.dynamicSmemBytes = smem_bytes;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-#define FN2_TN_LAUNCH(COV, SV)                                                                                          \
-    {                                                                                                                   \
-        static int set_ = 0;                                                                                            \
-        if (set_ < smem_bytes) { FN2_CUDA(cudaFuncSetAttribute(conv_tn_kernel<COV, SV>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes)); set_ = smem_bytes; } \
-        FN2_CUDA(cudaLaunchKernelEx(&cfg, conv_tn_kernel<COV, SV>, mapA, mapW, bias, out.p, p));                        \
-    }
-    if (d->co == 16 && p.S == 1) FN2_TN_LAUNCH(16, 1)
-    else if (d->co == 16) FN2_TN_LAUNCH(16, 2)
-    else if (p.S == 1) FN2_TN_LAUNCH(32, 1)
-    else FN2_TN_LAUNCH(32, 2)
-#undef FN2_TN_LAUNCH
-    FN2_LAUNCH_CHECK();
-    return FN2_OK;
+    const int smem = tn_smem_bytes(p);
+    if (d->co == 16 && p.S == 1) return tc_launch<conv_tn_kernel<16, 1>>(p.total, TN_THREADS, smem, true, st, mapA, mapW, bias, out.p, p);
+    if (d->co == 16) return tc_launch<conv_tn_kernel<16, 2>>(p.total, TN_THREADS, smem, true, st, mapA, mapW, bias, out.p, p);
+    if (p.S == 1) return tc_launch<conv_tn_kernel<32, 1>>(p.total, TN_THREADS, smem, true, st, mapA, mapW, bias, out.p, p);
+    return tc_launch<conv_tn_kernel<32, 2>>(p.total, TN_THREADS, smem, true, st, mapA, mapW, bias, out.p, p);
 }
 
 }  // namespace fn2

@@ -222,16 +222,12 @@ __global__ void corr_rearrange_generic_kernel(T4 in, float* __restrict__ ws, int
 }
 
 int make_map(CUtensorMap* m, float* base, int Ws, int Hs, int C, int NP, int bw, int bh) {
-    EncodeTiledFn fn = tc_encode_fn();
-    if (!fn) { set_error("cuTensorMapEncodeTiled is not available from the driver"); return FN2_ERR_CUDA; }
     cuuint64_t dims[4] = {(cuuint64_t)Ws, (cuuint64_t)Hs, (cuuint64_t)C, (cuuint64_t)NP};
     cuuint64_t strides[3] = {(cuuint64_t)Ws * 4, (cuuint64_t)Ws * Hs * 4, (cuuint64_t)Ws * Hs * C * 4};
     cuuint32_t box[4] = {(cuuint32_t)bw, (cuuint32_t)bh, (cuuint32_t)CC, 1};
     cuuint32_t es[4] = {1, 1, 1, 1};
-    CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, base, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                    CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed (%d)", (int)r); return FN2_ERR_CUDA; }
-    return FN2_OK;
+    return tc_tensor_map(m, "corr_fast", CU_TENSOR_MAP_DATA_TYPE_FLOAT32, base, dims, strides, box, es, CU_TENSOR_MAP_SWIZZLE_NONE,
+                         CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
 }
 
 int sub_extent(int v, int S) { return (v + S - 1) / S; }

@@ -1,16 +1,44 @@
 // wgmma / TMA / mbarrier PTX wrappers and constants shared by the tensor-core engines (fn2_conv_tc.cu, fn2_conv_tn.cu) and the
-// FP32 fast correlation (fn2_corr_fast.cu: mbarrier, TMA and the tensor-map encoder); sm_90a.
+// FP32 fast correlation (fn2_corr_fast.cu: mbarrier, TMA and the tensor-map helper), and the host helpers that encode their tensor
+// maps and launch them; sm_90a.
 #pragma once
 #include <cuda.h>
 #include "fn2_common.cuh"
 
 namespace fn2 {
 
-// The driver's cuTensorMapEncodeTiled, looked up once (fn2_conv_tc.cu); nullptr if the driver does not provide it.
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn tc_encode_fn();
+// Encodes a 4-D tiled tensor map of `base`: dims, byte strides of dims 1-3, box, element strides, no interleave, zero fill out of
+// bounds (fn2_conv_tc.cu).  FN2_ERR_CUDA, with "<what> tensor map ..." as the last error, when the driver has no encoder or the
+// encode fails.
+int tc_tensor_map(CUtensorMap* map, const char* what, CUtensorMapDataType dtype, const void* base, const cuuint64_t* dims,
+                  const cuuint64_t* strides, const cuuint32_t* box, const cuuint32_t* es, CUtensorMapSwizzle swizzle,
+                  CUtensorMapL2promotion l2);
+
+// Launches a persistent tensor-core kernel: min(units, SM count) CTAs of `threads` threads with `smem` bytes of dynamic shared
+// memory.  The kernel's shared-memory limit is raised when a launch needs more than the last one set; Kernel is a template
+// argument so that this state is per kernel (the instantiations of one kernel template share a function type), and it is per
+// process (one device per process, as num_sms assumes).  pdl: programmatic stream serialization, so that the kernel's CTAs may
+// start on SMs the previous kernel of the stream leaves; the kernel then waits in griddepcontrol.wait before it reads anything.
+template <auto Kernel, class... Args>
+int tc_launch(int units, int threads, int smem, bool pdl, cudaStream_t st, const Args&... args) {
+    static int smem_set = 0;
+    if (smem > smem_set) {
+        FN2_CUDA(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        smem_set = smem;
+    }
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3((unsigned)min(units, num_sms()));
+    cfg.blockDim = dim3(threads);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = st;
+    cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
+    FN2_CUDA(cudaLaunchKernelEx(&cfg, Kernel, args...));
+    FN2_LAUNCH_CHECK();
+    return FN2_OK;
+}
 
 // Mean relative loss of an FP32 accumulator per MMA that adds a non-zero product to it: the tensor core truncates (rounds
 // toward zero) its accumulator, so a chain of n MMAs shrinks the result by about n times this, and both engines add that

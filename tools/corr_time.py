@@ -1,5 +1,5 @@
 """Correlation at the bench shape: accuracy vs the oracle on a small case, timing of the route the layer takes (the tensor
-cores; FN2_TC=0 -> FP32 fast route) with algorithmic GB/s and TFLOP/s."""
+cores for these channel-fast maps with C % 32 == 0) with algorithmic GB/s and TFLOP/s."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch

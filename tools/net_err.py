@@ -1,5 +1,6 @@
 """End-to-end flow error of the engine vs the float64-accumulating oracle (same prototxt, same weights).
-Usage: [FN2_TC=0] python tools/net_err.py [model] [width] [height]"""
+Usage: [FN2_CONV_ENGINE=simt] python tools/net_err.py [model] [width] [height]
+FN2_CONV_ENGINE=simt runs every convolution on the exact-FP32 SIMT engine instead of the tensor cores."""
 import sys, os, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -22,6 +23,6 @@ else:
     want = OracleNet(proto, net.to_caffemodel(), batch=1, f64acc=True).forward(img0=img0, img1=img1)["predict_flow_final"]
     np.savez(cache, want=want)
     print("oracle %.1f s" % (time.time() - t))
-print("TC=%s %s %dx%d: flow max-abs err %.3e  (|flow| max %.2f, mean abs err %.3e)" % (
-    os.environ.get("FN2_TC", "1"), model, w, h, maxabs(got, want), np.abs(want).max(),
+print("conv engine %s, %s %dx%d: flow max-abs err %.3e  (|flow| max %.2f, mean abs err %.3e)" % (
+    os.environ.get("FN2_CONV_ENGINE", "default"), model, w, h, maxabs(got, want), np.abs(want).max(),
     float(np.abs(got - want).mean())), flush=True)
