@@ -39,6 +39,12 @@ FLOW_ERROR_FIELDS = tuple(sorted((k[len("FN2_FLOW_ERROR_"):].lower() for k in _D
                                  if k.startswith("FN2_FLOW_ERROR_") and k != "FN2_FLOW_ERROR_FIELDS"),
                                 key=lambda f: _DEFINES["FN2_FLOW_ERROR_" + f.upper()]))
 assert len(FLOW_ERROR_FIELDS) == _DEFINES["FN2_FLOW_ERROR_FIELDS"]
+# the per-pair record of fn2_flow_error_regions, the same way; and fn2_occlusion_boundary_dist2's value for a pair without boundary
+FLOW_REGION_FIELDS = tuple(sorted((k[len("FN2_FLOW_REGION_"):].lower() for k in _DEFINES
+                                  if k.startswith("FN2_FLOW_REGION_") and k != "FN2_FLOW_REGION_FIELDS"),
+                                 key=lambda f: _DEFINES["FN2_FLOW_REGION_" + f.upper()]))
+assert len(FLOW_REGION_FIELDS) == _DEFINES["FN2_FLOW_REGION_FIELDS"]
+DIST2_NONE = _DEFINES["FN2_DIST2_NONE"]
 
 
 class Fn2Error(RuntimeError):

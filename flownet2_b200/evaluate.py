@@ -1,7 +1,7 @@
 """Score a net against ground-truth flow: end-point error, outlier rate and Sintel speed bands over an image-and-flow list.
 
     python -m flownet2_b200.evaluate weights.caffemodel models/FlowNet2_deploy.prototxt.template val.txt [--batch B]
-                                     [--per-pair out.tsv] [--gpu G] [--kitti]
+                                     [--per-pair out.tsv] [--gpu G] [--kitti] [--occlusions LIST] [--objects LIST]
 
 The list is the train command's: one ``img0 img1 flow`` line per pair (files.read_list; an occlusion field is refused), flows
 as .flo or 'PF' PFM of either byte order.  Frame sizes may differ from line to line; a flow must have its frames' size
@@ -24,7 +24,19 @@ nonfinite_px and left out of every average.  Printed as one JSON line:
   fl_percent     counted pixels with EPE > 3 px and EPE > 5 % of |gt| (KITTI's Fl), in percent;
   s0-10, s10-40, s40+   pooled EPE over the pixels whose |gt| is in [0, 10), [10, 40), [40, inf) (null when a band is empty);
 and pairs, valid_px, invalid_px, nonfinite_px, batch, ranks and wall (s).  --per-pair writes a TSV row per list line: where,
-img0, img1, flow, valid pixels, EPE, Fl %.  A list with no valid pixel is refused (status 2).  When a prediction is not finite
+img0, img1, flow, valid pixels, EPE, Fl %.  A list with no valid pixel is refused (status 2).
+
+Regions (include/fn2_eval.h defines them).  --occlusions LIST and --objects LIST each name a list of 8-bit one-channel masks,
+one path per line for the pair list's lines in order (files.attach_masks, before any sharding; files.probe checks each mask's
+size).  The feeder reads the masks into each pair's payload stride; on the net's stream fn2_occlusion_boundary_dist2 computes
+the occlusion boundary distance and fn2_flow_error_regions scores the regions, and the records widen by FLOW_REGION_FIELDS.
+Pooled over the list, null when empty:
+  --occlusions   epe_matched, epe_unmatched (Sintel's matched / unmatched: the mask's zero / nonzero pixels), d0-10,
+                 d10-60, d60-140 (EPE of the pixels closer than 10, 10 to 60, 60 to 140 pixels to the occlusion boundary;
+                 this project's definition, see the header), matched_px, unmatched_px;
+  --objects      fl_bg, fl_fg (KITTI 2015's Fl-bg / Fl-fg, in percent; fl_percent is Fl-all), epe_bg, epe_fg, bg_px, fg_px.
+--per-pair appends the same scores per pair (NaN when empty), without the pixel counts.  Without either flag the output is
+exactly the plain command's.  When a prediction is not finite
 its pairs are named on stderr and the status is 1, as in run.
 
 Under torchrun (WORLD_SIZE, RANK, LOCAL_RANK) rank r scores the lines i with i % WORLD_SIZE == r; rank 0 gathers every rank's
@@ -39,51 +51,94 @@ import time
 
 import numpy as np
 
-from . import FLOW_ERROR_FIELDS
-from .files import FLOW_PX_BYTES, RunError, probe, read_list
+from . import FLOW_ERROR_FIELDS, FLOW_REGION_FIELDS
+from .feed import _align, mask_offset
+from .files import RunError, attach_masks, probe, read_list
 from .run import check_inputs, run_groups, shard
 
 FIELD = {name: i for i, name in enumerate(FLOW_ERROR_FIELDS)}
+REGION = {name: i for i, name in enumerate(FLOW_REGION_FIELDS)}
 BANDS = (("s0-10", "n_s0_10", "sum_s0_10"), ("s10-40", "n_s10_40", "sum_s10_40"), ("s40+", "n_s40", "sum_s40"))
+# the region scores each mask adds to the summary and the per-pair file: (key, region, pooled EPE or Fl %)
+REGION_KEYS = {"occlusions": (("epe_matched", "matched", "epe"), ("epe_unmatched", "unmatched", "epe"),
+                              ("d0-10", "d0_10", "epe"), ("d10-60", "d10_60", "epe"), ("d60-140", "d60_140", "epe")),
+               "objects": (("fl_bg", "bg", "fl"), ("fl_fg", "fg", "fl"), ("epe_bg", "bg", "epe"), ("epe_fg", "fg", "epe"))}
+
+
+def record_width(masks):
+    """Fields of a pair's record: FLOW_ERROR_FIELDS, then FLOW_REGION_FIELDS when the pairs carry masks."""
+    return len(FLOW_ERROR_FIELDS) + (len(FLOW_REGION_FIELDS) if masks else 0)
 
 
 class Scores(object):
     """evaluate's per-batch sink for run._run_size (the interface is described at run.FlowFiles): the ground-truth payloads
     ride in the frames' slots, each pair's at a stride that holds any format's, are converted on the net's stream before the
     forward, and each batch's flow is scored on the net's stream; the records of the real pairs land in
-    records[sample.index]."""
+    records[sample.index].
 
-    def __init__(self, n):
-        self.records = np.full((n, len(FLOW_ERROR_FIELDS)), np.nan)
+    masks: the kinds of mask each pair carries, in files.Pair.masks order ("occlusions", "objects" or both).  With masks the
+    records widen by FLOW_REGION_FIELDS: stage() computes the occlusion boundary distance straight from the slot and copies
+    the mask planes out of it (the slot is refilled while the forward runs), and score() adds fn2_flow_error_regions."""
+
+    def __init__(self, n, masks=()):
+        self.masks = tuple(masks)
+        self.records = np.full((n, record_width(self.masks)), np.nan)
         self.stats = {"collect": 0.0}
 
     def item_bytes(self, H, W):
-        return H * W * max(FLOW_PX_BYTES.values())
+        return _align(mask_offset(H, W) + len(self.masks) * H * W)
 
     def bind(self, torch, batch, H, W, flow_dev):
         from . import ops
-        self.ops = ops
-        fields = len(FLOW_ERROR_FIELDS)
+        self.ops, self.batch = ops, batch
+        nf, nr = len(FLOW_ERROR_FIELDS), record_width(self.masks) - len(FLOW_ERROR_FIELDS)
         self.pred = [f.permute(0, 3, 1, 2) for f in flow_dev]                       # (B, 2, H, W) views of the NHWC flow
         self.gt = [torch.empty((batch, 2, H, W), device="cuda") for _ in range(2)]
-        self.dev = [torch.empty((batch, fields), dtype=torch.float64, device="cuda") for _ in range(2)]
-        self.host = [torch.empty((batch, fields), dtype=torch.float64).pin_memory() for _ in range(2)]
-        self.workspace = torch.empty(max(ops.flow_error_workspace_bytes(batch, H, W), 8), dtype=torch.uint8, device="cuda")
+        # each batch's records in one buffer: fn2_flow_error's (B, nf), then fn2_flow_error_regions' (B, nr)
+        self.dev = [torch.empty(batch * (nf + nr), dtype=torch.float64, device="cuda") for _ in range(2)]
+        self.host = [torch.empty(batch * (nf + nr), dtype=torch.float64).pin_memory() for _ in range(2)]
+        self.err = [d[:batch * nf].view(batch, nf) for d in self.dev]
+        self.reg = [d[batch * nf:].view(batch, nr) for d in self.dev]
+        ws = ops.flow_error_workspace_bytes(batch, H, W)
+        if self.masks:
+            ws = max(ws, ops.flow_error_regions_workspace_bytes(batch, H, W))
+            self.planes = [torch.empty((len(self.masks), batch, H, W), dtype=torch.uint8, device="cuda") for _ in range(2)]
+            if "occlusions" in self.masks:
+                self.dist2 = [torch.empty((batch, H, W), dtype=torch.int32, device="cuda") for _ in range(2)]
+        self.workspace = torch.empty(max(ws, 8), dtype=torch.uint8, device="cuda")
 
     def stage(self, pairs, s, payload, stride):
-        """On the net's stream: pair i's payload, at payload[i * stride], into gt[s][i] (formats may differ per pair)."""
+        """On the net's stream: pair i's payload, at payload[i * stride], into gt[s][i] (formats may differ per pair); its masks
+        into planes[s][:, i] and, from its occlusion mask, the boundary distance into dist2[s][i]."""
         for i, p in enumerate(pairs):
             fh = p.flow_header
             self.ops.flow_to_tensor(payload[i * stride:i * stride + fh.nbytes], fh.format, 0, self.gt[s][i:i + 1])
+        if not self.masks:
+            return
+        _, B, H, W = self.planes[s].shape
+        items = payload[:B * stride].view(B, stride)
+        for m, kind in enumerate(self.masks):
+            off = mask_offset(H, W) + m * H * W
+            if kind == "occlusions":
+                self.ops.occlusion_boundary_dist2(payload[off:], out=self.dist2[s], pair_stride=stride)
+            self.planes[s][m].view(B, H * W).copy_(items[:, off:off + H * W])
 
     def score(self, s):
-        self.ops.flow_error(self.pred[s], self.gt[s], out=self.dev[s], workspace=self.workspace)
+        self.ops.flow_error(self.pred[s], self.gt[s], out=self.err[s], workspace=self.workspace)
+        if self.masks:
+            plane = {kind: self.planes[s][m] for m, kind in enumerate(self.masks)}
+            self.ops.flow_error_regions(self.pred[s], self.gt[s], occ=plane.get("occlusions"), obj=plane.get("objects"),
+                                        dist2=self.dist2[s] if "occlusions" in plane else None, out=self.reg[s],
+                                        workspace=self.workspace)
 
     def take(self, pairs, s, n_real):
         t0 = time.perf_counter()
-        rec = self.host[s].numpy()
+        buf = self.host[s].numpy()
+        nf = len(FLOW_ERROR_FIELDS)
+        err = buf[:self.batch * nf].reshape(self.batch, nf)
+        reg = buf[self.batch * nf:].reshape(self.batch, -1)
         for i, p in enumerate(pairs[:n_real]):
-            self.records[p.index] = rec[i]
+            self.records[p.index] = np.concatenate([err[i], reg[i]])
         self.stats["collect"] += time.perf_counter() - t0
 
 
@@ -100,9 +155,23 @@ def _ratio(num, den):
     return float(num / den) if den > 0 else None
 
 
-def summarize(records, pixels, name):
-    """The summary of per-pair records in list order ((n, FIELDS) float64) and each pair's pixel count -> dict; refuses a
-    list with no valid pixel, naming it."""
+def region_keys(occlusions, objects):
+    """The region scores of the summary and the per-pair file, in order: (key, region, EPE or Fl %)."""
+    return (REGION_KEYS["occlusions"] if occlusions else ()) + (REGION_KEYS["objects"] if objects else ())
+
+
+def region_scores(region, occlusions, objects):
+    """Region fields summed over some pairs (FLOW_REGION_FIELDS) -> [(key, pooled EPE or Fl %, None when the region is
+    empty)] of the masks given."""
+    at = lambda f: region[REGION[f]]
+    return [(key, _ratio(at("sum_" + r), at("n_" + r)) if what == "epe" else _ratio(100.0 * at("out_" + r), at("n_" + r)))
+            for key, r, what in region_keys(occlusions, objects)]
+
+
+def summarize(records, pixels, name, occlusions=False, objects=False):
+    """The summary of per-pair records in list order ((n, FIELDS) float64, or FIELDS + REGION FIELDS with masks) and each
+    pair's pixel count -> dict; with occlusions / objects, the pooled region scores and pixel counts of those masks are added.
+    Refuses a list with no valid pixel, naming it."""
     records = np.asarray(records, np.float64)
     col = lambda f: records[:, FIELD[f]]
     valid, nonfinite = col("valid"), col("nonfinite")
@@ -117,25 +186,34 @@ def summarize(records, pixels, name):
            "fl_percent": _ratio(100.0 * col("outliers").sum(), counted.sum())}
     for key, n, s in BANDS:
         out[key] = _ratio(col(s).sum(), col(n).sum())
+    if occlusions or objects:
+        region = records[:, len(FLOW_ERROR_FIELDS):].sum(axis=0)
+        out.update(region_scores(region, occlusions, objects))
+        for r in (("matched", "unmatched") if occlusions else ()) + (("bg", "fg") if objects else ()):
+            out[r + "_px"] = int(region[REGION["n_" + r]])
     return out
 
 
-def pair_rows(records):
-    """-> per pair (valid pixels, EPE, Fl %), NaN where no pixel counts."""
+def pair_rows(records, occlusions=False, objects=False):
+    """-> per pair (valid pixels, EPE, Fl %) followed by its region scores of the masks given, NaN where no pixel counts."""
     rows = []
+    nan = lambda v: float("nan") if v is None else v
     for r in np.asarray(records, np.float64):
         counted = r[FIELD["valid"]] - r[FIELD["nonfinite"]]
         epe = r[FIELD["epe_sum"]] / counted if counted > 0 else float("nan")
         fl = 100.0 * r[FIELD["outliers"]] / counted if counted > 0 else float("nan")
-        rows.append((int(r[FIELD["valid"]]), epe, fl))
+        regions = region_scores(r[len(FLOW_ERROR_FIELDS):], occlusions, objects) if occlusions or objects else []
+        rows.append((int(r[FIELD["valid"]]), epe, fl) + tuple(nan(v) for _, v in regions))
     return rows
 
 
-def write_per_pair(path, samples, records):
+def write_per_pair(path, samples, records, occlusions=False, objects=False):
+    extra = "".join("\t" + key for key, _, _ in region_keys(occlusions, objects))
     with open(path, "w") as f:
-        f.write("where\timg0\timg1\tflow\tvalid\tepe\tfl_percent\n")
-        for s, (valid, epe, fl) in zip(samples, pair_rows(records)):
-            f.write("%s\t%s\t%s\t%s\t%d\t%.9g\t%.9g\n" % (s.where, s.img0, s.img1, s.flow, valid, epe, fl))
+        f.write("where\timg0\timg1\tflow\tvalid\tepe\tfl_percent%s\n" % extra)
+        for s, (valid, epe, fl, *regions) in zip(samples, pair_rows(records, occlusions, objects)):
+            f.write("%s\t%s\t%s\t%s\t%d\t%.9g\t%.9g%s\n" % (s.where, s.img0, s.img1, s.flow, valid, epe, fl,
+                                                          "".join("\t%.9g" % v for v in regions)))
 
 
 def not_finite(samples, records):
@@ -147,25 +225,35 @@ def _list_name(samples):
     return samples[0].where.rsplit(":", 1)[0] if samples else "the list"
 
 
-def _score(caffemodel, template, samples, batch, device, threads, kitti=False):
-    """-> (records in the samples' order, per-stage busy seconds, number of sizes)."""
+def _mask_kinds(occlusions, objects):
+    """-> (mask kinds, their lists) of the mask lists given, in files.Pair.masks order."""
+    given = [(k, l) for k, l in (("occlusions", occlusions), ("objects", objects)) if l]
+    return tuple(k for k, _ in given), [l for _, l in given]
+
+
+def _score(caffemodel, template, samples, batch, device, threads, kitti=False, masks=()):
+    """-> (records in the samples' order, per-stage busy seconds, number of sizes).  masks: the kinds of the samples' masks."""
     t0 = time.perf_counter()
     check_inputs(caffemodel, template, batch)
     probe(samples, ground_truth=True, kitti=kitti)
     for i, s in enumerate(samples):
         s.index = i
-    sink = Scores(len(samples))
+    sink = Scores(len(samples), masks)
     stats, sizes = run_groups(caffemodel, template, samples, batch, device, threads, sink, t0)
     return sink.records, stats, sizes
 
 
-def evaluate(caffemodel, template, samples, batch=1, device=0, threads=None, kitti=False):
+def evaluate(caffemodel, template, samples, batch=1, device=0, threads=None, kitti=False, occlusions=None, objects=None):
     """Scores the net on every files.Pair -> (summary dict, per-pair records): the summary of summarize() plus batch, sizes,
     wall (s), per-stage busy seconds and the samples whose prediction is not finite; the records are an (n, FIELDS) float64
-    array in the samples' order (fields: flownet2_b200.FLOW_ERROR_FIELDS).  kitti: the flows are KITTI PNGs."""
+    array in the samples' order (fields: flownet2_b200.FLOW_ERROR_FIELDS, then FLOW_REGION_FIELDS with a mask list).  kitti:
+    the flows are KITTI PNGs.  occlusions, objects: mask lists (one path per sample, in order) of occlusion masks and object
+    maps, either or both, for the region scores of summarize()."""
     t0 = time.perf_counter()
-    records, stats, sizes = _score(caffemodel, template, samples, batch, device, threads, kitti)
-    summary = summarize(records, [s.size[0] * s.size[1] for s in samples], _list_name(samples))
+    masks, lists = _mask_kinds(occlusions, objects)
+    attach_masks(samples, lists)
+    records, stats, sizes = _score(caffemodel, template, samples, batch, device, threads, kitti, masks)
+    summary = summarize(records, [s.size[0] * s.size[1] for s in samples], _list_name(samples), bool(occlusions), bool(objects))
     summary.update({"batch": batch, "sizes": sizes, "wall": time.perf_counter() - t0, "busy": stats,
                     "not_finite": [s.where for s in not_finite(samples, records)]})
     return summary, records
@@ -196,6 +284,10 @@ def parse_args(argv):
     ap.add_argument("--per-pair", metavar="TSV", help="write one row per list line: where, img0, img1, flow, valid, EPE, Fl %%")
     ap.add_argument("--gpu", type=int, default=0, help="device to use without torchrun")
     ap.add_argument("--kitti", action="store_true", help="the flows are KITTI 16-bit PNGs (KITTI 2012 / 2015 ground truth)")
+    ap.add_argument("--occlusions", metavar="LIST", help="occlusion masks, one per list line (Sintel's occlusions/*.png): "
+                                                         "EPE matched / unmatched and by distance to the occlusion boundary")
+    ap.add_argument("--objects", metavar="LIST", help="object maps, one per list line (KITTI 2015's obj_map/*.png): "
+                                                      "Fl and EPE of the background and the foreground")
     return ap.parse_args(argv)
 
 
@@ -210,21 +302,23 @@ def main(argv=None):
         samples = read_list(a.listfile)
         if not samples:
             raise RunError("%s: the list holds no pairs" % a.listfile)
+        masks, lists = _mask_kinds(a.occlusions, a.objects)
+        attach_masks(samples, lists)                                    # before sharding: every rank sees the same lines
         if world > 1:
             import torch
             import torch.distributed as dist
             torch.cuda.set_device(device)
             dist.init_process_group("nccl")
         mine = shard(samples, world, rank)
-        local = np.empty((0, len(FLOW_ERROR_FIELDS) + 1))               # this rank's records, each pair's pixel count last
+        local = np.empty((0, record_width(masks) + 1))                  # this rank's records, each pair's pixel count last
         if mine:
-            records = _score(a.caffemodel, a.deployproto, mine, a.batch, device, None, a.kitti)[0]
+            records = _score(a.caffemodel, a.deployproto, mine, a.batch, device, None, a.kitti, masks)[0]
             local = np.concatenate([records, [[s.size[0] * s.size[1]] for s in mine]], axis=1)
         full = gather_records(local, len(samples), world, rank) if world > 1 else local
         if rank != 0:
             return 1 if np.any(local[:, FIELD["nonfinite"]] > 0) else 0
         records, pixels = full[:, :-1], full[:, -1]
-        summary = summarize(records, pixels, a.listfile)
+        summary = summarize(records, pixels, a.listfile, bool(a.occlusions), bool(a.objects))
     except RunError as e:
         sys.stderr.write("error: %s\n" % e)
         return 2
@@ -233,7 +327,7 @@ def main(argv=None):
             dist.destroy_process_group()
     summary.update({"batch": a.batch, "ranks": world, "wall": time.perf_counter() - t0})
     if a.per_pair:
-        write_per_pair(a.per_pair, samples, records)
+        write_per_pair(a.per_pair, samples, records, bool(a.occlusions), bool(a.objects))
     bad = not_finite(samples, records)
     for s in bad:
         sys.stderr.write("%s: the flow of %s %s is not finite\n" % (s.where, s.img0, s.img1))

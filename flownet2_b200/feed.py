@@ -8,8 +8,9 @@
 items_of(k) gives batch k's probed items (flownet2_b200.files.Pair; None past the end).  Each of the S slots is a pinned host
 buffer and a device buffer holding [img0 frames][img1 frames][payload]: the frames [B][H][W][K] bytes, K the batch's frame
 channel count (batch_channels), and from a 16-byte boundary item i's flow payload at i * item_bytes (none when item_bytes is
-0).  A reader pool on the net's device reads every part of a batch into its host slot: a PNM frame with K channels as stored,
-any other frame decoded, a payload through files.read_flow_into.  A call waits for the batch's reads, copies the slot to the
+0), followed by its masks (files.Pair.masks, H x W bytes each) from mask_offset(H, W) on.  A reader pool on the net's device
+reads every part of a batch into its host slot: a PNM frame with K channels as stored, any other frame decoded (a mask as one
+channel), a payload through files.read_flow_into.  A call waits for the batch's reads, copies the slot to the
 device on a copy stream, and on the net's stream waits for that copy, converts the frames into the net's first two inputs
 (fn2_net_set_input_frames_device), runs stage(payload, item_bytes) on the device payload and records the slot free.
 
@@ -24,7 +25,7 @@ import time
 from collections import deque
 from concurrent.futures import ThreadPoolExecutor
 
-from .files import RunError, read_flow_into, read_frame_into
+from .files import FLOW_PX_BYTES, RunError, read_flow_into, read_frame_into
 
 
 def _align(n, a=16):
@@ -38,16 +39,24 @@ def batch_channels(items):
     return ks.pop() if len(ks) == 1 else 3
 
 
+def mask_offset(H, W):
+    """Offset of an item's first mask plane in its payload stride: after the largest flow payload of an H x W pair."""
+    return H * W * max(FLOW_PX_BYTES.values())
+
+
 def read_part(p, j, size, k, out):
-    """Part j of item p -- 0: img0, 1: img1 as (H, W, k) bytes of `size` (W, H); 2: its flow's payload -- into the start of
-    the writable buffer `out`; a refusal names the list line."""
+    """Part j of item p -- 0: img0, 1: img1 as (H, W, k) bytes of `size` (W, H); 2: its flow's payload; 3 + m: its mask m as
+    (H, W) bytes -- into the start of the writable buffer `out`; a refusal names the list line (a mask's, its mask list's)."""
+    where = p.masks[j - 3][0] if j >= 3 else p.where
     try:
-        if j == 2:
+        if j >= 3:
+            read_frame_into(p.masks[j - 3][1], size, 1, out[:size[0] * size[1]])
+        elif j == 2:
             read_flow_into(p.flow, p.flow_header, out[:p.flow_header.nbytes])
         else:
             read_frame_into((p.img0, p.img1)[j], size, k, out[:size[0] * size[1] * k])
     except (OSError, RunError) as e:
-        raise RunError("%s: %s" % (p.where, e))
+        raise RunError("%s: %s" % (where, e))
 
 
 class Feeder(object):
@@ -88,13 +97,17 @@ class Feeder(object):
         if items is None:
             return
         s, K = k % self.slots, batch_channels(items)
-        parts = (0, 1, 2) if self.item_bytes else (0, 1)
-        self._reads[k] = (K, [self._pool.submit(self._read, s, K, i, j, p) for i, p in enumerate(items) for j in parts])
+        parts = lambda p: (0, 1, 2) + tuple(range(3, 3 + len(p.masks))) if self.item_bytes else (0, 1)
+        self._reads[k] = (K, [self._pool.submit(self._read, s, K, i, j, p) for i, p in enumerate(items) for j in parts(p)])
 
     def _read(self, s, K, i, j, p):
         self._ev_h2d[s].synchronize()                                  # the copy out of pin[s] `slots` batches ago is done
         t0 = time.perf_counter()
-        o = self.payload_off + i * self.item_bytes if j == 2 else (j * self.batch + i) * self.size[0] * self.size[1] * K
+        W, H = self.size
+        if j >= 3:
+            o = self.payload_off + i * self.item_bytes + mask_offset(H, W) + (j - 3) * H * W
+        else:
+            o = self.payload_off + i * self.item_bytes if j == 2 else (j * self.batch + i) * W * H * K
         read_part(p, j, self.size, K, self._host[s][o:])
         return time.perf_counter() - t0
 

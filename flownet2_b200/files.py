@@ -7,7 +7,8 @@ KITTI 16-bit PNGs; a flow file's payload is the bytes after its header as stored
 FLOW_PX_BYTES gives its bytes per pixel in each format.
 
 A list file holds one ``img0 img1 flow`` line per pair, blank lines skipped.  For run the third column is the flow to write;
-for evaluate and train it is the ground truth, and a fourth (occlusion) column is refused.
+for evaluate and train it is the ground truth, and a fourth (occlusion) column is refused.  Masks (evaluate's occlusion masks
+and object maps) come in lists of their own, one path per line in the pair list's order (attach_masks).
 """
 import os
 import struct
@@ -283,11 +284,12 @@ def write_pfm(path, hw3, big_endian=False):
 # ------------------------------------------------------------------------------------------------
 class Pair(object):
     """One list line: where ('list:line'), the frames img0 and img1, and flow, the flow file (written by run, ground truth
-    for evaluate and train).  probe() sets size (width, height), channels (img0's, img1's) and, with ground truth,
-    flow_header."""
+    for evaluate and train).  masks: the pair's 8-bit mask planes, [(where, path)] in the order attach_masks was given their
+    lists.  probe() sets size (width, height), channels (img0's, img1's) and, with ground truth, flow_header."""
 
     def __init__(self, where, img0, img1, flow):
         self.where, self.img0, self.img1, self.flow = where, img0, img1, flow
+        self.masks = ()
         self.size = self.channels = self.flow_header = None
 
 
@@ -311,10 +313,38 @@ def read_list(path, ground_truth=True):
     return out
 
 
+def read_mask_list(path, n):
+    """-> [(where, mask path)] of a mask list: one path per line, blank lines skipped, line k (counting non-blank lines) for
+    pair k of a pair list of n lines; refuses any other count, naming both."""
+    if not os.path.isfile(path):
+        raise RunError("%s: no such mask list" % path)
+    out = []
+    with open(path) as f:
+        for no, line in enumerate(f, 1):
+            fields = line.split()
+            if not fields:
+                continue
+            if len(fields) != 1:
+                raise RunError("%s:%d: %d fields, expected one mask path" % (path, no, len(fields)))
+            out.append(("%s:%d" % (path, no), fields[0]))
+    if len(out) != n:
+        raise RunError("%s: %d masks for a list of %d pairs" % (path, len(out), n))
+    return out
+
+
+def attach_masks(pairs, lists):
+    """Pair k of `pairs` (a whole list, before any sharding) gets line k of each mask list in `lists`, in that order, as its
+    masks."""
+    masks = [read_mask_list(path, len(pairs)) for path in lists]
+    for k, p in enumerate(pairs):
+        p.masks = tuple(m[k] for m in masks)
+
+
 def probe(pairs, ground_truth=False, kitti=False):
     """Checks every pair's frames without decoding them (present, 8-bit, a PNM's raster in full, one size per pair) and sets
     its size and channels; with ground truth also reads the flow's header (flow_header, or kitti.probe under kitti) into
-    flow_header and refuses a flow whose size is not its frames'.  Every refusal names the list line."""
+    flow_header and refuses a flow whose size is not its frames'; and checks each of its masks is a one-channel 8-bit image of
+    its frames' size.  Every refusal names the list line (a mask's: its mask list's line)."""
     if kitti:
         from . import kitti as kitti_png
     for p in pairs:
@@ -328,4 +358,13 @@ def probe(pairs, ground_truth=False, kitti=False):
             raise RunError("%s: %s is %dx%d but %s is %dx%d" % (p.where, p.img0, w0, h0, p.img1, w1, h1))
         if fh is not None and (fh.width, fh.height) != (w0, h0):
             raise RunError("%s: %s is %dx%d but its frames are %dx%d" % (p.where, p.flow, fh.width, fh.height, w0, h0))
+        for where, path in p.masks:
+            try:
+                w, h, k = probe_image(path)
+            except RunError as e:
+                raise RunError("%s: %s" % (where, e))
+            if k != 1:
+                raise RunError("%s: %s has %d channels, a mask is a one-channel 8-bit image" % (where, path, k))
+            if (w, h) != (w0, h0):
+                raise RunError("%s: %s is %dx%d but the frames of %s are %dx%d" % (where, path, w, h, p.where, w0, h0))
         p.size, p.channels, p.flow_header = (w0, h0), (k0, k1), fh

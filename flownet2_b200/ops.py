@@ -10,7 +10,7 @@ import ctypes as C
 
 import torch
 
-from . import FLOW_ERROR_FIELDS, LPQLOSS_STATE_FLOATS, check, fn2_conv_desc, fn2_l1loss_desc, fn2_lpqloss_desc, fn2_tensor, lib
+from . import FLOW_ERROR_FIELDS, FLOW_REGION_FIELDS, LPQLOSS_STATE_FLOATS, check, fn2_conv_desc, fn2_l1loss_desc, fn2_lpqloss_desc, fn2_tensor, lib
 
 
 def desc(t):
@@ -465,4 +465,52 @@ def flow_error(pred, gt, out=None, workspace=None):
     assert out.dtype == torch.float64 and out.is_contiguous() and out.numel() == N * len(FLOW_ERROR_FIELDS)
     check(lib().fn2_flow_error(desc(pred), desc(gt), C.cast(out.data_ptr(), C.POINTER(C.c_double)), _ptr(workspace),
                                workspace.numel(), _stream()))
+    return out
+
+
+def _planes(masks, N, H, W, pair_stride):
+    """A dense uint8 CUDA tensor holding N mask planes [H][W], pair i's at byte i * pair_stride -> its device address."""
+    assert masks.is_cuda and masks.dtype == torch.uint8 and masks.is_contiguous(), "need dense uint8 CUDA masks"
+    assert pair_stride >= H * W and masks.numel() >= (N - 1) * pair_stride + H * W, (tuple(masks.shape), pair_stride)
+    return masks.data_ptr()
+
+
+def occlusion_boundary_dist2(masks, out=None, pair_stride=None):
+    """Squared distance of every pixel to the nearest occlusion boundary (include/fn2_eval.h): masks is a dense uint8 CUDA
+    tensor, (N, H, W) occlusion masks, or any buffer holding them at pair_stride bytes with out given -> out, a dense int32
+    (N, H, W) CUDA tensor (a new one if None), DIST2_NONE throughout a pair without a boundary."""
+    if out is None:
+        out = torch.empty(masks.shape, dtype=torch.int32, device=masks.device)
+    assert out.is_cuda and out.dtype == torch.int32 and out.dim() == 3 and out.is_contiguous()
+    N, H, W = out.shape
+    pair_stride = H * W if pair_stride is None else pair_stride
+    check(lib().fn2_occlusion_boundary_dist2(_planes(masks, N, H, W, pair_stride), pair_stride, N, H, W,
+                                             C.cast(out.data_ptr(), C.POINTER(C.c_int32)), _stream()))
+    return out
+
+
+def flow_error_regions_workspace_bytes(N, H, W):
+    return _size(lib().fn2_flow_error_regions_workspace_bytes, N, H, W)
+
+
+def flow_error_regions(pred, gt, occ=None, obj=None, dist2=None, mask_pair_stride=None, out=None, workspace=None):
+    """Per-pair scores by region (include/fn2_eval.h): pred and gt as for flow_error; occ and obj are dense uint8 CUDA tensors
+    of (N, H, W) occlusion masks and object maps, or buffers holding them at mask_pair_stride bytes, each may be None; dist2 is
+    occlusion_boundary_dist2(occ), required with occ -> out, an (N, len(FLOW_REGION_FIELDS)) float64 CUDA tensor (a new one if
+    None).  workspace as for flow_error."""
+    N, _, H, W = pred.shape
+    stride = H * W if mask_pair_stride is None else mask_pair_stride
+    if workspace is None:
+        workspace = _ws(flow_error_regions_workspace_bytes(N, H, W), pred.device)
+    assert workspace.dtype == torch.uint8 and workspace.is_contiguous()
+    if out is None:
+        out = torch.empty((N, len(FLOW_REGION_FIELDS)), dtype=torch.float64, device=pred.device)
+    assert out.dtype == torch.float64 and out.is_contiguous() and out.numel() == N * len(FLOW_REGION_FIELDS)
+    if dist2 is not None:
+        assert dist2.is_cuda and dist2.dtype == torch.int32 and dist2.is_contiguous() and tuple(dist2.shape) == (N, H, W)
+    check(lib().fn2_flow_error_regions(desc(pred), desc(gt), None if occ is None else _planes(occ, N, H, W, stride),
+                                       None if obj is None else _planes(obj, N, H, W, stride), stride,
+                                       None if dist2 is None else C.cast(dist2.data_ptr(), C.POINTER(C.c_int32)),
+                                       C.cast(out.data_ptr(), C.POINTER(C.c_double)), _ptr(workspace), workspace.numel(),
+                                       _stream()))
     return out
