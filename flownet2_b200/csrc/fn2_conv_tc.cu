@@ -10,9 +10,10 @@
 //     straight into the wgmma A register fragment and splits them there (RS form: A from registers, W from shared memory).
 //   * FP16 route (NT == 128, plain K blocks: three quarters of FlowNet2's flops): FP16 has TF32's 11-bit significand at half
 //     the tensor-pipe cost, and a power-of-two scale covers its narrow exponent range exactly.  Per K step and pixel row,
-//     a 2^-e = hi + 2^-11 lo' (e from the row's largest |a|); per layer, w 2^-f = w_hi + 2^-11 w_lo' (f from the largest
-//     |w|), packed as W_A = 2^11 w_hi, W_B = w_lo', W_C = w_hi.  Per 16-channel half, lo' W_C + hi W_B + hi W_A =
-//     2^(11-e-f) a w (m64n128k16 f16 MMAs) into the chunk accumulator, scaled back exactly when it is folded.
+//     a 2^-e = hi + lo'' (e from the row's largest |a|); per layer, w 2^-f = w_hi + 2^-11 w_lo' (f from the largest |w|),
+//     packed as W_A = 2^11 w_hi, W_B = w_lo' (and W_C = w_hi, which no kernel reads).  Per 16-channel half,
+//     lo'' W_A + hi W_B + hi W_A = 2^(11-e-f) a w (m64n128k16 f16 MMAs, two weight tiles per K step) into the chunk
+//     accumulator, scaled back exactly when it is folded.
 //   * Accumulation: the tensor core truncates its FP32 accumulator, which over K up to 9216 and ~60 layers would shrink
 //     the flow.  Therefore the MMAs only chain over short chunks (kd K steps) in a register accumulator that is then added
 //     into a second, FP32 register accumulator with round-to-nearest, applying the mean truncation loss of a chain of that
@@ -74,11 +75,14 @@ struct TcParams {
     const uint32_t* wmax;                         // FP16 route: bits of the layer's largest |w|, behind the packed tiles
 };
 
-// FP16 route (NT == 128, plain K blocks): W stage = three FP16 tiles [NT][32 halves] (W_A, W_B, W_C, see tc_pack_f16_kernel)
+// W stage = two tiles: TF32 hi and lo [NT][32 floats], or on the FP16 route (NT == 128, plain K blocks) W_A and W_B
+// [NT][32 halves].  The packed FP16 layout still holds a third tile, W_C, after them (tc_pack_f16_kernel); no kernel reads it,
+// and it stays only because the packed format and its size are pinned: the stage box takes the first two.
 template <int NT, bool F16 = false> struct TcGeo {
     static constexpr int B_TILE_BYTES = F16 ? NT * 64 : NT * 128;
-    static constexpr int STAGE_BYTES = A_TILE_BYTES + (F16 ? 3 : 2) * B_TILE_BYTES;
+    static constexpr int STAGE_BYTES = A_TILE_BYTES + 2 * B_TILE_BYTES;
     // ring of R shared-memory stages (raw A tile + W tiles), then the epilogue's staging buffer [128 pixels][STG]
+    // (FP16: 5 stages of 32 KB would fit, and measured no faster than 4: the two-tile stage's gain is its bytes, DESIGN.md section 6)
     static constexpr int R = F16 ? 4 : (NT == 128 ? 3 : (NT == 64 ? 4 : 6));
     static constexpr int STG = NT + 4;                                             // floats per staged pixel row
     static constexpr int STG_BYTES = 128 * STG * 4;
@@ -251,7 +255,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                 const int cx0 = T.v0 * p.su, cy0 = T.u0 * p.sv;
                 auto load_w = [&](unsigned char* st, uint64_t* bar, int c0, int blk) {
                     if constexpr (F16) {
-                        // one box {32 halves, NT, 3 tiles} of K block (tap blk, channel block c0 / 32)
+                        // one box {32 halves, NT, 2 tiles: W_A | W_B} of K block (tap blk, channel block c0 / 32)
                         tma_load_4d(st + A_TILE_BYTES, &mapW, bar, 0, T.co0, 0, blk * cblocks + c0 / 32);
                     } else {
                         tma_load_4d(st + A_TILE_BYTES, &mapW, bar, c0, T.co0, blk, 0);
@@ -378,7 +382,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                 float rs[2];                       // FP16 route: 2^(e+f-11) of rows r0, r1
                 if constexpr (F16) {
                     // per row: e from the largest |a| of the row's 32 channels (8 per quad lane), so that |a| 2^-e < 2^15;
-                    // a 2^-e = hi + 2^-11 lo', both FP16 (a_hi / a_lo' in the fragments of the two 16-slot halves)
+                    // a 2^-e = hi + lo'', both FP16 (a_hi / a_lo'' in the fragments of the two 16-slot halves).  The
+                    // subtraction is exact; lo'' meets W_A = 2^11 w_hi, so no third weight tile is needed (DESIGN.md section 3)
 #pragma unroll
                     for (int e = 0; e < 2; e++) {
                         const int r = e ? r1 : r0;
@@ -390,17 +395,17 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                         mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
                         const int E = (int)(__float_as_uint(mx) >> 23);
                         const int ex = E == 255 ? 0 : min(max(E - 141, elo), ehi);          // E = 255: no finite max
-                        const float up = tc_pow2(-ex), up11 = tc_pow2(11 - ex);
+                        const float up = tc_pow2(-ex);
                         rs[e] = tc_pow2(ex + fw - 11);
                         const float4 vh[2] = {v0, v1};
 #pragma unroll
                         for (int hh = 0; hh < 2; hh++) {
-                            const float x[4] = {vh[hh].x, vh[hh].y, vh[hh].z, vh[hh].w};
+                            const float x[4] = {vh[hh].x * up, vh[hh].y * up, vh[hh].z * up, vh[hh].w * up};
 #pragma unroll
                             for (int q = 0; q < 2; q++) {
-                                const __half2 h = __floats2half2_rn(x[2 * q] * up, x[2 * q + 1] * up);
+                                const __half2 h = __floats2half2_rn(x[2 * q], x[2 * q + 1]);
                                 const float2 hf = __half22float2(h);
-                                const __half2 l = __floats2half2_rn(fmaf(-2048.f, hf.x, x[2 * q] * up11), fmaf(-2048.f, hf.y, x[2 * q + 1] * up11));
+                                const __half2 l = __floats2half2_rn(__fsub_rn(x[2 * q], hf.x), __fsub_rn(x[2 * q + 1], hf.y));
                                 ah[4 * hh + 2 * q + e] = *reinterpret_cast<const uint32_t*>(&h);
                                 al[4 * hh + 2 * q + e] = *reinterpret_cast<const uint32_t*>(&l);
                             }
@@ -444,12 +449,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                 for (int j = 0; j < (int)(sizeof(cx) / sizeof(float)); j++) reg_fence(cx[j]);
                 wgmma_fence();
                 if constexpr (F16) {
-                    // per 16-slot half: a_lo' * W_C and a_hi * W_B (2^-11 smaller) first, then a_hi * W_A
-                    const uint64_t dA = make_desc_sw64(bh), dB = make_desc_sw64(bh + G::B_TILE_BYTES), dC = make_desc_sw64(bh + 2 * G::B_TILE_BYTES);
+                    // per 16-slot half: a_lo'' * W_A and a_hi * W_B (2^-11 smaller) first, then a_hi * W_A
+                    const uint64_t dA = make_desc_sw64(bh), dB = make_desc_sw64(bh + G::B_TILE_BYTES);
                     const int acc0 = in_chunk != 0;
 #pragma unroll
                     for (int hh = 0; hh < 2; hh++) {
-                        WgmmaF16<NT>::mma(c, al + 4 * hh, dC + (uint64_t)(2 * hh), acc0 | hh);
+                        WgmmaF16<NT>::mma(c, al + 4 * hh, dA + (uint64_t)(2 * hh), acc0 | hh);
                         WgmmaF16<NT>::mma(c, ah + 4 * hh, dB + (uint64_t)(2 * hh), 1);
                     }
 #pragma unroll
@@ -614,7 +619,8 @@ __global__ void tc_absmax_kernel(const float* __restrict__ w, long long n, uint3
 
 // FP16 route: [tap][channel block][W_A | W_B | W_C][Co][32 K slots] halves (K slot order tc_f16_channel).  With f from the
 // layer's largest |w| (*wmax) and w_hi = fp16(w 2^-f): W_A = 2^11 w_hi, W_B = fp16(2^11 (w 2^-f - w_hi)), W_C = w_hi (all but
-// the rounding of W_B exact).
+// the rounding of W_B exact).  The forward reads only W_A and W_B (conv_tc_kernel multiplies the activations' low half by W_A);
+// W_C is still written because the packed format and its size are pinned, so that it can be dropped in one change with them.
 __global__ void tc_pack_f16_kernel(const float* __restrict__ w, __half* __restrict__ wp, int Ci, int Co, int kh, int kw, int cblocks,
                                    int deconv, const uint32_t* __restrict__ wmax) {
     const long long per = (long long)kh * kw * cblocks * 3 * Co * 32;
@@ -759,15 +765,16 @@ static int tc_chunk_steps(int NT) { return NT == 128 ? 1 : 4; }
 //   TF32, tap groups:      [hi|lo][group][Co][32]                  K index j*cs + ci for tap group*(32/cs) + j
 //   TF32, kernel rows:     [hi|lo][r*rblocks + kb][Co][32]         K index kb*32 + k = s*cs + ci of kernel row r
 //   FP16:                  [tap*cblocks + cb][W_A|W_B|W_C][Co][32 halves] (tc_pack_f16_kernel), then 4 floats holding the bits
-//                          of the largest |w| (tc_absmax_kernel)
+//                          of the largest |w| (tc_absmax_kernel).  The forward reads W_A and W_B only; W_C is no longer read
+//                          by any kernel and stays packed because the packed format and its size are pinned
 // Small-Ci packing (plain convolutions with at most 16 input channels): tap groups (several taps share a 32-wide K block, one small
 // TMA box per tap), or kernel rows where they take no more K blocks (needs a dense input whose pixel stride equals the padded
 // channel count, and a guard band around the tensor because the row runs of the edge pixels reach a little outside it).  The
-// NT = 128 layers in plain K-block mode run on FP16 operands (three FP16 products per K step with a power-of-two scale per pixel
-// row and per layer), every other layer on TF32 (3xTF32).
+// NT = 128 layers in plain K-block mode run on FP16 operands (three FP16 products per K step from two weight tiles, with a
+// power-of-two scale per pixel row and per layer), every other layer on TF32 (3xTF32).
 struct TcWeights {
     int mode;                 // TC_PLAIN, TC_GROUP or TC_ROW
-    bool f16;                 // FP16 operands (three tiles per K block), else TF32 hi and lo tiles
+    bool f16;                 // FP16 operands (three tiles per K block, of which the forward reads two), else TF32 hi and lo tiles
     int cs, rblocks;          // small-Ci packing: channels per tap padded to a multiple of 4, K blocks per kernel row
     int blocks, width, tiles; // K blocks, elements per output channel of a block, tiles per block
     size_t tile_floats;       // floats of the tiles
@@ -974,14 +981,14 @@ int conv_tc_forward(const fn2_conv_desc* d, const T4& in, const float* wp, const
     const int NT = pl.NT, su = p.su, sv = p.sv;
     p.out_sn = out.sn; p.out_sh = out.sh; p.out_sw = out.sw;
     // weights (tc_weights): TF32 {width, Co, blocks, hi|lo} read as boxes {32, NT}, one tile at a time; FP16 {32 halves, Co,
-    // W_A|W_B|W_C, blocks} read as one box {32, NT, 3} per K block
+    // W_A|W_B|W_C, blocks} read as one box {32, NT, 2} per K block: W_A | W_B, contiguous in each block (W_C is not read)
     CUtensorMap mapW;
     {
         const cuuint64_t row = (cuuint64_t)L.width * (L.f16 ? 2 : 4), tile = row * d->co;
         const int inner = L.f16 ? L.tiles : L.blocks, outer = L.f16 ? L.blocks : L.tiles;
         const cuuint64_t dims[4] = {(cuuint64_t)L.width, (cuuint64_t)d->co, (cuuint64_t)inner, (cuuint64_t)outer};
         const cuuint64_t strides[3] = {row, tile, tile * inner};
-        const cuuint32_t box[4] = {32, (cuuint32_t)NT, L.f16 ? 3u : 1u, 1};
+        const cuuint32_t box[4] = {32, (cuuint32_t)NT, L.f16 ? 2u : 1u, 1};
         const cuuint32_t es[4] = {1, 1, 1, 1};
         const int rc = tc_tensor_map(&mapW, "conv_tc: weight", L.f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32,
                                      wp, dims, strides, box, es, L.f16 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,

@@ -10,7 +10,8 @@ take turns on the card.  Per layer: its plan (NT, mode 0 plain / 1 tap groups / 
 2 N Co Ho Wo Ci kh kw for a convolution, 2 N Ci H W Co kh kw for a deconvolution), and per library the median over rounds of
 the mean time per call (CUDA events around --iters calls after 3 warm-up calls), TFLOP/s, the operand route its packed weights
 show (FP16 or TF32) and the bytes the plan's K steps read from L2: 16 KB of activations per step plus the weight stage, 2 NT 128 B
-as TF32 hi / lo or 3 NT 64 B as three FP16 tiles.  The card's name, power limit and maximum SM clock are read in the same call.
+as TF32 hi / lo or 2 NT 64 B as the FP16 tiles W_A and W_B (the packing's third tile, W_C, is not read).  The card's name, power
+limit and maximum SM clock are read in the same call.
 """
 import argparse
 import ctypes as C
@@ -130,7 +131,7 @@ def main():
             ts = sorted(r[name][0] for r in runs[lib])
             ms = ts[len(ts) // 2]
             f16 = f16_route(ci, co, k, pl, runs[lib][0][name][1])
-            wb = 3 * pl[0] * 64 if f16 else 2 * pl[0] * 128
+            wb = 2 * pl[0] * (64 if f16 else 128)
             row[lib] = {"ms": ms, "spread_ms": ts[-1] - ts[0], "tflops": gf / ms, "route": "FP16" if f16 else "TF32",
                         "l2_mb": pl[1] * pl[2] * (16384 + wb) / 2 ** 20}
         table.append(row)
