@@ -74,3 +74,10 @@ def backward(a, b, td, md, s2):
     a = _f64(a)
     b, td = _f64(b).to(a.device), _f64(td).to(a.device)
     return (_bwd0(b, td, md, s2), _bwd1(a, td, md, s2), _bwd0(b.abs(), td.abs(), md, s2), _bwd1(a.abs(), td.abs(), md, s2))
+
+
+def gradients(a, b, td, md, s2):
+    """The bottom gradients of `backward` without their absrefs: -> (d0, d1), float64 on a's device."""
+    a = _f64(a)
+    b, td = _f64(b).to(a.device), _f64(td).to(a.device)
+    return _bwd0(b, td, md, s2), _bwd1(a, td, md, s2)

@@ -14,7 +14,7 @@ from oracle.net import OracleNet, get, getall
 NO_BACKWARD = ("Resample", "DataAugmentation", "FlowAugmentation", "GenerateAugmentationParameters", "Downsample")
 
 
-def _lr_mults(l):
+def lr_mults(l):
     """lr_mult of each parameter blob of a layer (ParamSpec default 1); only convolutions have parameters in these graphs."""
     if get(l, "type") not in ("Convolution", "Deconvolution"):
         return []
@@ -30,7 +30,7 @@ class PrunedOracleNet(OracleNet):
         self.layer_need = {}
         for l in self.layers:
             typ = get(l, "type")
-            need = any(lr != 0 for lr in _lr_mults(l)) or any(blob_need.get(b, False) for b in getall(l, "bottom"))
+            need = any(lr != 0 for lr in lr_mults(l)) or any(blob_need.get(b, False) for b in getall(l, "bottom"))
             need = need and typ not in NO_BACKWARD
             self.layer_need[get(l, "name")] = need
             for t in getall(l, "top"):
@@ -46,7 +46,7 @@ class PrunedOracleNet(OracleNet):
         pd = getall(l, "propagate_down")
         grads = [g if self.blob_need.get(b, False) and not (i < len(pd) and pd[i] == "false") else None
                  for i, (b, g) in enumerate(zip(names, grads))]
-        lrs = _lr_mults(l)
+        lrs = lr_mults(l)
         if name in P and lrs and all(lr == 0 for lr in lrs):
             del P[name]
         return grads
