@@ -128,6 +128,13 @@ inline int ew_launch(void (*kernel)(P...), long long total, void* stream, const 
     return FN2_OK;
 }
 
+// A known flow pixel (Middlebury's rule, UNKNOWN_FLOW_THRESH = 1e9): both components finite and at most 1e9 in absolute value.
+// A ground-truth pixel is scored (fn2_eval.cu) and a flow pixel is coloured (fn2_ops.cu) only when it is known.
+constexpr float kUnknownFlow = 1e9f;
+__device__ __forceinline__ bool flow_known(float u, float v) {
+    return fabsf(u) <= kUnknownFlow && fabsf(v) <= kUnknownFlow;                   // false for NaN, Inf and unknown
+}
+
 // Grid-stride loops of the per-pixel and per-element kernels.  Each thread visits the same indices in the same order whatever
 // the kernel does with them, so per-thread partial sums (L1Loss, the eigenspace statistics) and index-seeded noise stay fixed.
 // f(n, y, x) for every pixel of an n x h x w extent, x fastest.

@@ -31,19 +31,15 @@ constexpr int kFields = FN2_FLOW_ERROR_FIELDS;
 constexpr int kRegionFields = FN2_FLOW_REGION_FIELDS;
 constexpr int kThreads = 256;
 constexpr int kUnroll = 4;
-constexpr float kUnknownFlow = 1e9f;                                    // Middlebury's UNKNOWN_FLOW_THRESH
 constexpr int kNone = FN2_DIST2_NONE;
 constexpr int kMaxSide = 16384;                                         // (2 * 16383^2 < 2^31: every dist2 fits in int32)
 constexpr int kColThreads = 32;                                         // a Sintel batch's 8 x 1024 columns: 256 blocks
 constexpr int kChunk = 8;
 constexpr int kRowThreads = 64;
 
-// fn2_flow_error's definitions, shared by both scoring kernels: a pixel counts when its ground truth is valid and its prediction
-// finite; its EPE and |gt| are float32 with separately rounded products; it is an outlier (KITTI's Fl) when EPE > 3 and
-// EPE > 5 % of |gt|.
-__device__ __forceinline__ bool gt_valid(float gu, float gv) {
-    return fabsf(gu) <= kUnknownFlow && fabsf(gv) <= kUnknownFlow;                 // false for NaN, Inf and unknown
-}
+// fn2_flow_error's definitions, shared by both scoring kernels: a pixel counts when its ground truth is valid (flow_known,
+// fn2_common.cuh) and its prediction finite; its EPE and |gt| are float32 with separately rounded products; it is an outlier
+// (KITTI's Fl) when EPE > 3 and EPE > 5 % of |gt|.
 __device__ __forceinline__ float pixel_epe(float gu, float gv, float pu, float pv) {
     const float du = pu - gu, dv = pv - gv;
     return sqrtf(du * du + dv * dv);
@@ -53,7 +49,7 @@ __device__ __forceinline__ bool outlier(float epe, float mag) { return epe > 3.f
 
 // Adds one pixel (ground truth gu, gv; prediction pu, pv) to the ten fields.
 __device__ __forceinline__ void score_pixel(float gu, float gv, float pu, float pv, double (&acc)[kFields]) {
-    if (!gt_valid(gu, gv)) return;
+    if (!flow_known(gu, gv)) return;
     acc[FN2_FLOW_ERROR_VALID] += 1.0;
     if (!(isfinite(pu) && isfinite(pv))) {
         acc[FN2_FLOW_ERROR_NONFINITE] += 1.0;
@@ -83,7 +79,7 @@ __device__ __forceinline__ void add_region(double epe, double out, double (&acc)
 // when has_obj.
 __device__ __forceinline__ void score_region(float gu, float gv, float pu, float pv, bool has_occ, bool occ, int d2, bool has_obj,
                                              bool fg, double (&acc)[kRegionFields]) {
-    if (!(gt_valid(gu, gv) && isfinite(pu) && isfinite(pv))) return;
+    if (!(flow_known(gu, gv) && isfinite(pu) && isfinite(pv))) return;
     const float epe = pixel_epe(gu, gv, pu, pv);
     const double e = (double)epe, o = outlier(epe, gt_mag(gu, gv)) ? 1.0 : 0.0;
     if (has_occ) {

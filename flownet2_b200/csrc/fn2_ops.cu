@@ -1,6 +1,6 @@
 // Streaming (HBM-bound) layers: FlowWarp, Resample, DataAugmentation kernels, ChannelNorm, the warp block, and the
 // element-wise ops of the forward and backward passes (ReLU and its backward, Eltwise SUM, y = alpha*x + beta*y, strided
-// copy and fill), and the conversion of 8-bit frames into an input blob.
+// copy and fill), the conversion of 8-bit frames into an input blob, the flow-file conversions and the flow colour coding.
 //
 // This translation unit is compiled with -fmad=false: every expression below is evaluated
 // with separately rounded multiplies and adds in the order written, which is also how the CPU
@@ -12,6 +12,7 @@
 // fn2_common.cuh.  The warp block is built from the device functions of the stand-alone FlowWarp, Resample, Eltwise and
 // ChannelNorm kernels: the compiler inlines the same functions in both places, so its tops are bit-identical to the layer chain's.
 #include <math.h>
+#include <algorithm>
 #include <cfloat>
 #include <initializer_list>
 
@@ -839,6 +840,115 @@ __global__ void flow_to_kitti_png_rows_kernel(T4 f, uint8_t* __restrict__ rows) 
     });
 }
 
+// ---------------------------------------------------------------------------------------------
+// Flow colour coding (include/fn2_flow.h): the Middlebury colour wheel (Baker et al., colorcode.cpp), every pixel divided by
+// a per-image scale.  flow_max_radius_kernel: grid (blocks, N), each block's largest float32 radius over its share of image
+// n's known pixels folded into max[n] with an integer atomicMax (non-negative floats order as their bits; max[n] starts at
+// -1, whose bits are negative), so the result is exact and independent of the order.  The colour kernels, one thread per
+// pixel: the dense form writes the pixel's 3 bytes; the PNG form colours the pixel and its left, up and up-left neighbours and
+// Paeth-filters its 3 bytes against them, as flow_to_kitti_png_rows_kernel does.  The arithmetic is float32 as written
+// (-fmad=false) except atan2, evaluated in double and rounded to float32: atan2f's last-ulp errors would flip the many bytes
+// that sit exactly on an integer (a channel whose two wheel entries are equal), so a host restatement could not reproduce them.
+// ---------------------------------------------------------------------------------------------
+__global__ void fill_minus_one_kernel(float* __restrict__ out, int n) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) out[i] = -1.f;
+}
+
+__global__ void flow_max_radius_kernel(T4 f, float* __restrict__ max_out) {
+    const int n = blockIdx.y;
+    const long long hw = (long long)f.h * f.w;
+    float m = -1.f;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < hw; i += (long long)gridDim.x * blockDim.x) {
+        const int y = (int)(i / f.w), x = (int)(i % f.w);
+        const float u = f.p[f.off(n, 0, y, x)], v = f.p[f.off(n, 1, y, x)];
+        if (flow_known(u, v)) m = fmaxf(m, sqrtf(u * u + v * v));
+    }
+    for (int o = 16; o; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    __shared__ float warp_max[32];
+    if ((threadIdx.x & 31) == 0) warp_max[threadIdx.x >> 5] = m;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (int w = 1; w < (int)(blockDim.x >> 5); w++) m = fmaxf(m, warp_max[w]);
+        if (m >= 0.f) atomicMax(reinterpret_cast<int*>(max_out + n), __float_as_int(m));
+    }
+}
+
+// Entry k of the 55-colour wheel, segments RY 15, YG 6, GC 4, CB 11, BM 13, MR 6, in integer arithmetic.
+__device__ __forceinline__ void wheel_entry(int k, int (&w)[3]) {
+    if (k < 15) { w[0] = 255; w[1] = 255 * k / 15; w[2] = 0; return; }
+    k -= 15;
+    if (k < 6) { w[0] = 255 - 255 * k / 6; w[1] = 255; w[2] = 0; return; }
+    k -= 6;
+    if (k < 4) { w[0] = 0; w[1] = 255; w[2] = 255 * k / 4; return; }
+    k -= 4;
+    if (k < 11) { w[0] = 0; w[1] = 255 - 255 * k / 11; w[2] = 255; return; }
+    k -= 11;
+    if (k < 13) { w[0] = 255 * k / 13; w[1] = 0; w[2] = 255; return; }
+    k -= 13;
+    w[0] = 255; w[1] = 0; w[2] = 255 - 255 * k / 6;
+}
+
+// The scale of image n: max_flow when positive, else max[n] (fallback[n] when max[n] is negative and fallback is given), and
+// 1 when that is not positive.
+__device__ __forceinline__ float colour_scale(const float* max, const float* fallback, float max_flow, int n) {
+    if (max_flow > 0.f) return max_flow;
+    float r = max[n];
+    if (r < 0.f && fallback) r = fallback[n];
+    return r > 0.f ? r : 1.f;
+}
+
+// The colour of flow pixel (n, y, x) as 0x00BBGGRR; 0 (black) for an unknown pixel and outside the image.
+__device__ __forceinline__ uint32_t flow_colour(const T4& f, int n, int y, int x, float scale) {
+    if (x < 0 || y < 0) return 0u;
+    const float u = f.p[f.off(n, 0, y, x)], v = f.p[f.off(n, 1, y, x)];
+    if (!flow_known(u, v)) return 0u;
+    const float fx = u / scale, fy = v / scale;
+    const float rad = sqrtf(fx * fx + fy * fy);
+    const float a = (float)atan2(-(double)fy, -(double)fx) / 3.14159265358979323846f;      // a correctly rounded atan2f
+    const float fk = (a + 1.f) / 2.f * 54.f;
+    const int k0 = (int)fk, k1 = (k0 + 1) % 55;
+    const float fr = fk - (float)k0;
+    int w0[3], w1[3];
+    wheel_entry(k0, w0);
+    wheel_entry(k1, w1);
+    uint32_t rgb = 0u;
+    #pragma unroll
+    for (int c = 0; c < 3; c++) {
+        float col = (1.f - fr) * (float)w0[c] / 255.f + fr * (float)w1[c] / 255.f;
+        col = rad <= 1.f ? 1.f - rad * (1.f - col) : col * 0.75f;
+        rgb |= (uint32_t)(int)(255.f * col) << (8 * c);
+    }
+    return rgb;
+}
+
+__global__ void flow_to_color_kernel(T4 f, const float* __restrict__ max, const float* __restrict__ fallback, float max_flow,
+                                     uint8_t* __restrict__ rgb) {
+    for_each_pixel(f.n, f.h, f.w, [&](int n, int y, int x) {
+        const uint32_t c = flow_colour(f, n, y, x, colour_scale(max, fallback, max_flow, n));
+        uint8_t* o = rgb + (((long long)n * f.h + y) * f.w + x) * 3;
+        o[0] = (uint8_t)c; o[1] = (uint8_t)(c >> 8); o[2] = (uint8_t)(c >> 16);
+    });
+}
+
+__global__ void flow_to_color_png_rows_kernel(T4 f, const float* __restrict__ max, const float* __restrict__ fallback,
+                                              float max_flow, uint8_t* __restrict__ rows) {
+    const long long row_bytes = 1 + 3LL * f.w;
+    for_each_pixel(f.n, f.h, f.w, [&](int n, int y, int x) {
+        const float s = colour_scale(max, fallback, max_flow, n);
+        const uint32_t self = flow_colour(f, n, y, x, s), left = flow_colour(f, n, y, x - 1, s),
+                       up = flow_colour(f, n, y - 1, x, s), upleft = flow_colour(f, n, y - 1, x - 1, s);
+        uint8_t* row = rows + ((long long)n * f.h + y) * row_bytes;
+        if (x == 0) row[0] = 4;
+        uint8_t* o = row + 1 + 3LL * x;
+        #pragma unroll
+        for (int c = 0; c < 3; c++) {
+            const int sh = 8 * c;
+            o[c] = (uint8_t)(((self >> sh) & 0xff) - paeth_predict((left >> sh) & 0xff, (up >> sh) & 0xff, (upleft >> sh) & 0xff));
+        }
+    });
+}
+
 }  // namespace fn2
 
 using namespace fn2;
@@ -1099,6 +1209,57 @@ int fn2_flow_to_kitti_png_rows(const fn2_tensor* src, void* dst_dev, void* strea
     T4 f = view(src);
     FN2_CHECK_ARG(f.c == 2, "flow_to_kitti_png_rows: src must have 2 channels (u, v), has %d", f.c);
     return ew_launch(flow_to_kitti_png_rows_kernel, (long long)f.n * f.h * f.w, stream, f, static_cast<uint8_t*>(dst_dev));
+}
+
+int fn2_flow_max_radius(const fn2_tensor* src, float* max_dev, void* stream) {
+    FN2_CHECK_ARG(valid(src), "flow_max_radius: src is null or empty");
+    FN2_CHECK_ARG(max_dev, "flow_max_radius: max is null");
+    FN2_CHECK_ARG((reinterpret_cast<uintptr_t>(src->data) & 3) == 0, "flow_max_radius: src must be 4-byte aligned");
+    FN2_CHECK_ARG((reinterpret_cast<uintptr_t>(max_dev) & 3) == 0, "flow_max_radius: max must be 4-byte aligned");
+    T4 f = view(src);
+    FN2_CHECK_ARG(f.c == 2, "flow_max_radius: src must have 2 channels (u, v), has %d", f.c);
+    FN2_CHECK_ARG(f.n <= 65535, "flow_max_radius: at most 65535 images, got %d", f.n);
+    cudaStream_t s = (cudaStream_t)stream;
+    fill_minus_one_kernel<<<(f.n + 255) / 256, 256, 0, s>>>(max_dev, f.n);
+    FN2_LAUNCH_CHECK();
+    const long long hw = (long long)f.h * f.w;
+    const int blocks = (int)std::max(1LL, std::min((hw + 255) / 256, (long long)ew_grid(hw * f.n, 256) / f.n));
+    flow_max_radius_kernel<<<dim3(blocks, f.n), 256, 0, s>>>(f, max_dev);
+    FN2_LAUNCH_CHECK();
+    return FN2_OK;
+}
+
+// The checks the two colour entry points share.
+static int colour_args(const char* who, const fn2_tensor* src, const float* max_dev, const float* fallback_dev, float max_flow,
+                       const void* dst_dev) {
+    FN2_CHECK_ARG(valid(src), "%s: src is null or empty", who);
+    FN2_CHECK_ARG(dst_dev, "%s: dst is null", who);
+    FN2_CHECK_ARG((reinterpret_cast<uintptr_t>(src->data) & 3) == 0, "%s: src must be 4-byte aligned", who);
+    FN2_CHECK_ARG(src->c == 2, "%s: src must have 2 channels (u, v), has %d", who, src->c);
+    FN2_CHECK_ARG(max_flow == 0.f || (max_flow > 0.f && isfinite(max_flow)),
+                  "%s: max_flow must be 0 (the per-image max) or finite and positive, got %g", who, (double)max_flow);
+    FN2_CHECK_ARG(max_flow > 0.f || max_dev, "%s: max is null and max_flow is 0", who);
+    FN2_CHECK_ARG(!((reinterpret_cast<uintptr_t>(max_dev) | reinterpret_cast<uintptr_t>(fallback_dev)) & 3),
+                  "%s: max and fallback must be 4-byte aligned", who);
+    return FN2_OK;
+}
+
+int fn2_flow_to_color(const fn2_tensor* src, const float* max_dev, const float* fallback_dev, float max_flow, void* dst_dev,
+                      void* stream) {
+    const int rc = colour_args("flow_to_color", src, max_dev, fallback_dev, max_flow, dst_dev);
+    if (rc != FN2_OK) return rc;
+    T4 f = view(src);
+    return ew_launch(flow_to_color_kernel, (long long)f.n * f.h * f.w, stream, f, max_dev, fallback_dev, max_flow,
+                     static_cast<uint8_t*>(dst_dev));
+}
+
+int fn2_flow_to_color_png_rows(const fn2_tensor* src, const float* max_dev, const float* fallback_dev, float max_flow,
+                               void* dst_dev, void* stream) {
+    const int rc = colour_args("flow_to_color_png_rows", src, max_dev, fallback_dev, max_flow, dst_dev);
+    if (rc != FN2_OK) return rc;
+    T4 f = view(src);
+    return ew_launch(flow_to_color_png_rows_kernel, (long long)f.n * f.h * f.w, stream, f, max_dev, fallback_dev, max_flow,
+                     static_cast<uint8_t*>(dst_dev));
 }
 
 }  // extern "C"

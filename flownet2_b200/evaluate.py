@@ -2,6 +2,7 @@
 
     python -m flownet2_b200.evaluate weights.caffemodel models/FlowNet2_deploy.prototxt.template val.txt [--batch B]
                                      [--per-pair out.tsv] [--gpu G] [--kitti] [--occlusions LIST] [--objects LIST]
+                                     [--visualize DIR [--max-flow F]]
 
 The list is the train command's: one ``img0 img1 flow`` line per pair (files.read_list; an occlusion field is refused), flows
 as .flo or 'PF' PFM of either byte order.  Frame sizes may differ from line to line; a flow must have its frames' size
@@ -39,6 +40,12 @@ Pooled over the list, null when empty:
 exactly the plain command's.  When a prediction is not finite
 its pairs are named on stderr and the status is 1, as in run.
 
+--visualize DIR [--max-flow F]: for list line k (counting pairs from 0) DIR/<k, 6 digits>_pred.png and _gt.png, the
+prediction and the ground truth colour-coded on the net's stream (fn2_flow_to_color_png_rows) at one scale, so that they can be
+compared: F, else the ground truth's largest known flow (the prediction's when no ground-truth pixel is known).  The
+scanlines come back with the records and the writer thread deflates them; under torchrun each rank writes its own pairs.
+The summary and --per-pair are the same with and without it.
+
 Under torchrun (WORLD_SIZE, RANK, LOCAL_RANK) rank r scores the lines i with i % WORLD_SIZE == r; rank 0 gathers every rank's
 records, puts them back in list order (combine_shards) and prints the summary, so at --batch 1 it does not depend on the
 number of ranks.  At larger batches a pair's flow, and so its record, can differ in the last bits (see run).
@@ -54,7 +61,7 @@ import numpy as np
 from . import FLOW_ERROR_FIELDS, FLOW_REGION_FIELDS
 from .feed import _align, mask_offset
 from .files import RunError, attach_masks, probe, read_list
-from .run import check_inputs, run_groups, shard
+from .run import check_inputs, check_max_flow, run_groups, shard
 
 FIELD = {name: i for i, name in enumerate(FLOW_ERROR_FIELDS)}
 REGION = {name: i for i, name in enumerate(FLOW_REGION_FIELDS)}
@@ -78,12 +85,17 @@ class Scores(object):
 
     masks: the kinds of mask each pair carries, in files.Pair.masks order ("occlusions", "objects" or both).  With masks the
     records widen by FLOW_REGION_FIELDS: stage() computes the occlusion boundary distance straight from the slot and copies
-    the mask planes out of it (the slot is refilled while the forward runs), and score() adds fn2_flow_error_regions."""
+    the mask planes out of it (the slot is refilled while the forward runs), and score() adds fn2_flow_error_regions.
 
-    def __init__(self, n, masks=()):
+    visualize: a directory; score() also colour-codes the prediction and the ground truth at one scale per pair (max_flow,
+    else the ground truth's largest known flow, else the prediction's) into PNG scanlines behind the records, and take() writes
+    them as <visualize>/<sample.number, 6 digits>_pred.png and _gt.png."""
+
+    def __init__(self, n, masks=(), visualize=None, max_flow=None):
         self.masks = tuple(masks)
         self.records = np.full((n, record_width(self.masks)), np.nan)
         self.stats = {"collect": 0.0}
+        self.visualize, self.max_flow = visualize, max_flow
 
     def item_bytes(self, H, W):
         return _align(mask_offset(H, W) + len(self.masks) * H * W)
@@ -94,11 +106,18 @@ class Scores(object):
         nf, nr = len(FLOW_ERROR_FIELDS), record_width(self.masks) - len(FLOW_ERROR_FIELDS)
         self.pred = [f.permute(0, 3, 1, 2) for f in flow_dev]                       # (B, 2, H, W) views of the NHWC flow
         self.gt = [torch.empty((batch, 2, H, W), device="cuda") for _ in range(2)]
-        # each batch's records in one buffer: fn2_flow_error's (B, nf), then fn2_flow_error_regions' (B, nr)
-        self.dev = [torch.empty(batch * (nf + nr), dtype=torch.float64, device="cuda") for _ in range(2)]
-        self.host = [torch.empty(batch * (nf + nr), dtype=torch.float64).pin_memory() for _ in range(2)]
-        self.err = [d[:batch * nf].view(batch, nf) for d in self.dev]
-        self.reg = [d[batch * nf:].view(batch, nr) for d in self.dev]
+        # each batch's records in one buffer: fn2_flow_error's (B, nf), then fn2_flow_error_regions' (B, nr), then with
+        # visualize the prediction's and the ground truth's colour scanlines
+        self.rec_bytes = batch * (nf + nr) * 8
+        self.size, self.vis_bytes = (W, H), H * (1 + 3 * W)
+        nb = self.rec_bytes + (2 * batch * self.vis_bytes if self.visualize else 0)
+        self.dev = [torch.empty(nb, dtype=torch.uint8, device="cuda") for _ in range(2)]
+        self.host = [torch.empty(nb, dtype=torch.uint8).pin_memory() for _ in range(2)]
+        rec = [d[:self.rec_bytes].view(torch.float64) for d in self.dev]
+        self.err = [r[:batch * nf].view(batch, nf) for r in rec]
+        self.reg = [r[batch * nf:].view(batch, nr) for r in rec]
+        if self.visualize:
+            self.radius = [torch.empty((2, batch), device="cuda") for _ in range(2)]      # the ground truth's, the prediction's
         ws = ops.flow_error_workspace_bytes(batch, H, W)
         if self.masks:
             ws = max(ws, ops.flow_error_regions_workspace_bytes(batch, H, W))
@@ -130,15 +149,31 @@ class Scores(object):
             self.ops.flow_error_regions(self.pred[s], self.gt[s], occ=plane.get("occlusions"), obj=plane.get("objects"),
                                         dist2=self.dist2[s] if "occlusions" in plane else None, out=self.reg[s],
                                         workspace=self.workspace)
+        if self.visualize:
+            gt_r = pred_r = None
+            if self.max_flow is None:
+                gt_r, pred_r = self.ops.flow_max_radius(self.gt[s], self.radius[s][0]), self.ops.flow_max_radius(
+                    self.pred[s], self.radius[s][1])
+            o, n = self.rec_bytes, self.batch * self.vis_bytes
+            for k, flow in enumerate((self.pred[s], self.gt[s])):
+                self.ops.flow_to_color_png_rows(flow, self.dev[s][o + k * n:o + (k + 1) * n], self.max_flow, max_radius=gt_r,
+                                                fallback=pred_r)
 
     def take(self, pairs, s, n_real):
         t0 = time.perf_counter()
-        buf = self.host[s].numpy()
+        raw = self.host[s].numpy()
+        buf = raw[:self.rec_bytes].view(np.float64)
         nf = len(FLOW_ERROR_FIELDS)
         err = buf[:self.batch * nf].reshape(self.batch, nf)
         reg = buf[self.batch * nf:].reshape(self.batch, -1)
         for i, p in enumerate(pairs[:n_real]):
             self.records[p.index] = np.concatenate([err[i], reg[i]])
+            if self.visualize:
+                from . import kitti
+                o, n, m = self.rec_bytes, self.batch * self.vis_bytes, self.vis_bytes
+                for k, tag in enumerate(("pred", "gt")):
+                    kitti.write_png_rows(os.path.join(self.visualize, "%06d_%s.png" % (p.number, tag)),
+                                         raw[o + k * n + i * m:o + k * n + (i + 1) * m], *self.size, 8)
         self.stats["collect"] += time.perf_counter() - t0
 
 
@@ -231,28 +266,41 @@ def _mask_kinds(occlusions, objects):
     return tuple(k for k, _ in given), [l for _, l in given]
 
 
-def _score(caffemodel, template, samples, batch, device, threads, kitti=False, masks=()):
-    """-> (records in the samples' order, per-stage busy seconds, number of sizes).  masks: the kinds of the samples' masks."""
+def _score(caffemodel, template, samples, batch, device, threads, kitti=False, masks=(), visualize=None, max_flow=None):
+    """-> (records in the samples' order, per-stage busy seconds, number of sizes).  masks: the kinds of the samples' masks.
+    visualize, max_flow: see Scores (each sample's number names its images)."""
     t0 = time.perf_counter()
     check_inputs(caffemodel, template, batch)
+    check_max_flow(max_flow)
     probe(samples, ground_truth=True, kitti=kitti)
     for i, s in enumerate(samples):
         s.index = i
-    sink = Scores(len(samples), masks)
+    if visualize:
+        os.makedirs(visualize, exist_ok=True)
+    sink = Scores(len(samples), masks, visualize, max_flow)
     stats, sizes = run_groups(caffemodel, template, samples, batch, device, threads, sink, t0)
     return sink.records, stats, sizes
 
 
-def evaluate(caffemodel, template, samples, batch=1, device=0, threads=None, kitti=False, occlusions=None, objects=None):
+def number(samples):
+    """Numbers the samples of a whole list, before any sharding, by their position: the names of evaluate --visualize."""
+    for k, s in enumerate(samples):
+        s.number = k
+
+
+def evaluate(caffemodel, template, samples, batch=1, device=0, threads=None, kitti=False, occlusions=None, objects=None,
+             visualize=None, max_flow=None):
     """Scores the net on every files.Pair -> (summary dict, per-pair records): the summary of summarize() plus batch, sizes,
     wall (s), per-stage busy seconds and the samples whose prediction is not finite; the records are an (n, FIELDS) float64
     array in the samples' order (fields: flownet2_b200.FLOW_ERROR_FIELDS, then FLOW_REGION_FIELDS with a mask list).  kitti:
     the flows are KITTI PNGs.  occlusions, objects: mask lists (one path per sample, in order) of occlusion masks and object
-    maps, either or both, for the region scores of summarize()."""
+    maps, either or both, for the region scores of summarize().  visualize: a directory for each pair's colour-coded
+    prediction and ground truth (Scores), at the fixed scale max_flow if given."""
     t0 = time.perf_counter()
     masks, lists = _mask_kinds(occlusions, objects)
     attach_masks(samples, lists)
-    records, stats, sizes = _score(caffemodel, template, samples, batch, device, threads, kitti, masks)
+    number(samples)
+    records, stats, sizes = _score(caffemodel, template, samples, batch, device, threads, kitti, masks, visualize, max_flow)
     summary = summarize(records, [s.size[0] * s.size[1] for s in samples], _list_name(samples), bool(occlusions), bool(objects))
     summary.update({"batch": batch, "sizes": sizes, "wall": time.perf_counter() - t0, "busy": stats,
                     "not_finite": [s.where for s in not_finite(samples, records)]})
@@ -288,6 +336,10 @@ def parse_args(argv):
                                                          "EPE matched / unmatched and by distance to the occlusion boundary")
     ap.add_argument("--objects", metavar="LIST", help="object maps, one per list line (KITTI 2015's obj_map/*.png): "
                                                       "Fl and EPE of the background and the foreground")
+    ap.add_argument("--visualize", metavar="DIR", help="write each pair's colour-coded prediction and ground truth, at one "
+                                                       "scale, as DIR/<list index>_pred.png and _gt.png")
+    ap.add_argument("--max-flow", type=float, metavar="F", help="with --visualize: colour at this scale (pixels) instead of "
+                                                                "each ground truth's largest flow")
     return ap.parse_args(argv)
 
 
@@ -298,12 +350,14 @@ def main(argv=None):
     t0 = time.perf_counter()
     dist = None
     try:
+        check_max_flow(a.max_flow)
         check_inputs(a.caffemodel, a.deployproto, a.batch)
         samples = read_list(a.listfile)
         if not samples:
             raise RunError("%s: the list holds no pairs" % a.listfile)
         masks, lists = _mask_kinds(a.occlusions, a.objects)
         attach_masks(samples, lists)                                    # before sharding: every rank sees the same lines
+        number(samples)
         if world > 1:
             import torch
             import torch.distributed as dist
@@ -312,7 +366,8 @@ def main(argv=None):
         mine = shard(samples, world, rank)
         local = np.empty((0, record_width(masks) + 1))                  # this rank's records, each pair's pixel count last
         if mine:
-            records = _score(a.caffemodel, a.deployproto, mine, a.batch, device, None, a.kitti, masks)[0]
+            records = _score(a.caffemodel, a.deployproto, mine, a.batch, device, None, a.kitti, masks, a.visualize,
+                             a.max_flow)[0]
             local = np.concatenate([records, [[s.size[0] * s.size[1]] for s in mine]], axis=1)
         full = gather_records(local, len(samples), world, rank) if world > 1 else local
         if rank != 0:

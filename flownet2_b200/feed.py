@@ -4,6 +4,7 @@
     feed.seek(k)                  # the next call feeds batch k; reading starts for batches k .. k + slots - 1
     feed(stage)                   # enqueues the next batch on the net's stream and starts reading the one `slots` ahead
     feed.busy(); feed.close()
+    Feeder(None, batch, (W, H), item_bytes, items_of, slots)     # payloads only, on a stream of its own (flownet2_b200.viz)
 
 items_of(k) gives batch k's probed items (flownet2_b200.files.Pair; None past the end).  Each of the S slots is a pinned host
 buffer and a device buffer holding [img0 frames][img1 frames][payload]: the frames [B][H][W][K] bytes, K the batch's frame
@@ -12,7 +13,8 @@ channel count (batch_channels), and from a 16-byte boundary item i's flow payloa
 reads every part of a batch into its host slot: a PNM frame with K channels as stored, any other frame decoded (a mask as one
 channel), a payload through files.read_flow_into.  A call waits for the batch's reads, copies the slot to the
 device on a copy stream, and on the net's stream waits for that copy, converts the frames into the net's first two inputs
-(fn2_net_set_input_frames_device), runs stage(payload, item_bytes) on the device payload and records the slot free.
+(fn2_net_set_input_frames_device), runs stage(payload, item_bytes) on the device payload and records the slot free.  Without
+a net (net None) a slot holds the payloads alone, from offset 0, and stage() runs on a stream of the feeder's own.
 
 Three orderings keep a slot from being overwritten while in use:
   * a reader writes host slot s only after the copy out of s from S batches ago has finished; it waits for that copy itself,
@@ -62,15 +64,15 @@ def read_part(p, j, size, k, out):
 class Feeder(object):
     def __init__(self, net, batch, size, item_bytes, items_of, slots, threads=None):
         import torch
-        self.torch, self.net, self.inputs = torch, net, net.inputs[:2]
+        self.torch, self.net = torch, net
         self.batch, self.size, self.item_bytes, self.items_of, self.slots = batch, size, item_bytes, items_of, slots
-        self.frame_bytes = batch * size[0] * size[1]                   # of one input at K = 1
+        self.frame_bytes = batch * size[0] * size[1] if net is not None else 0    # of one input at K = 1
         self.payload_off = _align(2 * self.frame_bytes * 4)             # after both inputs' frames, K <= 4
         nbytes = self.payload_off + batch * item_bytes
         self._pin = [torch.empty(nbytes, dtype=torch.uint8).pin_memory() for _ in range(slots)]
         self._host = [p.numpy() for p in self._pin]
         self._dev = [torch.empty(nbytes, dtype=torch.uint8, device="cuda") for _ in range(slots)]
-        self.stream = torch.cuda.ExternalStream(net.stream)
+        self.stream = torch.cuda.ExternalStream(net.stream) if net is not None else torch.cuda.Stream()
         self._copy_stream = torch.cuda.Stream()
         self._ev_h2d = [torch.cuda.Event() for _ in range(slots)]      # pin[s] has reached dev[s]
         self._ev_free = [torch.cuda.Event() for _ in range(slots)]     # the net has converted dev[s]
@@ -96,8 +98,9 @@ class Feeder(object):
         items = self.items_of(k)
         if items is None:
             return
-        s, K = k % self.slots, batch_channels(items)
-        parts = lambda p: (0, 1, 2) + tuple(range(3, 3 + len(p.masks))) if self.item_bytes else (0, 1)
+        s, K = k % self.slots, batch_channels(items) if self.net is not None else 0
+        frames = (0, 1) if self.net is not None else ()
+        parts = lambda p: frames + (2,) + tuple(range(3, 3 + len(p.masks))) if self.item_bytes else frames
         self._reads[k] = (K, [self._pool.submit(self._read, s, K, i, j, p) for i, p in enumerate(items) for j in parts(p)])
 
     def _read(self, s, K, i, j, p):
@@ -126,7 +129,8 @@ class Feeder(object):
         with torch.cuda.stream(self._copy_stream):
             self._copy_stream.wait_event(self._ev_free[s])             # dev[s] was converted `slots` batches ago
             ev[0].record(self._copy_stream)
-            self._dev[s][:n].copy_(self._pin[s][:n], non_blocking=True)
+            if n:
+                self._dev[s][:n].copy_(self._pin[s][:n], non_blocking=True)
             if pay:
                 self._dev[s][off:off + pay].copy_(self._pin[s][off:off + pay], non_blocking=True)
             ev[1].record(self._copy_stream)
@@ -135,9 +139,10 @@ class Feeder(object):
         ev[2].record(ns)
         ns.wait_event(self._ev_h2d[s])
         ev[3].record(ns)
-        base = self._dev[s].data_ptr()
-        self.net.set_input_image_device(self.inputs[0], base, K)
-        self.net.set_input_image_device(self.inputs[1], base + n // 2, K)
+        if self.net is not None:
+            base, inputs = self._dev[s].data_ptr(), self.net.inputs[:2]
+            self.net.set_input_image_device(inputs[0], base, K)
+            self.net.set_input_image_device(inputs[1], base + n // 2, K)
         if stage is not None:
             with torch.cuda.stream(ns):
                 stage(self._dev[s][off:], self.item_bytes)

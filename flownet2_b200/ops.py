@@ -448,6 +448,54 @@ def flow_to_kitti_png_rows(flow, out=None):
     return out
 
 
+def flow_max_radius(flow, out=None):
+    """A float32 (N, 2, H, W) CUDA view of any strides -> out, N float32 on the device (a new tensor if None): each image's
+    largest sqrt(u^2 + v^2) over its known pixels (include/fn2_flow.h), -1 for an image without one.  No host sync."""
+    if out is None:
+        out = torch.empty(flow.shape[0], dtype=torch.float32, device=flow.device)
+    assert out.is_cuda and out.dtype == torch.float32 and out.is_contiguous() and out.numel() == flow.shape[0]
+    check(lib().fn2_flow_max_radius(desc(flow), out.data_ptr(), _stream()))
+    return out
+
+
+def _colour_scale(flow, max_flow, max_radius, fallback):
+    """-> (max, fallback, max_flow) arguments of the colour entry points: a fixed max_flow, or per-image radii (max_radius, the
+    flow's own when None)."""
+    if max_flow is not None:
+        return None, None, float(max_flow)
+    if max_radius is None:
+        max_radius = flow_max_radius(flow)
+    for t in (max_radius, fallback):
+        assert t is None or (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.numel() == flow.shape[0])
+    return max_radius.data_ptr(), _ptr(fallback), 0.0
+
+
+def flow_to_color(flow, max_flow=None, out=None, max_radius=None, fallback=None):
+    """A float32 (N, 2, H, W) CUDA view of any strides -> out, a dense uint8 (N, H, W, 3) CUDA tensor (a new one if None) of
+    Middlebury colour-coded RGB (include/fn2_flow.h).  Scale: max_flow (> 0) for every image, else per image max_radius (N
+    device floats, flow_max_radius(flow) when None), fallback's where max_radius is negative, and 1 where the result is not
+    positive."""
+    N, _, H, W = flow.shape
+    if out is None:
+        out = torch.empty((N, H, W, 3), dtype=torch.uint8, device=flow.device)
+    assert out.is_cuda and out.dtype == torch.uint8 and out.is_contiguous() and out.numel() >= N * H * W * 3
+    m, fb, mf = _colour_scale(flow, max_flow, max_radius, fallback)
+    check(lib().fn2_flow_to_color(desc(flow), m, fb, mf, out.data_ptr(), _stream()))
+    return out
+
+
+def flow_to_color_png_rows(flow, out=None, max_flow=None, max_radius=None, fallback=None):
+    """As flow_to_color, written as N*H Paeth-filtered 8-bit RGB PNG scanlines of 1 + 3 W bytes -> out, a dense uint8 CUDA
+    tensor of at least N*H*(1 + 3 W) bytes (a new (N, H, 1 + 3 W) one if None)."""
+    N, _, H, W = flow.shape
+    if out is None:
+        out = torch.empty((N, H, 1 + 3 * W), dtype=torch.uint8, device=flow.device)
+    assert out.is_cuda and out.dtype == torch.uint8 and out.is_contiguous() and out.numel() >= N * H * (1 + 3 * W)
+    m, fb, mf = _colour_scale(flow, max_flow, max_radius, fallback)
+    check(lib().fn2_flow_to_color_png_rows(desc(flow), m, fb, mf, out.data_ptr(), _stream()))
+    return out
+
+
 def flow_error_workspace_bytes(N, H, W):
     return _size(lib().fn2_flow_error_workspace_bytes, N, H, W)
 

@@ -2,6 +2,7 @@
 
     python -m flownet2_b200.run weights.caffemodel models/FlowNet2_deploy.prototxt.template img0.png img1.png out.flo
     python -m flownet2_b200.run weights.caffemodel models/FlowNet2_deploy.prototxt.template pairs.txt [--batch 4] [--kitti]
+                                [--visualize [--max-flow F]]
 
 The list file holds one ``img0 img1 out.flo`` line per pair; blank lines are skipped.  The weights (.caffemodel or
 .caffemodel.h5) are read once.  Pairs are grouped by frame size in order of first appearance, and each size gets one
@@ -14,6 +15,12 @@ reference (palette to RGB or RGBA, LA to L; flownet2_b200.files, which probes ev
 back as (H, W, 2), the payload order of .flo (fn2_net_get_blob_nhwc_device).  The batches ahead are read on a thread pool
 into two pinned slots and copied to the device on a copy stream (flownet2_b200.feed) while batch k runs, and batch k-1's flow
 is copied back on another stream and written by a writer thread.
+
+--visualize also writes, beside each output, <output without its extension>.vis.png: the flow colour-coded on the net's stream
+(fn2_flow_to_color_png_rows, the Middlebury colour wheel scaled by the pair's largest known flow, or by --max-flow F), coming
+back in the same copy as the flow and deflated by the writer thread (flownet2_b200.viz).  It shows the net's float prediction,
+also under --kitti; a pixel whose flow is not finite is black.  A list in which two outputs map to one .vis.png, or a
+.vis.png is another line's output, is refused.
 
 --kitti writes every output as a KITTI flow PNG (flownet2_b200.kitti, the format the KITTI benchmark takes) instead of a
 .flo: the flow becomes Paeth-filtered PNG scanlines on the net's stream (fn2_flow_to_kitti_png_rows, 6 bytes a pixel instead
@@ -81,13 +88,17 @@ class FlowFiles(object):
 
     The sink interface of _run_size: item_bytes(H, W) the pinned payload bytes per pair the feeder reads (each pair's
     flow file, flownet2_b200.feed), stage(pairs, s, payload, stride) the net stream's use of them before the forward (None
-    without a payload); bind(...) allocates dev[s] / host[s] for one frame size, score(s) runs on the net's stream after the
-    flow is in flow_dev[s] and fills dev[s], which then goes to host[s] on the copy-back stream, and take(pairs, s, n_real)
-    consumes host[s] on the writer thread."""
+    without a payload); bind(...) allocates dev[s] / host[s] for one frame size (and may replace flow_dev[s] by a view into
+    dev[s]), score(s) runs on the net's stream after the flow is in flow_dev[s] and fills dev[s], which then goes to host[s]
+    on the copy-back stream, and take(pairs, s, n_real) consumes host[s] on the writer thread.
 
-    def __init__(self):
+    visualize: each batch's flow is also colour-coded into PNG scanlines at the end of dev[s] (fn2_flow_to_color_png_rows, at
+    the fixed scale max_flow, else at each pair's own largest radius), and take() writes each pair's vis_path(flow)."""
+
+    def __init__(self, visualize=False, max_flow=None):
         self.bad = []
         self.stats = {"write": 0.0}
+        self.visualize, self.max_flow = visualize, max_flow
 
     def item_bytes(self, H, W):
         return 0
@@ -95,20 +106,54 @@ class FlowFiles(object):
     stage = None
 
     def bind(self, torch, batch, H, W, flow_dev):
-        self.dev = flow_dev
-        self.host = [torch.empty((batch, H, W, 2)).pin_memory() for _ in range(2)]
+        if not self.visualize:
+            self.dev = flow_dev
+            self.host = [torch.empty((batch, H, W, 2)).pin_memory() for _ in range(2)]
+            return
+        self.flow_bytes = batch * H * W * 8
+        nb = self._bind_vis(torch, batch, H, W, flow_dev, self.flow_bytes)
+        self.dev = [torch.empty(nb, dtype=torch.uint8, device="cuda") for _ in range(2)]
+        self.host = [torch.empty(nb, dtype=torch.uint8).pin_memory() for _ in range(2)]
+        for s in range(2):                                                # the net writes its flow straight into dev[s]
+            flow_dev[s] = self.dev[s][:self.flow_bytes].view(torch.float32).view(batch, H, W, 2)
+            self.pred[s] = flow_dev[s].permute(0, 3, 1, 2)
+
+    def _bind_vis(self, torch, batch, H, W, flow_dev, offset):
+        """The colour rows' place in dev[s], from `offset` on -> dev[s]'s size."""
+        from . import ops
+        self.ops, self.size = ops, (W, H)
+        self.pred = [f.permute(0, 3, 1, 2) for f in flow_dev]             # (B, 2, H, W) views of the NHWC flow
+        self.vis_off, self.vis_bytes = _align(offset, 16), H * (1 + 3 * W)
+        self.radius = [torch.empty(batch, device="cuda") for _ in range(2)]
+        return self.vis_off + batch * self.vis_bytes
+
+    def _score_vis(self, s):
+        radius = None if self.max_flow is not None else self.ops.flow_max_radius(self.pred[s], self.radius[s])
+        self.ops.flow_to_color_png_rows(self.pred[s], self.dev[s][self.vis_off:], self.max_flow, max_radius=radius)
+
+    def _take_vis(self, buf, i, p):
+        from . import kitti
+        n, o = self.vis_bytes, self.vis_off
+        kitti.write_png_rows(vis_path(p.flow), buf[o + i * n:o + (i + 1) * n], *self.size, 8)
 
     def score(self, s):
-        pass
+        if self.visualize:
+            self._score_vis(s)
 
     def take(self, pairs, s, n_real):
         t0 = time.perf_counter()
-        flows = self.host[s].numpy()
+        buf = self.host[s].numpy()
+        if self.visualize:
+            flows = buf[:self.flow_bytes].view(np.float32).reshape(len(pairs), self.size[1], self.size[0], 2)
+        else:
+            flows = buf
         for i, p in enumerate(pairs[:n_real]):
             if not np.isfinite(flows[i]).all():
                 self.bad.append(p)
                 sys.stderr.write("%s: the flow of %s %s is not finite\n" % (p.where, p.img0, p.img1))
             write_flo(p.flow, flows[i])
+            if self.visualize:
+                self._take_vis(buf, i, p)
         self.stats["write"] += time.perf_counter() - t0
 
 
@@ -124,28 +169,61 @@ class KittiFiles(FlowFiles):
         self.row_bytes = H * (1 + kitti.BPP * W)                          # one pair's scanlines
         self.rec_off = _align(batch * self.row_bytes, 8)                  # then the pairs' float64 records
         nb = self.rec_off + batch * fields * 8
+        if self.visualize:                                                # then the colour rows
+            nb = self._bind_vis(torch, batch, H, W, flow_dev, nb)
         self.pred = [f.permute(0, 3, 1, 2) for f in flow_dev]             # (B, 2, H, W) views of the NHWC flow
         self.dev = [torch.empty(nb, dtype=torch.uint8, device="cuda") for _ in range(2)]
         self.host = [torch.empty(nb, dtype=torch.uint8).pin_memory() for _ in range(2)]
-        self.records = [d[self.rec_off:].view(torch.float64).view(batch, fields) for d in self.dev]
+        self.records = [d[self.rec_off:self.rec_off + batch * fields * 8].view(torch.float64).view(batch, fields)
+                        for d in self.dev]
         self.zero = torch.zeros((batch, 2, H, W), device="cuda")
         self.workspace = torch.empty(max(ops.flow_error_workspace_bytes(batch, H, W), 8), dtype=torch.uint8, device="cuda")
 
     def score(self, s):
         self.ops.flow_to_kitti_png_rows(self.pred[s], self.dev[s])
         self.ops.flow_error(self.pred[s], self.zero, out=self.records[s], workspace=self.workspace)
+        if self.visualize:
+            self._score_vis(s)
 
     def take(self, pairs, s, n_real):
         t0 = time.perf_counter()
         buf = self.host[s].numpy()
-        rec = buf[self.rec_off:].view(np.float64).reshape(len(pairs), -1)
+        rec = buf[self.rec_off:self.rec_off + len(pairs) * len(self.records[s][0]) * 8].view(np.float64).reshape(len(pairs), -1)
         n = self.row_bytes
         for i, p in enumerate(pairs[:n_real]):
             if rec[i, self.nonfinite] > 0:
                 self.bad.append(p)
                 sys.stderr.write("%s: the flow of %s %s is not finite\n" % (p.where, p.img0, p.img1))
             self.kitti.write_png_rows(p.flow, buf[i * n:(i + 1) * n], *self.size)
+            if self.visualize:
+                self._take_vis(buf, i, p)
         self.stats["write"] += time.perf_counter() - t0
+
+
+def vis_path(out):
+    """The colour-coded image run --visualize writes beside the output `out`: out without its extension, then .vis.png."""
+    return os.path.splitext(out)[0] + ".vis.png"
+
+
+def check_vis_paths(pairs):
+    """Refuses a list in which two different outputs have one vis_path, or a vis_path is an output, naming the lines."""
+    outs = {os.path.normpath(p.flow): p for p in pairs}
+    seen = {}
+    for p in pairs:
+        v, out = os.path.normpath(vis_path(p.flow)), os.path.normpath(p.flow)
+        if v in seen and os.path.normpath(seen[v].flow) != out:
+            raise RunError("%s: the outputs %s and %s (%s) both visualise to %s" % (p.where, p.flow, seen[v].flow, seen[v].where,
+                                                                                  vis_path(p.flow)))
+        if v in outs:
+            raise RunError("%s: the visualisation %s of %s is the output of %s" % (p.where, vis_path(p.flow), p.flow,
+                                                                                 outs[v].where))
+        seen[v] = p
+
+
+def check_max_flow(max_flow):
+    """Refuses a --max-flow that is not a finite positive number; None passes."""
+    if max_flow is not None and not (max_flow > 0 and np.isfinite(max_flow)):
+        raise RunError("--max-flow must be a finite positive number, got %r" % max_flow)
 
 
 def _run_size(torch, net, size, pairs, batch, threads, stats, sink):
@@ -244,14 +322,18 @@ def run_groups(caffemodel, template, pairs, batch, device, threads, sink, t0):
     return stats, len(groups)
 
 
-def run(caffemodel, template, pairs, batch=1, device=0, threads=None, kitti=False):
+def run(caffemodel, template, pairs, batch=1, device=0, threads=None, kitti=False, visualize=False, max_flow=None):
     """Flow of every files.Pair into its flow file, a .flo (kitti: a KITTI flow PNG) -> summary dict: pairs, sizes, nets, wall (s),
     per-stage busy seconds (build: checking the inputs, reading the weights and constructing the nets; decode: host, summed
-    over the pool's threads; h2d / forward / d2h: device; write: host) and the pairs whose flow is not finite."""
+    over the pool's threads; h2d / forward / d2h: device; write: host) and the pairs whose flow is not finite.  visualize:
+    also each flow colour-coded into vis_path(flow), at the fixed scale max_flow if given."""
     t0 = time.perf_counter()
     check_inputs(caffemodel, template, batch)
+    check_max_flow(max_flow)
     probe(pairs)
-    sink = KittiFiles() if kitti else FlowFiles()
+    if visualize:
+        check_vis_paths(pairs)
+    sink = (KittiFiles if kitti else FlowFiles)(visualize, max_flow)
     stats, sizes = run_groups(caffemodel, template, pairs, batch, device, threads, sink, t0)
     return {"pairs": len(pairs), "sizes": sizes, "nets": sizes, "batch": batch, "wall": time.perf_counter() - t0,
             "busy": stats, "not_finite": [p.where for p in sink.bad]}
@@ -267,6 +349,9 @@ def parse_args(argv):
     ap.add_argument("--verbose", action="store_true", help="accepted for compatibility; the engine does not log")
     ap.add_argument("--batch", type=int, default=1, help="pairs per forward (outputs bit-identical to single pairs only at 1)")
     ap.add_argument("--kitti", action="store_true", help="write each output as a KITTI 16-bit flow PNG instead of a .flo")
+    ap.add_argument("--visualize", action="store_true", help="also write each flow colour-coded, as <output>.vis.png")
+    ap.add_argument("--max-flow", type=float, metavar="F", help="with --visualize: colour every flow at this scale (pixels) "
+                                                                "instead of each pair's largest flow")
     a = ap.parse_args(argv)
     if len(a.files) not in (1, 3):
         ap.error("expected img0 img1 out, or one list file; got %d paths" % len(a.files))
@@ -278,8 +363,12 @@ def main(argv=None):
     world, rank = int(os.environ.get("WORLD_SIZE", "1")), int(os.environ.get("RANK", "0"))
     device = int(os.environ.get("LOCAL_RANK", a.gpu)) if "WORLD_SIZE" in os.environ else a.gpu
     try:
+        check_max_flow(a.max_flow)
         pairs = read_list(a.files[0], ground_truth=False) if len(a.files) == 1 else [Pair("command line", *a.files)]
-        s = run(a.caffemodel, a.deployproto, shard(pairs, world, rank), batch=a.batch, device=device, kitti=a.kitti)
+        if a.visualize:
+            check_vis_paths(pairs)                                 # the whole list: ranks must not collide either
+        s = run(a.caffemodel, a.deployproto, shard(pairs, world, rank), batch=a.batch, device=device, kitti=a.kitti,
+                visualize=a.visualize, max_flow=a.max_flow)
     except RunError as e:
         sys.stderr.write("error: %s\n" % e)
         return 2

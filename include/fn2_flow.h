@@ -2,7 +2,7 @@
  * fn2_flow.h -- C-ABI of libfn2.so for ground-truth flow files: the payloads of .flo, PFM and KITTI PNG files, copied to the
  * device as the bytes they hold after their header (a PNG: once the host has undone its container), converted there to a
  * network input (the input side of the reference's convert_imageset_and_flow + CustomData training path, without the
- * host-side conversions).  The sibling of fn2_frames.h; fn2.h, fn2_frames.h and this header together state the ABI, with
+ * host-side conversions), and for the flow going out: KITTI PNG scanlines and colour-coded images.  The sibling of fn2_frames.h; fn2.h, fn2_frames.h and this header together state the ABI, with
  * fn2.h's conventions: status 0 or negative with the message in fn2_last_error().
  *
  * Formats:
@@ -26,6 +26,18 @@
  * Encode (the devkit's writeFlowField): a pixel is valid when both components are finite; a valid pixel stores
  * (uint16) max(min(64 v + 32768, 65535), 0) for u and v (float32, truncating) and B = 1, any other pixel (0, 0, 0).  Every
  * encoded row is filtered with Paeth (type 4): the scanline is the filter byte 4, then the 6 W filtered bytes.
+ *
+ * Flow colour coding (the Middlebury colour code of Baker et al., colorcode.cpp): 8-bit R, G, B per pixel.  A pixel is known
+ * when both components are finite and at most 1e9 in absolute value (UNKNOWN_FLOW_THRESH, fn2_flow_error's valid ground
+ * truth); an unknown pixel is (0, 0, 0).  The wheel holds 55 colours in segments RY 15, YG 6, GC 4, CB 11, BM 13, MR 6; entry
+ * i of a segment of length L is, in integer arithmetic, RY (255, 255 i / L, 0), YG (255 - 255 i / L, 255, 0),
+ * GC (0, 255, 255 i / L), CB (0, 255 - 255 i / L, 255), BM (255 i / L, 0, 255), MR (255, 0, 255 - 255 i / L).  Image n's
+ * scale s: max_flow when it is positive, else max[n] (fallback[n] when max[n] is negative and a fallback is given), and 1 when
+ * that is not positive; max[n] is normally fn2_flow_max_radius's.  In float32, without FMA contraction, for a known (u, v):
+ * fx = u / s, fy = v / s; rad = sqrtf(fx fx + fy fy); a = t / pi, t the double atan2(-fy, -fx) rounded to float32 and pi
+ * the float32 pi (so (1, 0) gives exactly -1); fk = (a + 1) / 2 * 54,
+ * k0 = (int) fk, k1 = (k0 + 1) % 55, f = fk - k0; per channel col = (1 - f) w[k0] / 255 + f w[k1] / 255, then
+ * col = 1 - rad (1 - col) when rad <= 1, else 0.75 col; the byte is (int)(255 col).
  */
 #ifndef FN2_FLOW_H_
 #define FN2_FLOW_H_
@@ -53,6 +65,21 @@ FN2_API int fn2_net_set_input_flow_device(fn2_net* net, const char* blob, const 
  * (image n's row y at (n H + y)(1 + 6 W); the first row of every image is filtered against zeros), on stream.
  * FN2_ERR_INVALID for src.c != 2 or a misaligned src. */
 FN2_API int fn2_flow_to_kitti_png_rows(const fn2_tensor* src, void* dst_dev, void* stream);
+/* src, any float view of shape (N, 2, H, W), 4-byte aligned -> max_dev[n] (N floats, 4-byte aligned): the largest float32
+ * sqrtf(u u + v v) over image n's known pixels, -1 for an image without one; on stream, no host synchronisation.  Exact (a
+ * maximum).  FN2_ERR_INVALID for src.c != 2, N above 65535 or a misaligned pointer. */
+FN2_API int fn2_flow_max_radius(const fn2_tensor* src, float* max_dev, void* stream);
+/* src, any float view of shape (N, 2, H, W), 4-byte aligned -> dst_dev: the colour code above as dense [N][H][W][3] bytes
+ * (R, G, B), on stream.  Scale: max_flow > 0, or max_flow = 0 with max_dev (N floats on the device, 4-byte aligned) and
+ * optionally fallback_dev (the same, or null).  FN2_ERR_INVALID for src.c != 2, a misaligned pointer, a max_flow that is
+ * negative or not finite, and max_flow = 0 without max_dev. */
+FN2_API int fn2_flow_to_color(const fn2_tensor* src, const float* max_dev, const float* fallback_dev, float max_flow, void* dst_dev,
+                              void* stream);
+/* As fn2_flow_to_color, written as N*H PNG scanlines of 1 + 3 W bytes for 8-bit RGB (colour type 2, bit depth 8),
+ * Paeth-filtered with 3 bytes per pixel (image n's row y at (n H + y)(1 + 3 W); the first row of every image is filtered against
+ * zeros), the row layout of fn2_flow_to_kitti_png_rows. */
+FN2_API int fn2_flow_to_color_png_rows(const fn2_tensor* src, const float* max_dev, const float* fallback_dev, float max_flow,
+                                       void* dst_dev, void* stream);
 /* Host: undoes PNG's per-row filters (types 0-4) of `rows` scanlines of 1 + row_bytes bytes at src into rows * row_bytes
  * bytes at dst; bpp: bytes per complete pixel (1..8), the filters' left distance.  The first row is filtered against zeros.
  * FN2_ERR_INVALID for a filter type above 4, naming the row.  No device work. */
