@@ -147,7 +147,7 @@ def fill_train_template(text, crop_width, crop_height, data_width, data_height, 
 
 
 def model_template(name):
-    """Text of models/<name>_deploy.prototxt.template (FlowNet2, FlowNet2-C, -S, -CSS, -SD)."""
+    """Text of models/<name>_deploy.prototxt.template (FlowNet2, FlowNet2-C, -S, -CS, -CSS, -SD)."""
     p = os.path.join(os.path.dirname(_HERE), "models", "%s_deploy.prototxt.template" % name)
     with open(p) as f:
         return f.read()
@@ -234,6 +234,17 @@ class Net(object):
 
     def to_caffemodel(self):
         return sized_output(lib().fn2_net_to_caffemodel, self._h)
+
+    def param_layers(self):
+        """The layers that hold parameter blobs, in net order -> [(name, type, flags, blob shapes, lr_mults)]: flags "c" when
+        the layer takes its blobs through its own copy (DataAugmentation, adjusted to this net's crop), "t" when the template
+        alone defines its weights (a diagonal filler), "" otherwise (include/fn2_eval.h fn2_net_param_layers)."""
+        out = []
+        for line in sized_output(lib().fn2_net_param_layers, self._h)[:-1].decode().splitlines():
+            name, typ, flags, shapes, mults = line.split("\t")
+            out.append((name, typ, flags.strip("-"), [tuple(int(d) for d in s.split("x")) for s in shapes.split(",")],
+                        [float(m) for m in mults.split(",")]))
+        return out
 
     def to_hdf5(self):
         """Net::ToHDF5 (net.cpp:905-960): the weights as the bytes of a .caffemodel.h5 file."""

@@ -1,8 +1,10 @@
 // extern "C" net-level entry points of include/fn2.h, fn2_frames.h, fn2_flow.h and fn2_lpq.h over caffe::Net<float>, and the solver's of
 // include/fn2_solver.h over caffe::Solver.
+#include <cstdio>
 #include <cstring>
 #include <type_traits>
 
+#include "../../../include/fn2_eval.h"
 #include "../../../include/fn2_flow.h"
 #include "../../../include/fn2_frames.h"
 #include "../../../include/fn2_lpq.h"
@@ -91,6 +93,29 @@ int fn2_net_copy_trained_layers(fn2_net* net, const void* caffemodel, size_t byt
 int fn2_net_copy_trained_layers_prefixed(fn2_net* net, const void* caffemodel, size_t bytes, const char* prefix) {
     return net_call("copy_trained_layers_prefixed", net && caffemodel && prefix,
                     [&] { net->net->CopyTrainedLayersFrom(caffemodel, bytes, prefix); });
+}
+
+int fn2_net_param_layers(fn2_net* net, char* out, size_t* bytes) {
+    return net_call("param_layers", net && bytes, [&] {
+        caffe::Net<float>& n = *net->net;
+        std::string text;
+        for (size_t i = 0; i < n.layers().size(); i++) {
+            caffe::Layer<float>& l = *n.layers()[i];
+            if (l.blobs().empty()) continue;
+            std::string shapes, mults;
+            for (size_t j = 0; j < l.blobs().size(); j++) {
+                if (j) { shapes += ","; mults += ","; }
+                const std::vector<int>& s = l.blobs()[j]->shape();
+                for (size_t k = 0; k < s.size(); k++) shapes += (k ? "x" : "") + std::to_string(s[k]);
+                char m[32];
+                snprintf(m, sizeof(m), "%g", n.lr_mult((int)i, (int)j));
+                mults += m;
+            }
+            const char* flags = l.DoesUseCustomCopyBlobs() ? "c" : l.TemplateDefinedParams() ? "t" : "-";
+            text += n.layer_names()[i] + "\t" + l.type() + "\t" + flags + "\t" + shapes + "\t" + mults + "\n";
+        }
+        return emit("param_layers", text, true, out, bytes);
+    });
 }
 
 int fn2_net_to_caffemodel(fn2_net* net, void* buf, size_t* bytes) {

@@ -72,6 +72,9 @@ class Layer {
     virtual void ParamsChanged() {}
     // Fill parameters from the prototxt fillers (Net::FillParams); default: nothing to fill.
     virtual void FillParams(uint64_t seed) {}
+    // true when the prototxt alone defines the parameters (a seed-free filler such as "diagonal", so FillParams ignores the
+    // seed): Net::CopyTrainedLayersFrom fills them when the source does not name the layer, as Caffe's fillers have by then.
+    virtual bool TemplateDefinedParams() const { return false; }
     // Conv/Deconv: fuse an in-place ReLU that directly follows top[i].
     virtual bool FuseReLU(int top_index, float negative_slope) { return false; }
     // Algorithmic work of one Forward (for roofline reporting): flops and bytes moved if every

@@ -589,6 +589,10 @@ class BaseConvolutionLayer : public Layer<Dtype> {
             if (d_.has_bias) { this->blobs_[1].reset(new Blob<Dtype>()); this->blobs_[1]->Reshape(vector<int>{d_.co}); }
         }
     }
+    // the deploy nets' scale_conv1: a diagonal filler and no bias, so its weights follow from the template variables alone
+    bool TemplateDefinedParams() const override {
+        return !d_.has_bias && this->layer_param_.convolution_param().weight_filler().type() == "diagonal";
+    }
     void Reshape(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) override {
         CHECK_EQ(bottom[0]->channels(), d_.ci) << "Input size incompatible with convolution kernel.";
         for (size_t i = 1; i < bottom.size(); ++i)

@@ -320,9 +320,11 @@ void Net<Dtype>::CopyTrainedLayersFromHDF5(const void* h5, size_t bytes, const s
     CHECK(f.has("/data")) << "Error reading weights: the file has no /data group";
     std::map<string, int> index;
     for (size_t i = 0; i < layer_names_.size(); i++) index[layer_names_[i]] = (int)i;
+    std::set<int> filled;
     for (const string& src : f.links("/data")) {
         auto it = index.find(prefix + src);
         if (it == index.end()) continue;                               // "Ignoring source layer"
+        filled.insert(it->second);
         auto& target = layers_[it->second]->blobs();
         const string base = "/data/" + src;
         const vector<string> links = f.links(base);
@@ -349,7 +351,17 @@ void Net<Dtype>::CopyTrainedLayersFromHDF5(const void* h5, size_t bytes, const s
         }
         if (!staged.empty()) layers_[it->second]->CustomCopyBlobs(staged);
     }
+    FillTemplateDefined(filled);
     ParamsChanged();
+}
+
+// Caffe fills every layer from its prototxt fillers before it copies trained layers; this net does not (its parameters start
+// at zero), so a layer whose weights the template alone defines (TemplateDefinedParams: the deploy nets' diagonal
+// scale_conv1) is filled here when the source leaves it out, as a training snapshot does.
+template <typename Dtype>
+void Net<Dtype>::FillTemplateDefined(const std::set<int>& filled) {
+    for (size_t i = 0; i < layers_.size(); i++)
+        if (!filled.count((int)i) && layers_[i]->TemplateDefinedParams()) layers_[i]->FillParams(0);
 }
 
 template <typename Dtype>
@@ -358,10 +370,12 @@ void Net<Dtype>::CopyTrainedLayersFrom(const void* caffemodel, size_t bytes, con
     if (bytes >= 8 && !memcmp(caffemodel, h5sig, 8)) { CopyTrainedLayersFromHDF5(caffemodel, bytes, prefix); return; }   // .caffemodel.h5
     Caffe::stream() = stream_;
     vector<LayerBlobs> src = ParseCaffemodel(caffemodel, bytes);
+    std::set<int> filled;
     for (const LayerBlobs& sl : src) {
         size_t ti = 0;
         while (ti != layer_names_.size() && layer_names_[ti] != prefix + sl.name) ++ti;
         if (ti == layer_names_.size()) continue;                               // "Ignoring source layer"
+        filled.insert((int)ti);
         auto& target = layers_[ti]->blobs();
         if (layers_[ti]->DoesUseCustomCopyBlobs()) {                            // net.cpp:769-780 (fork)
             vector<shared_ptr<Blob<Dtype> > > tmp;
@@ -385,6 +399,7 @@ void Net<Dtype>::CopyTrainedLayersFrom(const void* caffemodel, size_t bytes, con
             target[j]->FromProto(sl.blobs[j], false);
         }
     }
+    FillTemplateDefined(filled);
     ParamsChanged();
 }
 

@@ -39,6 +39,7 @@ class Net {
     // trained sub-network inside the next stage's graph: conv1 -> net1_conv1); source layers with no target are ignored.
     void CopyTrainedLayersFrom(const void* caffemodel, size_t bytes, const string& prefix = "");
     void CopyTrainedLayersFromHDF5(const void* h5, size_t bytes, const string& prefix = "");
+    void FillTemplateDefined(const std::set<int>& filled);
     std::string ToCaffemodel();
     void FillParams(uint64_t seed);
     void ParamsChanged();

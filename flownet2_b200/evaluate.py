@@ -61,7 +61,7 @@ import numpy as np
 from . import FLOW_ERROR_FIELDS, FLOW_REGION_FIELDS
 from .feed import _align, mask_offset
 from .files import RunError, attach_masks, probe, read_list
-from .run import check_inputs, check_max_flow, run_groups, shard
+from .run import STAGES, _run_size, check_inputs, check_max_flow, group_by_size, run_groups, shard
 
 FIELD = {name: i for i, name in enumerate(FLOW_ERROR_FIELDS)}
 REGION = {name: i for i, name in enumerate(FLOW_REGION_FIELDS)}
@@ -321,6 +321,107 @@ def gather_records(local, n_total, world, rank):
     if rank != 0:
         return None
     return combine_shards([g[:len(range(r, n_total, world))].cpu().numpy() for r, g in enumerate(got)])
+
+
+def _squeeze(shape):
+    """A blob shape without its leading ones: the shapes Net.copy_from treats as equal."""
+    shape = tuple(shape)
+    while len(shape) > 1 and shape[0] == 1:
+        shape = shape[1:]
+    return shape
+
+
+def check_handover(train_layers, deploy_layers, deploy_name="the deploy net"):
+    """Refuses a deploy net that cannot score the training net's weights (Net.param_layers of each), naming the first
+    offending layer: a layer the training net trains (an lr_mult != 0) with no layer of that name and blob shapes in the
+    deploy net, a layer of both whose blobs the copy would refuse, or a deploy layer with parameters that gets none from the
+    training net and whose weights the template does not define (a diagonal filler)."""
+    train = {name: (flags, shapes) for name, _, flags, shapes, _ in train_layers}
+    deploy = {name: (flags, shapes) for name, _, flags, shapes, _ in deploy_layers}
+    same = lambda a, b: [_squeeze(s) for s in a] == [_squeeze(s) for s in b]
+    for name, _, flags, shapes, mults in train_layers:
+        if name in deploy:
+            if "c" not in flags and not same(shapes, deploy[name][1]):
+                raise RunError("the training net's layer %s has blobs %s, its namesake in %s %s" % (
+                    name, shapes, deploy_name, deploy[name][1]))
+        elif any(m != 0 for m in mults):
+            raise RunError("the training net trains layer %s, which %s lacks" % (name, deploy_name))
+    for name, _, flags, _, _ in deploy_layers:
+        if name not in train and "t" not in flags:
+            raise RunError("layer %s of %s gets no weights from the training net" % (name, deploy_name))
+
+
+class Validator(object):
+    """Scores weights held in memory against a list, again and again: the train command's --val.
+
+    At construction the list is read the way evaluate() reads it (files.probe, the mask lists attached, the pairs numbered),
+    so a bad list is refused before anything runs on the device.  Under torchrun (world, rank) this rank scores the lines i
+    with i % world == rank.  One deploy net per frame size (fill_template of `template`) is built on first use and kept;
+    score(weights) loads caffemodel bytes into each kept net with Net.copy_from and runs its pairs through run._run_size into
+    a Scores sink.  The summary and records are evaluate()'s for the same weights read from a file, bit for bit."""
+
+    def __init__(self, template, samples, batch=1, device=0, threads=None, kitti=False, occlusions=None, objects=None,
+                 world=1, rank=0):
+        if batch < 1:
+            raise RunError("--val-batch must be at least 1, got %d" % batch)
+        if not os.path.isfile(template):
+            raise RunError("%s: no such deploy prototxt template" % template)
+        if not samples:
+            raise RunError("the validation list holds no pairs")
+        with open(template) as f:
+            self.text = f.read()
+        self.masks, lists = _mask_kinds(occlusions, objects)
+        self.occlusions, self.objects = bool(occlusions), bool(objects)
+        attach_masks(samples, lists)
+        number(samples)
+        probe(samples, ground_truth=True, kitti=kitti)
+        self.samples, self.template, self.batch, self.device, self.threads = samples, template, batch, device, threads
+        self.world, self.rank = world, rank
+        self.mine = shard(samples, world, rank)
+        for i, s in enumerate(self.mine):
+            s.index = i
+        self.groups = group_by_size(self.mine)
+        self.nets = {}
+
+    def net(self, size):
+        """The kept deploy net of frame size (width, height), built on first use."""
+        if size not in self.nets:
+            import torch
+            import flownet2_b200 as F
+            torch.cuda.set_device(self.device)
+            self.nets[size] = F.Net(F.fill_template(self.text, size[0], size[1]), None, F.TEST, batch=self.batch)
+        return self.nets[size]
+
+    def check_handover(self, train_net):
+        """Refuses (check_handover) a training net whose weights this deploy template cannot score, before any validation."""
+        size = self.groups[0][0] if self.groups else self.samples[0].size
+        check_handover(train_net.param_layers(), self.net(size).param_layers(), self.template)
+
+    def score(self, weights):
+        """caffemodel bytes -> (summary, records) on rank 0, (None, None) elsewhere: evaluate()'s summary keys and records."""
+        import torch
+        t0 = time.perf_counter()
+        torch.cuda.set_device(self.device)
+        sink = Scores(len(self.mine), self.masks)
+        stats = dict.fromkeys(STAGES, 0.0)
+        stats.update(sink.stats)
+        for size, group in self.groups:
+            tb = time.perf_counter()
+            net = self.net(size)
+            net.copy_from(weights)
+            stats["build"] += time.perf_counter() - tb
+            _run_size(torch, net, size, group, self.batch, self.threads, stats, sink)
+        stats.update(sink.stats)
+        local = np.concatenate([sink.records, [[s.size[0] * s.size[1]] for s in self.mine]], axis=1) if self.mine \
+            else np.empty((0, record_width(self.masks) + 1))
+        full = gather_records(local, len(self.samples), self.world, self.rank) if self.world > 1 else local
+        if self.rank != 0:
+            return None, None
+        records = full[:, :-1]
+        summary = summarize(records, full[:, -1], _list_name(self.samples), self.occlusions, self.objects)
+        summary.update({"batch": self.batch, "sizes": len(group_by_size(self.samples)), "wall": time.perf_counter() - t0,
+                        "busy": stats, "not_finite": [s.where for s in not_finite(self.samples, records)]})
+        return summary, records
 
 
 def parse_args(argv):

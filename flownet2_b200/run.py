@@ -293,6 +293,9 @@ def check_inputs(caffemodel, template, batch):
             raise RunError("%s: no such %s" % (path, what))
 
 
+STAGES = ("build", "decode", "h2d", "forward", "d2h")                 # the busy seconds of run_groups, in this order
+
+
 def run_groups(caffemodel, template, pairs, batch, device, threads, sink, t0):
     """The pipeline of run and evaluate over probed pairs (files.probe): one net per frame size, the weights read once, each
     size's batches through _run_size into `sink` -> (per-stage busy seconds, number of sizes).  The build time counts
@@ -300,7 +303,7 @@ def run_groups(caffemodel, template, pairs, batch, device, threads, sink, t0):
     import torch
     import flownet2_b200 as F
     torch.cuda.set_device(device)
-    stats = {k: 0.0 for k in ("build", "decode", "h2d", "forward", "d2h")}
+    stats = dict.fromkeys(STAGES, 0.0)
     stats.update(sink.stats)
     with open(template) as f:
         text = f.read()

@@ -112,6 +112,18 @@ FN2_API int fn2_flow_error_regions(const fn2_tensor* pred, const fn2_tensor* gt,
                                    size_t mask_pair_stride, const int32_t* dist2_dev, double* out_dev, void* workspace,
                                    size_t workspace_bytes, void* stream);
 
+/* Scoring a training net's weights with a deploy net (the train command's --val) needs the two to fit: every layer the
+ * training net trains has a namesake in the deploy net with the same blob shapes, and every deploy layer with parameters gets
+ * them from the training net or from its own template.  fn2_net_param_layers lists what that check reads.
+ *
+ * The layers that hold parameter blobs, in net order, as text: one line per layer,
+ *   name TAB type TAB flags TAB shapes TAB lr_mults
+ * flags: 'c' when the layer takes its blobs through its own copy (DataAugmentation: adjusted to this net's crop, so the
+ * shapes need not match the source's), 't' when the template alone defines its weights (a diagonal filler, filled by
+ * fn2_net_copy_trained_layers when the source leaves the layer out), '-' for neither; shapes: each blob's dims joined by 'x', the blobs separated by ','; lr_mults: each blob's
+ * ParamSpec lr_mult, separated by ','.  The size-query convention of fn2_net_to_caffemodel (fn2.h); the text ends in a NUL. */
+FN2_API int fn2_net_param_layers(fn2_net* net, char* out, size_t* bytes);
+
 #ifdef __cplusplus
 }
 #endif

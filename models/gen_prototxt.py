@@ -231,6 +231,13 @@ def build_css():
     return p.text()
 
 
+def build_cs():
+    p = P(); header(p, "FlowNet2-CS"); a, b = preprocess(p)
+    flow = css_body(p, a, b, stages=(2,))
+    postprocess(p, flow)
+    return p.text()
+
+
 def build_sd():
     p = P(); header(p, "FlowNet2-SD"); a, b = preprocess(p)
     concat(p, "Concat_input", [a, b], "input")
@@ -401,8 +408,8 @@ def build_full_train():
     return p.text()
 
 
-MODELS = {"FlowNet2-S": build_s, "FlowNet2-C": build_c, "FlowNet2-CSS": build_css, "FlowNet2-SD": build_sd,
-          "FlowNet2": build_full}
+MODELS = {"FlowNet2-S": build_s, "FlowNet2-C": build_c, "FlowNet2-CS": build_cs, "FlowNet2-CSS": build_css,
+          "FlowNet2-SD": build_sd, "FlowNet2": build_full}
 TRAIN_MODELS = {"FlowNet2-C": build_c_train, "FlowNet2-CS": build_cs_train, "FlowNet2-CSS": build_css_train,
                 "FlowNet2-SD": build_sd_train, "FlowNet2": build_full_train}
 
