@@ -44,6 +44,11 @@ FLOW_REGION_FIELDS = tuple(sorted((k[len("FN2_FLOW_REGION_"):].lower() for k in 
                                   if k.startswith("FN2_FLOW_REGION_") and k != "FN2_FLOW_REGION_FIELDS"),
                                  key=lambda f: _DEFINES["FN2_FLOW_REGION_" + f.upper()]))
 assert len(FLOW_REGION_FIELDS) == _DEFINES["FN2_FLOW_REGION_FIELDS"]
+# the per-pair record of fn2_mask_confusion, the same way
+MASK_CONFUSION_FIELDS = tuple(sorted((k[len("FN2_MASK_CONFUSION_"):].lower() for k in _DEFINES
+                                     if k.startswith("FN2_MASK_CONFUSION_") and k != "FN2_MASK_CONFUSION_FIELDS"),
+                                    key=lambda f: _DEFINES["FN2_MASK_CONFUSION_" + f.upper()]))
+assert len(MASK_CONFUSION_FIELDS) == _DEFINES["FN2_MASK_CONFUSION_FIELDS"]
 DIST2_NONE = _DEFINES["FN2_DIST2_NONE"]
 
 

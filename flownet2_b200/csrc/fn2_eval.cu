@@ -1,6 +1,7 @@
 // Scoring a predicted flow against ground truth (include/fn2_eval.h): per pair, the valid-pixel count, the EPE sum, KITTI's Fl
 // outliers, the non-finite predictions and the three Sintel speed bands, in one pass over both flows; the same scores by region
-// (occlusion, distance to the occlusion boundary, object map) in a second pass; and the boundary distance itself.
+// (occlusion, distance to the occlusion boundary, object map) in a second pass; the boundary distance itself; and the
+// confusion counts of a predicted occlusion mask against a ground-truth one.
 //
 // flow_error_kernel: grid (blocks per pair, N); each thread visits its pair's pixels in a fixed grid-stride order and keeps the
 // ten fields in double registers; the block folds them with warp butterflies and a fixed-order sum over its warps into one
@@ -318,6 +319,46 @@ __global__ void __launch_bounds__(kRowThreads) boundary_row_kernel(int H, int W,
     }
 }
 
+// Confusion counts of two 8-bit masks: grid (blocks per pair, N).  Each thread counts its pixels' TP, FP and FN, each warp sums
+// them with a shuffle reduction and its lane 0 adds them to the pair's 64-bit counters (out, zeroed first) with atomicAdd:
+// integer sums, so the counts do not depend on the order.  confusion_final_kernel derives TN and stores the four as doubles
+// in place.
+__global__ void __launch_bounds__(kThreads) mask_confusion_kernel(const unsigned char* __restrict__ pred,
+                                                                  const unsigned char* __restrict__ gt, long long stride, int hw,
+                                                                  unsigned long long* __restrict__ out) {
+    const int n = blockIdx.y;
+    const unsigned char* p = pred + n * stride;
+    const unsigned char* g = gt + n * stride;
+    unsigned tp = 0, fp = 0, fn = 0;
+    for (int i = blockIdx.x * kThreads + threadIdx.x; i < hw; i += gridDim.x * kThreads) {
+        const bool a = __ldg(p + i) != 0, b = __ldg(g + i) != 0;
+        tp += a && b;
+        fp += a && !b;
+        fn += !a && b;
+    }
+    tp = __reduce_add_sync(0xffffffffu, tp);
+    fp = __reduce_add_sync(0xffffffffu, fp);
+    fn = __reduce_add_sync(0xffffffffu, fn);
+    if ((threadIdx.x & 31) == 0 && (tp | fp | fn)) {
+        unsigned long long* o = out + (long long)n * 4;
+        atomicAdd(o + 0, (unsigned long long)tp);
+        atomicAdd(o + 1, (unsigned long long)fp);
+        atomicAdd(o + 2, (unsigned long long)fn);
+    }
+}
+
+__global__ void confusion_final_kernel(int N, long long hw, unsigned long long* __restrict__ counts) {
+    const int n = blockIdx.x * blockDim.x + threadIdx.x;
+    if (n >= N) return;
+    unsigned long long* c = counts + (long long)n * 4;
+    const unsigned long long tp = c[0], fp = c[1], fn = c[2];
+    double* d = reinterpret_cast<double*>(c);
+    d[0] = (double)tp;
+    d[1] = (double)fp;
+    d[2] = (double)fn;
+    d[3] = (double)(hw - (long long)(tp + fp + fn));
+}
+
 }  // namespace
 }  // namespace fn2
 
@@ -402,6 +443,26 @@ int fn2_flow_error_regions(const fn2_tensor* pred, const fn2_tensor* gt, const v
     FN2_LAUNCH_CHECK();
     const int total = p.n * kRegionFields;
     final_kernel<kRegionFields><<<(total + 127) / 128, 128, 0, st>>>((const double*)workspace, p.n, bpp, out_dev);
+    FN2_LAUNCH_CHECK();
+    return FN2_OK;
+}
+
+int fn2_mask_confusion(const void* pred_dev, const void* gt_dev, size_t pair_stride, int N, int H, int W, double* out_dev,
+                       void* stream) {
+    FN2_CHECK_ARG(pred_dev && gt_dev && out_dev && N > 0 && H > 0 && W > 0, "mask_confusion: bad argument");
+    FN2_CHECK_ARG(N <= 65535 && (long long)H * W <= (1LL << 30), "mask_confusion: %d pairs of %dx%d is too large", N, W, H);
+    FN2_CHECK_ARG(pair_stride >= (size_t)H * W, "mask_confusion: pair stride %zu is below H * W = %lld", pair_stride,
+                  (long long)H * W);
+    FN2_CHECK_ARG(!((uintptr_t)out_dev & 7), "mask_confusion: out must be 8-byte aligned");
+    cudaStream_t st = (cudaStream_t)stream;
+    FN2_CUDA(cudaMemsetAsync(out_dev, 0, (size_t)N * 4 * sizeof(double), st));
+    const int hw = H * W;
+    const int bpp = (int)max(1LL, min(((long long)hw + kThreads - 1) / kThreads, (long long)ew_grid((long long)hw * N, kThreads) / N));
+    unsigned long long* counts = reinterpret_cast<unsigned long long*>(out_dev);
+    mask_confusion_kernel<<<dim3(bpp, N), kThreads, 0, st>>>((const unsigned char*)pred_dev, (const unsigned char*)gt_dev,
+                                                             (long long)pair_stride, hw, counts);
+    FN2_LAUNCH_CHECK();
+    confusion_final_kernel<<<(N + 127) / 128, 128, 0, st>>>(N, (long long)hw, counts);
     FN2_LAUNCH_CHECK();
     return FN2_OK;
 }

@@ -1,6 +1,7 @@
 // Streaming (HBM-bound) layers: FlowWarp, Resample, DataAugmentation kernels, ChannelNorm, the warp block, and the
 // element-wise ops of the forward and backward passes (ReLU and its backward, Eltwise SUM, y = alpha*x + beta*y, strided
-// copy and fill), the conversion of 8-bit frames into an input blob, the flow-file conversions and the flow colour coding.
+// copy and fill), the conversion of 8-bit frames into an input blob, the flow-file conversions, the flow colour coding and the
+// forward-backward occlusion check.
 //
 // This translation unit is compiled with -fmad=false: every expression below is evaluated
 // with separately rounded multiplies and adds in the order written, which is also how the CPU
@@ -949,6 +950,36 @@ __global__ void flow_to_color_png_rows_kernel(T4 f, const float* __restrict__ ma
     });
 }
 
+// ---------------------------------------------------------------------------------------------
+// Forward-backward consistency (include/fn2_flow.h; Sundaram, Brox and Keutzer, ECCV 2010).  The backward flow is sampled where
+// the forward flow lands with FlowWarp's own taps and mix (warp_taps, warp_channel), so the sample is fn2_flow_warp_forward's
+// output for image = bwd, flow = fwd, bit for bit.  Grid (blocks, N): pair blockIdx.y, its pixels in a grid-stride walk, one
+// byte written per pixel.  Each pixel reads 8 bytes of forward flow and four backward taps, mostly its neighbours' (cache hits).
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ bool fb_occluded(const T4& fwd, const T4& bwd, float alpha1, float alpha2, int n, int y, int x) {
+    const float fu = fwd.p[fwd.off(n, 0, y, x)], fv = fwd.p[fwd.off(n, 1, y, x)];
+    if (!isfinite(fu) || !isfinite(fv)) return true;
+    const WarpTaps t = warp_taps(bwd, n, y, x, fu, fv);
+    if (!t.inside) return true;
+    const float bu = warp_channel(t, bwd, 0), bv = warp_channel(t, bwd, 1);
+    if (!isfinite(bu) || !isfinite(bv)) return true;
+    const float du = fu + bu, dv = fv + bv;
+    const float lhs = du * du + dv * dv;
+    const float mag = (fu * fu + fv * fv) + (bu * bu + bv * bv);
+    return lhs > alpha1 * mag + alpha2;
+}
+
+__global__ void flow_fb_occlusion_kernel(T4 fwd, T4 bwd, float alpha1, float alpha2, uint8_t* __restrict__ out,
+                                         long long row_stride, long long pair_stride) {
+    const int n = blockIdx.y;
+    const long long hw = (long long)fwd.h * fwd.w;
+    uint8_t* o = out + n * pair_stride;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < hw; i += (long long)gridDim.x * blockDim.x) {
+        const int y = (int)(i / fwd.w), x = (int)(i - (long long)y * fwd.w);
+        o[y * row_stride + x] = fb_occluded(fwd, bwd, alpha1, alpha2, n, y, x) ? 255 : 0;
+    }
+}
+
 }  // namespace fn2
 
 using namespace fn2;
@@ -1260,6 +1291,31 @@ int fn2_flow_to_color_png_rows(const fn2_tensor* src, const float* max_dev, cons
     T4 f = view(src);
     return ew_launch(flow_to_color_png_rows_kernel, (long long)f.n * f.h * f.w, stream, f, max_dev, fallback_dev, max_flow,
                      static_cast<uint8_t*>(dst_dev));
+}
+
+int fn2_flow_fb_occlusion(const fn2_tensor* fwd, const fn2_tensor* bwd, float alpha1, float alpha2, void* out_dev,
+                          size_t row_stride, size_t pair_stride, void* stream) {
+    FN2_CHECK_ARG(valid(fwd) && valid(bwd), "flow_fb_occlusion: a flow is null or empty");
+    FN2_CHECK_ARG(out_dev, "flow_fb_occlusion: out is null");
+    FN2_CHECK_ARG(!((reinterpret_cast<uintptr_t>(fwd->data) | reinterpret_cast<uintptr_t>(bwd->data)) & 3),
+                  "flow_fb_occlusion: the flows must be 4-byte aligned");
+    const T4 f = view(fwd), b = view(bwd);
+    FN2_CHECK_ARG(same_dims(f, b), "flow_fb_occlusion: fwd is %dx%dx%dx%d but bwd is %dx%dx%dx%d", f.n, f.c, f.h, f.w, b.n, b.c,
+                  b.h, b.w);
+    FN2_CHECK_ARG(f.c == 2, "flow_fb_occlusion: flows need 2 channels (u, v), got %d", f.c);
+    FN2_CHECK_ARG(isfinite(alpha1) && alpha1 >= 0.f && isfinite(alpha2) && alpha2 >= 0.f,
+                  "flow_fb_occlusion: alpha1 and alpha2 must be finite and non-negative, got %g and %g", (double)alpha1,
+                  (double)alpha2);
+    FN2_CHECK_ARG(row_stride >= (size_t)f.w, "flow_fb_occlusion: row stride %zu is below W = %d", row_stride, f.w);
+    FN2_CHECK_ARG(pair_stride >= (size_t)f.h * row_stride, "flow_fb_occlusion: pair stride %zu is below H * row stride = %zu",
+                  pair_stride, (size_t)f.h * row_stride);
+    FN2_CHECK_ARG(f.n <= 65535, "flow_fb_occlusion: %d pairs, at most 65535", f.n);
+    const long long hw = (long long)f.h * f.w;
+    const int blocks = (int)std::max(1LL, std::min((hw + 255) / 256, (long long)ew_grid(hw * f.n, 256) / f.n));
+    flow_fb_occlusion_kernel<<<dim3(blocks, f.n), 256, 0, (cudaStream_t)stream>>>(f, b, alpha1, alpha2, static_cast<uint8_t*>(out_dev),
+                                                                                  (long long)row_stride, (long long)pair_stride);
+    FN2_LAUNCH_CHECK();
+    return FN2_OK;
 }
 
 }  // extern "C"

@@ -2,7 +2,7 @@
 
     python -m flownet2_b200.evaluate weights.caffemodel models/FlowNet2_deploy.prototxt.template val.txt [--batch B]
                                      [--per-pair out.tsv] [--gpu G] [--kitti] [--occlusions LIST] [--objects LIST]
-                                     [--visualize DIR [--max-flow F]]
+                                     [--visualize DIR [--max-flow F]] [--fb-check [--fb-alpha1 A] [--fb-alpha2 B]]
 
 The list is the train command's: one ``img0 img1 flow`` line per pair (files.read_list; an occlusion field is refused), flows
 as .flo or 'PF' PFM of either byte order.  Frame sizes may differ from line to line; a flow must have its frames' size
@@ -40,6 +40,16 @@ Pooled over the list, null when empty:
 exactly the plain command's.  When a prediction is not finite
 its pairs are named on stderr and the status is 1, as in run.
 
+--fb-check [--fb-alpha1 A] [--fb-alpha2 B]: the net also runs on every pair with its frames exchanged (run --backward's two
+forwards), and on the net's stream fn2_flow_fb_occlusion marks frame 0's pixels whose forward flow the backward flow does not
+undo (the forward-backward check of Sundaram, Brox and Keutzer, ECCV 2010; include/fn2_flow.h, alpha1 = A, 0.01, and
+alpha2 = B, 0.5).  fn2_flow_error_regions splits the EPE by that mask, and the summary gains, pooled over the list:
+  epe_fb_visible, epe_fb_flagged   EPE of the counted pixels the check keeps / flags (null when empty);
+  fb_visible_px, fb_flagged_px     their counts;
+and with --occlusions the mask is scored against the ground-truth masks by fn2_mask_confusion, "occluded" the positive class
+over all pixels: occ_tp, occ_fp, occ_fn, occ_precision, occ_recall, occ_f1 (null when undefined).  --per-pair gains the
+same columns.  Without the flag nothing of the output changes.
+
 --visualize DIR [--max-flow F]: for list line k (counting pairs from 0) DIR/<k, 6 digits>_pred.png and _gt.png, the
 prediction and the ground truth colour-coded on the net's stream (fn2_flow_to_color_png_rows) at one scale, so that they can be
 compared: F, else the ground truth's largest known flow (the prediction's when no ground-truth pixel is known).  The
@@ -58,13 +68,15 @@ import time
 
 import numpy as np
 
-from . import FLOW_ERROR_FIELDS, FLOW_REGION_FIELDS
+from . import FLOW_ERROR_FIELDS, FLOW_REGION_FIELDS, MASK_CONFUSION_FIELDS
 from .feed import _align, mask_offset
 from .files import RunError, attach_masks, probe, read_list
-from .run import STAGES, _run_size, check_inputs, check_max_flow, group_by_size, run_groups, shard
+from .run import STAGES, _run_size, check_fb_alphas, check_inputs, check_max_flow, group_by_size, run_groups, shard
 
 FIELD = {name: i for i, name in enumerate(FLOW_ERROR_FIELDS)}
 REGION = {name: i for i, name in enumerate(FLOW_REGION_FIELDS)}
+CONFUSION = {name: len(FLOW_REGION_FIELDS) + i for i, name in enumerate(MASK_CONFUSION_FIELDS)}     # in an --fb-check block
+FB_FIELDS = len(FLOW_REGION_FIELDS) + len(MASK_CONFUSION_FIELDS)
 BANDS = (("s0-10", "n_s0_10", "sum_s0_10"), ("s10-40", "n_s10_40", "sum_s10_40"), ("s40+", "n_s40", "sum_s40"))
 # the region scores each mask adds to the summary and the per-pair file: (key, region, pooled EPE or Fl %)
 REGION_KEYS = {"occlusions": (("epe_matched", "matched", "epe"), ("epe_unmatched", "unmatched", "epe"),
@@ -72,9 +84,10 @@ REGION_KEYS = {"occlusions": (("epe_matched", "matched", "epe"), ("epe_unmatched
                "objects": (("fl_bg", "bg", "fl"), ("fl_fg", "fg", "fl"), ("epe_bg", "bg", "epe"), ("epe_fg", "fg", "epe"))}
 
 
-def record_width(masks):
-    """Fields of a pair's record: FLOW_ERROR_FIELDS, then FLOW_REGION_FIELDS when the pairs carry masks."""
-    return len(FLOW_ERROR_FIELDS) + (len(FLOW_REGION_FIELDS) if masks else 0)
+def record_width(masks, fb=False):
+    """Fields of a pair's record: FLOW_ERROR_FIELDS, then FLOW_REGION_FIELDS when the pairs carry masks, then with fb (the
+    --fb-check block) FLOW_REGION_FIELDS split by the predicted mask and MASK_CONFUSION_FIELDS."""
+    return len(FLOW_ERROR_FIELDS) + (len(FLOW_REGION_FIELDS) if masks else 0) + (FB_FIELDS if fb else 0)
 
 
 class Scores(object):
@@ -89,38 +102,53 @@ class Scores(object):
 
     visualize: a directory; score() also colour-codes the prediction and the ground truth at one scale per pair (max_flow,
     else the ground truth's largest known flow, else the prediction's) into PNG scanlines behind the records, and take() writes
-    them as <visualize>/<sample.number, 6 digits>_pred.png and _gt.png."""
+    them as <visualize>/<sample.number, 6 digits>_pred.png and _gt.png.
 
-    def __init__(self, n, masks=(), visualize=None, max_flow=None):
-        self.masks = tuple(masks)
-        self.records = np.full((n, record_width(self.masks)), np.nan)
+    fb: (alpha1, alpha2) of the forward-backward check, or None.  With it _run_size also fills bwd_dev[s] with the flow of the
+    exchanged frames, and score() computes frame 0's occlusion mask (fn2_flow_fb_occlusion), splits the EPE by it
+    (fn2_flow_error_regions with the mask as the object map: BG visible, FG flagged) and, with occlusion masks, counts it
+    against them (fn2_mask_confusion); the records widen by FB_FIELDS (the confusion counts stay 0 without occlusions)."""
+
+    def __init__(self, n, masks=(), visualize=None, max_flow=None, fb=None):
+        self.masks, self.fb, self.backward = tuple(masks), fb, fb is not None
+        self.records = np.full((n, record_width(self.masks, self.backward)), np.nan)
         self.stats = {"collect": 0.0}
         self.visualize, self.max_flow = visualize, max_flow
 
     def item_bytes(self, H, W):
         return _align(mask_offset(H, W) + len(self.masks) * H * W)
 
-    def bind(self, torch, batch, H, W, flow_dev):
+    def bind(self, torch, batch, H, W, flow_dev, bwd_dev=None):
         from . import ops
         self.ops, self.batch = ops, batch
         nf, nr = len(FLOW_ERROR_FIELDS), record_width(self.masks) - len(FLOW_ERROR_FIELDS)
+        # each block of a pair's record: the fields of fn2_flow_error, fn2_flow_error_regions and, with fb, the regions split
+        # by the predicted mask and its confusion counts
+        self.widths = (nf, nr) + ((len(FLOW_REGION_FIELDS), len(MASK_CONFUSION_FIELDS)) if self.fb else ())
         self.pred = [f.permute(0, 3, 1, 2) for f in flow_dev]                       # (B, 2, H, W) views of the NHWC flow
         self.gt = [torch.empty((batch, 2, H, W), device="cuda") for _ in range(2)]
-        # each batch's records in one buffer: fn2_flow_error's (B, nf), then fn2_flow_error_regions' (B, nr), then with
-        # visualize the prediction's and the ground truth's colour scanlines
-        self.rec_bytes = batch * (nf + nr) * 8
+        # each batch's records in one buffer: per block of widths, its (B, width) fields; then with visualize the
+        # prediction's and the ground truth's colour scanlines
+        self.rec_bytes = batch * sum(self.widths) * 8
         self.size, self.vis_bytes = (W, H), H * (1 + 3 * W)
         nb = self.rec_bytes + (2 * batch * self.vis_bytes if self.visualize else 0)
         self.dev = [torch.empty(nb, dtype=torch.uint8, device="cuda") for _ in range(2)]
         self.host = [torch.empty(nb, dtype=torch.uint8).pin_memory() for _ in range(2)]
         rec = [d[:self.rec_bytes].view(torch.float64) for d in self.dev]
-        self.err = [r[:batch * nf].view(batch, nf) for r in rec]
-        self.reg = [r[batch * nf:].view(batch, nr) for r in rec]
+        self.blocks = [[b.view(batch, w) for b, w in zip(r.split([batch * w for w in self.widths]), self.widths)] for r in rec]
+        self.err = [b[0] for b in self.blocks]
+        self.reg = [b[1] for b in self.blocks]
+        if self.fb:
+            self.bwd = [b.permute(0, 3, 1, 2) for b in bwd_dev]
+            self.fbmask = [torch.empty((batch, H, W), dtype=torch.uint8, device="cuda") for _ in range(2)]
+            for b in self.blocks:
+                b[3].zero_()                                                        # the counts without occlusion masks
         if self.visualize:
             self.radius = [torch.empty((2, batch), device="cuda") for _ in range(2)]      # the ground truth's, the prediction's
         ws = ops.flow_error_workspace_bytes(batch, H, W)
-        if self.masks:
+        if self.masks or self.fb:
             ws = max(ws, ops.flow_error_regions_workspace_bytes(batch, H, W))
+        if self.masks:
             self.planes = [torch.empty((len(self.masks), batch, H, W), dtype=torch.uint8, device="cuda") for _ in range(2)]
             if "occlusions" in self.masks:
                 self.dist2 = [torch.empty((batch, H, W), dtype=torch.int32, device="cuda") for _ in range(2)]
@@ -149,6 +177,12 @@ class Scores(object):
             self.ops.flow_error_regions(self.pred[s], self.gt[s], occ=plane.get("occlusions"), obj=plane.get("objects"),
                                         dist2=self.dist2[s] if "occlusions" in plane else None, out=self.reg[s],
                                         workspace=self.workspace)
+        if self.fb:
+            fbreg, conf = self.blocks[s][2:]
+            self.ops.flow_fb_occlusion(self.pred[s], self.bwd[s], *self.fb, out=self.fbmask[s])
+            self.ops.flow_error_regions(self.pred[s], self.gt[s], obj=self.fbmask[s], out=fbreg, workspace=self.workspace)
+            if "occlusions" in self.masks:
+                self.ops.mask_confusion(self.fbmask[s], self.planes[s][self.masks.index("occlusions")], out=conf)
         if self.visualize:
             gt_r = pred_r = None
             if self.max_flow is None:
@@ -163,11 +197,10 @@ class Scores(object):
         t0 = time.perf_counter()
         raw = self.host[s].numpy()
         buf = raw[:self.rec_bytes].view(np.float64)
-        nf = len(FLOW_ERROR_FIELDS)
-        err = buf[:self.batch * nf].reshape(self.batch, nf)
-        reg = buf[self.batch * nf:].reshape(self.batch, -1)
+        ends = np.cumsum((0,) + self.widths) * self.batch
+        blocks = [buf[a:b].reshape(self.batch, -1) for a, b in zip(ends[:-1], ends[1:])]
         for i, p in enumerate(pairs[:n_real]):
-            self.records[p.index] = np.concatenate([err[i], reg[i]])
+            self.records[p.index] = np.concatenate([b[i] for b in blocks])
             if self.visualize:
                 from . import kitti
                 o, n, m = self.rec_bytes, self.batch * self.vis_bytes, self.vis_bytes
@@ -203,9 +236,28 @@ def region_scores(region, occlusions, objects):
             for key, r, what in region_keys(occlusions, objects)]
 
 
-def summarize(records, pixels, name, occlusions=False, objects=False):
+def fb_scores(block, occlusions):
+    """An --fb-check block (FB_FIELDS) summed over some pairs -> [(key, value)]: the EPE and counted pixels the check keeps
+    and flags and, with occlusions, the confusion counts against the ground-truth masks with precision, recall and F1
+    (None when undefined)."""
+    at = lambda f: block[REGION[f]]
+    out = [("epe_fb_visible", _ratio(at("sum_bg"), at("n_bg"))), ("epe_fb_flagged", _ratio(at("sum_fg"), at("n_fg"))),
+           ("fb_visible_px", int(at("n_bg"))), ("fb_flagged_px", int(at("n_fg")))]
+    if occlusions:
+        tp, fp, fn = (block[CONFUSION[f]] for f in ("tp", "fp", "fn"))
+        out += [("occ_tp", int(tp)), ("occ_fp", int(fp)), ("occ_fn", int(fn)), ("occ_precision", _ratio(tp, tp + fp)),
+                ("occ_recall", _ratio(tp, tp + fn)), ("occ_f1", _ratio(2 * tp, 2 * tp + fp + fn))]
+    return out
+
+
+def fb_keys(occlusions):
+    return [k for k, _ in fb_scores(np.zeros(FB_FIELDS), occlusions)]
+
+
+def summarize(records, pixels, name, occlusions=False, objects=False, fb=False):
     """The summary of per-pair records in list order ((n, FIELDS) float64, or FIELDS + REGION FIELDS with masks) and each
-    pair's pixel count -> dict; with occlusions / objects, the pooled region scores and pixel counts of those masks are added.
+    pair's pixel count -> dict; with occlusions / objects, the pooled region scores and pixel counts of those masks are added;
+    with fb (records ending in the --fb-check block), fb_scores of the block pooled over the list.
     Refuses a list with no valid pixel, naming it."""
     records = np.asarray(records, np.float64)
     col = lambda f: records[:, FIELD[f]]
@@ -226,11 +278,14 @@ def summarize(records, pixels, name, occlusions=False, objects=False):
         out.update(region_scores(region, occlusions, objects))
         for r in (("matched", "unmatched") if occlusions else ()) + (("bg", "fg") if objects else ()):
             out[r + "_px"] = int(region[REGION["n_" + r]])
+    if fb:
+        out.update(fb_scores(records[:, -FB_FIELDS:].sum(axis=0), occlusions))
     return out
 
 
-def pair_rows(records, occlusions=False, objects=False):
-    """-> per pair (valid pixels, EPE, Fl %) followed by its region scores of the masks given, NaN where no pixel counts."""
+def pair_rows(records, occlusions=False, objects=False, fb=False):
+    """-> per pair (valid pixels, EPE, Fl %) followed by its region scores of the masks given and with fb its fb_scores, NaN
+    where no pixel counts."""
     rows = []
     nan = lambda v: float("nan") if v is None else v
     for r in np.asarray(records, np.float64):
@@ -238,15 +293,17 @@ def pair_rows(records, occlusions=False, objects=False):
         epe = r[FIELD["epe_sum"]] / counted if counted > 0 else float("nan")
         fl = 100.0 * r[FIELD["outliers"]] / counted if counted > 0 else float("nan")
         regions = region_scores(r[len(FLOW_ERROR_FIELDS):], occlusions, objects) if occlusions or objects else []
+        regions += fb_scores(r[-FB_FIELDS:], occlusions) if fb else []
         rows.append((int(r[FIELD["valid"]]), epe, fl) + tuple(nan(v) for _, v in regions))
     return rows
 
 
-def write_per_pair(path, samples, records, occlusions=False, objects=False):
+def write_per_pair(path, samples, records, occlusions=False, objects=False, fb=False):
     extra = "".join("\t" + key for key, _, _ in region_keys(occlusions, objects))
+    extra += "".join("\t" + key for key in fb_keys(occlusions)) if fb else ""
     with open(path, "w") as f:
         f.write("where\timg0\timg1\tflow\tvalid\tepe\tfl_percent%s\n" % extra)
-        for s, (valid, epe, fl, *regions) in zip(samples, pair_rows(records, occlusions, objects)):
+        for s, (valid, epe, fl, *regions) in zip(samples, pair_rows(records, occlusions, objects, fb)):
             f.write("%s\t%s\t%s\t%s\t%d\t%.9g\t%.9g%s\n" % (s.where, s.img0, s.img1, s.flow, valid, epe, fl,
                                                           "".join("\t%.9g" % v for v in regions)))
 
@@ -266,10 +323,12 @@ def _mask_kinds(occlusions, objects):
     return tuple(k for k, _ in given), [l for _, l in given]
 
 
-def _score(caffemodel, template, samples, batch, device, threads, kitti=False, masks=(), visualize=None, max_flow=None):
+def _score(caffemodel, template, samples, batch, device, threads, kitti=False, masks=(), visualize=None, max_flow=None, fb=None):
     """-> (records in the samples' order, per-stage busy seconds, number of sizes).  masks: the kinds of the samples' masks.
-    visualize, max_flow: see Scores (each sample's number names its images)."""
+    visualize, max_flow, fb: see Scores (each sample's number names its images)."""
     t0 = time.perf_counter()
+    if fb is not None:
+        check_fb_alphas(*fb)
     check_inputs(caffemodel, template, batch)
     check_max_flow(max_flow)
     probe(samples, ground_truth=True, kitti=kitti)
@@ -277,7 +336,7 @@ def _score(caffemodel, template, samples, batch, device, threads, kitti=False, m
         s.index = i
     if visualize:
         os.makedirs(visualize, exist_ok=True)
-    sink = Scores(len(samples), masks, visualize, max_flow)
+    sink = Scores(len(samples), masks, visualize, max_flow, fb)
     stats, sizes = run_groups(caffemodel, template, samples, batch, device, threads, sink, t0)
     return sink.records, stats, sizes
 
@@ -289,19 +348,21 @@ def number(samples):
 
 
 def evaluate(caffemodel, template, samples, batch=1, device=0, threads=None, kitti=False, occlusions=None, objects=None,
-             visualize=None, max_flow=None):
+             visualize=None, max_flow=None, fb=None):
     """Scores the net on every files.Pair -> (summary dict, per-pair records): the summary of summarize() plus batch, sizes,
     wall (s), per-stage busy seconds and the samples whose prediction is not finite; the records are an (n, FIELDS) float64
     array in the samples' order (fields: flownet2_b200.FLOW_ERROR_FIELDS, then FLOW_REGION_FIELDS with a mask list).  kitti:
     the flows are KITTI PNGs.  occlusions, objects: mask lists (one path per sample, in order) of occlusion masks and object
     maps, either or both, for the region scores of summarize().  visualize: a directory for each pair's colour-coded
-    prediction and ground truth (Scores), at the fixed scale max_flow if given."""
+    prediction and ground truth (Scores), at the fixed scale max_flow if given.  fb: (alpha1, alpha2) of the forward-backward
+    check, which adds fb_scores to the summary and the --fb-check block to the records, or None."""
     t0 = time.perf_counter()
     masks, lists = _mask_kinds(occlusions, objects)
     attach_masks(samples, lists)
     number(samples)
-    records, stats, sizes = _score(caffemodel, template, samples, batch, device, threads, kitti, masks, visualize, max_flow)
-    summary = summarize(records, [s.size[0] * s.size[1] for s in samples], _list_name(samples), bool(occlusions), bool(objects))
+    records, stats, sizes = _score(caffemodel, template, samples, batch, device, threads, kitti, masks, visualize, max_flow, fb)
+    summary = summarize(records, [s.size[0] * s.size[1] for s in samples], _list_name(samples), bool(occlusions), bool(objects),
+                        fb is not None)
     summary.update({"batch": batch, "sizes": sizes, "wall": time.perf_counter() - t0, "busy": stats,
                     "not_finite": [s.where for s in not_finite(samples, records)]})
     return summary, records
@@ -441,6 +502,12 @@ def parse_args(argv):
                                                        "scale, as DIR/<list index>_pred.png and _gt.png")
     ap.add_argument("--max-flow", type=float, metavar="F", help="with --visualize: colour at this scale (pixels) instead of "
                                                                 "each ground truth's largest flow")
+    ap.add_argument("--fb-check", action="store_true", help="also run each pair backward and score the forward-backward "
+                                                            "occlusion mask (against --occlusions when given)")
+    ap.add_argument("--fb-alpha1", type=float, default=0.01, metavar="A", help="with --fb-check: the check's relative term "
+                                                                               "(default 0.01)")
+    ap.add_argument("--fb-alpha2", type=float, default=0.5, metavar="B", help="with --fb-check: the check's constant term, "
+                                                                              "in squared pixels (default 0.5)")
     return ap.parse_args(argv)
 
 
@@ -450,8 +517,10 @@ def main(argv=None):
     device = int(os.environ.get("LOCAL_RANK", a.gpu)) if "WORLD_SIZE" in os.environ else a.gpu
     t0 = time.perf_counter()
     dist = None
+    fb = (a.fb_alpha1, a.fb_alpha2) if a.fb_check else None
     try:
         check_max_flow(a.max_flow)
+        check_fb_alphas(a.fb_alpha1, a.fb_alpha2)
         check_inputs(a.caffemodel, a.deployproto, a.batch)
         samples = read_list(a.listfile)
         if not samples:
@@ -465,16 +534,16 @@ def main(argv=None):
             torch.cuda.set_device(device)
             dist.init_process_group("nccl")
         mine = shard(samples, world, rank)
-        local = np.empty((0, record_width(masks) + 1))                  # this rank's records, each pair's pixel count last
+        local = np.empty((0, record_width(masks, a.fb_check) + 1))      # this rank's records, each pair's pixel count last
         if mine:
             records = _score(a.caffemodel, a.deployproto, mine, a.batch, device, None, a.kitti, masks, a.visualize,
-                             a.max_flow)[0]
+                             a.max_flow, fb)[0]
             local = np.concatenate([records, [[s.size[0] * s.size[1]] for s in mine]], axis=1)
         full = gather_records(local, len(samples), world, rank) if world > 1 else local
         if rank != 0:
             return 1 if np.any(local[:, FIELD["nonfinite"]] > 0) else 0
         records, pixels = full[:, :-1], full[:, -1]
-        summary = summarize(records, pixels, a.listfile, bool(a.occlusions), bool(a.objects))
+        summary = summarize(records, pixels, a.listfile, bool(a.occlusions), bool(a.objects), a.fb_check)
     except RunError as e:
         sys.stderr.write("error: %s\n" % e)
         return 2
@@ -483,7 +552,7 @@ def main(argv=None):
             dist.destroy_process_group()
     summary.update({"batch": a.batch, "ranks": world, "wall": time.perf_counter() - t0})
     if a.per_pair:
-        write_per_pair(a.per_pair, samples, records, bool(a.occlusions), bool(a.objects))
+        write_per_pair(a.per_pair, samples, records, bool(a.occlusions), bool(a.objects), a.fb_check)
     bad = not_finite(samples, records)
     for s in bad:
         sys.stderr.write("%s: the flow of %s %s is not finite\n" % (s.where, s.img0, s.img1))

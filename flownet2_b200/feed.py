@@ -3,6 +3,7 @@
     feed = Feeder(net, batch, (W, H), item_bytes, items_of, slots)
     feed.seek(k)                  # the next call feeds batch k; reading starts for batches k .. k + slots - 1
     feed(stage)                   # enqueues the next batch on the net's stream and starts reading the one `slots` ahead
+    feed.swap()                   # with swap=True, after the first forward: the slot's frames again, the two inputs exchanged
     feed.busy(); feed.close()
     Feeder(None, batch, (W, H), item_bytes, items_of, slots)     # payloads only, on a stream of its own (flownet2_b200.viz)
 
@@ -13,14 +14,17 @@ channel count (batch_channels), and from a 16-byte boundary item i's flow payloa
 reads every part of a batch into its host slot: a PNM frame with K channels as stored, any other frame decoded (a mask as one
 channel), a payload through files.read_flow_into.  A call waits for the batch's reads, copies the slot to the
 device on a copy stream, and on the net's stream waits for that copy, converts the frames into the net's first two inputs
-(fn2_net_set_input_frames_device), runs stage(payload, item_bytes) on the device payload and records the slot free.  Without
-a net (net None) a slot holds the payloads alone, from offset 0, and stage() runs on a stream of the feeder's own.
+(fn2_net_set_input_frames_device), runs stage(payload, item_bytes) on the device payload and records the slot free.  A
+feeder built with swap=True (run --backward, evaluate --fb-check) leaves the slot in use after the call: swap(), once the
+first forward has been enqueued, converts the same frames into the two inputs exchanged (img1 first) and only then records
+the slot free.  Without a net (net None) a slot holds the payloads alone, from offset 0, and stage() runs on a stream of the
+feeder's own.
 
 Three orderings keep a slot from being overwritten while in use:
   * a reader writes host slot s only after the copy out of s from S batches ago has finished; it waits for that copy itself,
     so the caller's thread never synchronises with the device;
   * the copy into device slot s waits until the net's stream has converted s from S batches ago;
-  * slot s is recorded free only after its frames and stage() have been enqueued.
+  * slot s is recorded free only after its frames and stage() have been enqueued (with swap, after swap()'s conversion).
 """
 import os
 import time
@@ -62,9 +66,9 @@ def read_part(p, j, size, k, out):
 
 
 class Feeder(object):
-    def __init__(self, net, batch, size, item_bytes, items_of, slots, threads=None):
+    def __init__(self, net, batch, size, item_bytes, items_of, slots, threads=None, swap=False):
         import torch
-        self.torch, self.net = torch, net
+        self.torch, self.net, self.swap_inputs, self._held = torch, net, swap, None
         self.batch, self.size, self.item_bytes, self.items_of, self.slots = batch, size, item_bytes, items_of, slots
         self.frame_bytes = batch * size[0] * size[1] if net is not None else 0    # of one input at K = 1
         self.payload_off = _align(2 * self.frame_bytes * 4)             # after both inputs' frames, K <= 4
@@ -118,6 +122,7 @@ class Feeder(object):
         """Enqueues the next batch on the net's stream: its frames into the net's first two inputs, then stage(payload,
         item_bytes) with the device payload (a uint8 tensor) and the net's stream current."""
         torch = self.torch
+        assert self._held is None, "swap() was not called for the last batch"
         k = self.next
         s = k % self.slots
         K, futs = self._reads.pop(k)
@@ -147,11 +152,26 @@ class Feeder(object):
             with torch.cuda.stream(ns):
                 stage(self._dev[s][off:], self.item_bytes)
         ev[4].record(ns)
-        self._ev_free[s].record(ns)
+        if self.swap_inputs:
+            self._held = (s, K)                                        # swap() converts dev[s] again, then frees it
+        else:
+            self._ev_free[s].record(ns)
         self._timing.append(ev)
         self._harvest(block=False)
         self.next = k + 1
         self._submit(k + self.slots)                                   # reads into pin[s] once its copy is done
+
+    def swap(self):
+        """Enqueues the last batch's frames again on the net's stream, into the net's first two inputs exchanged (img1 into the
+        first), then records its slot free.  For a feeder built with swap=True, once per call, after that batch's first
+        forward."""
+        s, K = self._held
+        n = 2 * self.frame_bytes * K
+        base, inputs = self._dev[s].data_ptr(), self.net.inputs[:2]
+        self.net.set_input_image_device(inputs[0], base + n // 2, K)
+        self.net.set_input_image_device(inputs[1], base, K)
+        self._ev_free[s].record(self.stream)
+        self._held = None
 
     def _harvest(self, block):
         while self._timing and (block or self._timing[0][4].query()):

@@ -5,6 +5,7 @@ predictions.  This module is the only place that knows the container; the value 
     read_payload(path, info, out)           # inflate + unfilter into `out`: [H][W][3] big-endian uint16, the file's own bytes
     write_png_rows(path, rows, w, h)        # scanlines already filtered (fn2_flow_to_kitti_png_rows) -> a PNG file
     write_png_rows(path, rows, w, h, 8)     # the same for 8-bit RGB (fn2_flow_to_color_png_rows, flownet2_b200.viz)
+    write_png_rows(path, rows, w, h, 8, 1)  # 8-bit grey (fn2_flow_fb_occlusion's masks, run --backward)
     read_kitti_flow(path) / write_kitti_flow(path, flow_hw2)     # host helpers in numpy, float32 (H, W, 2) with NaN = invalid
 
 The host only undoes (or makes) the PNG container: the chunks, zlib's deflate and the per-row filters.  The conversion
@@ -119,19 +120,20 @@ def _chunk(kind, body):
     return struct.pack(">I", len(body)) + kind + body + struct.pack(">I", zlib.crc32(body, zlib.crc32(kind)))
 
 
-def png_bytes(rows, w, h, depth=16):
-    """An RGB PNG (colour type 2) of bit depth 16 (a KITTI flow) or 8 (a colour-coded flow, flownet2_b200.viz) from h filtered
-    scanlines of 1 + 3 (depth / 8) w bytes: IHDR, one IDAT deflated at level 6, IEND."""
-    assert depth in (8, 16), depth
+def png_bytes(rows, w, h, depth=16, channels=3):
+    """An RGB PNG (colour type 2) of bit depth 16 (a KITTI flow) or 8 (a colour-coded flow, flownet2_b200.viz), or with
+    channels 1 an 8-bit grey one (colour type 0, an occlusion mask), from h filtered scanlines of 1 + channels (depth / 8) w
+    bytes: IHDR, one IDAT deflated at level 6, IEND."""
+    assert (depth, channels) in ((8, 3), (16, 3), (8, 1)), (depth, channels)
     rows = memoryview(rows).cast("B")
-    assert len(rows) == h * (1 + 3 * depth // 8 * w), (len(rows), w, h, depth)
-    return (SIGNATURE + _chunk(b"IHDR", struct.pack(">IIBBBBB", w, h, depth, 2, 0, 0, 0))
+    assert len(rows) == h * (1 + channels * depth // 8 * w), (len(rows), w, h, depth, channels)
+    return (SIGNATURE + _chunk(b"IHDR", struct.pack(">IIBBBBB", w, h, depth, 2 if channels == 3 else 0, 0, 0, 0))
             + _chunk(b"IDAT", zlib.compress(rows, LEVEL)) + _chunk(b"IEND", b""))
 
 
-def write_png_rows(path, rows, w, h, depth=16):
+def write_png_rows(path, rows, w, h, depth=16, channels=3):
     with open(path, "wb") as f:
-        f.write(png_bytes(rows, w, h, depth))
+        f.write(png_bytes(rows, w, h, depth, channels))
     return str(path)
 
 

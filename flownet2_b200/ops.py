@@ -10,7 +10,7 @@ import ctypes as C
 
 import torch
 
-from . import FLOW_ERROR_FIELDS, FLOW_REGION_FIELDS, LPQLOSS_STATE_FLOATS, check, fn2_conv_desc, fn2_l1loss_desc, fn2_lpqloss_desc, fn2_tensor, lib
+from . import FLOW_ERROR_FIELDS, FLOW_REGION_FIELDS, LPQLOSS_STATE_FLOATS, MASK_CONFUSION_FIELDS, check, fn2_conv_desc, fn2_l1loss_desc, fn2_lpqloss_desc, fn2_tensor, lib
 
 
 def desc(t):
@@ -493,6 +493,35 @@ def flow_to_color_png_rows(flow, out=None, max_flow=None, max_radius=None, fallb
     assert out.is_cuda and out.dtype == torch.uint8 and out.is_contiguous() and out.numel() >= N * H * (1 + 3 * W)
     m, fb, mf = _colour_scale(flow, max_flow, max_radius, fallback)
     check(lib().fn2_flow_to_color_png_rows(desc(flow), m, fb, mf, out.data_ptr(), _stream()))
+    return out
+
+
+def flow_fb_occlusion(fwd, bwd, alpha1=0.01, alpha2=0.5, out=None, row_stride=None, pair_stride=None):
+    """Frame 0's occlusion mask by the forward-backward check (include/fn2_flow.h): fwd and bwd are float32 (N, 2, H, W) CUDA
+    views of any strides -> out, a uint8 CUDA tensor (a new dense (N, H, W) one if None), 255 where occluded and 0 where
+    visible.  With row_stride / pair_stride, pixel (n, y, x) goes to byte n * pair_stride + y * row_stride + x of out (a dense
+    uint8 buffer), and no other byte is written."""
+    N, _, H, W = fwd.shape
+    if out is None:
+        out = torch.empty((N, H, W), dtype=torch.uint8, device=fwd.device)
+    rs = W if row_stride is None else row_stride
+    ps = H * rs if pair_stride is None else pair_stride
+    assert out.is_cuda and out.dtype == torch.uint8 and out.is_contiguous() and out.numel() >= (N - 1) * ps + (H - 1) * rs + W
+    check(lib().fn2_flow_fb_occlusion(desc(fwd), desc(bwd), float(alpha1), float(alpha2), out.data_ptr(), rs, ps, _stream()))
+    return out
+
+
+def mask_confusion(pred, gt, out=None):
+    """Per-pair confusion counts of predicted against ground-truth occlusion masks (include/fn2_eval.h): pred and gt are dense
+    uint8 (N, H, W) CUDA tensors, nonzero meaning occluded -> out, an (N, len(MASK_CONFUSION_FIELDS)) float64 CUDA tensor (a
+    new one if None) with the fields of MASK_CONFUSION_FIELDS (tp, fp, fn, tn)."""
+    N, H, W = pred.shape
+    assert tuple(gt.shape) == (N, H, W), (tuple(pred.shape), tuple(gt.shape))
+    if out is None:
+        out = torch.empty((N, len(MASK_CONFUSION_FIELDS)), dtype=torch.float64, device=pred.device)
+    assert out.is_cuda and out.dtype == torch.float64 and out.is_contiguous() and out.numel() == N * len(MASK_CONFUSION_FIELDS)
+    check(lib().fn2_mask_confusion(_planes(pred, N, H, W, H * W), _planes(gt, N, H, W, H * W), H * W, N, H, W,
+                                   C.cast(out.data_ptr(), C.POINTER(C.c_double)), _stream()))
     return out
 
 

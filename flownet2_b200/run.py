@@ -2,7 +2,7 @@
 
     python -m flownet2_b200.run weights.caffemodel models/FlowNet2_deploy.prototxt.template img0.png img1.png out.flo
     python -m flownet2_b200.run weights.caffemodel models/FlowNet2_deploy.prototxt.template pairs.txt [--batch 4] [--kitti]
-                                [--visualize [--max-flow F]]
+                                [--visualize [--max-flow F]] [--backward [--fb-alpha1 A] [--fb-alpha2 B]]
 
 The list file holds one ``img0 img1 out.flo`` line per pair; blank lines are skipped.  The weights (.caffemodel or
 .caffemodel.h5) are read once.  Pairs are grouped by frame size in order of first appearance, and each size gets one
@@ -21,6 +21,17 @@ is copied back on another stream and written by a writer thread.
 back in the same copy as the flow and deflated by the writer thread (flownet2_b200.viz).  It shows the net's float prediction,
 also under --kitti; a pixel whose flow is not finite is black.  A list in which two outputs map to one .vis.png, or a
 .vis.png is another line's output, is refused.
+
+--backward also runs the net on every pair with its frames exchanged, at the same batch on the same net (the feeder converts
+each batch's frames a second time, flownet2_b200.feed), and writes two more files beside each output:
+<output without its extension>.bwd<extension>, the backward flow in the output's format, and <output without its
+extension>.occ.png, frame 0's occlusion mask as an 8-bit grey PNG (255 occluded, 0 visible; Sintel's convention).  The mask
+is the forward-backward consistency check of Sundaram, Brox and Keutzer (ECCV 2010) on the two flows, computed on the net's
+stream (fn2_flow_fb_occlusion, include/fn2_flow.h, which states the arithmetic), with alpha1 = --fb-alpha1 (0.01) and
+alpha2 = --fb-alpha2 (0.5).  Its scanlines come back in the batch's one copy with the flows and the writer thread deflates
+them.  The forward outputs are the files run writes without the flag, and each .bwd file is the output run writes for the
+pair with its frames exchanged, bit for bit at the same --batch.  Every derived path (.vis.png, .bwd, .occ.png) is checked
+against every output and every other derived path before a net is built.
 
 --kitti writes every output as a KITTI flow PNG (flownet2_b200.kitti, the format the KITTI benchmark takes) instead of a
 .flo: the flow becomes Paeth-filtered PNG scanlines on the net's stream (fn2_flow_to_kitti_png_rows, 6 bytes a pixel instead
@@ -93,30 +104,67 @@ class FlowFiles(object):
     on the copy-back stream, and take(pairs, s, n_real) consumes host[s] on the writer thread.
 
     visualize: each batch's flow is also colour-coded into PNG scanlines at the end of dev[s] (fn2_flow_to_color_png_rows, at
-    the fixed scale max_flow, else at each pair's own largest radius), and take() writes each pair's vis_path(flow)."""
+    the fixed scale max_flow, else at each pair's own largest radius), and take() writes each pair's vis_path(flow).
 
-    def __init__(self, visualize=False, max_flow=None):
+    backward (alphas: alpha1, alpha2): _run_size also fills bwd_dev[s] with the flow of the exchanged frames; score() turns the
+    two flows into frame 0's occlusion mask as 8-bit grey PNG scanlines in dev[s] (fn2_flow_fb_occlusion), and take() writes
+    each pair's bwd_path(flow) and occ_path(flow)."""
+
+    def __init__(self, visualize=False, max_flow=None, backward=False, alphas=(0.01, 0.5)):
         self.bad = []
         self.stats = {"write": 0.0}
         self.visualize, self.max_flow = visualize, max_flow
+        self.backward, self.alphas = backward, alphas
 
     def item_bytes(self, H, W):
         return 0
 
     stage = None
 
-    def bind(self, torch, batch, H, W, flow_dev):
-        if not self.visualize:
+    def bind(self, torch, batch, H, W, flow_dev, bwd_dev=None):
+        if not (self.visualize or self.backward):
             self.dev = flow_dev
             self.host = [torch.empty((batch, H, W, 2)).pin_memory() for _ in range(2)]
             return
-        self.flow_bytes = batch * H * W * 8
-        nb = self._bind_vis(torch, batch, H, W, flow_dev, self.flow_bytes)
+        self.flow_bytes = batch * H * W * 8                               # the flow, then with backward the backward flow
+        nb = self.flow_bytes * (2 if self.backward else 1)
+        if self.backward:
+            nb = self._bind_occ(batch, H, W, nb)
+        if self.visualize:
+            nb = self._bind_vis(torch, batch, H, W, flow_dev, nb)
         self.dev = [torch.empty(nb, dtype=torch.uint8, device="cuda") for _ in range(2)]
         self.host = [torch.empty(nb, dtype=torch.uint8).pin_memory() for _ in range(2)]
-        for s in range(2):                                                # the net writes its flow straight into dev[s]
-            flow_dev[s] = self.dev[s][:self.flow_bytes].view(torch.float32).view(batch, H, W, 2)
-            self.pred[s] = flow_dev[s].permute(0, 3, 1, 2)
+        flows = lambda s, k: self.dev[s][k * self.flow_bytes:(k + 1) * self.flow_bytes].view(torch.float32).view(batch, H, W, 2)
+        for s in range(2):                                                # the net writes its flows straight into dev[s]
+            flow_dev[s] = flows(s, 0)
+            if self.backward:
+                bwd_dev[s] = flows(s, 1)
+        self.pred = [f.permute(0, 3, 1, 2) for f in flow_dev]
+        if self.backward:
+            self._zero_occ(bwd_dev)
+
+    def _bind_occ(self, batch, H, W, offset):
+        """The mask rows' place in dev[s], from `offset` on -> the offset after them."""
+        from . import ops
+        self.ops, self.size, self.occ_off, self.occ_bytes = ops, (W, H), offset, H * (1 + W)
+        return offset + batch * self.occ_bytes
+
+    def _zero_occ(self, bwd_dev):
+        """Zeroes the mask rows of both dev[s] once: the check writes each row from byte 1 on, so every filter byte stays 0
+        (None)."""
+        self.bwd = [b.permute(0, 3, 1, 2) for b in bwd_dev]               # (B, 2, H, W) views of the NHWC backward flow
+        for d in self.dev:
+            d[self.occ_off:self.occ_off + len(bwd_dev[0]) * self.occ_bytes].zero_()
+
+    def _score_occ(self, s):
+        W, H = self.size
+        self.ops.flow_fb_occlusion(self.pred[s], self.bwd[s], *self.alphas, out=self.dev[s][self.occ_off + 1:],
+                                   row_stride=1 + W, pair_stride=self.occ_bytes)
+
+    def _take_occ(self, buf, i, p):
+        from . import kitti
+        n, o = self.occ_bytes, self.occ_off
+        kitti.write_png_rows(occ_path(p.flow), buf[o + i * n:o + (i + 1) * n], *self.size, 8, 1)
 
     def _bind_vis(self, torch, batch, H, W, flow_dev, offset):
         """The colour rows' place in dev[s], from `offset` on -> dev[s]'s size."""
@@ -137,21 +185,27 @@ class FlowFiles(object):
         kitti.write_png_rows(vis_path(p.flow), buf[o + i * n:o + (i + 1) * n], *self.size, 8)
 
     def score(self, s):
+        if self.backward:
+            self._score_occ(s)
         if self.visualize:
             self._score_vis(s)
 
     def take(self, pairs, s, n_real):
         t0 = time.perf_counter()
         buf = self.host[s].numpy()
-        if self.visualize:
-            flows = buf[:self.flow_bytes].view(np.float32).reshape(len(pairs), self.size[1], self.size[0], 2)
+        if self.visualize or self.backward:
+            flows = buf[:self.flow_bytes * (2 if self.backward else 1)].view(np.float32).reshape(-1, len(pairs), self.size[1],
+                                                                                                  self.size[0], 2)
         else:
-            flows = buf
+            flows = buf[None]
         for i, p in enumerate(pairs[:n_real]):
-            if not np.isfinite(flows[i]).all():
+            if not np.isfinite(flows[0, i]).all():
                 self.bad.append(p)
                 sys.stderr.write("%s: the flow of %s %s is not finite\n" % (p.where, p.img0, p.img1))
-            write_flo(p.flow, flows[i])
+            write_flo(p.flow, flows[0, i])
+            if self.backward:
+                write_flo(bwd_path(p.flow), flows[1, i])
+                self._take_occ(buf, i, p)
             if self.visualize:
                 self._take_vis(buf, i, p)
         self.stats["write"] += time.perf_counter() - t0
@@ -160,19 +214,24 @@ class FlowFiles(object):
 class KittiFiles(FlowFiles):
     """run --kitti's sink: on the net's stream each batch's flow becomes KITTI PNG scanlines (fn2_flow_to_kitti_png_rows) and
     fn2_flow_error against a zero flow counts each pair's non-finite pixels; both come back in one copy, and the writer
-    thread deflates each pair's rows into its file.  A pair with a non-finite pixel is named on stderr and kept in `bad`."""
+    thread deflates each pair's rows into its file.  A pair with a non-finite pixel is named on stderr and kept in `bad`.
+    With backward the backward flow's scanlines follow the flow's, and the mask rows the records."""
 
-    def bind(self, torch, batch, H, W, flow_dev):
+    def bind(self, torch, batch, H, W, flow_dev, bwd_dev=None):
         from . import FLOW_ERROR_FIELDS, kitti, ops
         self.ops, self.kitti, self.size = ops, kitti, (W, H)
         self.nonfinite, fields = FLOW_ERROR_FIELDS.index("nonfinite"), len(FLOW_ERROR_FIELDS)
         self.row_bytes = H * (1 + kitti.BPP * W)                          # one pair's scanlines
-        self.rec_off = _align(batch * self.row_bytes, 8)                  # then the pairs' float64 records
+        self.rec_off = _align(batch * self.row_bytes * (2 if self.backward else 1), 8)   # then the pairs' float64 records
         nb = self.rec_off + batch * fields * 8
+        if self.backward:                                                 # then the mask rows
+            nb = self._bind_occ(batch, H, W, nb)
         if self.visualize:                                                # then the colour rows
             nb = self._bind_vis(torch, batch, H, W, flow_dev, nb)
         self.pred = [f.permute(0, 3, 1, 2) for f in flow_dev]             # (B, 2, H, W) views of the NHWC flow
         self.dev = [torch.empty(nb, dtype=torch.uint8, device="cuda") for _ in range(2)]
+        if self.backward:
+            self._zero_occ(bwd_dev)
         self.host = [torch.empty(nb, dtype=torch.uint8).pin_memory() for _ in range(2)]
         self.records = [d[self.rec_off:self.rec_off + batch * fields * 8].view(torch.float64).view(batch, fields)
                         for d in self.dev]
@@ -182,6 +241,10 @@ class KittiFiles(FlowFiles):
     def score(self, s):
         self.ops.flow_to_kitti_png_rows(self.pred[s], self.dev[s])
         self.ops.flow_error(self.pred[s], self.zero, out=self.records[s], workspace=self.workspace)
+        if self.backward:
+            B = len(self.zero)
+            self.ops.flow_to_kitti_png_rows(self.bwd[s], self.dev[s][B * self.row_bytes:2 * B * self.row_bytes])
+            self._score_occ(s)
         if self.visualize:
             self._score_vis(s)
 
@@ -195,6 +258,10 @@ class KittiFiles(FlowFiles):
                 self.bad.append(p)
                 sys.stderr.write("%s: the flow of %s %s is not finite\n" % (p.where, p.img0, p.img1))
             self.kitti.write_png_rows(p.flow, buf[i * n:(i + 1) * n], *self.size)
+            if self.backward:
+                b = len(pairs) * n
+                self.kitti.write_png_rows(bwd_path(p.flow), buf[b + i * n:b + (i + 1) * n], *self.size)
+                self._take_occ(buf, i, p)
             if self.visualize:
                 self._take_vis(buf, i, p)
         self.stats["write"] += time.perf_counter() - t0
@@ -205,19 +272,50 @@ def vis_path(out):
     return os.path.splitext(out)[0] + ".vis.png"
 
 
-def check_vis_paths(pairs):
-    """Refuses a list in which two different outputs have one vis_path, or a vis_path is an output, naming the lines."""
+def bwd_path(out):
+    """The backward flow run --backward writes beside the output `out`: out without its extension, .bwd, then the extension."""
+    root, ext = os.path.splitext(out)
+    return root + ".bwd" + ext
+
+
+def occ_path(out):
+    """Frame 0's occlusion mask run --backward writes beside the output `out`: out without its extension, then .occ.png."""
+    return os.path.splitext(out)[0] + ".occ.png"
+
+
+# what each derived path is, in the refusals of check_vis_paths
+DERIVED = {vis_path: ("visualisation", "visualise to"), bwd_path: ("backward flow", "have the backward flow"),
+           occ_path: ("occlusion mask", "have the occlusion mask")}
+
+
+def check_vis_paths(pairs, derived=(vis_path,)):
+    """Refuses a list in which two different outputs have one derived path (each function of `derived` maps an output to one
+    of the files written beside it), or a derived path is an output, naming the lines."""
     outs = {os.path.normpath(p.flow): p for p in pairs}
     seen = {}
     for p in pairs:
-        v, out = os.path.normpath(vis_path(p.flow)), os.path.normpath(p.flow)
-        if v in seen and os.path.normpath(seen[v].flow) != out:
-            raise RunError("%s: the outputs %s and %s (%s) both visualise to %s" % (p.where, p.flow, seen[v].flow, seen[v].where,
-                                                                                  vis_path(p.flow)))
-        if v in outs:
-            raise RunError("%s: the visualisation %s of %s is the output of %s" % (p.where, vis_path(p.flow), p.flow,
-                                                                                 outs[v].where))
-        seen[v] = p
+        out = os.path.normpath(p.flow)
+        for f in derived:
+            what, verb = DERIVED[f]
+            v = os.path.normpath(f(p.flow))
+            if v in seen and os.path.normpath(seen[v].flow) != out:
+                raise RunError("%s: the outputs %s and %s (%s) both %s %s" % (p.where, p.flow, seen[v].flow, seen[v].where, verb,
+                                                                          f(p.flow)))
+            if v in outs:
+                raise RunError("%s: the %s %s of %s is the output of %s" % (p.where, what, f(p.flow), p.flow, outs[v].where))
+            seen[v] = p
+
+
+def derived_paths(visualize, backward):
+    """The functions of the files run writes beside each output, for check_vis_paths."""
+    return ((vis_path,) if visualize else ()) + ((bwd_path, occ_path) if backward else ())
+
+
+def check_fb_alphas(alpha1, alpha2):
+    """Refuses forward-backward thresholds that are negative or not finite."""
+    for name, a in (("--fb-alpha1", alpha1), ("--fb-alpha2", alpha2)):
+        if not (np.isfinite(a) and a >= 0):
+            raise RunError("%s must be a finite non-negative number, got %r" % (name, a))
 
 
 def check_max_flow(max_flow):
@@ -230,9 +328,12 @@ def _run_size(torch, net, size, pairs, batch, threads, stats, sink):
     """Runs one size's pairs through `net`, B per forward, with reads, copies, forward and the sink's work overlapped."""
     W, H = size
     todo = batches(pairs, batch)
+    both = sink.backward                                           # also the flow of the exchanged frames, into bwd_dev[s]
     flow_dev = [torch.empty((batch, H, W, 2), device="cuda") for _ in range(2)]
-    sink.bind(torch, batch, H, W, flow_dev)
-    feed = Feeder(net, batch, size, sink.item_bytes(H, W), lambda k: todo[k][0] if k < len(todo) else None, 2, threads)
+    bwd_dev = [torch.empty((batch, H, W, 2), device="cuda") for _ in range(2)] if both else None
+    sink.bind(torch, batch, H, W, flow_dev, bwd_dev)
+    feed = Feeder(net, batch, size, sink.item_bytes(H, W), lambda k: todo[k][0] if k < len(todo) else None, 2, threads,
+                  swap=both)
     net_stream, d2h_stream = feed.stream, torch.cuda.Stream()
     ev = lambda: torch.cuda.Event(enable_timing=True)
     ev_flow = [torch.cuda.Event() for _ in range(2)]               # sink.dev[s] holds the batch's result
@@ -256,6 +357,10 @@ def _run_size(torch, net, size, pairs, batch, threads, stats, sink):
                     net.forward_async()
                     net_stream.wait_event(ev_d2h[s])               # sink.dev[s] has left for the host two batches ago
                     net.get_blob_nhwc_device("predict_flow_final", flow_dev[s].data_ptr())
+                    if both:
+                        feed.swap()                                # the same frames, img1 first; frees the feeder's slot
+                        net.forward_async()
+                        net.get_blob_nhwc_device("predict_flow_final", bwd_dev[s].data_ptr())
                     sink.score(s)
                     t[1].record(net_stream)
                     ev_flow[s].record(net_stream)
@@ -325,18 +430,22 @@ def run_groups(caffemodel, template, pairs, batch, device, threads, sink, t0):
     return stats, len(groups)
 
 
-def run(caffemodel, template, pairs, batch=1, device=0, threads=None, kitti=False, visualize=False, max_flow=None):
+def run(caffemodel, template, pairs, batch=1, device=0, threads=None, kitti=False, visualize=False, max_flow=None,
+        backward=False, fb_alpha1=0.01, fb_alpha2=0.5):
     """Flow of every files.Pair into its flow file, a .flo (kitti: a KITTI flow PNG) -> summary dict: pairs, sizes, nets, wall (s),
     per-stage busy seconds (build: checking the inputs, reading the weights and constructing the nets; decode: host, summed
     over the pool's threads; h2d / forward / d2h: device; write: host) and the pairs whose flow is not finite.  visualize:
-    also each flow colour-coded into vis_path(flow), at the fixed scale max_flow if given."""
+    also each flow colour-coded into vis_path(flow), at the fixed scale max_flow if given.  backward: also the flow of the
+    exchanged frames into bwd_path(flow) and frame 0's forward-backward occlusion mask (thresholds fb_alpha1, fb_alpha2)
+    into occ_path(flow)."""
     t0 = time.perf_counter()
+    check_fb_alphas(fb_alpha1, fb_alpha2)
     check_inputs(caffemodel, template, batch)
     check_max_flow(max_flow)
     probe(pairs)
-    if visualize:
-        check_vis_paths(pairs)
-    sink = (KittiFiles if kitti else FlowFiles)(visualize, max_flow)
+    if visualize or backward:
+        check_vis_paths(pairs, derived_paths(visualize, backward))
+    sink = (KittiFiles if kitti else FlowFiles)(visualize, max_flow, backward, (fb_alpha1, fb_alpha2))
     stats, sizes = run_groups(caffemodel, template, pairs, batch, device, threads, sink, t0)
     return {"pairs": len(pairs), "sizes": sizes, "nets": sizes, "batch": batch, "wall": time.perf_counter() - t0,
             "busy": stats, "not_finite": [p.where for p in sink.bad]}
@@ -355,6 +464,12 @@ def parse_args(argv):
     ap.add_argument("--visualize", action="store_true", help="also write each flow colour-coded, as <output>.vis.png")
     ap.add_argument("--max-flow", type=float, metavar="F", help="with --visualize: colour every flow at this scale (pixels) "
                                                                 "instead of each pair's largest flow")
+    ap.add_argument("--backward", action="store_true", help="also write the backward flow, as <output>.bwd<ext>, and frame 0's "
+                                                            "forward-backward occlusion mask, as <output>.occ.png")
+    ap.add_argument("--fb-alpha1", type=float, default=0.01, metavar="A", help="with --backward: the check's relative term "
+                                                                               "(default 0.01)")
+    ap.add_argument("--fb-alpha2", type=float, default=0.5, metavar="B", help="with --backward: the check's constant term, in "
+                                                                              "squared pixels (default 0.5)")
     a = ap.parse_args(argv)
     if len(a.files) not in (1, 3):
         ap.error("expected img0 img1 out, or one list file; got %d paths" % len(a.files))
@@ -367,11 +482,13 @@ def main(argv=None):
     device = int(os.environ.get("LOCAL_RANK", a.gpu)) if "WORLD_SIZE" in os.environ else a.gpu
     try:
         check_max_flow(a.max_flow)
+        check_fb_alphas(a.fb_alpha1, a.fb_alpha2)
         pairs = read_list(a.files[0], ground_truth=False) if len(a.files) == 1 else [Pair("command line", *a.files)]
-        if a.visualize:
-            check_vis_paths(pairs)                                 # the whole list: ranks must not collide either
+        if a.visualize or a.backward:
+            check_vis_paths(pairs, derived_paths(a.visualize, a.backward))     # the whole list: ranks must not collide either
         s = run(a.caffemodel, a.deployproto, shard(pairs, world, rank), batch=a.batch, device=device, kitti=a.kitti,
-                visualize=a.visualize, max_flow=a.max_flow)
+                visualize=a.visualize, max_flow=a.max_flow, backward=a.backward, fb_alpha1=a.fb_alpha1,
+                fb_alpha2=a.fb_alpha2)
     except RunError as e:
         sys.stderr.write("error: %s\n" % e)
         return 2

@@ -54,6 +54,14 @@
  * fn2_occlusion_boundary_dist2 writes it) is required when occ_dev is given and refused when it is not.  Both masks are
  * read at mask_pair_stride.  The reduction, its bit-identical records and the workspace convention are fn2_flow_error's,
  * with its own size query.
+ *
+ * fn2_mask_confusion(pred_dev, gt_dev, pair_stride, N, H, W, out_dev, stream) -- a predicted occlusion mask (fn2_flow_fb_occlusion,
+ * include/fn2_flow.h) against a ground-truth one, both 8-bit planes read as above (nonzero: occluded, the positive class), at
+ * pair_stride.  out_dev: N x FN2_MASK_CONFUSION_FIELDS device doubles, 8-byte aligned, per pair the pixels that are TP
+ * (occluded in both), FP (pred only), FN (gt only) and TN (neither), TP + FP + FN + TN = H * W.  Counted in integers and
+ * stored as doubles (exact below 2^53), so equal inputs give bit-identical records; no workspace.  The EPE split by the
+ * predicted mask is fn2_flow_error_regions with that mask as obj_dev (BG: visible, FG: occluded).  FN2_ERR_INVALID for N
+ * above 65535, H * W above 2^30, pair_stride < H * W or a misaligned out_dev.
  */
 #ifndef FN2_EVAL_H_
 #define FN2_EVAL_H_
@@ -95,6 +103,12 @@
 #define FN2_FLOW_REGION_SUM_FG 19
 #define FN2_FLOW_REGION_OUT_FG 20
 
+#define FN2_MASK_CONFUSION_FIELDS 4
+#define FN2_MASK_CONFUSION_TP 0
+#define FN2_MASK_CONFUSION_FP 1
+#define FN2_MASK_CONFUSION_FN 2
+#define FN2_MASK_CONFUSION_TN 3
+
 /* dist2 of every pixel of a pair without an occlusion boundary: INT32_MAX */
 #define FN2_DIST2_NONE 2147483647
 
@@ -111,6 +125,8 @@ FN2_API int fn2_flow_error_regions_workspace_bytes(int N, int H, int W, size_t* 
 FN2_API int fn2_flow_error_regions(const fn2_tensor* pred, const fn2_tensor* gt, const void* occ_dev, const void* obj_dev,
                                    size_t mask_pair_stride, const int32_t* dist2_dev, double* out_dev, void* workspace,
                                    size_t workspace_bytes, void* stream);
+FN2_API int fn2_mask_confusion(const void* pred_dev, const void* gt_dev, size_t pair_stride, int N, int H, int W, double* out_dev,
+                               void* stream);
 
 /* Scoring a training net's weights with a deploy net (the train command's --val) needs the two to fit: every layer the
  * training net trains has a namesake in the deploy net with the same blob shapes, and every deploy layer with parameters gets

@@ -2,7 +2,8 @@
  * fn2_flow.h -- C-ABI of libfn2.so for ground-truth flow files: the payloads of .flo, PFM and KITTI PNG files, copied to the
  * device as the bytes they hold after their header (a PNG: once the host has undone its container), converted there to a
  * network input (the input side of the reference's convert_imageset_and_flow + CustomData training path, without the
- * host-side conversions), and for the flow going out: KITTI PNG scanlines and colour-coded images.  The sibling of fn2_frames.h; fn2.h, fn2_frames.h and this header together state the ABI, with
+ * host-side conversions), and for the flow going out: KITTI PNG scanlines, colour-coded images and forward-backward occlusion
+ * masks.  The sibling of fn2_frames.h; fn2.h, fn2_frames.h and this header together state the ABI, with
  * fn2.h's conventions: status 0 or negative with the message in fn2_last_error().
  *
  * Formats:
@@ -38,6 +39,22 @@
  * the float32 pi (so (1, 0) gives exactly -1); fk = (a + 1) / 2 * 54,
  * k0 = (int) fk, k1 = (k0 + 1) % 55, f = fk - k0; per channel col = (1 - f) w[k0] / 255 + f w[k1] / 255, then
  * col = 1 - rad (1 - col) when rad <= 1, else 0.75 col; the byte is (int)(255 col).
+ *
+ * Forward-backward consistency (Sundaram, Brox and Keutzer, ECCV 2010; this project's occlusion estimate, see DESIGN §7): with
+ * fwd the flow from frame 0 to frame 1 and bwd the flow from frame 1 to frame 0, a pixel of frame 0 is occluded (255) or
+ * visible (0).  For pixel (n, y, x), (fu, fv) = fwd(n, y, x):
+ *   255 when fu or fv is not finite;
+ *   255 when the point (x + fu, y + fv) is outside the image: FlowWarp's test x2 >= 0, y2 >= 0, x2 < W, y2 < H on the float32
+ *       x2 = x + fu, y2 = y + fv;
+ *   else (bu, bv) = bwd sampled there with FlowWarp's bilinear taps and mix, the values fn2_flow_warp_forward(image = bwd,
+ *       flow = fwd) writes: ix = (int) x2, iy = (int) y2, ix1 = min(ix + 1, W - 1), iy1 = min(iy + 1, H - 1),
+ *       a = x2 - ix, b = y2 - iy, per channel ((1-a)(1-b) TL + a(1-b) TR) + (1-a) b BL) + a b BR;
+ *   255 when bu or bv is not finite (a tap that is not finite makes the sample so even at weight 0);
+ *   else du = fu + bu, dv = fv + bv, lhs = du du + dv dv, mag = (fu fu + fv fv) + (bu bu + bv bv), and the pixel is 255 iff
+ *       lhs > alpha1 mag + alpha2.
+ * All in float32 with every product rounded separately (no FMA), in the order written, so a float32 restatement reproduces
+ * every byte.  Sundaram et al. use alpha1 = 0.01, alpha2 = 0.5.  The mask of frame 1 is the same call with fwd and bwd
+ * exchanged.
  */
 #ifndef FN2_FLOW_H_
 #define FN2_FLOW_H_
@@ -80,6 +97,13 @@ FN2_API int fn2_flow_to_color(const fn2_tensor* src, const float* max_dev, const
  * zeros), the row layout of fn2_flow_to_kitti_png_rows. */
 FN2_API int fn2_flow_to_color_png_rows(const fn2_tensor* src, const float* max_dev, const float* fallback_dev, float max_flow,
                                        void* dst_dev, void* stream);
+/* fwd, bwd: float views of one shape (N, 2, H, W), any strides, 4-byte aligned -> frame 0's occlusion mask by the
+ * forward-backward check above, one byte per pixel: pixel (n, y, x) at out_dev + n pair_stride + y row_stride + x, on stream.
+ * Nothing else of out_dev is written, so row_stride = 1 + W with out_dev one byte into a buffer gives PNG scanlines of
+ * 8-bit grey (filter None where the buffer holds zeros).  FN2_ERR_INVALID for shapes that differ, c != 2, an alpha that is
+ * negative or not finite, row_stride < W, pair_stride < H row_stride, N above 65535 (the grid's limit) or a misaligned flow. */
+FN2_API int fn2_flow_fb_occlusion(const fn2_tensor* fwd, const fn2_tensor* bwd, float alpha1, float alpha2, void* out_dev,
+                                  size_t row_stride, size_t pair_stride, void* stream);
 /* Host: undoes PNG's per-row filters (types 0-4) of `rows` scanlines of 1 + row_bytes bytes at src into rows * row_bytes
  * bytes at dst; bpp: bytes per complete pixel (1..8), the filters' left distance.  The first row is filtered against zeros.
  * FN2_ERR_INVALID for a filter type above 4, naming the row.  No device work. */
